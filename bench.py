@@ -191,7 +191,7 @@ def measured_peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return d.get("bf16_tflops_sustained", 1443.3), d.get("hbm_gbs", 6567.7), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.0, 3350.0, "fallback (H100 SXM data sheet: dense bf16, HBM3; not measured)"
 
 
 class ClockSampler:
@@ -374,6 +374,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-strong", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     spec = MODELS[args.model]
@@ -462,14 +464,21 @@ def main():
     sync_all()
     launches0 = eng.launches
     sampler = ClockSampler(local_rank) if rank == 0 else None
+    last = {}
+    if args.dump_outputs:                                     # keep the embeddings the step scores (a reference, no copy)
+        score = job.score
+        job.score = lambda emb: (last.__setitem__("emb", emb), score(emb))[1]
     ms, _, res = timed(lambda: job.run_device(pcm), args.steps, 0)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs:
+        job.score = score
+        dump_outputs(Path(args.dump_outputs), rank, res, last["emb"])
     launches = eng.launches - launches0
     fad_value = float(res[0].item())
     audio_s = total_clips * CLIP_SECONDS * args.steps
     value = audio_s / (ms / 1000.0)
 
-    # ---- separate profiled pass -> roofline of the dominant kernel (tcgen05 conv / FC GEMM)
+    # ---- separate profiled pass -> roofline of the dominant kernel (wgmma conv / FC GEMM)
     peak_tf, peak_hbm, peak_src = measured_peaks()
     eng.profile_collect()
     eng.profile(True)
@@ -498,18 +507,15 @@ def main():
         per_layer_factor = 1.5 if wlo_fp8 else 2.0            # an fp8 low-part MMA takes half the tensor-pipe time of an fp16 one
         issued_factor = sum(UMMA_LAYER_FLOP[k] * (per_layer_factor if (split_mask >> i) & 1 else 1.0)
                             for i, k in enumerate(UMMA_LAYER_FLOP)) / sum(UMMA_LAYER_FLOP.values())
-        pair_env = os.environ.get("FADTK_PAIR", "auto")
-        pairs = {"auto": "CTA pairs (cta_group::2, M = 256) on conv3_2, conv4_1, conv4_2, fc1, fc2", "1": "CTA pairs (cta_group::2) on every layer",
-                 "0": "single-CTA MMAs"}.get(pair_env, f"CTA pairs mask {pair_env}")
-        kernel = (f"fad::conv_gemm_kernel<128, STAGES, {2 if wlo_fp8 else 1}, PAIR> (tcgen05 kind::f16, {pairs}; fp16 hi/lo split weights on "
-                  f"{bin(split_mask).count('1')}/8 layers: " + ("low parts as kind::f8f6f4 E4M3 MMAs)" if wlo_fp8 else "2 fp16 MMAs per K slice into one TMEM accumulator)"))
+        kernel = (f"fad::conv_gemm_kernel<128, STAGES, {2 if wlo_fp8 else 1}> (wgmma m64n128k16 f16; fp16 hi/lo split weights on "
+                  f"{bin(split_mask).count('1')}/8 layers: " + ("low parts as E4M3 wgmmas)" if wlo_fp8 else "2 fp16 wgmmas per K slice into one register accumulator)"))
     else:
         # the GEMM category does not cover every GEMM of these forwards (front-end convolutions are timed with the
         # front end): rate over the WHOLE forward - a lower bound of the kernel's own rate that cannot exceed the peak
         denom_ms = forward_ms
         basis = "algorithmic GEMM FLOPs / whole forward time of the profiled pass (lower bound of the kernel's own rate)"
         issued_factor = None
-        kernel = "fad::conv_gemm_kernel (tcgen05 kind::f16; every Linear / convolution-as-GEMM of the forward)"
+        kernel = "fad::conv_gemm_kernel (wgmma f16; every Linear / convolution-as-GEMM of the forward)"
     achieved = flop / (denom_ms / 1000.0) / 1e12 if denom_ms > 0 else 0.0
     per_layer = {k: {"ms_per_launch": prof[k][0] / prof[k][1], "tflops": UMMA_LAYER_FLOP[k] * units / (prof[k][0] / 1000.0) / 1e12}
                  for k in UMMA_LAYER_FLOP if k in prof and prof[k][0] > 0} if args.model == "vggish" else None
@@ -688,6 +694,19 @@ def main():
             "cpu_baseline": cpu, "parity_sample": parity}
     print(json.dumps(line))
     dist.shutdown()
+
+
+def dump_outputs(out_dir: Path, rank: int, res: torch.Tensor, emb: torch.Tensor, max_bytes: int = 60 << 20) -> None:
+    """The last timed step's result vector (fp64[8]: FAD and its terms) and its fp16 embeddings as float32 - all rows
+    when they fit in `max_bytes`, else a fixed seeded sample of rows (sorted, so the same rows for the same shape)."""
+    out_dir.mkdir(parents=True, exist_ok=True)
+    sfx = f"_rank{rank}" if rank else ""
+    np.save(out_dir / f"result{sfx}.npy", res.detach().cpu().numpy().astype(np.float64))
+    n, d = emb.shape
+    keep = max(1, min(n, (max_bytes - 4096) // (4 * d)))
+    rows = np.arange(n) if keep == n else np.sort(np.random.default_rng(0).choice(n, keep, replace=False))
+    np.save(out_dir / f"embeddings{sfx}.npy", emb[torch.from_numpy(rows).to(emb.device)].float().cpu().numpy())
+    np.save(out_dir / f"embedding_rows{sfx}.npy", rows.astype(np.float64))
 
 
 def files_flow(ml, clips: int, baseline_clips: int, sr: int, workers: int = 16) -> dict:

@@ -25,7 +25,7 @@ for S, d, n, scale in ((199, 768, 8, 1.0), (199, 768, 8, 2.5), (1500, 768, 2, 1.
     want = (p @ v).permute(0, 2, 1, 3).reshape(n * S, d)
     rms = want.pow(2).mean().sqrt().item()
     row = {"S": S, "score_scale": scale, "max_p_mean": p.max(-1).values.mean().item()}
-    for name, legacy in (("tcgen05", False), ("mma_sync", True)):
+    for name, legacy in (("wgmma", False), ("mma_sync", True)):
         got = eng.attention(qkv, n, legacy=legacy).double()
         err = got - want
         row[name] = {"rms_rel": err.pow(2).mean().sqrt().item() / rms, "mean_rel": err.mean().item() / rms,

@@ -25,4 +25,4 @@ for seed in range(int(sys.argv[1]) if len(sys.argv) > 1 else 4):
     fg = fk.calc_frechet_distance(*fk.calc_embd_statistics(gpu["base"]), *fk.calc_embd_statistics(gpu["eval"]))
     fc = fo.frechet_distance(*fo.embd_statistics(cpu["base"]), *fo.embd_statistics(cpu["eval"]))
     out.append({"seed": seed, "fad_gpu": float(fg), "fad_cpu": float(fc), "rel": float((fg - fc) / fc)})
-print(json.dumps({"attention": os.environ.get("FADTK_ATTN", "tcgen05"), "sets": out}))
+print(json.dumps({"attention": os.environ.get("FADTK_ATTN", "wgmma"), "sets": out}))

@@ -1,7 +1,7 @@
 """End to end through FILES on one GPU: .wav directories -> convert cache -> embeddings (.npy) -> statistics -> FAD,
 i.e. what `python -m fadtk_b200 vggish <baseline dir> <eval dir>` does (fadtk/__main__.py:39-70), timed as a whole.
 Synthetic 10-s clips at the model rate; prints one JSON line.
-Usage (on a B200): python benchmarks/file_flow.py [--clips 3000] [--baseline-clips 500] [--workers 16]
+Usage (on an H100): python benchmarks/file_flow.py [--clips 3000] [--baseline-clips 500] [--workers 16]
 """
 import argparse
 import json

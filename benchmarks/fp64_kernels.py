@@ -61,7 +61,7 @@ def main():
     dev = eng.torch_device
     peaks = json.loads((ROOT / "MEASURED_PEAKS.json").read_text()) if (ROOT / "MEASURED_PEAKS.json").exists() else {}
     hbm = peaks.get("hbm_gbs", 6650.0)
-    out = {"hbm_peak_gbs": hbm, "hbm_peak_source": "MEASURED_PEAKS.json" if peaks else "fallback (B200_PROFILING.md)"}
+    out = {"hbm_peak_gbs": hbm, "hbm_peak_source": "MEASURED_PEAKS.json" if peaks else "fallback (H100 SXM data sheet, not measured)"}
     dmma = eng.dmma_peak_tflops() if "peak" in what else None
     if dmma:
         dmma = max(dmma, eng.dmma_peak_tflops())

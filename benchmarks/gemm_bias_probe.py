@@ -1,4 +1,4 @@
-"""Does the tcgen05 GEMM (fp16 activations, fp16 hi/lo weights, fp32 TMEM accumulation cut every 512 of K) carry a SYSTEMATIC
+"""Does the wgmma GEMM (fp16 activations, fp16 hi/lo weights, fp32 register accumulation cut every 512 of K) carry a SYSTEMATIC
 per-output-channel error?  fp32 outputs of fad_umma_layer vs an fp64 product of the same fp16 activations and fp32 weights:
 rms error, error of the per-channel mean over all rows, and what that would be if the errors were independent."""
 import json

@@ -17,7 +17,7 @@ for line in txt.splitlines():
         rows.append((cur, int(m.group(1)), int(m.group(2)), int(m.group(3))))
         cur = None
 names = subprocess.run(["c++filt"] + [r[0] for r in rows], capture_output=True, text=True).stdout.splitlines()
-print("# Kernel resource audit, end of round 2 (`cuobjdump -res-usage fadtk_b200/csrc/libfadtk_b200.so`, sm_100a)\n")
+print("# Kernel resource audit, end of round 2 (`cuobjdump -res-usage fadtk_b200/csrc/libfadtk_b200.so`, sm_90a)\n")
 print("Registers per thread, stack bytes (spills / local arrays), static shared memory; dynamic shared memory (conv_gemm,")
 print("attention_umma, logmel, stats_umma) is set at launch.  New this round: `attention_umma_kernel` (320 threads, two CTAs per")
 print("SM), the fp64 tensor-pipe kernels (`dgemm_kernel`, `dgemm_strided_kernel`, `stats_dmma_kernel<__half | double>`,")

@@ -1,4 +1,4 @@
-"""Per-shape rate of the tcgen05 GEMM kernel on the Linear layers of the transformer forwards (stage entry
+"""Per-shape rate of the wgmma GEMM kernel on the Linear layers of the transformer forwards (stage entry
 fad_umma_layer, H = W = 1): split weights with and without CTA pairs, and plain fp16 weights for scale.
 TFLOP/s are ALGORITHMIC (2 M N K once).  One JSON list on stdout."""
 import json

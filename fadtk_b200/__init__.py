@@ -1,8 +1,8 @@
-"""fadtk_b200 - B200-native drop-in for the embedding -> statistics -> FAD path of microsoft/fadtk.
+"""fadtk_b200 - H100-native drop-in for the embedding -> statistics -> FAD path of microsoft/fadtk.
 
 Export surface mirrors fadtk/__init__.py:1-4 (star re-exports of fad, fad_batch, model_loader,
 utils).  Importing the package needs neither a GPU nor the compiled library; the first compute
-call loads csrc/libfadtk_b200.so and fails loudly if it or a B200 is missing.
+call loads csrc/libfadtk_b200.so and fails loudly if it or an H100 is missing.
 """
 from .fad import *            # noqa: F401,F403
 from .fad import FADInfResults, FrechetAudioDistance, calc_embd_statistics, calc_frechet_distance, log  # noqa: F401

@@ -1,7 +1,7 @@
 """ctypes binding of the C ABI in include/fadtk_b200.h (csrc/libfadtk_b200.so).
 
 PyTorch tensors are only containers here: every call passes ``tensor.data_ptr()`` and the
-current CUDA stream.  There is no CPU fallback - if the shared library or a B200 is missing
+current CUDA stream.  There is no CPU fallback - if the shared library or an H100 is missing
 the import of a compute entry point raises.
 """
 from __future__ import annotations
@@ -74,7 +74,6 @@ SIGNATURES = {
     "fad_frechet_batched": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_attention": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "fad_bench_dmma_peak": (C.c_int, [c_vp, C.c_int, c_vp]),
-    "fad_bench_umma_mode": (C.c_int, [c_vp, C.c_int, C.c_int, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -185,12 +184,6 @@ class Engine:
         out = torch.empty((qkv.shape[0], d), dtype=torch.float16, device=qkv.device)
         _check(lib().fad_attention(self._h, qkv.data_ptr(), n_clips, S, d, out.data_ptr(), int(legacy), _stream()))
         return out
-
-    def umma_mode_ms(self, mode: int, ksteps: int = 40000) -> float:
-        """tensor-pipe microbenchmark (csrc/umma_bench.cuh): ms for `ksteps` split-weight K steps per SM under issue pattern `mode`"""
-        out = C.c_double(0.0)
-        _check(lib().fad_bench_umma_mode(self._h, int(mode), int(ksteps), C.byref(out)))
-        return float(out.value)
 
     def dmma_peak_tflops(self, iters: int = 0) -> float:
         """measured fp64 tensor-pipe (DMMA) rate, TFLOP/s: roofline denominator of the fp64 kernels"""

@@ -1,5 +1,5 @@
 // CLAP-LAION audio branch (HTSAT-tiny Swin transformer) - the CUDA-core kernels around the
-// tcgen05 GEMMs.  Replaces laion_clap / torchlibrosa behind CLAPLaionModel._get_embedding
+// wgmma GEMMs.  Replaces laion_clap / torchlibrosa behind CLAPLaionModel._get_embedding
 // (fadtk/model_loader.py:389-411); architecture per SURVEY.md appendix B and the HF port of
 // htsat.py (oracle/clap_oracle.py is pinned to it).
 //
@@ -368,7 +368,7 @@ clap_copy_rows_kernel(float* __restrict__ x, const float* __restrict__ y, long l
 }
 
 // Window attention on the warp-level tensor-core path (mma.sync m16n8k16 / m16n8k8, fp16 in / fp32
-// accumulate): a 64 x 64 x 24 problem per (window, head) is far too small for a tcgen05/TMEM tile,
+// accumulate): a 64 x 64 x 24 problem per (window, head) is far too small for a wgmma tile,
 // but maps exactly onto 16x8 fragments.  One warp per (window, head):
 //   staging  Q, K, V rows (24 halves = 48 B each) with 16-B cp.async into warp-private smem, row
 //            stride 48 B: conflict-free for the fragment loads below and for ldmatrix

@@ -1,4 +1,4 @@
-// Implicit-GEMM 3x3 convolution / fully-connected layer on tcgen05 tensor cores.
+// Implicit-GEMM 3x3 convolution / fully-connected layer on Hopper tensor cores (wgmma).
 //
 //   D[128 pixels, N_TILE channels] = sum over (tap, 64-channel block) of
 //         X_tap[128 pixels, 64 ch] (fp16, K-major, TMA im2col-by-coordinates)
@@ -12,22 +12,20 @@
 // BW x BH x BN box of pixels (BW*BH*BN = 128); for filter tap (kh, kw) the A operand is the
 // same box shifted by (kh-1, kw-1), fetched with ONE 4-D TMA whose out-of-bounds elements are
 // zero-filled by hardware - that is the conv padding, and there is no im2col buffer.  TMA
-// writes the 128-byte swizzled K-major layout tcgen05.mma consumes directly.
+// writes the 128-byte swizzled K-major layout wgmma consumes directly.
 //
-// Accumulation.  The tensor core adds into its fp32 accumulator with truncation: measured on
-// B200, a K-long reduction comes out scaled by (1 - 1.0e-9 K) (tests/diag_accum_bias.py: -1.25e-5
-// at K = 12288) - over the eight layers that alone moves the FAD by ~6e-5 relative.  So the MMA
-// warp accumulates at most kChunkSteps x 64 = 512 of K into one TMEM buffer, and the epilogue
-// warps sum the chunks in registers with ordinary round-to-nearest fp32 adds.  The two TMEM
-// buffers alternate per CHUNK, so draining chunk c overlaps the MMAs of chunk c+1.
+// Accumulation.  The tensor core adds into its fp32 accumulator with truncation, so a long K
+// reduction comes out slightly shrunk (tests/diag_accum_bias.py measures it).  So each consumer
+// warpgroup accumulates at most kChunkSteps x 64 = 512 of K into its wgmma accumulator, then adds
+// the chunk into a second register array with ordinary round-to-nearest fp32 adds.
 //
 // Warp roles (384 threads, persistent over tiles):
-//   warp 0  TMA producer (one elected lane)        warp 2  TMEM allocator
-//   warp 1  MMA issuer   (one elected lane)        warps 4-11 epilogue: TMEM lane quarter = warp%4,
-//                                                  column half = (warp-4)/4
-// Pipelines: smem ring full[]/empty[] (TMA <-> MMA), TMEM chunk buffers tmem_full[]/tmem_empty[].
+//   warpgroup 0     TMA producer (one elected lane of warp 0)
+//   warpgroups 1-2  consumers: warpgroup 1 + c issues the wgmmas of tile rows [64 c, 64 c + 64) and runs
+//                   their epilogue (accumulator -> shared-memory tile -> one row per thread)
+// Pipeline: smem ring full[] (TMA -> consumers) / empty[] (consumers -> TMA).
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace fad {
 
@@ -72,46 +70,41 @@ __device__ __forceinline__ long long window_row_to_token(long long o, int res, i
 constexpr int kTileM = 128;
 constexpr int kBlockK = 64;                        // fp16 elements per 128-B swizzled row
 constexpr int kConvGemmThreads = 384;
-constexpr int kEpilogueWarps = 8;
-constexpr int kChunkSteps = 8;                     // k-steps (of 64) per TMEM accumulation chunk
+constexpr int kConsumers = 2;                      // consumer warpgroups, 64 tile rows each
+constexpr int kChunkSteps = 8;                     // k-steps (of 64) per accumulation chunk
 // The tensor core truncates when it adds into its fp32 accumulator: a sum over T accumulated elements (T = K of the
-// chunk, x 2 when the hi and lo weight MMAs share the accumulator) comes out scaled by (1 - 1.0e-9 T) - measured on
-// B200 for random and post-ReLU operands, shapes K = 384 ... 12288 (tests/diag_accum_bias.py; profiles/
-// r2_gemm_bias_probe_before.json: -8.1e-7 at T = 768, -1.08e-6 at T = 1024, -4.1e-7 at T = 384).  Cutting K into chunks
-// bounds it, but what is left is SYSTEMATIC: through the ~50 GEMMs of a transformer encoder it adds up to a per-
-// dimension offset of the hidden states (wav2vec: 8e-5 of their rms at layer 12, 10x what independent errors would
-// give, and a -2e-4 offset of the FAD, profiles/r2_w2v_layer_bias_before.json).  The epilogue therefore scales every
-// chunk by the inverse of its expected shrink when it sums the chunks in registers: v + v * eps as one FMA (1 + eps
-// itself is not representable finely enough in fp32: eps ~ 1e-6 is only 8 ulps of 1).
+// chunk) comes out scaled by (1 - c T), c = 1.06e-9 measured on H100 with tests/diag_accum_bias.py.  Cutting K into
+// chunks bounds it, but what is left is SYSTEMATIC: through the ~50 GEMMs of a transformer encoder it adds up to a
+// per-dimension offset of the hidden states and of the FAD.  The consumer therefore scales every chunk by the inverse
+// of its expected shrink when it sums the chunks in registers: v + v * eps as one FMA (1 + eps itself is not
+// representable finely enough in fp32: eps ~ 1e-6 is only 8 ulps of 1).  c is what tests/diag_accum_bias.py measures.
 constexpr float kAccumShrinkPerElement = 1.06e-9f;
 constexpr uint32_t kABytes = kTileM * kBlockK * 2; // 16 KiB per stage
-constexpr uint32_t kStagingBytes = 32 * 128;       // per epilogue warp: 32 rows x 128 B output staging
+constexpr uint32_t kEpiRowBytes = 128 * 4;         // one fp32 row of a 128-column accumulator tile
+constexpr uint32_t kEpiBytes = 64 * kEpiRowBytes;  // per consumer: 64 rows x 128 fp32 (32 KiB)
+constexpr uint32_t kStagingBytes = 32 * 128;       // per epilogue warp: 32 rows x 128 B output staging (inside kEpiBytes)
 
 // SPLIT_W: the weights are an fp16 hi/lo pair (W = Wh + Wl, 22 bits).  fp16 rounding of the
 // weights is a fixed perturbation of the model that does not average out over samples: it alone
 // moves the FAD by ~1.4e-4 relative (CPU experiment, DESIGN.md), more than the whole 1e-4 budget,
 // whereas fp16 activations cost 2e-5.  The hi and lo rows of one N tile are stored back to back
-// ([Wh: N_TILE rows | Wl: N_TILE rows] per tile), so ONE TMA box brings both and the MMA warp
-// issues A x Wh and A x Wl into the same TMEM accumulator.
-// WMODE 0: fp16 weights.  1: fp16 hi/lo pair, two kind::f16 MMAs per K step.  2: fp16 hi + E4M3 lo:
-// the low part (|Wl| <= 2^-11 |W|, needed to ~4 bits) is applied by a kind::f8f6f4 MMA - twice the
-// rate and half the operand bytes of a second fp16 MMA - against an E4M3 copy of the activation
+// ([Wh: N_TILE rows | Wl: N_TILE rows] per tile), so ONE TMA box brings both and each consumer
+// issues A x Wh and A x Wl into the same accumulator.
+// WMODE 0: fp16 weights.  1: fp16 hi/lo pair, two fp16 wgmmas per K slice.  2: fp16 hi + E4M3 lo:
+// the low part (|Wl| <= 2^-11 |W|, needed to ~4 bits) is applied by an E4M3 wgmma - twice the
+// rate and half the operand bytes of a second fp16 one - against an E4M3 copy of the activation
 // (written next to the fp16 one by the producing kernel, fetched by its own TMA box), into its own
-// TMEM accumulator that the epilogue adds with the power-of-two scale of the E4M3 weights.
-// PAIR: two CTAs (one cluster, the two SMs of a TPC) share every MMA with cta_group::2 - M = 256, each CTA holds its
-// own 128-row A tile and HALF of the weight tile, so a stage carries half the weight bytes per CTA (the kernel is
-// bound by what each SM pulls from L2 per k-step, not by the tensor pipe: ncu, profiles/r2_ncu_conv_gemm_pair.md).
-template <int N_TILE, int WMODE, int PAIR = 0>
+// register accumulator that the epilogue adds with the power-of-two scale of the E4M3 weights.
+template <int N_TILE, int WMODE>
 __host__ __device__ constexpr uint32_t conv_gemm_stage_bytes() {
-    constexpr int kNLoc = PAIR ? N_TILE / 2 : N_TILE;
-    return WMODE == 2 ? kABytes + kNLoc * kBlockK * 2 + kNLoc * kBlockK + kTileM * kBlockK
-                      : kABytes + (WMODE == 1 ? 2 : 1) * kNLoc * kBlockK * 2;
+    return WMODE == 2 ? kABytes + N_TILE * kBlockK * 2 + N_TILE * kBlockK + kTileM * kBlockK
+                      : kABytes + (WMODE == 1 ? 2 : 1) * N_TILE * kBlockK * 2;
 }
 
-template <int N_TILE, int STAGES, int WMODE, int PAIR = 0>
+template <int N_TILE, int STAGES, int WMODE>
 __host__ __device__ constexpr uint32_t conv_gemm_smem_bytes() {
-    return STAGES * conv_gemm_stage_bytes<N_TILE, WMODE, PAIR>() + 1024 /*align slack*/ + 256 /*barriers*/
-         + kEpilogueWarps * kStagingBytes;
+    return STAGES * conv_gemm_stage_bytes<N_TILE, WMODE>() + 1024 /*align slack*/ + 256 /*barriers*/
+         + kConsumers * kEpiBytes;
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
@@ -164,7 +157,7 @@ __device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
     return *reinterpret_cast<uint32_t*>(&r);
 }
 
-template <int N_TILE, int STAGES, int WMODE, int PAIR = 0, int STACK = 0>
+template <int N_TILE, int STAGES, int WMODE>
 __global__ void __launch_bounds__(kConvGemmThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                  const __grid_constant__ CUtensorMap map_w,
@@ -172,40 +165,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                  const __grid_constant__ CUtensorMap map_x8,        // WMODE 2: E4M3 copy of the activation
                  const ConvGemmParams p)
 {
-    using namespace sm100;
+    using namespace sm90;
+    static_assert(N_TILE == 128, "one m64n128 accumulator per consumer warpgroup");
     constexpr bool SPLIT_W = WMODE == 1;
     constexpr bool LO8 = WMODE == 2;
-    constexpr uint32_t kStageBytes = conv_gemm_stage_bytes<N_TILE, WMODE, PAIR>();
+    constexpr uint32_t kStageBytes = conv_gemm_stage_bytes<N_TILE, WMODE>();
     constexpr int kBRows = (WMODE != 0 ? 2 : 1) * N_TILE;           // rows of the packed weight tensor per N tile
-    constexpr int kNLoc = PAIR ? N_TILE / 2 : N_TILE;               // weight rows (output channels) THIS CTA stages
-    // STACKED (SPLIT_W && STACK; measurement variant, off by default): hi and lo weight rows as ONE B operand of N = 2 N_TILE
-    // rows ([Wh | Wl] is how a stage holds them); the product lands in two column halves of the accumulator (hi: [0, N_TILE),
-    // lo: [N_TILE, 2 N_TILE)) that the epilogue adds.  One MMA per K slice instead of two, A fetched from shared memory
-    // once: 16 % faster on the bare tensor pipe (profiles/r2_umma_issue_patterns.json: 2.24 vs 1.89 PFLOP/s issued) - but
-    // not in this kernel, which runs against the power cap, and it costs a second TMEM read per epilogue group
-    // (profiles/r2_ncu_vggish_pair.md); the default accumulates A Wh^T and A Wl^T into the same TMEM tile.
-    constexpr bool STACKED = SPLIT_W && STACK != 0;
-    constexpr uint32_t kBufCols = (STACKED ? 2 : 1) * N_TILE;       // TMEM columns of one chunk buffer
-    constexpr uint32_t kTmemCols = LO8 ? 4 * N_TILE : 2 * kBufCols; // two chunk buffers (+ two low-part buffers)
-    constexpr uint32_t kIdesc = make_idesc(FMT_F16, PAIR ? 2 * kTileM : kTileM, STACKED ? 2 * N_TILE : N_TILE);
-    constexpr uint32_t kIdesc8 = make_idesc(FMT_E4M3, PAIR ? 2 * kTileM : kTileM, N_TILE);
-    constexpr uint32_t kWhBytes = kNLoc * kBlockK * 2;
+    constexpr uint32_t kWhBytes = N_TILE * kBlockK * 2;
     constexpr uint32_t kOffWl8 = kABytes + kWhBytes;                // stage layout (LO8): A16 | Wh | Wl8 | A8
-    constexpr uint32_t kOffA8 = kOffWl8 + kNLoc * kBlockK;
-    static_assert(!PAIR || WMODE != 0, "pairs are built for the split-weight modes");
-    constexpr int kColsPerWarp = N_TILE / 2;            // each lane quarter is shared by two warps
-    constexpr int kGroups = kColsPerWarp / 32;
+    constexpr uint32_t kOffA8 = kOffWl8 + N_TILE * kBlockK;
+    constexpr int kColsPerThread = N_TILE / 2;          // epilogue: one row, one column half per thread
+    constexpr int kGroups = kColsPerThread / 32;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * kStageBytes);
     uint64_t* full = bars;
     uint64_t* empty = bars + STAGES;
-    uint64_t* tmem_full = bars + 2 * STAGES;
-    uint64_t* tmem_empty = bars + 2 * STAGES + 2;
-    uint64_t* corr_empty = bars + 2 * STAGES + 4;                    // LO8: low-part accumulator drained
-    uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 6);
-    uint8_t* staging = smem + STAGES * kStageBytes + 256;            // kEpilogueWarps x kStagingBytes
+    uint8_t* epi = smem + STAGES * kStageBytes + 256;                // kConsumers x kEpiBytes
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -213,13 +190,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
     const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;       // balanced chunks
     const int m_tiles = p.img_groups * p.tiles_h * p.tiles_w;
-    // work unit = one N tile x (one M tile | PAIR: two consecutive M tiles, one per CTA of the pair; the second of an
-    // odd count is past the batch: its TMA boxes are zero-filled and its rows masked in the epilogue)
-    const uint32_t rank = PAIR ? cluster_ctarank() : 0;
-    const int n_workers = PAIR ? (int)gridDim.x / 2 : (int)gridDim.x;
-    const int worker = PAIR ? (int)blockIdx.x / 2 : (int)blockIdx.x;
-    const int m_units = PAIR ? (m_tiles + 1) / 2 : m_tiles;
-    const int total_tiles = m_units * p.n_tiles;
+    const int total_tiles = m_tiles * p.n_tiles;                    // work unit = one M tile x one N tile
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_x);
@@ -227,29 +198,20 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
         if (LO8) { tma_prefetch_desc(&map_wl8); tma_prefetch_desc(&map_x8); }
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        // PAIR: the leader's tmem_empty / corr_empty collect the epilogue warps of BOTH CTAs
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], kEpilogueWarps * (PAIR ? 2 : 1)); }
-        for (int a = 0; a < 2; ++a) mbar_init(&corr_empty[a], kEpilogueWarps * (PAIR ? 2 : 1));
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers * 4); }
         mbar_fence_init();
     }
-    if (warp == 2) { if (PAIR) tmem_alloc_pair<kTmemCols>(tmem_base_slot); else tmem_alloc<kTmemCols>(tmem_base_slot); }
-    tc_fence_before_sync();
-    if (PAIR) cluster_sync(); else __syncthreads();           // PAIR: the peer's barriers exist before anything signals them
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_base_slot;
+    __syncthreads();
 
-    // warps 0-3 (one warpgroup) only issue TMA / MMA: hand their registers to the two epilogue
-    // warpgroups, which hold N_TILE/2 fp32 partial sums per thread.  128*88 + 256*208 <= 64 K.
     if (warp < 4) {
-      setmaxnreg_dec<88>();
-      if (warp == 0) {
         // ------------------------------------------------------------ TMA producer
-        if (elect_one()) {
+        // hand the registers of this warpgroup to the two consumers, which hold 2 x 64 (+ 64) fp32 accumulators
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
             int s = 0; uint32_t ph = 0;
-            for (int tile = worker; tile < total_tiles; tile += n_workers) {
+            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
                 const int nt = tile % p.n_tiles;
-                const int m = PAIR ? 2 * (tile / p.n_tiles) + (int)rank : tile / p.n_tiles;
+                const int m = tile / p.n_tiles;
                 const int w0 = (m % p.tiles_w) * p.box_w;
                 const int h0 = ((m / p.tiles_w) % p.tiles_h) * p.box_h;
                 const int n0 = (m / (p.tiles_w * p.tiles_h)) * p.box_n;
@@ -260,25 +222,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     if (p.taps == 9) { dh = tap / 3 - 1; dw = tap % 3 - 1; }
                     mbar_wait(&empty[s], ph ^ 1);
                     uint8_t* st = smem + s * kStageBytes;
-                    if (PAIR) {
-                        // both CTAs' bytes land on the LEADER's barrier (the MMA issuer waits there); a peer's bytes may
-                        // complete before the leader arms the phase - the transaction count is signed, that is fine
-                        if (rank == 0) mbar_expect_tx(&full[s], 2 * kStageBytes);
-                        const uint32_t bar = mapa_u32(smem_u32(&full[s]), 0);
-                        tma_load_4d_pair(st, &map_x, bar, cb * kBlockK, w0 + dw, h0 + dh, n0);
-                        // this CTA's half of the hi rows (and of the lo rows: a second box).  STACKED: B of the pair's N = 2 N_TILE
-                        // MMA is [Wh | Wl]: rank 0 stages all hi rows, rank 1 all lo rows (one box of N_TILE rows each)
-                        if (STACKED) tma_load_2d_pair(st + kABytes, &map_w, bar, ks * kBlockK, nt * kBRows + (int)rank * N_TILE);
-                        else {
-                            tma_load_2d_pair(st + kABytes, &map_w, bar, ks * kBlockK, nt * kBRows + (int)rank * kNLoc);
-                            if (SPLIT_W)
-                                tma_load_2d_pair(st + kABytes + kWhBytes, &map_w, bar, ks * kBlockK, nt * kBRows + N_TILE + (int)rank * kNLoc);
-                        }
-                        if (LO8) {
-                            tma_load_2d_pair(st + kOffWl8, &map_wl8, bar, ks * kBlockK, nt * N_TILE + (int)rank * kNLoc);
-                            tma_load_4d_pair(st + kOffA8, &map_x8, bar, cb * kBlockK, w0 + dw, h0 + dh, n0);
-                        }
-                    } else {
                     mbar_expect_tx(&full[s], kStageBytes);
                     tma_load_4d(st, &map_x, &full[s], cb * kBlockK, w0 + dw, h0 + dh, n0);
                     tma_load_2d(st + kABytes, &map_w, &full[s], ks * kBlockK, nt * kBRows);
@@ -286,94 +229,29 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                         tma_load_2d(st + kOffWl8, &map_wl8, &full[s], ks * kBlockK, nt * N_TILE);
                         tma_load_4d(st + kOffA8, &map_x8, &full[s], cb * kBlockK, w0 + dw, h0 + dh, n0);
                     }
-                    }
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
             }
         }
-      } else if (warp == 1 && rank == 0) {
-        // -------------------------------------------------------------- MMA issuer (PAIR: the leader CTA only)
-        if (elect_one()) {
-            int s = 0; uint32_t ph = 0;
-            int buf = 0; uint32_t buf_ph = 0;
-            int cpar = 0; uint32_t cpar_ph = 0;
-            int pend_stage[4] = {0, 0, 0, 0}; bool pend_first[4] = {false, false, false, false}; int n_pend = 0;
-            for (int tile = worker; tile < total_tiles; tile += n_workers) {
-                const uint32_t d_corr = tmem_base + 2 * N_TILE + cpar * N_TILE;
-                if (LO8) { mbar_wait(&corr_empty[cpar], cpar_ph ^ 1); tc_fence_after_sync(); }
-                for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
-                    const int ks1 = min(ks0 + chunk_len, ksteps);
-                    mbar_wait(&tmem_empty[buf], buf_ph ^ 1);
-                    tc_fence_after_sync();
-                    const uint32_t d_tmem = tmem_base + buf * kBufCols;
-                    for (int ks = ks0; ks < ks1; ++ks) {
-                        mbar_wait(&full[s], ph);
-                        tc_fence_after_sync();
-                        const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
-                        const uint64_t a_desc = kmajor_sw128_desc(a_addr);
-                        const uint64_t b_desc = kmajor_sw128_desc(a_addr + kABytes);
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 16; ++k) {
-                            // +32 B along K inside the 128-B swizzle atom == +2 in the 16-B address field
-                            if (PAIR) umma_f16_pair(d_tmem, a_desc + 2 * k, b_desc + 2 * k, kIdesc, (ks > ks0) || (k > 0));
-                            else      umma_f16(d_tmem, a_desc + 2 * k, b_desc + 2 * k, kIdesc, (ks > ks0) || (k > 0));
-                            if (SPLIT_W && !STACKED) {         // lo rows: kNLoc rows (x 128 B) further down the stage, same accumulator
-                                if (PAIR) umma_f16_pair(d_tmem, a_desc + 2 * k, b_desc + 2 * k + (kNLoc * 128 / 16), kIdesc, 1);
-                                else      umma_f16(d_tmem, a_desc + 2 * k, b_desc + 2 * k + (kNLoc * 128 / 16), kIdesc, 1);
-                            }
-                        }
-                        if (LO8) {
-                            // The E4M3 low-part MMAs of the last `lo8_group` k-steps are issued together, after their
-                            // fp16 MMAs: alternating kind::f16 / kind::f8f6f4 every k-step drains the tensor pipe at
-                            // each switch (ncu: tensor pipe 58-71 % with per-k-step alternation, r2_ncu_wlo8).  A stage
-                            // is released once BOTH its MMAs have been issued, so a group holds `lo8_group` stages.
-                            pend_stage[n_pend] = s; pend_first[n_pend] = (ks == 0); ++n_pend;
-                            if (n_pend == p.lo8_group || ks == ks1 - 1) {
-                                for (int q = 0; q < n_pend; ++q) {
-                                    const uint32_t q_addr = smem_u32(smem + pend_stage[q] * kStageBytes);
-                                    const uint64_t a8_desc = kmajor_sw64_desc(q_addr + kOffA8);
-                                    const uint64_t w8_desc = kmajor_sw64_desc(q_addr + kOffWl8);
-#pragma unroll
-                                    for (int k = 0; k < kBlockK / 32; ++k) { // K = 32 per kind::f8f6f4 MMA, +32 B inside the 64-B atom
-                                        if (PAIR) umma_f8_pair(d_corr, a8_desc + 2 * k, w8_desc + 2 * k, kIdesc8, !pend_first[q] || (k > 0));
-                                        else      umma_f8(d_corr, a8_desc + 2 * k, w8_desc + 2 * k, kIdesc8, !pend_first[q] || (k > 0));
-                                    }
-                                    if (PAIR) umma_commit_pair(&empty[pend_stage[q]]); else umma_commit(&empty[pend_stage[q]]);
-                                }
-                                n_pend = 0;
-                            }
-                        } else {
-                            if (PAIR) umma_commit_pair(&empty[s]); else umma_commit(&empty[s]);   // smem slot(s) free once these MMAs retire
-                        }
-                        if (++s == STAGES) { s = 0; ph ^= 1; }
-                    }
-                    if (PAIR) umma_commit_pair(&tmem_full[buf]); else umma_commit(&tmem_full[buf]);   // chunk complete -> epilogue warps
-                    if (++buf == 2) { buf = 0; buf_ph ^= 1; }
-                }
-                if (++cpar == 2) { cpar = 0; cpar_ph ^= 1; }
-            }
-        }
-      }
     } else {
-        // ---------------------------------------------------------------- epilogue
-        setmaxnreg_inc<208>();
-        const int q = warp & 3;                           // TMEM lane quarter this warp may read
-        const int half = (warp - 4) >> 2;                 // which half of the tile's columns
-        const int r = q * 32 + lane;                      // row of the tile == TMEM lane
+        // ------------------------------------------------------------ consumers: wgmma + epilogue
+        setmaxnreg_inc<232>();
+        const int c = (warp >> 2) - 1;                    // consumer index: tile rows [64 c, 64 c + 64)
+        const int wg_t = threadIdx.x & 127;               // thread within the warpgroup
+        const int wq = wg_t >> 5;                         // warp within the warpgroup
+        // epilogue role: row rr of this consumer's 64, column half `half`
+        const int rr = wg_t & 63;
+        const int half = wg_t >> 6;
+        const int r = c * 64 + rr;                        // row of the tile
         const int bw = p.box_w, bh = p.box_h;
         const int pw = r % bw;
         const int phh = (r / bw) % bh;
         const int pn = r / (bw * bh);
-        int buf = 0; uint32_t buf_ph = 0;
-        int cpar = 0;
+        const uint32_t epi_base = smem_u32(epi) + c * kEpiBytes;
+        const uint32_t bar_id = 1 + c;
+        int s = 0; uint32_t ph = 0;
         // plain row-major GEMM (1x1 "image", 128 rows per tile): no per-tile divisions
         const bool plain = p.tiles_w == 1 && p.tiles_h == 1 && bw == 1 && bh == 1;
-        // (nt, mu) of this worker's current unit, stepped without divisions; m = the M tile of THIS CTA
-        int nt = worker % p.n_tiles, mu = worker / p.n_tiles;
-        const int step_nt = n_workers % p.n_tiles, step_m = n_workers / p.n_tiles;
-        int m = PAIR ? 2 * mu + (int)rank : mu;
-        const uint32_t te_addr[2] = {PAIR ? mapa_u32(smem_u32(&tmem_empty[0]), 0) : 0u, PAIR ? mapa_u32(smem_u32(&tmem_empty[1]), 0) : 0u};
-        const uint32_t ce_addr[2] = {PAIR ? mapa_u32(smem_u32(&corr_empty[0]), 0) : 0u, PAIR ? mapa_u32(smem_u32(&corr_empty[1]), 0) : 0u};
         // residual rows are read-modify-written in the epilogue: pull the NEXT tile's rows into L2
         // while this tile is computed, so the loads do not pay HBM latency on the critical path
         auto prefetch_resid = [&](int nt_, int m_) {
@@ -381,21 +259,99 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
             const int n_ = m_ * kTileM + r;
             if (n_ >= p.NB) return;
             const long long tok = p.resid_res ? window_row_to_token((long long)n_, p.resid_res, p.resid_shift) : (long long)n_;
-            const int c0 = nt_ * N_TILE + half * kColsPerWarp;
-            for (int c = c0; c < c0 + kColsPerWarp && c < p.resid_C; c += 32)
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(p.resid + tok * p.resid_C + c));
+            const int c0 = nt_ * N_TILE + half * kColsPerThread;
+            for (int cc = c0; cc < c0 + kColsPerThread && cc < p.resid_C; cc += 32)
+                asm volatile("prefetch.global.L2 [%0];" :: "l"(p.resid + tok * p.resid_C + cc));
         };
-        if (mu < m_units) prefetch_resid(nt, m);
-        // The unit index itself is not carried: unit = mu * n_tiles + nt < total_tiles  <=>  mu < m_units.  (One loop scalar
-        // less: the round-1 form kept the counter and tmem_base in LOCAL memory - ptxas spills what crosses the setmaxnreg
-        // split - and reloaded both on the critical path of every tile: 9 % of the epilogue warps' stall samples on the
-        // CLAP layers, profiles/r2_ncu_clap_gemm.md.)
+        if ((int)blockIdx.x < total_tiles) prefetch_resid((int)blockIdx.x % p.n_tiles, (int)blockIdx.x / p.n_tiles);
         auto load_bias = [&](float4 (&b)[8], int col0) {
             const float4* src = reinterpret_cast<const float4*>(p.bias + col0);
 #pragma unroll
             for (int j = 0; j < 8; ++j) b[j] = __ldg(src + j);
         };
-        while (mu < m_units) {
+
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int nt = tile % p.n_tiles;
+            const int m = tile / p.n_tiles;
+            if (tile + (int)gridDim.x < total_tiles)
+                prefetch_resid((tile + (int)gridDim.x) % p.n_tiles, (tile + (int)gridDim.x) / p.n_tiles);
+
+            // ---- main loop: chunks of <= kChunkSteps k-steps into `acc`, summed into `sum` (round-to-nearest adds,
+            // undoing the expected truncation shrink of each chunk); LO8: the low-part products into `corr`
+            float sum[64], acc[64], corr[LO8 ? 64 : 1];
+#pragma unroll
+            for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+            for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
+                const int ks1 = min(ks0 + chunk_len, ksteps);
+                // K products per accumulator element: the lo-part products that share the accumulator are ~2^-11 of the
+                // hi ones and add no measurable shrink on H100 (tests/diag_accum_bias.py: counting them over-corrects by
+                // exactly one K's worth, +5.4e-7 at K = 512 per chunk)
+                const float unshrink = kAccumShrinkPerElement * (float)((ks1 - ks0) * kBlockK);
+                int prev_s = -1;
+                for (int ks = ks0; ks < ks1; ++ks) {
+                    mbar_wait(&full[s], ph);
+                    const uint32_t a_addr = smem_u32(smem + s * kStageBytes);
+                    const uint64_t a_desc = kmajor_sw128_desc(a_addr + c * 64 * 128);     // this consumer's 64 rows
+                    const uint64_t b_desc = kmajor_sw128_desc(a_addr + kABytes);
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < kBlockK / 16; ++k) {
+                        // +32 B along K inside the 128-B swizzle atom == +2 in the 16-B address field
+                        wgmma_m64n128k16_f16<0, 0>(acc, a_desc + 2 * k, b_desc + 2 * k, (ks > ks0) || (k > 0));
+                        if (SPLIT_W)                   // lo rows: N_TILE rows (x 128 B) further down the stage, same accumulator
+                            wgmma_m64n128k16_f16<0, 0>(acc, a_desc + 2 * k, b_desc + 2 * k + (N_TILE * 128 / 16), 1);
+                    }
+                    if constexpr (LO8) {
+                        const uint64_t a8_desc = kmajor_sw64_desc(a_addr + kOffA8 + c * 64 * 64);
+                        const uint64_t w8_desc = kmajor_sw64_desc(a_addr + kOffWl8);
+#pragma unroll
+                        for (int k = 0; k < kBlockK / 32; ++k)   // K = 32 per E4M3 wgmma, +32 B inside the 64-B atom
+                            wgmma_m64n128k32_e4m3(corr, a8_desc + 2 * k, w8_desc + 2 * k, (ks > 0) || (k > 0));
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                   // the previous k-step's wgmmas have retired: release its stage
+                    if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+                    prev_s = s;
+                    if (++s == STAGES) { s = 0; ph ^= 1; }
+                }
+                wgmma_wait<0>();
+                fence_regs(acc);
+                if constexpr (LO8) fence_regs(corr);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[prev_s]);
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
+            }
+            if constexpr (LO8) {                       // + A8 * Wl8^T / 2^s
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sum[i] = fmaf(corr[i], p.lo_scale, sum[i]);
+            }
+
+            // ---- accumulator fragment -> fp32 tile [64 rows][128 cols] in shared memory, 16-B chunks XOR-swizzled by row
+            named_bar_sync(bar_id, 128);               // the previous tile's epilogue is done with the region
+            {
+                const int fr = wq * 16 + (lane >> 2);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int row = fr + 8 * i, col = 8 * j + 2 * (lane & 3);
+                        const uint32_t addr = epi_base + row * kEpiRowBytes + ((((col >> 2) ^ (row & 7))) << 4) + (col & 3) * 4;
+                        sts64(addr, sum[4 * j + 2 * i], sum[4 * j + 2 * i + 1]);
+                    }
+                }
+            }
+            named_bar_sync(bar_id, 128);
+            float accr[kColsPerThread];
+#pragma unroll
+            for (int q4 = 0; q4 < kColsPerThread / 4; ++q4) {
+                const int ch = half * (kColsPerThread / 4) + q4;
+                const uint4 u = lds128(epi_base + rr * kEpiRowBytes + ((ch ^ (rr & 7)) << 4));
+                accr[4 * q4 + 0] = __uint_as_float(u.x); accr[4 * q4 + 1] = __uint_as_float(u.y);
+                accr[4 * q4 + 2] = __uint_as_float(u.z); accr[4 * q4 + 3] = __uint_as_float(u.w);
+            }
+            named_bar_sync(bar_id, 128);               // the tile region becomes the four warps' output staging
+
             int w, h, n;
             if (plain) { w = 0; h = 0; n = m * kTileM + r; }
             else {
@@ -404,76 +360,11 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 n = (m / (p.tiles_w * p.tiles_h)) * p.box_n + pn;
             }
             const bool valid = n < p.NB;
-            int nt_next = nt + step_nt, mu_next = mu + step_m;
-            if (nt_next >= p.n_tiles) { nt_next -= p.n_tiles; ++mu_next; }
-            const int m_next = PAIR ? 2 * mu_next + (int)rank : mu_next;
-            if (mu_next < m_units) prefetch_resid(nt_next, m_next);
-            // bias of the first 32-column group: requested BEFORE the wait for the accumulator (the mbarrier / TMEM asm
-            // statements are compiler barriers: a load written after them is issued after them, and its latency then
-            // sits on the critical path of the tile - the single largest stall of the epilogue in the ncu source page)
-            constexpr bool kBiasAhead = kColsPerWarp <= 64;  // N_TILE = 256 holds 128 partial sums per thread: no room for it
-            float4 bnext[8];
-            if (kBiasAhead) load_bias(bnext, nt * N_TILE + half * kColsPerWarp);
-            uint32_t tmem_base_e;                            // re-read per tile (LDS) instead of a local-memory reload
-            asm volatile("ld.shared.b32 %0, [%1];" : "=r"(tmem_base_e) : "r"(smem_u32(tmem_base_slot)));
-
-            // sum the K chunks in registers (round-to-nearest adds), undoing the expected truncation shrink of each
-            float acc[kColsPerWarp];
-            for (int c = 0; c < n_chunks; ++c) {
-                const int len_c = min(chunk_len, ksteps - c * chunk_len);
-                // products accumulated per TMEM element: hi and lo share one accumulator (x 2) unless they are stacked side by side
-                const float unshrink = kAccumShrinkPerElement * (float)(len_c * kBlockK * (SPLIT_W && !STACKED ? 2 : 1));
-                mbar_wait(&tmem_full[buf], buf_ph);
-                tc_fence_after_sync();
-                const uint32_t t_row = tmem_base_e + (uint32_t(q * 32) << 16) + buf * kBufCols + half * kColsPerWarp;
-#pragma unroll
-                for (int g = 0; g < kGroups; ++g) {
-                    uint32_t v[32];
-                    tmem_ld_32x32(t_row + g * 32, v);
-                    if (STACKED) {                             // A Wh^T + A Wl^T: the two column halves of the stacked product
-                        uint32_t w[32];
-                        tmem_ld_32x32(t_row + N_TILE + g * 32, w);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(w[j]));
-                    } else {
-                        tmem_ld_wait();
-                    }
-                    if (c == 0) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[g * 32 + j] = fmaf(__uint_as_float(v[j]), unshrink, __uint_as_float(v[j]));
-                    } else {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[g * 32 + j] += fmaf(__uint_as_float(v[j]), unshrink, __uint_as_float(v[j]));
-                    }
-                    if (LO8 && c == n_chunks - 1) {           // + A8 * Wl8^T / 2^s: complete once the last chunk is
-                        tmem_ld_32x32(tmem_base_e + (uint32_t(q * 32) << 16) + 2 * N_TILE + cpar * N_TILE + half * kColsPerWarp + g * 32, v);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) acc[g * 32 + j] = fmaf(__uint_as_float(v[j]), p.lo_scale, acc[g * 32 + j]);
-                    }
-                }
-                tc_fence_before_sync();
-                __syncwarp();
-                if (lane == 0) {
-                    if (PAIR) {                               // the leader's MMA warp waits for both CTAs' drains
-                        mbar_arrive_cluster(te_addr[buf]);
-                        if (LO8 && c == n_chunks - 1) mbar_arrive_cluster(ce_addr[cpar]);
-                    } else {
-                        mbar_arrive(&tmem_empty[buf]);
-                        if (LO8 && c == n_chunks - 1) mbar_arrive(&corr_empty[cpar]);
-                    }
-                }
-                if (++buf == 2) { buf = 0; buf_ph ^= 1; }
-            }
-            cpar ^= 1;
-
-            const int ch0 = nt * N_TILE + half * kColsPerWarp;
+            const int ch0 = nt * N_TILE + half * kColsPerThread;
             // Destination of this lane's row (element offsets, -1 = row beyond the batch).  Stores go
             // through a per-warp staging tile (32 rows x 128 B, 16-B chunks XOR-swizzled by row) so a
             // warp writes whole 128-B lines of 4 rows per instruction instead of 16 B into 32
-            // different rows: the direct pattern made the small-K GEMMs LSU-bound (ncu: 32 sectors
-            // per store request, stall_lg/long_scoreboard on the bias loads queued behind them).
+            // different rows.
             long long out_off = -1, res_off = -1;
             if (valid && !p.pool) {
                 out_off = (long long)((size_t(n) * p.H + h) * p.W + w) * p.ld_out;
@@ -481,24 +372,24 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     res_off = (p.resid_res ? window_row_to_token((long long)n, p.resid_res, p.resid_shift) : (long long)n)
                               * p.resid_C;
             }
-            const uint32_t stg = smem_u32(staging) + (warp - 4) * kStagingBytes;     // shared-space addresses (sts128 / lds128)
+            const uint32_t stg = epi_base + wq * kStagingBytes;
             const uint32_t stg_mine = stg + lane * 128;
             const int sw = lane & 7;
             const int cq = lane & 7, rq = lane >> 3;      // flush role: 16-B chunk cq of rows it*4 + rq
             const bool f32_path = p.out_f32 != nullptr || p.resid != nullptr;
+            float4 bnext[8];
 #pragma unroll
             for (int g = 0; g < kGroups; ++g) {
                 float f[32];
-                if (!kBiasAhead) load_bias(bnext, ch0 + g * 32);
+                load_bias(bnext, ch0 + g * 32);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
                     const float4 b = bnext[j];
-                    f[4 * j + 0] = acc[g * 32 + 4 * j + 0] + b.x;
-                    f[4 * j + 1] = acc[g * 32 + 4 * j + 1] + b.y;
-                    f[4 * j + 2] = acc[g * 32 + 4 * j + 2] + b.z;
-                    f[4 * j + 3] = acc[g * 32 + 4 * j + 3] + b.w;
+                    f[4 * j + 0] = accr[g * 32 + 4 * j + 0] + b.x;
+                    f[4 * j + 1] = accr[g * 32 + 4 * j + 1] + b.y;
+                    f[4 * j + 2] = accr[g * 32 + 4 * j + 2] + b.z;
+                    f[4 * j + 3] = accr[g * 32 + 4 * j + 3] + b.w;
                 }
-                if (kBiasAhead && g + 1 < kGroups) load_bias(bnext, ch0 + (g + 1) * 32);   // the next group's, one group ahead
                 if (p.relu == 1) {
 #pragma unroll
                     for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.0f);
@@ -607,13 +498,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     }
                 }
             }
-            nt = nt_next; mu = mu_next; m = m_next;
         }
     }
-
-    tc_fence_before_sync();
-    if (PAIR) cluster_sync(); else __syncthreads();           // PAIR: neither CTA may exit while the other still signals it
-    if (warp == 2) { if (PAIR) tmem_dealloc_pair<kTmemCols>(tmem_base); else tmem_dealloc<kTmemCols>(tmem_base); }
 }
 
 }  // namespace fad

@@ -1,5 +1,5 @@
 // Encodec-24 kHz SEANet encoder (EncodecEmbModel, fadtk/model_loader.py:111-176: model.encoder(audio) ->
-// [T/320, 128]) around the tcgen05 GEMM: every causal weight-normalised Conv1d is an im2col + GEMM (the
+// [T/320, 128]) around the wgmma GEMM: every causal weight-normalised Conv1d is an im2col + GEMM (the
 // pre-activation ELU is applied while gathering; reflect padding by index), residual blocks use the
 // epilogue's fp32 read-modify-write, the 2-layer LSTM runs its input projections as one GEMM per layer and
 // its recurrence as one small GEMM + cell kernel per time step.

@@ -1,5 +1,5 @@
 // Host side of the C ABI declared in include/fadtk_b200.h: owns device weights and workspaces,
-// encodes TMA descriptors, launches the sm_100a kernels.  No torch, no CUTLASS.
+// encodes TMA descriptors, launches the sm_90a kernels.  No torch, no CUTLASS.
 #include "../../include/fadtk_b200.h"
 
 #include <cuda.h>
@@ -25,8 +25,7 @@
 #include "whisper.cuh"
 #include "encodec.cuh"
 #include "wav2vec.cuh"
-#include "umma_bench.cuh"
-#include "attention_umma.cuh"
+#include "attention_wgmma.cuh"
 
 namespace {
 
@@ -83,9 +82,7 @@ struct LayerGeom {
     int taps, Cin, Cout, H, W, relu, pool;
     int box_w, box_h, box_n, n_tile;
     int split_w;      // 0: fp16 weights; 1: fp16 hi/lo pair (interleaved per 128-row tile), two fp16 MMAs;
-                      // 2: same packed tensor, low part applied as E4M3 (kind::f8f6f4) - see conv_gemm.cuh
-    int pair;         // 1: CTA pairs (cta_group::2, M = 256 per MMA, each CTA stages half of the weight tile)
-    int stack;        // 1 (mode 1 only, FADTK_STACK=1): hi | lo rows as one N = 2 n_tile MMA operand (measurement variant)
+                      // 2: same packed tensor, low part applied by an E4M3 wgmma - see conv_gemm.cuh
 };
 
 // how the low part of split weights is applied: FADTK_WLO=fp16 (two fp16 MMAs) | fp8 (E4M3 correction MMA)
@@ -93,32 +90,9 @@ int wlo_mode() {
     static const int mode = [] { const char* e = getenv("FADTK_WLO"); return (e && std::string(e) == "fp8") ? 2 : 1; }();
     return mode;
 }
-// CTA pairs (cta_group::2) per VGGish tensor-core layer, bit i = conv2, conv3_1, conv3_2, conv4_1, conv4_2, fc1, fc2, fc3.
-// FADTK_PAIR = auto (default) | 0 | 1 (every layer) | 0x<mask>.  auto = the layers where the pair measured faster
-// (profiles/r2_bench_pair_*.json): K >= 2304 convolutions and the FC layers; conv2 / conv3_1 (K = 576 / 1152, epilogue-
-// heavy: one output tile per 9 / 18 k-steps) lose a little to the lock-step of two SMs and stay single-CTA.
-unsigned pair_mask() {
-    static const unsigned mask = [] {
-        const char* e = getenv("FADTK_PAIR");
-        if (!e || std::string(e) == "auto") return 0x7Cu;
-        if (std::string(e) == "1") return 0xFFu;
-        return (unsigned)strtoul(e, nullptr, 0) & 0xFFu;
-    }();
-    return mask;
-}
-int pair_all() {                    // stage-test entry (fad_umma_layer): pairs only when explicitly forced on
-    const char* e = getenv("FADTK_PAIR");
-    return (e && std::string(e) == "1") ? 1 : 0;
-}
-
 int make_geom(LayerGeom& g, int H, int W, int Cin, int Cout, int taps, int relu, int pool, int split_w) {
     g.taps = taps; g.Cin = Cin; g.Cout = Cout; g.H = H; g.W = W; g.relu = relu; g.pool = pool;
     g.split_w = split_w;                     // 0, 1 or 2 - the caller decides (wlo_mode() for the VGGish pipeline)
-    g.pair = 0;                              // set by the caller after make_geom (split modes only)
-    {
-        static const int stk = [] { const char* e = getenv("FADTK_STACK"); return (e && e[0] == '1') ? 1 : 0; }();
-        g.stack = (g.split_w == 1 && stk) ? 1 : 0;
-    }
     if (Cin % 64 != 0) return fail("Cin must be a multiple of 64");
     if (taps != 1 && taps != 9) return fail("taps must be 1 or 9");
     if (H == 1 && W == 1) { g.box_w = 1; g.box_h = 1; g.box_n = 128; }
@@ -133,7 +107,7 @@ int make_geom(LayerGeom& g, int H, int W, int Cin, int Cout, int taps, int relu,
     }
     if (pool && (g.box_h % 2 != 0 || g.box_w % 2 != 0)) return fail("pooling needs even tile boxes");
     if (Cout % 128 != 0) return fail("Cout must be a multiple of 128");
-    g.n_tile = (!g.split_w && Cout % 256 == 0) ? 256 : 128;
+    g.n_tile = 128;                          // one m64n128 wgmma accumulator per consumer warpgroup
     return 0;
 }
 
@@ -203,35 +177,21 @@ struct fad_handle {
 
 namespace {
 
-template <int N_TILE, int STAGES, int WMODE, int PAIR = 0, int STACK = 0>
+template <int N_TILE, int STAGES, int WMODE>
 int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mw8,
                      const CUtensorMap& mx8, const fad::ConvGemmParams& p, cudaStream_t st) {
     static bool attr_set = false;
-    constexpr uint32_t smem = fad::conv_gemm_smem_bytes<N_TILE, STAGES, WMODE, PAIR>();
+    constexpr uint32_t smem = fad::conv_gemm_smem_bytes<N_TILE, STAGES, WMODE>();
     static_assert(smem <= 227 * 1024, "over the per-CTA shared-memory limit");
-    auto kern = fad::conv_gemm_kernel<N_TILE, STAGES, WMODE, PAIR, STACK>;
+    auto kern = fad::conv_gemm_kernel<N_TILE, STAGES, WMODE>;
     if (!attr_set) {
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
-    const int m_tiles = p.img_groups * p.tiles_h * p.tiles_w;
-    const int total = (PAIR ? (m_tiles + 1) / 2 : m_tiles) * p.n_tiles;           // work units (PAIR: two M tiles each)
+    const int total = p.img_groups * p.tiles_h * p.tiles_w * p.n_tiles;
     if (total == 0) return 0;
-    if (PAIR) {
-        // one cluster of two CTAs per unit in flight: the pair lands on the two SMs of a TPC
-        const int pairs = total < h->num_sms / 2 ? total : h->num_sms / 2;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(2 * pairs); cfg.blockDim = dim3(fad::kConvGemmThreads);
-        cfg.dynamicSmemBytes = smem; cfg.stream = st;
-        cudaLaunchAttribute attr[1];
-        attr[0].id = cudaLaunchAttributeClusterDimension;
-        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-        cfg.attrs = attr; cfg.numAttrs = 1;
-        CK(cudaLaunchKernelEx(&cfg, kern, mx, mw, mw8, mx8, p));
-    } else {
-        const int grid = total < h->num_sms ? total : h->num_sms;
-        kern<<<grid, fad::kConvGemmThreads, smem, st>>>(mx, mw, mw8, mx8, p);
-    }
+    const int grid = total < h->num_sms ? total : h->num_sms;
+    kern<<<grid, fad::kConvGemmThreads, smem, st>>>(mx, mw, mw8, mx8, p);
     CK(cudaGetLastError());
     h->launches++;
     return 0;
@@ -253,29 +213,26 @@ int encode_layer_maps(const LayerGeom& g, const void* x, long long nb_dim, const
     const uint64_t rows_mul = g.split_w ? 2 : 1;
     const uint64_t wd[2] = {K, (uint64_t)g.Cout * rows_mul};
     const uint64_t ws[1] = {K * 2};
-    // rows per weight box: mode 1 fetches hi + lo of a tile at once, mode 2 the hi rows only; a CTA of a pair fetches
-    // its half of the hi rows and its half of the lo rows as two boxes
-    // (mode 1 pair: one box of n_tile rows - rank 0 the hi rows, rank 1 the lo rows of the stacked N = 2 n_tile operand)
-    const uint32_t wb[2] = {64, (uint32_t)(g.pair ? (g.stack ? g.n_tile : g.n_tile / 2) : g.n_tile * (g.split_w == 1 ? 2 : 1))};
+    // rows per weight box: mode 1 fetches hi + lo of a tile at once, mode 2 the hi rows only
+    const uint32_t wb[2] = {64, (uint32_t)(g.n_tile * (g.split_w == 1 ? 2 : 1))};
     return encode_f16_map(mw, w, 2, wd, ws, wb);
 }
 
 int lo8_for(fad_handle* h, const LayerGeom& g, const void* w, CUtensorMap* mw8, float* inv_scale, cudaStream_t st);
 
-// Encoder self-attention on tcgen05 (attention_umma.cuh).  qkv: fp16 [clips * S][3 d] (q | k | v, head h at column h * 64),
+// Encoder self-attention on wgmma (attention_wgmma.cuh).  qkv: fp16 [clips * S][3 d] (q | k | v, head h at column h * 64),
 // out: fp16 [clips * S][d].  FADTK_ATTN=legacy selects the mma.sync flash kernel (whisper.cuh) instead.
-bool attention_umma_enabled() {
+bool attention_wgmma_enabled() {
     static const bool on = [] { const char* e = getenv("FADTK_ATTN"); return !(e && std::string(e) == "legacy"); }();
     return on;
 }
-int launch_attention_umma(fad_handle* h, const __half* qkv, long long n_clips, int S, int d, int heads, __half* out, cudaStream_t st) {
+int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, int S, int d, int heads, __half* out, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        CK(cudaFuncSetAttribute(fad::attention_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kAtSmem));
-        CK(cudaFuncSetAttribute(fad::attention_umma_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutMaxShared));   // two CTAs of 112 KiB per SM
+        CK(cudaFuncSetAttribute(fad::attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kAtSmem));
         attr_set = true;
     }
-    if (heads * 64 != d) return fail("attention_umma: head dimension must be 64");
+    if (heads * 64 != d) return fail("attention_wgmma: head dimension must be 64");
     CUtensorMap map;
     const uint64_t dims[3] = {(uint64_t)3 * d, (uint64_t)S, (uint64_t)n_clips};
     const uint64_t strides[2] = {(uint64_t)3 * d * 2, (uint64_t)S * 3 * d * 2};
@@ -283,7 +240,7 @@ int launch_attention_umma(fad_handle* h, const __half* qkv, long long n_clips, i
     if (encode_f16_map(&map, qkv, 3, dims, strides, box)) return 1;
     fad::AttnParams p;
     p.S = S; p.d = d; p.heads = heads; p.out = out;
-    fad::attention_umma_kernel<<<dim3((S + 127) / 128, heads, (unsigned)n_clips), fad::kAtThreads, fad::kAtSmem, st>>>(map, p);
+    fad::attention_wgmma_kernel<<<dim3((S + 127) / 128, heads, (unsigned)n_clips), fad::kAtThreads, fad::kAtSmem, st>>>(map, p);
     CK(cudaGetLastError());
     h->launches++;
     return 0;
@@ -326,24 +283,15 @@ int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CU
     p.bias = bias; p.out = reinterpret_cast<__half*>(out); p.out_f32 = out_f32; p.out8 = out8;
     p.resid = resid; p.resid_C = resid_C; p.resid_res = resid_res; p.resid_shift = resid_shift;
     p.lo_scale = 0.0f;
-    p.lo8_group = 1;
-    {
-        static const int grp = [] { const char* e = getenv("FADTK_LO8_GROUP"); const int v = e ? atoi(e) : 2; return v < 1 ? 1 : (v > 3 ? 3 : v); }();
-        p.lo8_group = grp;                                 // <= STAGES - 2 so the producer always has a stage to fill
-    }
+    // stages: as many 48 / 32 KiB stages as fit next to the two 32 KiB epilogue tiles in 227 KiB
     if (g.split_w == 2) {
         if (mx8 == nullptr) return fail("fp8 low-part mode needs the E4M3 copy of the activation");
         CUtensorMap mw8;
         if (lo8_for(h, g, w, &mw8, &p.lo_scale, st)) return 1;
-        if (g.pair) return launch_conv_gemm<128, 5, 2, 1>(h, mx, mw, mw8, *mx8, p, st);
-        return launch_conv_gemm<128, 4, 2>(h, mx, mw, mw8, *mx8, p, st);
+        return launch_conv_gemm<128, 3, 2>(h, mx, mw, mw8, *mx8, p, st);
     }
-    if (g.split_w && g.pair && g.stack) return launch_conv_gemm<128, 6, 1, 1, 1>(h, mx, mw, mw, mx, p, st);
-    if (g.split_w && g.pair) return launch_conv_gemm<128, 6, 1, 1>(h, mx, mw, mw, mx, p, st);
-    if (g.split_w && g.stack) return launch_conv_gemm<128, 4, 1, 0, 1>(h, mx, mw, mw, mx, p, st);
-    if (g.split_w) return launch_conv_gemm<128, 4, 1>(h, mx, mw, mw, mx, p, st);
-    if (g.n_tile == 256) return launch_conv_gemm<256, 4, 0>(h, mx, mw, mw, mx, p, st);
-    return launch_conv_gemm<128, 6, 0>(h, mx, mw, mw, mx, p, st);
+    if (g.split_w) return launch_conv_gemm<128, 3, 1>(h, mx, mw, mw, mx, p, st);
+    return launch_conv_gemm<128, 4, 0>(h, mx, mw, mw, mx, p, st);
 }
 
 // E4M3 copy of the low parts of a packed hi/lo weight tensor, scaled by a power of two so the largest
@@ -403,7 +351,7 @@ int lo8_for(fad_handle* h, const LayerGeom& g, const void* w, CUtensorMap* mw8, 
     if (!fn) return fail("cuTensorMapEncodeTiled entry point not available");
     cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)(n_tiles * 128)};
     cuuint64_t gstr[1] = {(cuuint64_t)K};
-    cuuint32_t bdim[2] = {64, (cuuint32_t)(g.pair ? 64 : 128)}, estr[2] = {1, 1};
+    cuuint32_t bdim[2] = {64, 128}, estr[2] = {1, 1};
     CUresult r = fn(mw8, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, it->second.w8, gdim, gstr, bdim, estr,
                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -522,7 +470,7 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(cudaSetDevice(device));
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail("fadtk_b200 kernels are built for sm_100a (Blackwell B200) only");
+    if (prop.major != 9) return fail("fadtk_b200 kernels are built for sm_90a (Hopper H100) only");
     fad_handle* h = new fad_handle();
     h->device = device;
     h->num_sms = prop.multiProcessorCount;
@@ -609,7 +557,6 @@ int fad_vggish_load(fad_handle* h, const fad_vggish_weights* w) {
     for (int i = 0; i < 8; ++i) {
         const VggLayer& L = kVgg[i];
         if (make_geom(h->geom[i], L.H, L.W, L.Cin, L.Cout, L.taps, L.relu, L.pool, ((w->split_mask >> i) & 1) ? wlo_mode() : 0)) return 1;
-        h->geom[i].pair = (h->geom[i].split_w && ((pair_mask() >> i) & 1)) ? 1 : 0;
         const void* wptr = i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5];
         if (encode_layer_maps(h->geom[i], h->act[i], (long long)B, wptr, &h->map_x[i], &h->map_w[i])) return 1;
         if (h->geom[i].split_w == 2) {
@@ -721,7 +668,6 @@ int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int C
     CK(cudaSetDevice(h->device));
     LayerGeom g;
     if (make_geom(g, H, W, Cin, Cout, taps, relu, pool, split_w)) return 1;
-    g.pair = (g.split_w && pair_all()) ? 1 : 0;
     if (pool && out_f32_or_null) return fail("fp32 copy is only available for un-pooled layers");
     CUtensorMap mx, mw, mx8;
     if (encode_layer_maps(g, x_f16, NB, w_f16, &mx, &mw)) return 1;
@@ -749,7 +695,7 @@ int fad_stats_accumulate(fad_handle* h, const void* emb_f16, long long n_rows, i
     cudaStream_t st = (cudaStream_t)stream;
     const __half* E = reinterpret_cast<const __half*>(emb_f16);
     const __half* shift = reinterpret_cast<const __half*>(shift_f16);
-    // mode 0 (default): exact fp64 Gram on the FP64 tensor pipe (DMMA); 1: tcgen05 fp16 hi/lo (fp32 accumulation,
+    // mode 0 (default): exact fp64 Gram on the FP64 tensor pipe (DMMA); 1: wgmma fp16 hi/lo (fp32 accumulation,
     // full-rank well-conditioned sets only); 2: fp64 CUDA-core kernel (verification).  FADTK_STATS overrides.
     static const int forced = [] {
         const char* e = getenv("FADTK_STATS");
@@ -948,7 +894,7 @@ extern "C" int fad_attention(fad_handle* h, const void* qkv_f16, long long n_cli
     if (d % 64 != 0 || S <= 0 || n_clips <= 0) return fail("bad shape");
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
-    if (!legacy) return launch_attention_umma(h, reinterpret_cast<const __half*>(qkv_f16), n_clips, S, d, d / 64, reinterpret_cast<__half*>(out_f16), st);
+    if (!legacy) return launch_attention_wgmma(h, reinterpret_cast<const __half*>(qkv_f16), n_clips, S, d, d / 64, reinterpret_cast<__half*>(out_f16), st);
     fad::whisper_flash_attention_kernel<<<dim3((S + 63) / 64, d / 64, (unsigned)n_clips), 128, 0, st>>>(
         reinterpret_cast<const __half*>(qkv_f16), S, d, reinterpret_cast<__half*>(out_f16));
     CK(cudaGetLastError());
@@ -956,27 +902,6 @@ extern "C" int fad_attention(fad_handle* h, const void* qkv_f16, long long n_cli
     return 0;
 }
 
-// time (ms) of `ksteps` hi/lo-split K steps per SM under issue pattern `mode` (umma_bench.cuh), every SM busy
-extern "C" int fad_bench_umma_mode(fad_handle* h, int mode, int ksteps, double* ms_out_host) {
-    if (!h || !ms_out_host) return fail("null argument");
-    if (mode < 0 || mode > 5 || ksteps < 16) return fail("bad mode / ksteps");
-    CK(cudaSetDevice(h->device));
-    CK(cudaFuncSetAttribute(fad::umma_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kUbSmem));
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    fad::umma_bench_kernel<<<h->num_sms, fad::kUbThreads, fad::kUbSmem>>>(mode, ksteps / 8);     // warm-up
-    CK(cudaEventRecord(e0));
-    fad::umma_bench_kernel<<<h->num_sms, fad::kUbThreads, fad::kUbSmem>>>(mode, ksteps);
-    CK(cudaEventRecord(e1));
-    CK(cudaEventSynchronize(e1));
-    CK(cudaGetLastError());
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    *ms_out_host = ms;
-    h->launches += 2;
-    return 0;
-}
 
 extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_host) {
     if (!h || !tflops_out_host) return fail("null argument");

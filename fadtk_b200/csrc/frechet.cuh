@@ -33,7 +33,7 @@ struct DgemmBatch {
 };
 
 // One 64 x 64 tile of C = alpha A B + beta_diag I per 256-thread CTA on the FP64 TENSOR pipe
-// (mma.sync m8n8k4 f64 -> SASS DMMA.8x8x4, the only fp64 MMA shape sm_100a has; tcgen05 has no f64 kind).
+// (mma.sync m8n8k4 f64 -> SASS DMMA.8x8x4, the fp64 MMA shape of sm_90a; wgmma has no f64 kind).
 // Returns max |C - I| over this thread's outputs and its share of tr C.
 // Layout: 8 warps as 2 (M) x 4 (N); a warp owns 32 x 16 outputs = 4 x 2 DMMA blocks (16 fp64 accumulators
 // per thread).  Per 4-wide k-step a warp issues 6 conflict-free LDS.64 (4 A + 2 B fragments) for 8 DMMAs,

@@ -12,7 +12,7 @@
 //                  <= 1.5e-6 relative vs the reference's float64 numpy (CPU experiment, DESIGN.md);
 //                  T = double matches float64 to 2e-6 in the fp32 output.
 //  conv1_kernel    3x3 conv 1->64 + bias + ReLU + 2x2 max-pool on fp32 input (K = 9 is too thin
-//                  for the tensor pipe); writes NHWC fp16 [B, 48, 32, 64] for the tcgen05 layers.
+//                  for the tensor pipe); writes NHWC fp16 [B, 48, 32, 64] for the wgmma layers.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>

@@ -12,19 +12,20 @@
 //   range); Y tiles are staged in shared memory as doubles with pitch 68 (== 4 mod 16: conflict-free fragment loads)
 //   and double-buffered; each job's tile goes to a workspace and stats_dmma_reduce_kernel sums the jobs in a fixed
 //   order (deterministic).  In = double with no shift is the variant score() feeds with per-file fp16-rounded means
-//   (fad_stats_accumulate_f64).  ncu: profiles/r2_ncu_fp64_dmma.md.
+//   (fad_stats_accumulate_f64).
 //
-// stats_umma_kernel  (mode 1, opt-in)   tcgen05 fp16 hi/lo: yh = fp16(y), yl = fp16(y - yh),
+// stats_umma_kernel  (mode 1, opt-in)   tensor-core (wgmma) fp16 hi/lo: yh = fp16(y), yl = fp16(y - yh),
 //       sum y y^T ~= sum yh yh^T + yh yl^T + yl yh^T            (yl yl^T ~ 2^-22 is dropped)
 //   Every fp16 x fp16 product is exact in the fp32 accumulator; the accumulation itself is cut every 256 rows and
 //   drained into an fp64 tile, because tensor-core fp32 adds truncate.  One CTA = (128x128 output tile, row range).
 //   E is row-major, so both operands of E^T E are "MN-major": a TMA box [32 rows x 64 cols] with 128-B swizzle IS
-//   the canonical MN-major SWIZZLE_128B UMMA layout (K = row index).
+//   the canonical MN-major SWIZZLE_128B wgmma layout (K = row index).
 //     warp 0       TMA producer: per 32-row stage, two 64-column boxes per panel
 //     warps 4-11   transform: in smem, x -> (yh in place, yl into a second panel), zero rows past the end, exact
 //                  column sums of x - s and of yh + yl in fp64 registers
-//     warp 1       MMA issuer: per stage 2 k-steps x {hh, hl, lh} tcgen05.mma, fp32 in TMEM
-//     warps 12-15  drain: every 256 rows the TMEM tile is added into an fp64 tile in shared memory
+//     warps 12-19  two MMA warpgroups, one per 64-row half of the output tile: per stage 2 k-steps x {hh, hl, lh}
+//                  wgmmas into an fp32 register accumulator that is added into an fp64 tile in shared memory
+//                  every 256 rows
 //   Good to ~1e-6 relative: fine for full-rank, well-conditioned sets only.
 //
 // stats_simt_kernel  (mode 2)   fp64 CUDA-core contraction of the exact y: the round-1 default, kept as the
@@ -34,18 +35,18 @@
 //   acc[0] = n,  acc[1 .. d] = sum(x - s) (exact),  acc[1+d .. 1+d+d*d) = sum(y y^T)
 //   (d x d, full, row-major),  acc[1+d+d*d ..] = sum(yh + yl)  (centring term of the covariance; = sum y in modes 0, 2)
 #pragma once
-#include "sm100.cuh"
+#include "sm90.cuh"
 
 namespace fad {
 
 constexpr int kStTile = 128;
 constexpr int kStStageRows = 32;
-constexpr int kStStagesPerChunk = 8;               // 256 rows per fp32 TMEM accumulation
+constexpr int kStStagesPerChunk = 8;               // 256 rows per fp32 register accumulation
 constexpr int kStStages = 3;
 constexpr uint32_t kStBlockBytes = kStStageRows * 128;            // one 64-col box: 4 KiB
 constexpr uint32_t kStPanelBytes = 2 * kStBlockBytes;             // 128 cols x 32 rows: 8 KiB
 constexpr uint32_t kStStageBytes = 4 * kStPanelBytes;             // Ah | Bh | Al | Bl = 32 KiB
-constexpr int kStThreads = 512;
+constexpr int kStThreads = 640;
 constexpr int kStTransformThreads = 256;
 constexpr uint32_t kStSmemBytes = kStStages * kStStageBytes + kStTile * kStTile * 8 + 1024 + 256;
 
@@ -80,8 +81,7 @@ __device__ __forceinline__ void split_hi_lo(__half2 x, __half2 s, __half2& hi, _
 __global__ void __launch_bounds__(kStThreads, 1)
 stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParams p)
 {
-    using namespace sm100;
-    constexpr uint32_t kIdesc = make_idesc(FMT_F16, kStTile, kStTile, /*a MN-major*/1, /*b MN-major*/1);
+    using namespace sm90;
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -90,9 +90,7 @@ stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParam
     uint64_t* full = bars;                       // TMA landed
     uint64_t* ready = bars + kStStages;          // transform done
     uint64_t* empty = bars + 2 * kStStages;      // MMAs retired
-    uint64_t* tmem_full = bars + 3 * kStStages;
-    uint64_t* tmem_empty = bars + 3 * kStStages + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * kStStages + 4);
+    uint64_t* mma_done = bars + 3 * kStStages;   // every MMA of the job retired: stage 0 may be reused
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int job = blockIdx.x;
@@ -110,17 +108,13 @@ stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParam
     if (warp == 0 && lane == 0) tma_prefetch_desc(&map_e);
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < kStStages; ++s) {
-            mbar_init(&full[s], 1); mbar_init(&ready[s], kStTransformThreads / 32); mbar_init(&empty[s], 1);
+            mbar_init(&full[s], 1); mbar_init(&ready[s], kStTransformThreads / 32); mbar_init(&empty[s], 8);
         }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tmem_full[a], 1); mbar_init(&tmem_empty[a], 4); }
+        mbar_init(mma_done, 8);
         mbar_fence_init();
     }
-    if (warp == 2) tmem_alloc<256>(tmem_slot);
     for (int i = threadIdx.x; i < kStTile * kStTile; i += kStThreads) acc64[i] = 0.0;
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_slot;
 
     if (warp == 0) {
         if (elect_one()) {
@@ -137,41 +131,6 @@ stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParam
                     tma_load_2d(st + kStPanelBytes + kStBlockBytes, &map_e, &full[s], tj * kStTile + 64, r0);
                 }
                 if (++s == kStStages) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp == 1) {
-        if (elect_one()) {
-            int s = 0; uint32_t ph = 0;
-            int acc = 0; uint32_t acc_ph = 0;
-            int it = 0;
-            for (int c = 0; c < n_chunks; ++c) {
-                mbar_wait(&tmem_empty[acc], acc_ph ^ 1);
-                tc_fence_after_sync();
-                const uint32_t d_tmem = tmem_base + acc * kStTile;
-                const int n_st = min(kStStagesPerChunk, n_stages_total - it);
-                for (int q = 0; q < n_st; ++q, ++it) {
-                    mbar_wait(&ready[s], ph);
-                    tc_fence_after_sync();
-                    const uint32_t base = smem_u32(smem + s * kStStageBytes);
-                    const uint32_t ah = base, bh = diag ? base : base + kStPanelBytes;
-                    const uint32_t al = base + 2 * kStPanelBytes, bl = diag ? al : al + kStPanelBytes;
-                    // MN-major SW128: 64-col blocks kStBlockBytes apart (LBO), 8-row K groups 1024 B apart (SBO)
-                    const uint64_t d_ah = mnmajor_sw128_desc(ah, kStBlockBytes, 1024);
-                    const uint64_t d_bh = mnmajor_sw128_desc(bh, kStBlockBytes, 1024);
-                    const uint64_t d_al = mnmajor_sw128_desc(al, kStBlockBytes, 1024);
-                    const uint64_t d_bl = mnmajor_sw128_desc(bl, kStBlockBytes, 1024);
-#pragma unroll
-                    for (int k = 0; k < kStStageRows / 16; ++k) {
-                        const uint32_t off = 128 * k;          // 16 K-rows = 2048 B = 128 x 16 B
-                        umma_f16(d_tmem, d_ah + off, d_bh + off, kIdesc, (q | k) != 0);
-                        umma_f16(d_tmem, d_ah + off, d_bl + off, kIdesc, 1);
-                        umma_f16(d_tmem, d_al + off, d_bh + off, kIdesc, 1);
-                    }
-                    umma_commit(&empty[s]);
-                    if (++s == kStStages) { s = 0; ph ^= 1; }
-                }
-                umma_commit(&tmem_full[acc]);
-                if (++acc == 2) { acc = 0; acc_ph ^= 1; }
             }
         }
     } else if (warp >= 4 && warp < 12) {
@@ -237,10 +196,7 @@ stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParam
         }
         // column sums: reduce the 16 row lanes through stage 0 once every MMA has retired
         if (diag) {
-            if (n_chunks > 0) {
-                const int last = n_chunks - 1;
-                mbar_wait(&tmem_full[last & 1], (uint32_t)((last >> 1) & 1));
-            }
+            mbar_wait(mma_done, 0);
             asm volatile("bar.sync 1, 256;");
             double* red = reinterpret_cast<double*>(smem);       // [2][16 row lanes][128 cols] = 32 KiB
             const int lane16 = hf * 8 + rl;
@@ -259,35 +215,58 @@ stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParam
             }
         }
     } else if (warp >= 12) {
-        // -------------------------------------------------- drain TMEM -> fp64 smem
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        int acc = 0; uint32_t acc_ph = 0;
+        // -------------------------------------- wgmma: output rows [64 mh, 64 mh + 64) of the tile, fp32 -> fp64 smem
+        const int mh = (warp - 12) >> 2;
+        const int wq = warp & 3;
+        int s = 0; uint32_t ph = 0;
+        int it = 0;
+        float d[64];
         for (int c = 0; c < n_chunks; ++c) {
-            mbar_wait(&tmem_full[acc], acc_ph);
-            tc_fence_after_sync();
-            const uint32_t t_row = tmem_base + (uint32_t(q * 32) << 16) + acc * kStTile;
-#pragma unroll 1
-            for (int cc = 0; cc < kStTile / 32; ++cc) {
-                uint32_t v[32];
-                tmem_ld_32x32(t_row + cc * 32, v);
-                tmem_ld_wait();
+            const int n_st = min(kStStagesPerChunk, n_stages_total - it);
+            for (int q = 0; q < n_st; ++q, ++it) {
+                mbar_wait(&ready[s], ph);
+                const uint32_t base = smem_u32(smem + s * kStStageBytes);
+                const uint32_t ah = base + mh * kStBlockBytes, bh = diag ? base : base + kStPanelBytes;
+                const uint32_t al = base + 2 * kStPanelBytes + mh * kStBlockBytes, bl = diag ? base + 2 * kStPanelBytes : base + 3 * kStPanelBytes;
+                // MN-major SW128: 64-col blocks kStBlockBytes apart (LBO), 8-row K groups 1024 B apart (SBO)
+                const uint64_t d_ah = mnmajor_sw128_desc(ah, kStBlockBytes, 1024);
+                const uint64_t d_bh = mnmajor_sw128_desc(bh, kStBlockBytes, 1024);
+                const uint64_t d_al = mnmajor_sw128_desc(al, kStBlockBytes, 1024);
+                const uint64_t d_bl = mnmajor_sw128_desc(bl, kStBlockBytes, 1024);
+                wgmma_fence();
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    acc64[(cc * 32 + j) * kStTile + row] += (double)__uint_as_float(v[j]);
+                for (int k = 0; k < kStStageRows / 16; ++k) {
+                    const uint32_t off = 128 * k;          // 16 K-rows = 2048 B = 128 x 16 B
+                    wgmma_m64n128k16_f16<1, 1>(d, d_ah + off, d_bh + off, (q | k) != 0);
+                    wgmma_m64n128k16_f16<1, 1>(d, d_ah + off, d_bl + off, 1);
+                    wgmma_m64n128k16_f16<1, 1>(d, d_al + off, d_bh + off, 1);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                fence_regs(d);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);
+                if (++s == kStStages) { s = 0; ph ^= 1; }
             }
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tmem_empty[acc]);
-            if (++acc == 2) { acc = 0; acc_ph ^= 1; }
+            // fragment (row 16 wq + lane / 4 + 8 i, col 8 j + 2 (lane % 4) + e) -> acc64[col][row]; one owner per element
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int row = mh * 64 + wq * 16 + (lane >> 2) + 8 * i, col = 8 * j + 2 * (lane & 3) + e;
+                        acc64[col * kStTile + row] += (double)d[4 * j + 2 * i + e];
+                    }
         }
-        double* dst = p.ws_tiles + (size_t)job * kStTile * kStTile;
-        for (int col = 0; col < kStTile; ++col) dst[col * kStTile + row] = acc64[col * kStTile + row];
+        __syncwarp();
+        if (lane == 0) mbar_arrive(mma_done);
     }
-
-    tc_fence_before_sync();
     __syncthreads();
-    if (warp == 2) tmem_dealloc<256>(tmem_base);
+    {
+        double* dst = p.ws_tiles + (size_t)job * kStTile * kStTile;
+        for (int i = threadIdx.x; i < kStTile * kStTile; i += kStThreads) dst[i] = acc64[i];
+    }
 }
 
 // acc += sum over row splits of the job tiles (fixed order => deterministic).

@@ -1,6 +1,6 @@
 // wav2vec 2.0 / HuBERT / MERT style encoders (W2V2Model, HuBERTModel, MERTModel of fadtk/model_loader.py:
 // processor normalisation -> 7-layer conv feature encoder -> feature projection -> grouped positional conv ->
-// post-LN transformer layers -> hidden_states[layer]).  Convs and Linears run on the tcgen05 GEMM
+// post-LN transformer layers -> hidden_states[layer]).  Convs and Linears run on the wgmma GEMM
 // (operands read in place through overlapping-row tensor maps), attention on whisper_flash_attention_kernel, LayerNorm on clap_ln_kernel;
 // this file adds the pieces those do not cover.
 #pragma once

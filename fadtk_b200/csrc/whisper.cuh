@@ -1,7 +1,7 @@
 // Whisper (openai/whisper-{tiny..large}) as the reference uses it for embeddings
 // (fadtk/model_loader.py:636-672): WhisperFeatureExtractor log-mel of the clip padded to 30 s ->
 // WhisperModel(input_features, decoder_input_ids = [[sot, sot]]).last_hidden_state -> [2, d_model].
-// The Linear / Conv1d layers run on the tcgen05 GEMM (conv_gemm.cuh, split fp16 weights); this file holds
+// The Linear / Conv1d layers run on the wgmma GEMM (conv_gemm.cuh, split fp16 weights); this file holds
 // the CUDA-core / warp-MMA kernels around them:
 //   whisper_logmel_kernel      |STFT_400|^2 (centre, reflect), 80 Slaney mel bands, log10, per-clip max
 //   whisper_finish_im2col1     max(x, clipmax - 8), (x + 4) / 4, fp16, 3-tap im2col rows for conv1

@@ -1,5 +1,5 @@
 """FAD engine (mirror of fadtk/fad.py): same functions, class, methods, on-disk layout and
-error behaviour; the arithmetic runs on the B200 through the C ABI.
+error behaviour; the arithmetic runs on the H100 through the C ABI.
 
     calc_embd_statistics      fad.py:42-48   -> shifted E^T E tensor-core kernel (csrc/stats.cuh)
     calc_frechet_distance     fad.py:51-120  -> Newton-Schulz GEMM chain on the PSD form (csrc/frechet.cuh)

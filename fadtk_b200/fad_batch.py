@@ -5,7 +5,7 @@ of the model on cuda:0 and looping file by file at batch size one - three filesy
 per clip through Python (SURVEY.md section 8 a4).  Here one process owns one GPU and the host
 side is batched too: the PCM16 payloads of a whole chunk of files are read by native threads
 straight into ONE pinned buffer (libfadtk_io.so, include/fadtk_b200_io.h), packed into large
-batches for the sm_100a forward, and the convert cache and the fp16 ``.npy`` embedding cache
+batches for the sm_90a forward, and the convert cache and the fp16 ``.npy`` embedding cache
 are written back by the same native threads - byte-compatible with what the reference writes.
 Files the native reader cannot take as they are (other sample rates, multi-channel, non-PCM16,
 other containers) go through FrechetAudioDistance.convert_audio (GPU resampler) on ``workers``

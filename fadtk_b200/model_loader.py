@@ -3,8 +3,8 @@
 ``ModelLoader`` keeps the reference's contract verbatim - constructor arguments and attributes,
 ``load_model`` / ``_get_embedding`` / ``get_embedding`` / ``load_wav`` / ``enforce_min_len``,
 picklable before ``load_model`` - so third-party plugins written against fadtk (README plugin
-template, README.md:113-138) keep working.  ``VGGishModel`` is the B200-native implementation:
-its forward is hand-written sm_100a CUDA behind the C ABI (include/fadtk_b200.h), not torchvggish.
+template, README.md:113-138) keep working.  ``VGGishModel`` is the H100-native implementation:
+its forward is hand-written sm_90a CUDA behind the C ABI (include/fadtk_b200.h), not torchvggish.
 
 One addition: ``embed_pcm_batch(list_of_int16_arrays)`` lets the batch driver push many clips
 through the GPU in one launch sequence; the default implementation falls back to the per-clip
@@ -204,7 +204,7 @@ class VGGishModel(_DeviceBatch, ModelLoader):
     def __init__(self, use_pca=False, use_activation=False, checkpoint=None, seed: int = 0):
         super().__init__("vggish", 128, 16000, min_len=1)
         if use_pca or use_activation:
-            raise NotImplementedError("the B200 path implements the reference's default (no PCA, no final ReLU)")
+            raise NotImplementedError("the GPU path implements the reference's default (no PCA, no final ReLU)")
         self.use_pca = use_pca
         self.use_activation = use_activation
         self.checkpoint = checkpoint
@@ -315,7 +315,7 @@ class VGGishModel(_DeviceBatch, ModelLoader):
 
 
 class CLAPLaionModel(_DeviceBatch, ModelLoader):
-    """CLAP from https://github.com/LAION-AI/CLAP, audio branch, B200-native.
+    """CLAP from https://github.com/LAION-AI/CLAP, audio branch, H100-native.
 
     Same registry names, dimensionality and sample rate as the reference (model_loader.py:296-297):
     ``type='audio'`` = HTSAT-tiny (630k-audioset-best), ``type='music'`` = HTSAT-base
@@ -371,7 +371,7 @@ class CLAPLaionModel(_DeviceBatch, ModelLoader):
 
 
 class WhisperModel(_DeviceBatch, ModelLoader):
-    """Whisper from https://huggingface.co/openai/whisper-<size>, B200-native (model_loader.py:636-672).
+    """Whisper from https://huggingface.co/openai/whisper-<size>, H100-native (model_loader.py:636-672).
 
     Same registry names (``whisper-tiny|base|small|medium|large``), dimensionality and sample rate.  The
     reference's three transformers calls - feature extractor (clip padded / truncated to 30 s),
@@ -426,7 +426,7 @@ class WhisperModel(_DeviceBatch, ModelLoader):
 
 
 class EncodecEmbModel(_DeviceBatch, ModelLoader):
-    """Encodec (https://github.com/facebookresearch/encodec) continuous encoder output, B200-native
+    """Encodec (https://github.com/facebookresearch/encodec) continuous encoder output, H100-native
     (model_loader.py:111-176).  ``variant='24k'`` (registry name ``encodec-emb``): the causal SEANet encoder
     of ``EncodecModel.encodec_model_24khz()`` on the whole file -> [T/320, 128].  ``variant='48k'``
     (``encodec-emb-48k``): the non-causal GroupNorm encoder of ``encodec_model_48khz()`` on 1-s segments with
@@ -498,7 +498,7 @@ class EncodecEmbModel(_DeviceBatch, ModelLoader):
 
 
 class Wav2VecFamilyModel(_DeviceBatch, ModelLoader):
-    """wav2vec 2.0 / HuBERT / MERT hidden-state embedders, B200-native (model_loader.py:254-288, 525-596).
+    """wav2vec 2.0 / HuBERT / MERT hidden-state embedders, H100-native (model_loader.py:254-288, 525-596).
 
     One class for the three reference loaders whose checkpoints share the "group-norm conv feature encoder +
     post-LN transformer" architecture: ``w2v2-base[-k]`` (facebook/wav2vec2-base-960h), ``hubert-base[-k]``
@@ -595,7 +595,7 @@ def MERTModel(size: str = 'v1-95M', layer: int = 12, **kw):
 
 
 class UnbuiltModel(ModelLoader):
-    """Registry entry whose forward pass has no B200-native implementation yet.
+    """Registry entry whose forward pass has no H100-native implementation yet.
 
     The names stay valid ``choices`` for the CLI (fadtk/__main__.py:13,17); statistics / Frechet
     scoring from cached ``.npy`` embeddings or ``.npz`` statistics works for every name, only
@@ -604,7 +604,7 @@ class UnbuiltModel(ModelLoader):
 
     def load_model(self):
         raise NotImplementedError(
-            f"{self.name}: no sm_100a forward pass in fadtk_b200 yet (see DESIGN.md, scope table)")
+            f"{self.name}: no sm_90a forward pass in fadtk_b200 yet (see DESIGN.md, scope table)")
 
     def _get_embedding(self, audio):
         raise NotImplementedError(self.name)

@@ -130,7 +130,7 @@ def split_hi_lo_tiles(w32: torch.Tensor, tile: int = 128) -> torch.Tensor:
 
 
 def pack_vggish(sd: dict, split_mask: int = ALL_LAYERS_SPLIT) -> dict:
-    """Re-lay the state-dict for the sm_100a kernels (all on CPU, contiguous).
+    """Re-lay the state-dict for the sm_90a kernels (all on CPU, contiguous).
 
     ``split_mask`` bit i (LAYER_NAMES order) stores that layer's weights as an fp16 hi/lo pair
     (split_hi_lo_tiles); default: every tensor-core layer.

@@ -1,4 +1,4 @@
-/* fadtk_b200 - C ABI of the B200-native Frechet-Audio-Distance hot path.
+/* fadtk_b200 - C ABI of the H100-native (sm_90a) Frechet-Audio-Distance hot path.
  *
  * The reference (microsoft/fadtk) has no native layer: its hot path is Python calling
  * third-party PyTorch models and numpy/scipy.  This header is the boundary a maintainer
@@ -170,7 +170,7 @@ size_t fad_stats_acc_len(int d);
  * accumulation is fp64 in a fixed order, so the result is the Gram matrix of the data to ~1e-16,
  * positive semi-definite and bit-reproducible (rank-deficient per-song sets and covariances with
  * cond ~1e9 need that, DESIGN.md section 5.4).
- * tensor_core = 1: tcgen05 kind::f16 hi/lo-split E^T E (fp32 accumulation in TMEM, ~1e-6 relative)
+ * tensor_core = 1: wgmma fp16 hi/lo-split E^T E (fp32 register accumulation, ~1e-6 relative)
  * for well-conditioned, full-rank sets.
  * tensor_core = 2: the same exact arithmetic on the CUDA cores (DFMA + fp64 atomics): verification. */
 int fad_stats_accumulate(fad_handle* h, const void* emb_f16, long long n_rows, int d,
@@ -263,7 +263,7 @@ int fad_resample(fad_handle* h, const int16_t* in_i16, const float* in_f32, int 
 #define FAD_PROF_STATS_REDUCE 11
 #define FAD_PROF_FRECHET      12
 #define FAD_PROF_CLAP_FRONT   13   /* log-mel + patch embedding */
-#define FAD_PROF_CLAP_GEMM    14   /* tcgen05 GEMMs of the Swin blocks */
+#define FAD_PROF_CLAP_GEMM    14   /* wgmma GEMMs of the Swin blocks */
 #define FAD_PROF_CLAP_ATTN    15   /* window attention */
 #define FAD_PROF_CLAP_OTHER   16   /* LayerNorm, residual adds, head */
 #define FAD_PROF_CATEGORIES   20
@@ -275,7 +275,7 @@ long long fad_launch_count(fad_handle* h);
 
 /* Stage entry (parity test / profiling): the encoder self-attention of the Whisper and wav2vec-family forwards alone.
  * qkv: fp16 [n_clips * S][3 d] (q | k | v, head i at columns i * 64), out: fp16 [n_clips * S][d], softmax(q k^T / 8) v per
- * head.  legacy = 0: tcgen05 kernel (csrc/attention_umma.cuh); 1: the mma.sync flash kernel it replaced. */
+ * head.  legacy = 0: wgmma kernel (csrc/attention_wgmma.cuh); 1: the mma.sync flash kernel it replaced. */
 int fad_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int S, int d, void* out_f16, int legacy, void* stream);
 
 /* ---- measurement utility -------------------------------------------------------------
@@ -283,10 +283,6 @@ int fad_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int S, 
  * issue loop: the roofline denominator of the exact-Gram and Newton-Schulz kernels, which
  * MEASURED_PEAKS.json (bf16 GEMM, HBM copy) does not carry.  Synchronous; iters <= 0 = default. */
 int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_host);
-/* Milliseconds that `ksteps` K steps (128 x 128 x 64, hi/lo split weights) take on every SM at once under tcgen05 issue
- * pattern `mode` (0..5, csrc/umma_bench.cuh): operands resident in shared memory, no TMA, no epilogue - what the
- * tensor pipe itself (and the power cap) allows for each way of applying the low weight parts. */
-int fad_bench_umma_mode(fad_handle* h, int mode, int ksteps, double* ms_out_host);
 
 #ifdef __cplusplus
 }

@@ -10,16 +10,16 @@ Contents
 ``fad_oracle``      numpy restatement of the reference's statistics + Frechet code
                     (reference: fadtk/fad.py:42-120, :304-395, fadtk/utils.py:13-46).
                     PINNED: checked against the reference's own functions imported
-                    from /root/reference (see ``ref_shims`` / ``make_golden``); the
+                    from the reference checkout (see ``ref_shims`` / ``make_golden``); the
                     outputs are committed under ``tests/golden/``.
 ``vggish_oracle``   numpy (fp64) log-mel front-end + torch-CPU fp32 VGG stack that
                     the reference reaches through ``torch.hub.load('harritaylor/
                     torchvggish', 'vggish')`` (fadtk/model_loader.py:99-108).
                     PARITY UNPINNED for the network: torchvggish is an un-vendored,
                     un-pinned hub dependency with no source, weights or golden
-                    embeddings in /root/reference, so this is a restatement of the
+                    embeddings in the reference checkout, so this is a restatement of the
                     published algorithm anchored on the reference's call site.
-``ref_shims``       import the real ``fadtk`` package from /root/reference with
+``ref_shims``       import the real ``fadtk`` package from the reference checkout with
                     no-arithmetic stub modules (only usable in the build container).
 ``make_golden``     regenerates ``tests/golden/*.npz`` from the real reference.
 """

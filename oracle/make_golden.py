@@ -1,6 +1,6 @@
 """Regenerate tests/golden/*.npz by running the REAL reference (imported unchanged from
-/root/reference through oracle/ref_shims.py).  Build-container only; the outputs are committed
-because /root/reference does not exist on the GPU box.
+the reference checkout through oracle/ref_shims.py).  Build-container only; the outputs are committed
+because the reference checkout is not available where the GPU tests run.
 
     python -m oracle.make_golden
 

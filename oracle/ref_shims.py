@@ -1,4 +1,4 @@
-"""Import the *real* reference package from /root/reference (build container only).
+"""Import the *real* reference package from the reference checkout (build container only).
 
 Test infrastructure.  The reference's numeric core (fadtk/fad.py, fadtk/utils.py)
 imports cleanly once a handful of no-arithmetic helper modules exist:
@@ -11,18 +11,20 @@ imports cleanly once a handful of no-arithmetic helper modules exist:
   (the lock file pins 1.15.3); fad.py:88 only uses that result for a warning, the
   returned score comes from ``linalg.eig`` (fad.py:91-92,119-120).
 
-Nothing here is reachable from the product package, and /root/reference does not
+Nothing here is reachable from the product package, and the reference checkout does not
 exist on the GPU box: the golden vectors this produces are committed instead.
 """
 from __future__ import annotations
 
 import importlib
 import logging
+import os
 import sys
 import types
 from pathlib import Path
 
-REFERENCE_ROOT = Path("/root/reference")
+# a microsoft/fadtk checkout: $FADTK_REFERENCE_ROOT, else a sibling directory named fadtk
+REFERENCE_ROOT = Path(os.environ.get("FADTK_REFERENCE_ROOT", Path(__file__).resolve().parents[2] / "fadtk"))
 
 
 def _stub(name: str, **attrs) -> types.ModuleType:

@@ -3,7 +3,7 @@
 TEST INFRASTRUCTURE (see oracle/__init__.py).  PARITY UNPINNED for the network:
 the reference obtains the model with ``torch.hub.load('harritaylor/torchvggish',
 'vggish')`` (fadtk/model_loader.py:99) - an un-vendored, un-pinned hub dependency
-whose source and weights are absent from /root/reference and from this image.
+whose source and weights are absent from the reference checkout and from this image.
 What follows restates the *published* algorithm (Hershey et al., ICASSP 2017; the
 AudioSet ``vggish_input`` / ``mel_features`` / ``vggish_params`` definitions that
 torchvggish reuses), anchored on the reference's call site and its two

@@ -16,7 +16,7 @@ os.environ.setdefault("FADTK_SYNTHETIC", "1")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
 
 
 def _has_gpu() -> bool:

@@ -1,4 +1,4 @@
-"""Diagnostic (not a test): does tcgen05 fp32 accumulation shrink results systematically?
+"""Diagnostic (not a test): does tensor-core fp32 accumulation shrink results systematically?
 
 For each layer shape, run the tensor-core layer on post-ReLU-like operands and regress its fp32
 output on the exact fp64 result computed from the SAME fp16 operands:
@@ -45,7 +45,7 @@ def main():
         # magnitude-wise: mean of (|out| - |ref|) / mean |ref|
         shrink = ((o.abs() - ref.abs()).mean() / ref.abs().mean()).item()
         os_ = out32s.double(); slope_s = (os_ * ref).sum() / (ref * ref).sum()
-        print(f"K={taps * cin:6d} N={cout:5d}: split-W slope-1 = {slope_s.item() - 1:+.3e} rms {((os_ - slope_s * ref).norm() / ref.norm()).item():.2e} | tcgen05 slope-1 = {slope.item() - 1:+.3e}  |.|-shrink = {shrink:+.3e}  "
+        print(f"K={taps * cin:6d} N={cout:5d}: split-W slope-1 = {slope_s.item() - 1:+.3e} rms {((os_ - slope_s * ref).norm() / ref.norm()).item():.2e} | fp16-W slope-1 = {slope.item() - 1:+.3e}  |.|-shrink = {shrink:+.3e}  "
               f"noise rms = {rms:.2e}   (torch fp32 CUDA slope-1 = {s32.item() - 1:+.3e})")
 
 

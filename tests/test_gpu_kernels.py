@@ -1,4 +1,4 @@
-"""Stage-by-stage parity of the sm_100a kernels (through the C ABI) against the CPU oracle.
+"""Stage-by-stage parity of the sm_90a kernels (through the C ABI) against the CPU oracle.
 
 Tolerances: the embedder computes with fp16 operands and fp32 accumulation (DESIGN.md
 "precision budget"), so layer outputs are compared with a torch fp32 reference fed the SAME
@@ -154,7 +154,7 @@ def test_statistics_match_numpy_float64(engine, n, d, tensor_core):
     assert np.abs(mu.cpu().numpy() - mu_ref).max() < 1e-9 * (1 + np.abs(mu_ref).max())
     err = np.abs(cov.cpu().numpy() - cov_ref).max() / np.abs(cov_ref).max()
     # exact paths (0 = DMMA on the fp64 tensor pipe, the default; 2 = CUDA-core fp64): Gram matrix of exact
-    # (x - shift) values.  tcgen05 path (1): y carried as an fp16 hi/lo pair (2^-22), fp32 accumulation cut
+    # (x - shift) values.  wgmma path (1): y carried as an fp16 hi/lo pair (2^-22), fp32 accumulation cut
     # every 256 rows -> ~1e-6 of the largest entry
     assert err < (5e-6 if tensor_core == 1 else 1e-12), f"cov rel err {err}"
 
@@ -221,11 +221,13 @@ def test_frechet_golden_fma_pop(engine, golden_dir):
     assert rel < 1e-6, f"FAD {out[0]} vs golden {float(g['fad'])} rel {rel}"
 
 
+# "tcgen05" is the stable id of the default tensor-core attention kernel (legacy=False); on sm_90a that kernel is
+# attention_wgmma_kernel.  The id is kept so the test keeps its identity across architectures.
 @pytest.mark.parametrize("legacy", [False, True], ids=["tcgen05", "mma_sync"])
 @pytest.mark.parametrize("n_clips,S,d", [(2, 1500, 768), (3, 499, 768), (1, 128, 128), (2, 77, 256), (1, 129, 64), (2, 640, 1024)])
 def test_encoder_attention_matches_torch(engine, n_clips, S, d, legacy):
-    """Encoder self-attention stage (Whisper / wav2vec family; heads of 64 dims, scores scaled by 1/8): tcgen05 kernel
-    (S = Q K^T and P V as UMMA tiles, scores in TMEM) and the mma.sync kernel it replaced, against torch in fp32 on the
+    """Encoder self-attention stage (Whisper / wav2vec family; heads of 64 dims, scores scaled by 1/8): wgmma kernel
+    (S = Q K^T and P V as wgmma tiles, scores in registers) and the mma.sync kernel it replaced, against torch in fp32 on the
     same fp16 inputs.  Ragged sizes exercise the zero-filled key rows of the last 128-key block."""
     g = torch.Generator(device="cpu").manual_seed(S * 7 + d)
     qkv = (torch.randn((n_clips * S, 3 * d), generator=g) * 1.5).to(torch.float16)

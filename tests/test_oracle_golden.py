@@ -1,7 +1,7 @@
 """Pin the CPU oracle (oracle/fad_oracle.py) to outputs of the REAL reference functions.
 
 tests/golden/*.npz were produced by oracle/make_golden.py, which imports fadtk/fad.py and
-fadtk/utils.py unchanged from /root/reference.  Bit-level agreement is expected wherever the
+fadtk/utils.py unchanged from the reference checkout.  Bit-level agreement is expected wherever the
 oracle performs the same numpy/LAPACK calls; 1e-12 relative elsewhere.
 """
 import numpy as np

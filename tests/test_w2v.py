@@ -112,7 +112,7 @@ def test_w2v_fad_parity_on_identical_audio(engine):
     1000 + 1000 clips, CLAP 8e-5 at 200 + 200: profiles/r2_parity_*.json).  What it is (DESIGN.md section 3, finding 6):
     under seeded random weights the hidden state of layer 12 is 99.2 % per-dimension mean (mean / rms = 0.996,
     profiles/r2_w2v_fad_terms_32clips.json), so the covariances the score is made of are those of a fluctuation 11x
-    smaller than the values the fp16 GEMM operands round - not the attention kernel (tcgen05 and mma.sync agree,
+    smaller than the values the fp16 GEMM operands round - not the attention kernel (the tensor-core and mma.sync kernels agree,
     profiles/r2_attention_accuracy.json) and, since the epilogue compensates the tensor core's accumulator truncation
     (gain error of a GEMM -8e-7 -> -9e-9, profiles/r2_gemm_bias_probe_*.json), not a gain error of the GEMMs either.
     The reference path itself with fp16-rounded Linear / Conv1d inputs moves the FAD of these sets by +6e-5 ... +1.1e-4 on the
