@@ -45,6 +45,8 @@ SIGNATURES = {
     "fad_vggish_conv1": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_umma_layer": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp,
                                  C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_linear": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_ll, c_vp, C.c_int, c_vp, C.c_int, C.c_int, c_vp, c_vp,
+                             c_vp, C.c_int, C.c_int, C.c_int, c_vp]),
     "fad_clap_load": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_clap_plan": (c_ll, [c_vp, c_ll, c_vp, c_vp, c_ll, c_vp]),
     "fad_clap_plan_frames": (c_ll, [c_vp, c_ll, c_vp, c_vp, c_vp, c_ll, c_vp]),
@@ -268,6 +270,16 @@ class Engine:
                                     cout, taps, int(relu), int(pool), int(split_w), out.data_ptr(), _ptr(out32),
                                     _stream()))
         return (out, out32) if want_f32 else out
+
+    def linear(self, a, rows: int, k_cols: int, w, bias, n_cols: int, act: int = 0, *, lda: int = 0, split_w: int = 1,
+               out16=None, out32=None, resid=None, resid_C: int = 0, resid_res: int = 0, resid_shift: int = 0):
+        """fad_linear: act(A W^T + bias) into the caller's buffers (cuda tensors, any of out16 / out32 / resid).
+        a fp16 rows of k_cols elements lda apart (0: k_cols); w packed fp16 [(2 if split_w else 1) * pad128(n_cols),
+        pad64(k_cols)]; bias fp32 [pad128(n_cols)]; out16 / out32 [rows, n_cols] from their first element;
+        resid fp32 [tokens, resid_C] updated in place.  Raises NativeError on rejected arguments."""
+        _check(lib().fad_linear(self._h, _ptr(a), int(rows), int(k_cols), int(lda), _ptr(w), int(split_w),
+                                _ptr(bias), int(n_cols), int(act), _ptr(out16), _ptr(out32), _ptr(resid),
+                                int(resid_C), int(resid_res), int(resid_shift), _stream()))
 
     # -------------------------------------------------------------------- CLAP
     def clap_load(self, tensors: list, max_chunks: int = 32):

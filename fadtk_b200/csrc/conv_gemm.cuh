@@ -38,6 +38,7 @@ struct ConvGemmParams {
     int n_tiles;               // Cout / N_TILE
     int H, W, NB, Cout;
     float lo_scale;            // WMODE 2: 2^-s of the E4M3 low parts
+    int lo_adds;               // WMODE 1: 1 = the lo parts are not all zero, so their wgmmas truncate the accumulator too
     int lo8_group;             // WMODE 2: k-steps whose E4M3 MMAs are issued together (1 .. min(4, STAGES - 2))
     int ld_out, n_valid;       // un-pooled outputs: row stride and number of columns actually stored
                                // (Cout is padded to the tile width; columns >= n_valid are dropped)
@@ -283,10 +284,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
             for (int i = 0; i < 64; ++i) sum[i] = 0.f;
             for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
                 const int ks1 = min(ks0 + chunk_len, ksteps);
-                // K products per accumulator element: the lo-part products that share the accumulator are ~2^-11 of the
-                // hi ones and add no measurable shrink on H100 (tests/diag_accum_bias.py: counting them over-corrects by
-                // exactly one K's worth, +5.4e-7 at K = 512 per chunk)
-                const float unshrink = kAccumShrinkPerElement * (float)((ks1 - ks0) * kBlockK);
+                // products accumulated per accumulator element: the truncation acts on the running sum, so the lo-part
+                // wgmmas that share the accumulator (SPLIT_W) shrink it as much as the hi ones although their products
+                // are ~2^-11 of them (tests/test_gpu_gemm.py::test_accumulation_is_unbiased: counting only K leaves
+                // -5e-7 per 512-K chunk on H100).  All-zero lo parts (weights exact in fp16, p.lo_adds = 0) add exact
+                // zeros, which do not truncate: counting them would over-correct by +5.4e-7 per chunk.  The E4M3 low
+                // parts have their own accumulator.
+                const float unshrink = kAccumShrinkPerElement * (float)((ks1 - ks0) * kBlockK * (SPLIT_W && p.lo_adds ? 2 : 1));
                 int prev_s = -1;
                 for (int ks = ks0; ks < ks1; ++ks) {
                     mbar_wait(&full[s], ph);
@@ -448,11 +452,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                             }
                         }
                         __syncwarp();
-                        if (p.out != nullptr && out_off >= 0 && ch0 + g * 32 + 32 <= p.n_valid) {   // rare (last VGGish layer): both precisions, direct
+                        if (p.out != nullptr && out_off >= 0) {   // rare: both precisions, direct, in 8-column pieces
                             uint4* dst = reinterpret_cast<uint4*>(p.out + out_off + ch0 + g * 32);
 #pragma unroll
-                            for (int j = 0; j < 4; ++j)
-                                dst[j] = make_uint4(h2[4 * j], h2[4 * j + 1], h2[4 * j + 2], h2[4 * j + 3]);
+                            for (int j = 0; j < 4; ++j)          // n_valid is a multiple of 8: a partial last group
+                                if (ch0 + g * 32 + 8 * j < p.n_valid)
+                                    dst[j] = make_uint4(h2[4 * j], h2[4 * j + 1], h2[4 * j + 2], h2[4 * j + 3]);
                         }
                     } else if (p.out != nullptr) {
                         // fp16 output: two groups (64 columns) fill the 128-B row segment, then flush

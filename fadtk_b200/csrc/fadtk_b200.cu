@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -156,6 +157,7 @@ struct fad_handle {
     float* rs_mono = nullptr;  size_t rs_mono_cap = 0;
     struct Lo8 { uint8_t* w8; float inv_scale; };
     std::map<const void*, Lo8> lo8;          // E4M3 low parts per packed weight tensor (built on first use)
+    std::set<const void*> zero_lo;           // hi/lo weight tensors whose lo parts are all zero (note_split_weights)
     double* fr_scal = nullptr;   // 32 doubles
 
     void* nccl_comm = nullptr;   // ncclComm_t created by fad_comm_init (NCCL is dlopen'ed, never linked)
@@ -250,6 +252,7 @@ int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, 
 void lo8_forget(fad_handle* h, const void* w) {
     auto it = h->lo8.find(w);
     if (it != h->lo8.end()) { cudaFree(it->second.w8); h->lo8.erase(it); }
+    h->zero_lo.erase(w);
 }
 
 // E4M3 copy of an NHWC activation: same box geometry as the fp16 map, 64-B rows, SWIZZLE_64B
@@ -283,6 +286,7 @@ int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CU
     p.bias = bias; p.out = reinterpret_cast<__half*>(out); p.out_f32 = out_f32; p.out8 = out8;
     p.resid = resid; p.resid_C = resid_C; p.resid_res = resid_res; p.resid_shift = resid_shift;
     p.lo_scale = 0.0f;
+    p.lo_adds = g.split_w == 1 && h->zero_lo.count(w) == 0;
     // stages: as many 48 / 32 KiB stages as fit next to the two 32 KiB epilogue tiles in 227 KiB
     if (g.split_w == 2) {
         if (mx8 == nullptr) return fail("fp8 low-part mode needs the E4M3 copy of the activation");
@@ -320,6 +324,28 @@ __global__ void wlo_to_e4m3_kernel(const __half* __restrict__ w, long long n_til
 __global__ void f16_to_e4m3_kernel(const __half* __restrict__ x, size_t count, uint8_t* __restrict__ out) {
     for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < count; e += (size_t)gridDim.x * blockDim.x)
         out[e] = (uint8_t)__nv_cvt_float_to_fp8(__half2float(x[e]), __NV_SATFINITE, __NV_E4M3);
+}
+
+// Whether the lo parts of a hi/lo weight tensor ([2 * 128 * n_tiles, K], device) are all zero, as they are for weights
+// that are exact in fp16.  Their lo wgmmas then add exact zeros, which do not truncate the accumulator, and the GEMM's
+// unshrink counts the hi products only (ConvGemmParams::lo_adds).  Every hi/lo tensor is noted when it is uploaded;
+// caller-owned tensors (the stage entries) on every call.  Synchronous.
+int note_split_weights(fad_handle* h, const void* w, long long n_tiles, long long K, cudaStream_t st) {
+    unsigned int* d_max = nullptr;
+    CK(cudaMalloc(&d_max, 4));
+    unsigned int mx = 0;
+    cudaError_t e = cudaMemsetAsync(d_max, 0, 4, st);
+    if (e == cudaSuccess) {
+        const unsigned blocks = (unsigned)std::max<long long>(1, std::min<long long>((n_tiles * 128 * K + 255) / 256, (long long)h->num_sms * 16));
+        wlo_absmax_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __half*>(w), n_tiles, K, d_max);
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&mx, d_max, 4, cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    cudaFree(d_max);
+    if (e != cudaSuccess) return fail(std::string("note_split_weights: ") + cudaGetErrorString(e));
+    if (mx == 0) h->zero_lo.insert(w); else h->zero_lo.erase(w);
+    return 0;
 }
 
 int lo8_for(fad_handle* h, const LayerGeom& g, const void* w, CUtensorMap* mw8, float* inv_scale, cudaStream_t st) {
@@ -548,6 +574,12 @@ int fad_vggish_load(fad_handle* h, const fad_vggish_weights* w) {
         if (up((void**)&h->fc_w[i], w->fc_w_host[i], mul * L.Cout * L.Cin * 2)) return 1;
         if (up((void**)&h->fc_b[i], w->fc_b_host[i], (size_t)L.Cout * 4)) return 1;
     }
+    for (int i = 0; i < 8; ++i)
+        if ((w->split_mask >> i) & 1) {
+            const VggLayer& L = kVgg[i];
+            if (note_split_weights(h, i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5], L.Cout / 128,
+                                   (long long)L.taps * L.Cin, 0)) return 1;
+        }
     const size_t B = (size_t)h->max_examples;
     if (!h->logmel) CK(cudaMalloc(&h->logmel, B * 96 * 64 * 4));
     for (int i = 0; i < 8; ++i)
@@ -669,6 +701,7 @@ int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int C
     LayerGeom g;
     if (make_geom(g, H, W, Cin, Cout, taps, relu, pool, split_w)) return 1;
     if (pool && out_f32_or_null) return fail("fp32 copy is only available for un-pooled layers");
+    if (g.split_w == 1 && note_split_weights(h, w_f16, Cout / 128, (long long)taps * Cin, (cudaStream_t)stream)) return 1;
     CUtensorMap mx, mw, mx8;
     if (encode_layer_maps(g, x_f16, NB, w_f16, &mx, &mw)) return 1;
     if (g.split_w == 2) {                    // stage test entry: make the E4M3 copy a producer would have written
@@ -1241,6 +1274,22 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
 #include "clap_host.inc"
 
 static void clap_free_state(void* p) { clap_free(reinterpret_cast<ClapState*>(p)); }
+
+extern "C" int fad_linear(fad_handle* h, const void* a_f16, long long rows, int k_cols, long long lda, const void* w_f16,
+                          int split_w, const float* bias, int n_cols, int act, void* out_f16, float* out_f32,
+                          float* resid, int resid_C, int resid_res, int resid_shift, void* stream) {
+    if (!h) return fail("null handle");
+    CK(cudaSetDevice(h->device));
+    const __half* A = reinterpret_cast<const __half*>(a_f16);
+    const __half* W = reinterpret_cast<const __half*>(w_f16);
+    __half* out16 = reinterpret_cast<__half*>(out_f16);
+    if (clap_gemm_check(A, rows, k_cols, W, bias, n_cols, act, out16, out_f32, resid, resid_C, resid_res, resid_shift, lda, split_w))
+        return 1;
+    // caller-owned weights: whether their lo parts are zero is decided on every call, never taken from a cache
+    if (split_w == 1 && note_split_weights(h, W, pad_to(n_cols, 128) / 128, pad_to(k_cols, 64), (cudaStream_t)stream)) return 1;
+    return clap_gemm(h, A, rows, k_cols, W, bias, n_cols, act, out16, out_f32, (cudaStream_t)stream,
+                     resid, resid_C, resid_res, resid_shift, lda, split_w);
+}
 
 #include "whisper_host.inc"
 #include "encodec_host.inc"

@@ -84,6 +84,21 @@ int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int C
                    const void* w_f16, const float* bias, int Cout, int taps, int relu, int pool,
                    int split_w /* weights are [2*Cout, K] hi/lo tiles */,
                    void* out_f16, float* out_f32_or_null, void* stream);
+/* The Linear / 1-D convolution GEMM every transformer and Encodec layer runs (csrc/clap_host.inc clap_gemm):
+ *   C = act(A W^T + bias), act 0 none, 1 ReLU, 2 GELU (erf form), 3 ELU (alpha = 1).
+ * a_f16: fp16 rows of k_cols elements, row r starting at a_f16 + r * lda (lda = 0: k_cols; lda < k_cols gives
+ * overlapping rows); w_f16: [2 * pad128(n_cols), pad64(k_cols)] fp16 hi/lo tiles (split_w = 1, see
+ * weights.split_hi_lo_tiles) or [pad128(n_cols), pad64(k_cols)] fp16 (split_w = 0); bias: fp32 [pad128(n_cols)].
+ * Outputs (any of them may be NULL): out_f16 / out_f32 [rows, n_cols]; resid fp32 [tokens, resid_C]:
+ * resid[token(r)][0:resid_C] += C[r][0:resid_C], token(r) = r (resid_res = 0) or the token of window-ordered row r
+ * of resid_res x resid_res images in 8 x 8 windows cyclically shifted by resid_shift.
+ * k_cols, n_cols and lda must be multiples of 8, resid_C a multiple of 32 and at most n_cols, every pointer
+ * 16-byte aligned; otherwise the call fails and launches nothing.  With split_w = 1 every call first checks, on the
+ * stream and synchronously, whether the lo parts are all zero (weights exact in fp16): the truncation compensation
+ * depends on it. */
+int fad_linear(fad_handle* h, const void* a_f16, long long rows, int k_cols, long long lda, const void* w_f16,
+               int split_w, const float* bias, int n_cols, int act, void* out_f16, float* out_f32,
+               float* resid, int resid_C, int resid_res, int resid_shift, void* stream);
 
 /* ---- CLAP-LAION audio embedder (HTSAT-tiny): replaces CLAPLaionModel.load_model/_get_embedding
  * (fadtk/model_loader.py:382-418 -> laion_clap.CLAP_Module + torchlibrosa front-end).
