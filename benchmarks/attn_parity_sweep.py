@@ -1,5 +1,5 @@
 """How much of the w2v2-base FAD parity error is the attention kernel and how much is chance: FAD(gpu) vs FAD(cpu oracle) for
-several independent 8 + 8 clip sets (4 s clips), under the attention kernel selected by $FADTK_ATTN.  One JSON line."""
+several independent 8 + 8 clip sets (4 s clips).  One JSON line."""
 import json
 import os
 import sys
@@ -25,4 +25,4 @@ for seed in range(int(sys.argv[1]) if len(sys.argv) > 1 else 4):
     fg = fk.calc_frechet_distance(*fk.calc_embd_statistics(gpu["base"]), *fk.calc_embd_statistics(gpu["eval"]))
     fc = fo.frechet_distance(*fo.embd_statistics(cpu["base"]), *fo.embd_statistics(cpu["eval"]))
     out.append({"seed": seed, "fad_gpu": float(fg), "fad_cpu": float(fc), "rel": float((fg - fc) / fc)})
-print(json.dumps({"attention": os.environ.get("FADTK_ATTN", "wgmma"), "sets": out}))
+print(json.dumps({"sets": out}))

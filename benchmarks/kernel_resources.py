@@ -17,13 +17,11 @@ for line in txt.splitlines():
         rows.append((cur, int(m.group(1)), int(m.group(2)), int(m.group(3))))
         cur = None
 names = subprocess.run(["c++filt"] + [r[0] for r in rows], capture_output=True, text=True).stdout.splitlines()
-print("# Kernel resource audit, end of round 2 (`cuobjdump -res-usage fadtk_b200/csrc/libfadtk_b200.so`, sm_90a)\n")
+print("# Kernel resource audit (`cuobjdump -res-usage fadtk_b200/csrc/libfadtk_b200.so`, sm_90a)\n")
 print("Registers per thread, stack bytes (spills / local arrays), static shared memory; dynamic shared memory (conv_gemm,")
-print("attention_umma, logmel, stats_umma) is set at launch.  New this round: `attention_umma_kernel` (320 threads, two CTAs per")
-print("SM), the fp64 tensor-pipe kernels (`dgemm_kernel`, `dgemm_strided_kernel`, `stats_dmma_kernel<__half | double>`,")
-print("`song_stats_dmma_kernel`: <= 128 registers for two CTAs per SM, no spills), the `conv_gemm_kernel<N_TILE, STAGES, WMODE,")
-print("PAIR, STACK>` pair instantiations (tens of bytes of spills in the epilogue warps).\n")
+print("attention_wgmma, logmel) is set at launch.  The fp64 tensor-pipe kernels (`dgemm_kernel`, `dgemm_strided_kernel`,")
+print("`stats_dmma_kernel<__half | double>`, `song_stats_dmma_kernel`) stay at <= 128 registers for two CTAs per SM.\n")
 print("| kernel | registers | stack bytes | static smem |\n|---|---|---|---|")
 for (m, r, st, sh), n in sorted(zip(rows, names), key=lambda t: t[1]):
-    n = re.sub(r"\(.*", "", n).replace("void ", "").replace("(anonymous namespace)::", "")
+    n = re.sub(r"\(.*", "", n.replace("(anonymous namespace)::", "")).replace("void ", "")
     print(f"| `{n}` | {r} | {st} | {sh} |")

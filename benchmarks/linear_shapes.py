@@ -1,5 +1,5 @@
 """Per-shape rate of the wgmma GEMM kernel on the Linear layers of the transformer forwards (stage entry
-fad_umma_layer, H = W = 1): split weights with and without CTA pairs, and plain fp16 weights for scale.
+fad_umma_layer, H = W = 1): split weights, and plain fp16 weights for scale.
 TFLOP/s are ALGORITHMIC (2 M N K once).  One JSON list on stdout."""
 import json
 import os
@@ -29,8 +29,7 @@ for name, rows, K, N, act in SHAPES:
     w32[:N] = torch.randn(N, K) / K ** 0.5
     bias = torch.zeros(npad, dtype=torch.float32, device=dev)
     rec = {"layer": name, "rows": rows, "K": K, "N": N, "act": act}
-    for label, split, pair in (("split", True, "0"), ("split_pair", True, "1"), ("fp16", False, "0")):
-        os.environ["FADTK_PAIR"] = pair
+    for label, split in (("split", True), ("fp16", False)):
         w = (weights.split_hi_lo_tiles(w32, 128) if split else w32.to(torch.float16)).to(dev).contiguous()
         for _ in range(3):
             eng.umma_layer(x, w, bias, 1, act, 0, split_w=split)

@@ -458,7 +458,8 @@ class Engine:
     def stats_new(self, d: int) -> torch.Tensor:
         return torch.zeros(self.stats_acc_len(d), dtype=torch.float64, device=self.torch_device)
 
-    def stats_accumulate(self, emb, shift, acc, tensor_core=False):
+    def stats_accumulate(self, emb, shift, acc, tensor_core: int = 0):
+        """tensor_core 0: exact Gram on the FP64 tensor pipe (the product path); 2: the CUDA-core fp64 cross-check."""
         assert emb.dtype == torch.float16 and emb.is_contiguous() and shift.dtype == torch.float16
         n, d = emb.shape
         _check(lib().fad_stats_accumulate(self._h, emb.data_ptr(), n, d, shift.data_ptr(),

@@ -37,16 +37,13 @@ struct ConvGemmParams {
     int img_groups;            // ceil(NB / box_n)
     int n_tiles;               // Cout / N_TILE
     int H, W, NB, Cout;
-    float lo_scale;            // WMODE 2: 2^-s of the E4M3 low parts
     int lo_adds;               // WMODE 1: 1 = the lo parts are not all zero, so their wgmmas truncate the accumulator too
-    int lo8_group;             // WMODE 2: k-steps whose E4M3 MMAs are issued together (1 .. min(4, STAGES - 2))
     int ld_out, n_valid;       // un-pooled outputs: row stride and number of columns actually stored
                                // (Cout is padded to the tile width; columns >= n_valid are dropped)
     int relu, pool;            // relu: 0 = none, 1 = ReLU, 2 = GELU (erf form), 3 = ELU
     const float* bias;         // [Cout]
     __half* out;               // NHWC fp16 [NB, H(/2), W(/2), Cout]; may be null when out_f32 is set
     float* out_f32;            // optional fp32 copy of the un-pooled output (may be null)
-    uint8_t* out8;             // optional E4M3 copy of `out` (same layout) for a WMODE 2 consumer (may be null)
     // optional fused residual update (transformer blocks): resid[token(row)][0:resid_C] += result,
     // where row -> token undoes the (shifted-)window ordering of the rows (resid_res = 0: identity)
     float* resid;
@@ -91,15 +88,11 @@ constexpr uint32_t kStagingBytes = 32 * 128;       // per epilogue warp: 32 rows
 // whereas fp16 activations cost 2e-5.  The hi and lo rows of one N tile are stored back to back
 // ([Wh: N_TILE rows | Wl: N_TILE rows] per tile), so ONE TMA box brings both and each consumer
 // issues A x Wh and A x Wl into the same accumulator.
-// WMODE 0: fp16 weights.  1: fp16 hi/lo pair, two fp16 wgmmas per K slice.  2: fp16 hi + E4M3 lo:
-// the low part (|Wl| <= 2^-11 |W|, needed to ~4 bits) is applied by an E4M3 wgmma - twice the
-// rate and half the operand bytes of a second fp16 one - against an E4M3 copy of the activation
-// (written next to the fp16 one by the producing kernel, fetched by its own TMA box), into its own
-// register accumulator that the epilogue adds with the power-of-two scale of the E4M3 weights.
+// WMODE 0: fp16 weights, one wgmma per K slice.  WMODE 1: fp16 hi/lo pair (SPLIT_W), two fp16
+// wgmmas per K slice into one accumulator.
 template <int N_TILE, int WMODE>
 __host__ __device__ constexpr uint32_t conv_gemm_stage_bytes() {
-    return WMODE == 2 ? kABytes + N_TILE * kBlockK * 2 + N_TILE * kBlockK + kTileM * kBlockK
-                      : kABytes + (WMODE == 1 ? 2 : 1) * N_TILE * kBlockK * 2;
+    return kABytes + (WMODE == 1 ? 2 : 1) * N_TILE * kBlockK * 2;
 }
 
 template <int N_TILE, int STAGES, int WMODE>
@@ -141,18 +134,6 @@ __device__ __forceinline__ float elu_ex2(float x) {
     return x > 0.f ? x : (x > -0.0625f ? t : e - 1.0f);
 }
 
-// 8 halves -> 8 E4M3 bytes (round to nearest, saturate)
-__device__ __forceinline__ uint32_t f16x4_to_e4m3x4(uint32_t a, uint32_t b) {
-    __half2_raw h0, h1;
-    h0.x = (unsigned short)(a & 0xffffu); h0.y = (unsigned short)(a >> 16);
-    h1.x = (unsigned short)(b & 0xffffu); h1.y = (unsigned short)(b >> 16);
-    return (uint32_t)__nv_cvt_halfraw2_to_fp8x2(h0, __NV_SATFINITE, __NV_E4M3)
-         | ((uint32_t)__nv_cvt_halfraw2_to_fp8x2(h1, __NV_SATFINITE, __NV_E4M3) << 16);
-}
-__device__ __forceinline__ uint2 f16x8_to_e4m3x8(uint4 v) {
-    return make_uint2(f16x4_to_e4m3x4(v.x, v.y), f16x4_to_e4m3x4(v.z, v.w));
-}
-
 __device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
     __half2 r = __hmax2(*reinterpret_cast<__half2*>(&a), *reinterpret_cast<__half2*>(&b));
     return *reinterpret_cast<uint32_t*>(&r);
@@ -162,19 +143,14 @@ template <int N_TILE, int STAGES, int WMODE>
 __global__ void __launch_bounds__(kConvGemmThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                  const __grid_constant__ CUtensorMap map_w,
-                 const __grid_constant__ CUtensorMap map_wl8,       // WMODE 2: E4M3 low parts [Cout, K]
-                 const __grid_constant__ CUtensorMap map_x8,        // WMODE 2: E4M3 copy of the activation
                  const ConvGemmParams p)
 {
     using namespace sm90;
     static_assert(N_TILE == 128, "one m64n128 accumulator per consumer warpgroup");
+    static_assert(WMODE == 0 || WMODE == 1, "WMODE 0: fp16 weights, 1: fp16 hi/lo pair");
     constexpr bool SPLIT_W = WMODE == 1;
-    constexpr bool LO8 = WMODE == 2;
     constexpr uint32_t kStageBytes = conv_gemm_stage_bytes<N_TILE, WMODE>();
-    constexpr int kBRows = (WMODE != 0 ? 2 : 1) * N_TILE;           // rows of the packed weight tensor per N tile
-    constexpr uint32_t kWhBytes = N_TILE * kBlockK * 2;
-    constexpr uint32_t kOffWl8 = kABytes + kWhBytes;                // stage layout (LO8): A16 | Wh | Wl8 | A8
-    constexpr uint32_t kOffA8 = kOffWl8 + N_TILE * kBlockK;
+    constexpr int kBRows = (SPLIT_W ? 2 : 1) * N_TILE;              // rows of the packed weight tensor per N tile
     constexpr int kColsPerThread = N_TILE / 2;          // epilogue: one row, one column half per thread
     constexpr int kGroups = kColsPerThread / 32;
 
@@ -196,7 +172,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_x);
         tma_prefetch_desc(&map_w);
-        if (LO8) { tma_prefetch_desc(&map_wl8); tma_prefetch_desc(&map_x8); }
     }
     if (warp == 1 && lane == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers * 4); }
@@ -206,7 +181,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
 
     if (warp < 4) {
         // ------------------------------------------------------------ TMA producer
-        // hand the registers of this warpgroup to the two consumers, which hold 2 x 64 (+ 64) fp32 accumulators
+        // hand the registers of this warpgroup to the two consumers, which hold 2 x 64 fp32 accumulators
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
             int s = 0; uint32_t ph = 0;
@@ -226,10 +201,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     mbar_expect_tx(&full[s], kStageBytes);
                     tma_load_4d(st, &map_x, &full[s], cb * kBlockK, w0 + dw, h0 + dh, n0);
                     tma_load_2d(st + kABytes, &map_w, &full[s], ks * kBlockK, nt * kBRows);
-                    if (LO8) {
-                        tma_load_2d(st + kOffWl8, &map_wl8, &full[s], ks * kBlockK, nt * N_TILE);
-                        tma_load_4d(st + kOffA8, &map_x8, &full[s], cb * kBlockK, w0 + dw, h0 + dh, n0);
-                    }
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
             }
@@ -278,8 +249,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 prefetch_resid((tile + (int)gridDim.x) % p.n_tiles, (tile + (int)gridDim.x) / p.n_tiles);
 
             // ---- main loop: chunks of <= kChunkSteps k-steps into `acc`, summed into `sum` (round-to-nearest adds,
-            // undoing the expected truncation shrink of each chunk); LO8: the low-part products into `corr`
-            float sum[64], acc[64], corr[LO8 ? 64 : 1];
+            // undoing the expected truncation shrink of each chunk)
+            float sum[64], acc[64];
 #pragma unroll
             for (int i = 0; i < 64; ++i) sum[i] = 0.f;
             for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
@@ -288,8 +259,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 // wgmmas that share the accumulator (SPLIT_W) shrink it as much as the hi ones although their products
                 // are ~2^-11 of them (tests/test_gpu_gemm.py::test_accumulation_is_unbiased: counting only K leaves
                 // -5e-7 per 512-K chunk on H100).  All-zero lo parts (weights exact in fp16, p.lo_adds = 0) add exact
-                // zeros, which do not truncate: counting them would over-correct by +5.4e-7 per chunk.  The E4M3 low
-                // parts have their own accumulator.
+                // zeros, which do not truncate: counting them would over-correct by +5.4e-7 per chunk.
                 const float unshrink = kAccumShrinkPerElement * (float)((ks1 - ks0) * kBlockK * (SPLIT_W && p.lo_adds ? 2 : 1));
                 int prev_s = -1;
                 for (int ks = ks0; ks < ks1; ++ks) {
@@ -305,13 +275,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                         if (SPLIT_W)                   // lo rows: N_TILE rows (x 128 B) further down the stage, same accumulator
                             wgmma_m64n128k16_f16<0, 0>(acc, a_desc + 2 * k, b_desc + 2 * k + (N_TILE * 128 / 16), 1);
                     }
-                    if constexpr (LO8) {
-                        const uint64_t a8_desc = kmajor_sw64_desc(a_addr + kOffA8 + c * 64 * 64);
-                        const uint64_t w8_desc = kmajor_sw64_desc(a_addr + kOffWl8);
-#pragma unroll
-                        for (int k = 0; k < kBlockK / 32; ++k)   // K = 32 per E4M3 wgmma, +32 B inside the 64-B atom
-                            wgmma_m64n128k32_e4m3(corr, a8_desc + 2 * k, w8_desc + 2 * k, (ks > 0) || (k > 0));
-                    }
                     wgmma_commit();
                     wgmma_wait<1>();                   // the previous k-step's wgmmas have retired: release its stage
                     if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
@@ -320,15 +283,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 }
                 wgmma_wait<0>();
                 fence_regs(acc);
-                if constexpr (LO8) fence_regs(corr);
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[prev_s]);
 #pragma unroll
                 for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
-            }
-            if constexpr (LO8) {                       // + A8 * Wl8^T / 2^s
-#pragma unroll
-                for (int i = 0; i < 64; ++i) sum[i] = fmaf(corr[i], p.lo_scale, sum[i]);
             }
 
             // ---- accumulator fragment -> fp32 tile [64 rows][128 cols] in shared memory, 16-B chunks XOR-swizzled by row
@@ -472,10 +430,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                                 const int rr = it * 4 + rq;
                                 const uint4 v = lds128(stg + rr * 128 + ((cq ^ (rr & 7)) << 4));
                                 const long long off = __shfl_sync(0xffffffffu, out_off, rr);
-                                if (off >= 0 && col < p.n_valid) {
-                                    *reinterpret_cast<uint4*>(p.out + off + col) = v;
-                                    if (p.out8 != nullptr) *reinterpret_cast<uint2*>(p.out8 + off + col) = f16x8_to_e4m3x8(v);
-                                }
+                                if (off >= 0 && col < p.n_valid) *reinterpret_cast<uint4*>(p.out + off + col) = v;
                             }
                             __syncwarp();
                         }
@@ -499,7 +454,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     if (valid) {
                         const size_t pix = (size_t(n) * (p.H >> 1) + (h >> 1)) * (p.W >> 1) + (w >> 1);
                         *reinterpret_cast<uint4*>(p.out + pix * p.Cout + ch0 + g * 32 + sub * 8) = o;
-                        if (p.out8 != nullptr) *reinterpret_cast<uint2*>(p.out8 + pix * p.Cout + ch0 + g * 32 + sub * 8) = f16x8_to_e4m3x8(o);
                     }
                 }
             }

@@ -5,13 +5,11 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
-#include <cuda_fp8.h>
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <map>
 #include <set>
 #include <string>
 #include <vector>
@@ -82,18 +80,12 @@ int encode_f16_map(CUtensorMap* map, const void* base, int rank, const uint64_t*
 struct LayerGeom {
     int taps, Cin, Cout, H, W, relu, pool;
     int box_w, box_h, box_n, n_tile;
-    int split_w;      // 0: fp16 weights; 1: fp16 hi/lo pair (interleaved per 128-row tile), two fp16 MMAs;
-                      // 2: same packed tensor, low part applied by an E4M3 wgmma - see conv_gemm.cuh
+    int split_w;      // 0: fp16 weights; 1: fp16 hi/lo pair (interleaved per 128-row tile), two fp16 MMAs
 };
 
-// how the low part of split weights is applied: FADTK_WLO=fp16 (two fp16 MMAs) | fp8 (E4M3 correction MMA)
-int wlo_mode() {
-    static const int mode = [] { const char* e = getenv("FADTK_WLO"); return (e && std::string(e) == "fp8") ? 2 : 1; }();
-    return mode;
-}
 int make_geom(LayerGeom& g, int H, int W, int Cin, int Cout, int taps, int relu, int pool, int split_w) {
     g.taps = taps; g.Cin = Cin; g.Cout = Cout; g.H = H; g.W = W; g.relu = relu; g.pool = pool;
-    g.split_w = split_w;                     // 0, 1 or 2 - the caller decides (wlo_mode() for the VGGish pipeline)
+    g.split_w = split_w;
     if (Cin % 64 != 0) return fail("Cin must be a multiple of 64");
     if (taps != 1 && taps != 9) return fail("taps must be 1 or 9");
     if (H == 1 && W == 1) { g.box_w = 1; g.box_h = 1; g.box_n = 128; }
@@ -137,9 +129,7 @@ struct fad_handle {
     __half* act[9] = {};       // act[0]=conv1 out ... act[5]=conv6 out (flattened), act[6..7]=fc1, fc2 out
 
     // per-layer cached descriptors for the fixed VGGish pipeline
-    CUtensorMap map_x[8], map_w[8], map_x8[8];
-    uint8_t* act8[8] = {};     // E4M3 copies of act[0..7] (inputs of the 8 tensor-core layers) when the low parts run in fp8
-    uint8_t* x8_scratch = nullptr;  size_t x8_scratch_cap = 0;   // fad_umma_layer (stage test) only
+    CUtensorMap map_x[8], map_w[8];
     LayerGeom geom[8];
 
     // statistics workspace
@@ -155,8 +145,6 @@ struct fad_handle {
     size_t frb_cap = 0;
     float* rs_bank = nullptr;  size_t rs_bank_cap = 0;  int rs_in = 0, rs_out = 0;     // resampler filter bank
     float* rs_mono = nullptr;  size_t rs_mono_cap = 0;
-    struct Lo8 { uint8_t* w8; float inv_scale; };
-    std::map<const void*, Lo8> lo8;          // E4M3 low parts per packed weight tensor (built on first use)
     std::set<const void*> zero_lo;           // hi/lo weight tensors whose lo parts are all zero (note_split_weights)
     double* fr_scal = nullptr;   // 32 doubles
 
@@ -180,8 +168,7 @@ struct fad_handle {
 namespace {
 
 template <int N_TILE, int STAGES, int WMODE>
-int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const CUtensorMap& mw8,
-                     const CUtensorMap& mx8, const fad::ConvGemmParams& p, cudaStream_t st) {
+int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const fad::ConvGemmParams& p, cudaStream_t st) {
     static bool attr_set = false;
     constexpr uint32_t smem = fad::conv_gemm_smem_bytes<N_TILE, STAGES, WMODE>();
     static_assert(smem <= 227 * 1024, "over the per-CTA shared-memory limit");
@@ -193,7 +180,7 @@ int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw
     const int total = p.img_groups * p.tiles_h * p.tiles_w * p.n_tiles;
     if (total == 0) return 0;
     const int grid = total < h->num_sms ? total : h->num_sms;
-    kern<<<grid, fad::kConvGemmThreads, smem, st>>>(mx, mw, mw8, mx8, p);
+    kern<<<grid, fad::kConvGemmThreads, smem, st>>>(mx, mw, p);
     CK(cudaGetLastError());
     h->launches++;
     return 0;
@@ -215,19 +202,13 @@ int encode_layer_maps(const LayerGeom& g, const void* x, long long nb_dim, const
     const uint64_t rows_mul = g.split_w ? 2 : 1;
     const uint64_t wd[2] = {K, (uint64_t)g.Cout * rows_mul};
     const uint64_t ws[1] = {K * 2};
-    // rows per weight box: mode 1 fetches hi + lo of a tile at once, mode 2 the hi rows only
-    const uint32_t wb[2] = {64, (uint32_t)(g.n_tile * (g.split_w == 1 ? 2 : 1))};
+    // rows per weight box: a split layer fetches hi + lo of a tile at once
+    const uint32_t wb[2] = {64, (uint32_t)(g.n_tile * rows_mul)};
     return encode_f16_map(mw, w, 2, wd, ws, wb);
 }
 
-int lo8_for(fad_handle* h, const LayerGeom& g, const void* w, CUtensorMap* mw8, float* inv_scale, cudaStream_t st);
-
 // Encoder self-attention on wgmma (attention_wgmma.cuh).  qkv: fp16 [clips * S][3 d] (q | k | v, head h at column h * 64),
-// out: fp16 [clips * S][d].  FADTK_ATTN=legacy selects the mma.sync flash kernel (whisper.cuh) instead.
-bool attention_wgmma_enabled() {
-    static const bool on = [] { const char* e = getenv("FADTK_ATTN"); return !(e && std::string(e) == "legacy"); }();
-    return on;
-}
+// out: fp16 [clips * S][d].
 int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, int S, int d, int heads, __half* out, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
@@ -248,31 +229,12 @@ int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, 
     return 0;
 }
 
-// the E4M3 low parts are cached per weight POINTER: drop the entry whenever that memory is rewritten
-void lo8_forget(fad_handle* h, const void* w) {
-    auto it = h->lo8.find(w);
-    if (it != h->lo8.end()) { cudaFree(it->second.w8); h->lo8.erase(it); }
-    h->zero_lo.erase(w);
-}
-
-// E4M3 copy of an NHWC activation: same box geometry as the fp16 map, 64-B rows, SWIZZLE_64B
-int encode_x8_map(const LayerGeom& g, const void* x8, long long nb_dim, CUtensorMap* mx8) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t gdim[4] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W, (cuuint64_t)g.H, (cuuint64_t)nb_dim};
-    cuuint64_t gstr[3] = {(cuuint64_t)g.Cin, (cuuint64_t)g.W * g.Cin, (cuuint64_t)g.H * g.W * g.Cin};
-    cuuint32_t bdim[4] = {64, (cuuint32_t)g.box_w, (cuuint32_t)g.box_h, (cuuint32_t)g.box_n}, estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(mx8, CU_TENSOR_MAP_DATA_TYPE_UINT8, 4, const_cast<void*>(x8), gdim, gstr, bdim, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (E4M3 activation) failed");
-    return 0;
-}
+// zero_lo is keyed by weight POINTER: drop the entry whenever that memory is freed or reallocated
+void forget_zero_lo(fad_handle* h, const void* w) { h->zero_lo.erase(w); }
 
 int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CUtensorMap& mw, const void* w,
               int NB, const float* bias, void* out, float* out_f32, cudaStream_t st,
-              float* resid = nullptr, int resid_C = 0, int resid_res = 0, int resid_shift = 0, int n_valid = 0,
-              const CUtensorMap* mx8 = nullptr, uint8_t* out8 = nullptr) {
+              float* resid = nullptr, int resid_C = 0, int resid_res = 0, int resid_shift = 0, int n_valid = 0) {
     fad::ConvGemmParams p;
     p.taps = g.taps; p.cblks = g.Cin / 64;
     p.box_w = g.box_w; p.box_h = g.box_h; p.box_n = g.box_n;
@@ -283,23 +245,15 @@ int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CU
     p.n_valid = n_valid > 0 ? n_valid : g.Cout;
     p.ld_out = p.n_valid;
     p.relu = g.relu; p.pool = g.pool;
-    p.bias = bias; p.out = reinterpret_cast<__half*>(out); p.out_f32 = out_f32; p.out8 = out8;
+    p.bias = bias; p.out = reinterpret_cast<__half*>(out); p.out_f32 = out_f32;
     p.resid = resid; p.resid_C = resid_C; p.resid_res = resid_res; p.resid_shift = resid_shift;
-    p.lo_scale = 0.0f;
     p.lo_adds = g.split_w == 1 && h->zero_lo.count(w) == 0;
     // stages: as many 48 / 32 KiB stages as fit next to the two 32 KiB epilogue tiles in 227 KiB
-    if (g.split_w == 2) {
-        if (mx8 == nullptr) return fail("fp8 low-part mode needs the E4M3 copy of the activation");
-        CUtensorMap mw8;
-        if (lo8_for(h, g, w, &mw8, &p.lo_scale, st)) return 1;
-        return launch_conv_gemm<128, 3, 2>(h, mx, mw, mw8, *mx8, p, st);
-    }
-    if (g.split_w) return launch_conv_gemm<128, 3, 1>(h, mx, mw, mw, mx, p, st);
-    return launch_conv_gemm<128, 4, 0>(h, mx, mw, mw, mx, p, st);
+    if (g.split_w) return launch_conv_gemm<128, 3, 1>(h, mx, mw, p, st);
+    return launch_conv_gemm<128, 4, 0>(h, mx, mw, p, st);
 }
 
-// E4M3 copy of the low parts of a packed hi/lo weight tensor, scaled by a power of two so the largest
-// |Wl| lands near 224 (E4M3 max 448), plus its tensor map (64-B rows, SWIZZLE_64B).  Built once per tensor.
+// max |Wl| over the lo parts of a packed hi/lo weight tensor ([hi: 128 rows | lo: 128 rows] per tile), as float bits
 __global__ void wlo_absmax_kernel(const __half* __restrict__ w, long long n_tiles, long long K, unsigned int* __restrict__ out) {
     float m = 0.f;
     const long long total = n_tiles * 128 * K;
@@ -311,21 +265,6 @@ __global__ void wlo_absmax_kernel(const __half* __restrict__ w, long long n_tile
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));
 }
-__global__ void wlo_to_e4m3_kernel(const __half* __restrict__ w, long long n_tiles, long long K, float scale, uint8_t* __restrict__ out) {
-    const long long total = n_tiles * 128 * K;
-    for (long long e = blockIdx.x * (long long)blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
-        const long long row = e / K, k = e - row * K;
-        const long long t = row >> 7, j = row & 127;
-        const float v = __half2float(w[((t * 256 + 128 + j) * K) + k]) * scale;
-        out[e] = (uint8_t)__nv_cvt_float_to_fp8(v, __NV_SATFINITE, __NV_E4M3);
-    }
-}
-
-__global__ void f16_to_e4m3_kernel(const __half* __restrict__ x, size_t count, uint8_t* __restrict__ out) {
-    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < count; e += (size_t)gridDim.x * blockDim.x)
-        out[e] = (uint8_t)__nv_cvt_float_to_fp8(__half2float(x[e]), __NV_SATFINITE, __NV_E4M3);
-}
-
 // Whether the lo parts of a hi/lo weight tensor ([2 * 128 * n_tiles, K], device) are all zero, as they are for weights
 // that are exact in fp16.  Their lo wgmmas then add exact zeros, which do not truncate the accumulator, and the GEMM's
 // unshrink counts the hi products only (ConvGemmParams::lo_adds).  Every hi/lo tensor is noted when it is uploaded;
@@ -345,43 +284,6 @@ int note_split_weights(fad_handle* h, const void* w, long long n_tiles, long lon
     cudaFree(d_max);
     if (e != cudaSuccess) return fail(std::string("note_split_weights: ") + cudaGetErrorString(e));
     if (mx == 0) h->zero_lo.insert(w); else h->zero_lo.erase(w);
-    return 0;
-}
-
-int lo8_for(fad_handle* h, const LayerGeom& g, const void* w, CUtensorMap* mw8, float* inv_scale, cudaStream_t st) {
-    const long long K = (long long)g.taps * g.Cin, n_tiles = g.Cout / 128;
-    auto it = h->lo8.find(w);
-    if (it == h->lo8.end()) {
-        unsigned int* d_max = nullptr;
-        uint8_t* w8 = nullptr;
-        CK(cudaMalloc(&d_max, 4));
-        CK(cudaMalloc(&w8, (size_t)(n_tiles * 128 * K)));
-        CK(cudaMemsetAsync(d_max, 0, 4, st));
-        const unsigned blocks = (unsigned)std::min<long long>((n_tiles * 128 * K + 255) / 256, (long long)h->num_sms * 16);
-        wlo_absmax_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __half*>(w), n_tiles, K, d_max);
-        float mx = 0.f;
-        CK(cudaMemcpyAsync(&mx, d_max, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        int e = 0;
-        if (mx > 0.f) e = (int)std::floor(std::log2(224.0f / mx));
-        if (e > 100) e = 100;
-        const float scale = std::ldexp(1.0f, e);
-        wlo_to_e4m3_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __half*>(w), n_tiles, K, scale, w8);
-        CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(st));
-        cudaFree(d_max);
-        it = h->lo8.emplace(w, fad_handle::Lo8{w8, 1.0f / scale}).first;
-    }
-    *inv_scale = it->second.inv_scale;
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) return fail("cuTensorMapEncodeTiled entry point not available");
-    cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)(n_tiles * 128)};
-    cuuint64_t gstr[1] = {(cuuint64_t)K};
-    cuuint32_t bdim[2] = {64, 128}, estr[2] = {1, 1};
-    CUresult r = fn(mw8, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, it->second.w8, gdim, gstr, bdim, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail("cuTensorMapEncodeTiled (E4M3 low parts) failed");
     return 0;
 }
 
@@ -455,6 +357,38 @@ void prof_end(fad_handle* h, int cat, size_t e0, cudaStream_t st) {
     h->spans.push_back({cat, e0, e1});
 }
 
+// Exact Gram statistics on the FP64 tensor pipe (stats.cuh): acc += the packed statistics of E [n_rows, d] - shift.
+// In = __half (embeddings) or double (per-file mean rows, no shift).  Only the embedding statistics are profiled.
+template <typename In>
+int launch_stats_dmma(fad_handle* h, const In* E, long long n_rows, int d, const __half* shift, double* acc, cudaStream_t st) {
+    constexpr bool kProf = sizeof(In) == 2;
+    if (d % 64 != 0) return fail("d must be a multiple of 64");
+    fad::StatsDmmaParams p;
+    p.n_rows = n_rows; p.d = d; p.n_tiles = d / fad::kSdTile;
+    p.n_pairs = p.n_tiles * (p.n_tiles + 1) / 2;
+    const long long stages = (n_rows + fad::kSdRows - 1) / fad::kSdRows;
+    long long want = (4LL * h->num_sms + p.n_pairs - 1) / p.n_pairs;       // ~2 waves at 2 CTAs per SM
+    if (want < 1) want = 1;
+    long long per = (stages + want - 1) / want;                             // 16-row stages per split
+    if (per < 4) per = 4;
+    p.n_splits = (int)((stages + per - 1) / per);
+    p.rows_per_split = per * fad::kSdRows;
+    p.shift = shift;
+    const size_t jobs = (size_t)p.n_pairs * p.n_splits;
+    if (ensure((void**)&h->ws_tiles, &h->ws_tiles_cap, jobs * fad::kSdTile * fad::kSdTile * 8)) return 1;
+    if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
+    p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
+    size_t ev = kProf ? prof_begin(h, st) : 0;
+    fad::stats_dmma_kernel<In><<<(unsigned)jobs, 256, 0, st>>>(E, p);
+    CK(cudaGetLastError());
+    if (kProf) { prof_end(h, FAD_PROF_STATS, ev, st); ev = prof_begin(h, st); }
+    fad::stats_dmma_reduce_kernel<<<dim3(p.n_pairs, fad::kSdTile * fad::kSdTile / 256), 256, 0, st>>>(p, acc);
+    CK(cudaGetLastError());
+    if (kProf) prof_end(h, FAD_PROF_STATS_REDUCE, ev, st);
+    h->launches += 2;
+    return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -514,8 +448,6 @@ int fad_create(int device, int max_examples, fad_handle** out) {
                             (int)fad::logmel_smem_bytes<double>()));
     CK(cudaFuncSetAttribute(fad::logmel_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)fad::logmel_smem_bytes<float>()));
-    CK(cudaFuncSetAttribute(fad::stats_umma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)fad::kStSmemBytes));
     *out = h;
     return 0;
 }
@@ -536,12 +468,9 @@ int fad_destroy(fad_handle* h) {
     void* ptrs[] = {h->d_twiddle, h->d_hann, h->d_melw, h->d_mel_start, h->d_mel_count, h->conv1_w, h->conv1_b,
                     h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->fr_scal, h->frb_buf, h->rs_bank, h->rs_mono};
     for (void* p : ptrs) if (p) cudaFree(p);
-    for (auto& kv : h->lo8) cudaFree(kv.second.w8);
     for (int i = 0; i < 5; ++i) { if (h->conv_w[i]) cudaFree(h->conv_w[i]); if (h->conv_b[i]) cudaFree(h->conv_b[i]); }
     for (int i = 0; i < 3; ++i) { if (h->fc_w[i]) cudaFree(h->fc_w[i]); if (h->fc_b[i]) cudaFree(h->fc_b[i]); }
     for (int i = 0; i < 9; ++i) if (h->act[i]) cudaFree(h->act[i]);
-    for (int i = 0; i < 8; ++i) if (h->act8[i]) cudaFree(h->act8[i]);
-    if (h->x8_scratch) cudaFree(h->x8_scratch);
     delete h;
     return 0;
 }
@@ -554,9 +483,9 @@ int fad_vggish_load(fad_handle* h, const fad_vggish_weights* w) {
     CK(cudaSetDevice(h->device));
     auto up = [&](void** dst, const void* src, size_t bytes) -> int {
         if (!src) return fail("missing weight pointer");
-        if (*dst) { lo8_forget(h, *dst); cudaFree(*dst); *dst = nullptr; }          // sizes depend on split_mask
+        if (*dst) { forget_zero_lo(h, *dst); cudaFree(*dst); *dst = nullptr; }      // sizes depend on split_mask
         CK(cudaMalloc(dst, bytes));
-        lo8_forget(h, *dst);
+        forget_zero_lo(h, *dst);
         CK(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
         return 0;
     };
@@ -588,13 +517,9 @@ int fad_vggish_load(fad_handle* h, const fad_vggish_weights* w) {
     // batch are never scheduled and rows past it are masked in the epilogue)
     for (int i = 0; i < 8; ++i) {
         const VggLayer& L = kVgg[i];
-        if (make_geom(h->geom[i], L.H, L.W, L.Cin, L.Cout, L.taps, L.relu, L.pool, ((w->split_mask >> i) & 1) ? wlo_mode() : 0)) return 1;
+        if (make_geom(h->geom[i], L.H, L.W, L.Cin, L.Cout, L.taps, L.relu, L.pool, (w->split_mask >> i) & 1)) return 1;
         const void* wptr = i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5];
         if (encode_layer_maps(h->geom[i], h->act[i], (long long)B, wptr, &h->map_x[i], &h->map_w[i])) return 1;
-        if (h->geom[i].split_w == 2) {
-            if (!h->act8[i]) CK(cudaMalloc(&h->act8[i], B * kActElems[i]));
-            if (encode_x8_map(h->geom[i], h->act8[i], (long long)B, &h->map_x8[i])) return 1;
-        }
     }
     h->vgg_loaded = true;
     return 0;
@@ -660,11 +585,7 @@ int fad_vggish_forward(fad_handle* h, const int16_t* pcm, const long long* ex_st
         if (launch_logmel(h, pcm, ex_start + base, nb, h->logmel, fe_double, st)) return 1;
         prof_end(h, FAD_PROF_LOGMEL, ev, st);
         ev = prof_begin(h, st);
-        {
-            static const bool simt = []() { const char* e = getenv("FADTK_CONV1"); return !(e && std::string(e) == "mma"); }();   // default: CUDA-core stencil
-            if (simt) fad::conv1_kernel<<<dim3(6, nb), 256, 0, st>>>(h->logmel, h->conv1_w, h->conv1_b, h->act[0], h->act8[0]);
-            else      fad::conv1_mma_kernel<<<nb, 256, 0, st>>>(h->logmel, h->conv1_w, h->conv1_b, h->act[0], h->act8[0]);
-        }
+        fad::conv1_kernel<<<dim3(6, nb), 256, 0, st>>>(h->logmel, h->conv1_w, h->conv1_b, h->act[0]);
         CK(cudaGetLastError());
         h->launches++;
         prof_end(h, FAD_PROF_CONV1, ev, st);
@@ -672,8 +593,7 @@ int fad_vggish_forward(fad_handle* h, const int16_t* pcm, const long long* ex_st
             const float* bias = i < 5 ? h->conv_b[i] : h->fc_b[i - 5];
             void* out = (i == 7) ? (void*)((__half*)emb_out_f16 + (size_t)base * 128) : (void*)h->act[i + 1];
             ev = prof_begin(h, st);
-            if (run_layer(h, h->geom[i], h->map_x[i], h->map_w[i], (i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5]), nb, bias, out, nullptr, st,
-                          nullptr, 0, 0, 0, 0, h->geom[i].split_w == 2 ? &h->map_x8[i] : nullptr, i < 7 ? h->act8[i + 1] : nullptr)) return 1;
+            if (run_layer(h, h->geom[i], h->map_x[i], h->map_w[i], (i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5]), nb, bias, out, nullptr, st)) return 1;
             prof_end(h, FAD_PROF_LAYER0 + i, ev, st);
         }
     }
@@ -687,7 +607,7 @@ int fad_vggish_conv1(fad_handle* h, const float* logmel, long long n_examples, v
     if (n_examples <= 0) return 0;
     CK(cudaSetDevice(h->device));
     fad::conv1_kernel<<<dim3(6, (unsigned)n_examples), 256, 0, (cudaStream_t)stream>>>(
-        logmel, h->conv1_w, h->conv1_b, reinterpret_cast<__half*>(out_f16), nullptr);
+        logmel, h->conv1_w, h->conv1_b, reinterpret_cast<__half*>(out_f16));
     CK(cudaGetLastError());
     h->launches++;
     return 0;
@@ -697,24 +617,15 @@ int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int C
                    const void* w_f16, const float* bias, int Cout, int taps, int relu, int pool,
                    int split_w, void* out_f16, float* out_f32_or_null, void* stream) {
     if (!h) return fail("null handle");
+    if (split_w != 0 && split_w != 1) return fail("fad_umma_layer: split_w must be 0 (fp16 weights) or 1 (fp16 hi/lo pair)");
     CK(cudaSetDevice(h->device));
     LayerGeom g;
     if (make_geom(g, H, W, Cin, Cout, taps, relu, pool, split_w)) return 1;
     if (pool && out_f32_or_null) return fail("fp32 copy is only available for un-pooled layers");
     if (g.split_w == 1 && note_split_weights(h, w_f16, Cout / 128, (long long)taps * Cin, (cudaStream_t)stream)) return 1;
-    CUtensorMap mx, mw, mx8;
+    CUtensorMap mx, mw;
     if (encode_layer_maps(g, x_f16, NB, w_f16, &mx, &mw)) return 1;
-    if (g.split_w == 2) {                    // stage test entry: make the E4M3 copy a producer would have written
-        lo8_forget(h, w_f16);                // caller-owned weights: never trust a cached conversion
-        const size_t count = (size_t)NB * H * W * Cin;
-        if (ensure((void**)&h->x8_scratch, &h->x8_scratch_cap, count)) return 1;
-        f16_to_e4m3_kernel<<<(unsigned)std::min<size_t>((count / 8 + 255) / 256 + 1, (size_t)h->num_sms * 16), 256, 0, (cudaStream_t)stream>>>(
-            reinterpret_cast<const __half*>(x_f16), count, h->x8_scratch);
-        CK(cudaGetLastError());
-        if (encode_x8_map(g, h->x8_scratch, NB, &mx8)) return 1;
-    }
-    return run_layer(h, g, mx, mw, w_f16, NB, bias, out_f16, out_f32_or_null, (cudaStream_t)stream,
-                     nullptr, 0, 0, 0, 0, g.split_w == 2 ? &mx8 : nullptr, nullptr);
+    return run_layer(h, g, mx, mw, w_f16, NB, bias, out_f16, out_f32_or_null, (cudaStream_t)stream);
 }
 
 // -------------------------------------------------------------------------- statistics
@@ -723,87 +634,19 @@ size_t fad_stats_acc_len(int d) { return 1 + 2 * (size_t)d + (size_t)d * d; }
 int fad_stats_accumulate(fad_handle* h, const void* emb_f16, long long n_rows, int d,
                          const void* shift_f16, double* acc, int tensor_core, void* stream) {
     if (!h) return fail("null handle");
+    // 0: exact fp64 Gram on the FP64 tensor pipe (DMMA), the product path; 2: fp64 CUDA-core kernel (cross-check)
+    if (tensor_core != 0 && tensor_core != 2) return fail("fad_stats_accumulate: tensor_core must be 0 (DMMA) or 2 (CUDA-core fp64)");
     if (n_rows <= 0) return 0;
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
     const __half* E = reinterpret_cast<const __half*>(emb_f16);
     const __half* shift = reinterpret_cast<const __half*>(shift_f16);
-    // mode 0 (default): exact fp64 Gram on the FP64 tensor pipe (DMMA); 1: wgmma fp16 hi/lo (fp32 accumulation,
-    // full-rank well-conditioned sets only); 2: fp64 CUDA-core kernel (verification).  FADTK_STATS overrides.
-    static const int forced = [] {
-        const char* e = getenv("FADTK_STATS");
-        if (!e) return -1;
-        const std::string v(e);
-        return v == "dmma" ? 0 : v == "umma" ? 1 : v == "simt" ? 2 : -1;
-    }();
-    if (forced >= 0) tensor_core = forced;
-    if (tensor_core == 2) {
-        if (d % 64 != 0) return fail("d must be a multiple of 64");
-        dim3 grid((unsigned)((n_rows + fad::kSimtRows - 1) / fad::kSimtRows), d / 64, d / 64);
-        fad::stats_simt_kernel<<<grid, 256, 0, st>>>(E, n_rows, d, shift, acc);
-        CK(cudaGetLastError());
-        h->launches++;
-        return 0;
-    }
-    if (tensor_core == 0) {
-        if (d % 64 != 0) return fail("d must be a multiple of 64");
-        fad::StatsDmmaParams p;
-        p.n_rows = n_rows; p.d = d; p.n_tiles = d / fad::kSdTile;
-        p.n_pairs = p.n_tiles * (p.n_tiles + 1) / 2;
-        const long long stages = (n_rows + fad::kSdRows - 1) / fad::kSdRows;
-        long long want = (4LL * h->num_sms + p.n_pairs - 1) / p.n_pairs;       // ~2 waves at 2 CTAs per SM
-        if (want < 1) want = 1;
-        long long per = (stages + want - 1) / want;                             // 16-row stages per split
-        if (per < 4) per = 4;
-        p.n_splits = (int)((stages + per - 1) / per);
-        p.rows_per_split = per * fad::kSdRows;
-        p.shift = shift;
-        const size_t jobs = (size_t)p.n_pairs * p.n_splits;
-        if (ensure((void**)&h->ws_tiles, &h->ws_tiles_cap, jobs * fad::kSdTile * fad::kSdTile * 8)) return 1;
-        if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
-        p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
-        size_t ev = prof_begin(h, st);
-        fad::stats_dmma_kernel<__half><<<(unsigned)jobs, 256, 0, st>>>(E, p);
-        CK(cudaGetLastError());
-        prof_end(h, FAD_PROF_STATS, ev, st);
-        ev = prof_begin(h, st);
-        fad::stats_dmma_reduce_kernel<<<dim3(p.n_pairs, fad::kSdTile * fad::kSdTile / 256), 256, 0, st>>>(p, acc);
-        CK(cudaGetLastError());
-        prof_end(h, FAD_PROF_STATS_REDUCE, ev, st);
-        h->launches += 2;
-        return 0;
-    }
-    if (d % 128 != 0) return fail("d must be a multiple of 128 for the tensor-core statistics kernel");
-    fad::StatsJobParams p;
-    p.n_rows = n_rows; p.d = d; p.n_tiles = d / 128;
-    p.n_pairs = p.n_tiles * (p.n_tiles + 1) / 2;
-    const long long stages = (n_rows + fad::kStStageRows - 1) / fad::kStStageRows;
-    long long want = (2LL * h->num_sms) / p.n_pairs;          // ~2 waves of jobs
-    if (p.n_pairs == 1) want = h->num_sms;
-    if (want < 1) want = 1;
-    long long per = (stages + want - 1) / want;                // 32-row stages per split
-    if (per < fad::kStStagesPerChunk) per = fad::kStStagesPerChunk;   // at least one 256-row chunk
-    p.n_splits = (int)((stages + per - 1) / per);
-    p.rows_per_split = per * fad::kStStageRows;
-    p.shift = shift;
-    const size_t jobs = (size_t)p.n_pairs * p.n_splits;
-    if (ensure((void**)&h->ws_tiles, &h->ws_tiles_cap, jobs * 128 * 128 * 8)) return 1;
-    if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * 2 * 128 * 8)) return 1;
-    p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
-    CUtensorMap me;
-    const uint64_t ed[2] = {(uint64_t)d, (uint64_t)n_rows};
-    const uint64_t es[1] = {(uint64_t)d * 2};
-    const uint32_t eb[2] = {64, (uint32_t)fad::kStStageRows};
-    if (encode_f16_map(&me, E, 2, ed, es, eb)) return 1;
-    size_t ev = prof_begin(h, st);
-    fad::stats_umma_kernel<<<(unsigned)jobs, fad::kStThreads, fad::kStSmemBytes, st>>>(me, p);
+    if (tensor_core == 0) return launch_stats_dmma(h, E, n_rows, d, shift, acc, st);
+    if (d % 64 != 0) return fail("d must be a multiple of 64");
+    dim3 grid((unsigned)((n_rows + fad::kSimtRows - 1) / fad::kSimtRows), d / 64, d / 64);
+    fad::stats_simt_kernel<<<grid, 256, 0, st>>>(E, n_rows, d, shift, acc);
     CK(cudaGetLastError());
-    prof_end(h, FAD_PROF_STATS, ev, st);
-    ev = prof_begin(h, st);
-    fad::stats_reduce_kernel<<<p.n_pairs, 256, 0, st>>>(p, acc);
-    CK(cudaGetLastError());
-    prof_end(h, FAD_PROF_STATS_REDUCE, ev, st);
-    h->launches += 2;
+    h->launches++;
     return 0;
 }
 
@@ -826,29 +669,8 @@ int fad_file_means(fad_handle* h, const void* emb_f16, long long n_files, int ro
 int fad_stats_accumulate_f64(fad_handle* h, const double* rows, long long n_rows, int d, double* acc, void* stream) {
     if (!h) return fail("null handle");
     if (n_rows <= 0) return 0;
-    if (d % 64 != 0) return fail("d must be a multiple of 64");
     CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    fad::StatsDmmaParams p;
-    p.n_rows = n_rows; p.d = d; p.n_tiles = d / fad::kSdTile;
-    p.n_pairs = p.n_tiles * (p.n_tiles + 1) / 2;
-    const long long stages = (n_rows + fad::kSdRows - 1) / fad::kSdRows;
-    long long want = (4LL * h->num_sms + p.n_pairs - 1) / p.n_pairs;
-    if (want < 1) want = 1;
-    long long per = (stages + want - 1) / want;
-    if (per < 4) per = 4;
-    p.n_splits = (int)((stages + per - 1) / per);
-    p.rows_per_split = per * fad::kSdRows;
-    p.shift = nullptr;
-    const size_t jobs = (size_t)p.n_pairs * p.n_splits;
-    if (ensure((void**)&h->ws_tiles, &h->ws_tiles_cap, jobs * fad::kSdTile * fad::kSdTile * 8)) return 1;
-    if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
-    p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
-    fad::stats_dmma_kernel<double><<<(unsigned)jobs, 256, 0, st>>>(rows, p);
-    fad::stats_dmma_reduce_kernel<<<dim3(p.n_pairs, fad::kSdTile * fad::kSdTile / 256), 256, 0, st>>>(p, acc);
-    CK(cudaGetLastError());
-    h->launches += 2;
-    return 0;
+    return launch_stats_dmma(h, rows, n_rows, d, nullptr, acc, (cudaStream_t)stream);
 }
 
 int fad_stats_finalize_mirrored(fad_handle* h, const double* acc, const double* acc_means64, const double* acc_means16,
@@ -882,7 +704,7 @@ int fad_stats_accumulate_gather(fad_handle* h, const void* emb_f16, long long n_
         reinterpret_cast<const __half*>(emb_f16), idx, n_idx, d, h->gather_buf);
     CK(cudaGetLastError());
     h->launches++;
-    return fad_stats_accumulate(h, h->gather_buf, n_idx, d, shift_f16, acc, 0, stream);   // exact fp64 path
+    return launch_stats_dmma(h, h->gather_buf, n_idx, d, reinterpret_cast<const __half*>(shift_f16), acc, (cudaStream_t)stream);
 }
 
 int fad_stats_finalize(fad_handle* h, const double* acc, const void* shift_f16, int d,

@@ -15,7 +15,6 @@
 //                  for the tensor pipe); writes NHWC fp16 [B, 48, 32, 64] for the wgmma layers.
 #pragma once
 #include <cuda_fp16.h>
-#include <cuda_fp8.h>
 #include <stdint.h>
 
 namespace fad {
@@ -177,6 +176,7 @@ logmel_kernel(const int16_t* __restrict__ pcm, const long long* __restrict__ ex_
     }
 }
 
+// warp-level fp16 x fp16 -> fp32 MMA, C += A[16 x 16] B[16 x 8] (the attention kernels of clap.cuh and whisper.cuh)
 __device__ __forceinline__ void mma_m16n8k16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
                                              uint32_t b0, uint32_t b1) {
     asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
@@ -184,131 +184,11 @@ __device__ __forceinline__ void mma_m16n8k16(float (&c)[4], uint32_t a0, uint32_
                  : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// conv1 on the warp-level tensor cores (mma.sync m16n8k16, fp16 x fp16 -> fp32) at fp32-equivalent
-// accuracy: input and weights are split into fp16 hi/lo pairs (22 bits each) and the three
-// significant products go into one K = 32 reduction per output,
-//   k =  0.. 8: xh(tap) * wh(tap)     k =  9..17: xl(tap) * wh(tap)     k = 18..26: xh(tap) * wl(tap)
-// (xl * wl ~ 2^-22 is dropped; k = 27..31 multiply zero weights).  A tile row = one pooled pixel, the
-// four conv pixels of its 2x2 window are four successive m-tiles whose accumulators are max-ed in
-// registers; bias + ReLU commute with the max.  The CUDA-core version needed 72 FFMA per pooled pixel
-// per lane and was issue-bound; this needs 16 HMMA per 16 pooled pixels x 64 channels.
-// grid = B examples; block = 256 threads = 8 warps looping over the 6 strips of 8 pooled rows (the weight
-// fragments are built once per block), warp w owns pooled row w of the strip.
-__global__ void __launch_bounds__(256, 2)
-conv1_mma_kernel(const float* __restrict__ logmel /*[B,96,64]*/, const float* __restrict__ w /*[64,9]*/,
-                 const float* __restrict__ bias, __half* __restrict__ out /*[B,48,32,64]*/,
-                 uint8_t* __restrict__ out8 /* optional E4M3 copy, may be null */)
-{
-    __shared__ __half tile[2][18][72];                      // [hi | lo][input row + halo][input col + 1]
-    const int e = blockIdx.x;
-    const float* src = logmel + (size_t)e * 96 * 64;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int g = lane >> 2, t = lane & 3;
-
-    // B fragments: B[k][ch], ch = 8 j + g; b[j][s][0] = {B[16s + 2t][ch], B[16s + 2t + 1][ch]}, [1] = k + 8
-    auto bval = [&](int k, int ch) -> __half {
-        if (k >= 27) return __float2half_rn(0.f);
-        const float wf = w[ch * 9 + k % 9];
-        const __half wh = __float2half_rn(wf);
-        return k < 18 ? wh : __float2half_rn(wf - __half2float(wh));
-    };
-    uint32_t bf[8][2][2];
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int s = 0; s < 2; ++s)
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int k = 16 * s + 8 * hh + 2 * t;
-                const __half2 v = __halves2half2(bval(k, 8 * j + g), bval(k + 1, 8 * j + g));
-                bf[j][s][hh] = *reinterpret_cast<const uint32_t*>(&v);
-            }
-    // A operand: smem offset (in halves, relative to the conv pixel's top-left tap) of K index k
-    auto aoff = [&](int k) -> int {
-        const int kk = k < 27 ? k : 0;                      // padded K: weight is zero, any finite value will do
-        const int term = kk / 9, tap = kk % 9;
-        return (term == 1 ? 18 * 72 : 0) + (tap / 3) * 72 + tap % 3;
-    };
-    int off[2][2][2];                                       // [k-step][k / k+8][k, k+1]
-#pragma unroll
-    for (int s = 0; s < 2; ++s)
-#pragma unroll
-        for (int hh = 0; hh < 2; ++hh) {
-            off[s][hh][0] = aoff(16 * s + 8 * hh + 2 * t);
-            off[s][hh][1] = aoff(16 * s + 8 * hh + 2 * t + 1);
-        }
-    float2 bia[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) bia[j] = make_float2(bias[8 * j + 2 * t], bias[8 * j + 2 * t + 1]);
-
-    const __half* tl = &tile[0][0][0];
-    const int py = warp;                                   // pooled row inside the strip
-#pragma unroll 1
-  for (int strip = 0; strip < 6; ++strip) {                // strip: pooled rows [8*strip, 8*strip+8)
-    const int row0 = strip * 16 - 1;
-    __syncthreads();                                       // previous strip fully consumed
-    for (int i = threadIdx.x; i < 18 * 66; i += 256) {
-        const int r = i / 66, c = i % 66;
-        const int gr = row0 + r, gc = c - 1;
-        const float x = (gr >= 0 && gr < 96 && gc >= 0 && gc < 64) ? src[gr * 64 + gc] : 0.0f;
-        const __half xh = __float2half_rn(x);
-        tile[0][r][c] = xh;
-        tile[1][r][c] = __float2half_rn(x - __half2float(xh));
-    }
-    __syncthreads();
-#pragma unroll 1
-    for (int grp = 0; grp < 2; ++grp) {                    // 16 pooled pixels per group
-        float mx[8][4];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { mx[j][0] = mx[j][1] = mx[j][2] = mx[j][3] = -3.0e38f; }
-#pragma unroll
-        for (int sub = 0; sub < 4; ++sub) {                // (dy, dx) of the 2x2 window
-            const int dy = sub >> 1, dx = sub & 1;
-            const int p0 = (2 * py + dy) * 72 + 2 * (grp * 16 + g) + dx;        // row g   -> pooled col grp*16 + g
-            const int p1 = p0 + 16;                                              // row g+8 -> pooled col + 8
-            float acc[8][4];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) { acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f; }
-#pragma unroll
-            for (int s = 0; s < 2; ++s) {
-                auto pair = [&](int base, int hh) -> uint32_t {
-                    const __half2 v = __halves2half2(tl[base + off[s][hh][0]], tl[base + off[s][hh][1]]);
-                    return *reinterpret_cast<const uint32_t*>(&v);
-                };
-                const uint32_t a0 = pair(p0, 0), a1 = pair(p1, 0), a2 = pair(p0, 1), a3 = pair(p1, 1);
-#pragma unroll
-                for (int j = 0; j < 8; ++j) mma_m16n8k16(acc[j], a0, a1, a2, a3, bf[j][s][0], bf[j][s][1]);
-            }
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                mx[j][0] = fmaxf(mx[j][0], acc[j][0]); mx[j][1] = fmaxf(mx[j][1], acc[j][1]);
-                mx[j][2] = fmaxf(mx[j][2], acc[j][2]); mx[j][3] = fmaxf(mx[j][3], acc[j][3]);
-            }
-        }
-        const size_t pix0 = ((size_t)e * 48 + strip * 8 + py) * 32 + grp * 16 + g;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-            const __half2 h0 = __floats2half2_rn(fmaxf(mx[j][0] + bia[j].x, 0.f), fmaxf(mx[j][1] + bia[j].y, 0.f));
-            const __half2 h1 = __floats2half2_rn(fmaxf(mx[j][2] + bia[j].x, 0.f), fmaxf(mx[j][3] + bia[j].y, 0.f));
-            *reinterpret_cast<__half2*>(out + pix0 * 64 + 8 * j + 2 * t) = h0;
-            *reinterpret_cast<__half2*>(out + (pix0 + 8) * 64 + 8 * j + 2 * t) = h1;
-            if (out8 != nullptr) {
-                *reinterpret_cast<unsigned short*>(out8 + pix0 * 64 + 8 * j + 2 * t) =
-                    __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(h0), __NV_SATFINITE, __NV_E4M3);
-                *reinterpret_cast<unsigned short*>(out8 + (pix0 + 8) * 64 + 8 * j + 2 * t) =
-                    __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(h1), __NV_SATFINITE, __NV_E4M3);
-            }
-        }
-    }
-  }
-}
-
 // conv1: grid = (6 strips, B); block = 256 threads.  Lane = output-channel pair, warp loops
 // over pooled pixels of an 8-row strip; the fp32 input strip (with halo) sits in smem.
 __global__ void __launch_bounds__(256)
 conv1_kernel(const float* __restrict__ logmel /*[B,96,64]*/, const float* __restrict__ w /*[64,9]*/,
-             const float* __restrict__ bias, __half* __restrict__ out /*[B,48,32,64]*/,
-             uint8_t* __restrict__ out8 /* optional E4M3 copy of `out` (fp8 low-part mode of conv2), may be null */)
+             const float* __restrict__ bias, __half* __restrict__ out /*[B,48,32,64]*/)
 {
     __shared__ float tile[18][68];
     const int e = blockIdx.y, strip = blockIdx.x;          // strip: pooled rows [8*strip, 8*strip+8)
@@ -352,11 +232,7 @@ conv1_kernel(const float* __restrict__ logmel /*[B,96,64]*/, const float* __rest
             }
         m0 = fmaxf(m0 + b0, 0.f); m1 = fmaxf(m1 + b1, 0.f);
         const size_t pix = ((size_t)e * 48 + strip * 8 + py) * 32 + px;
-        const __half2 hv = __floats2half2_rn(m0, m1);
-        *reinterpret_cast<__half2*>(out + pix * 64 + 2 * lane) = hv;
-        if (out8 != nullptr)                               // E4M3 of the fp16 value the next layer sees
-            *reinterpret_cast<unsigned short*>(out8 + pix * 64 + 2 * lane) =
-                __nv_cvt_halfraw2_to_fp8x2(static_cast<__half2_raw>(hv), __NV_SATFINITE, __NV_E4M3);
+        *reinterpret_cast<__half2*>(out + pix * 64 + 2 * lane) = __floats2half2_rn(m0, m1);
     }
 }
 

@@ -156,10 +156,6 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 __device__ __forceinline__ uint64_t kmajor_sw128_desc(uint32_t saddr) {
     return make_smem_desc(saddr, 16, 1024, SWZ_128B);
 }
-// K-major tile of 8-bit elements with 64-B rows (64 elements), SWIZZLE_64B: 8-row atoms of 512 B.
-__device__ __forceinline__ uint64_t kmajor_sw64_desc(uint32_t saddr) {
-    return make_smem_desc(saddr, 16, 512, SWZ_64B);
-}
 // MN-major operand tile, SWIZZLE_128B, 16-bit elements: each K row holds 64 contiguous M/N
 // elements (128 B); 8 K-rows form a 1024-B atom.  LBO = stride between successive 64-element
 // blocks along M/N, SBO = stride between 8-row K groups.
@@ -206,15 +202,6 @@ __device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " FAD_WG_D64 ", %64, %65, p, 1, 1, %67, %68;\n\t}\n"
         : FAD_WG_OUT64(d)
         : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
-}
-// E4M3 x E4M3 -> fp32, K = 32 per instruction, both operands K-major
-__device__ __forceinline__ void wgmma_m64n128k32_e4m3(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 " FAD_WG_D64 ", %64, %65, p, 1, 1;\n\t}\n"
-        : FAD_WG_OUT64(d)
-        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
 #define FAD_WG_D32                                                                                                 \

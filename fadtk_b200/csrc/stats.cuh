@@ -2,9 +2,9 @@
 // s a shared fp16 shift vector.  Replaces np.mean / np.cov in fadtk/fad.py:42-48 and the per-file scatter + Chan
 // merge in fadtk/utils.py:13-46 with one shifted E^T E contraction.
 //
-// Three kernels compute the same packed accumulator (fad_stats_accumulate's `mode`):
+// Two kernels compute the same packed accumulator (fad_stats_accumulate's `tensor_core`):
 //
-// stats_dmma_kernel<In>  (mode 0, the product default)   fp64 tensor pipe.  x and s are fp16, so y = x - s is exact
+// stats_dmma_kernel<In>  (0, the product path)   fp64 tensor pipe.  x and s are fp16, so y = x - s is exact
 //   in fp64; products and sums are fp64 (mma.sync m8n8k4.f64 -> SASS DMMA.8x8x4): the result is the Gram matrix of
 //   the data to ~1e-16, hence positive semi-definite.  Parity needs that: a covariance with cond ~1e9 (CLAP/MERT) or
 //   a rank-deficient per-song covariance perturbed at the 1e-6 level of an fp32-accumulating path is indefinite -
@@ -14,291 +14,23 @@
 //   order (deterministic).  In = double with no shift is the variant score() feeds with per-file fp16-rounded means
 //   (fad_stats_accumulate_f64).
 //
-// stats_umma_kernel  (mode 1, opt-in)   tensor-core (wgmma) fp16 hi/lo: yh = fp16(y), yl = fp16(y - yh),
-//       sum y y^T ~= sum yh yh^T + yh yl^T + yl yh^T            (yl yl^T ~ 2^-22 is dropped)
-//   Every fp16 x fp16 product is exact in the fp32 accumulator; the accumulation itself is cut every 256 rows and
-//   drained into an fp64 tile, because tensor-core fp32 adds truncate.  One CTA = (128x128 output tile, row range).
-//   E is row-major, so both operands of E^T E are "MN-major": a TMA box [32 rows x 64 cols] with 128-B swizzle IS
-//   the canonical MN-major SWIZZLE_128B wgmma layout (K = row index).
-//     warp 0       TMA producer: per 32-row stage, two 64-column boxes per panel
-//     warps 4-11   transform: in smem, x -> (yh in place, yl into a second panel), zero rows past the end, exact
-//                  column sums of x - s and of yh + yl in fp64 registers
-//     warps 12-19  two MMA warpgroups, one per 64-row half of the output tile: per stage 2 k-steps x {hh, hl, lh}
-//                  wgmmas into an fp32 register accumulator that is added into an fp64 tile in shared memory
-//                  every 256 rows
-//   Good to ~1e-6 relative: fine for full-rank, well-conditioned sets only.
-//
-// stats_simt_kernel  (mode 2)   fp64 CUDA-core contraction of the exact y: the round-1 default, kept as the
-//   independent cross-check of mode 0 (tests/test_gpu_kernels.py compares all three).
+// stats_simt_kernel  (2)   fp64 CUDA-core contraction of the exact y, with atomics: the independent cross-check of
+//   the DMMA kernel (tests/test_gpu_kernels.py compares the two).
 //
 // Packed accumulator (fp64, caller-owned, all-reduced across GPUs as-is):
 //   acc[0] = n,  acc[1 .. d] = sum(x - s) (exact),  acc[1+d .. 1+d+d*d) = sum(y y^T)
-//   (d x d, full, row-major),  acc[1+d+d*d ..] = sum(yh + yl)  (centring term of the covariance; = sum y in modes 0, 2)
+//   (d x d, full, row-major),  acc[1+d+d*d ..] = sum y  (centring term of the covariance; the same values as
+//   acc[1 .. d], kept so that the layout and the all-reduce length stay as they are)
 #pragma once
 #include "sm90.cuh"
 
 namespace fad {
-
-constexpr int kStTile = 128;
-constexpr int kStStageRows = 32;
-constexpr int kStStagesPerChunk = 8;               // 256 rows per fp32 register accumulation
-constexpr int kStStages = 3;
-constexpr uint32_t kStBlockBytes = kStStageRows * 128;            // one 64-col box: 4 KiB
-constexpr uint32_t kStPanelBytes = 2 * kStBlockBytes;             // 128 cols x 32 rows: 8 KiB
-constexpr uint32_t kStStageBytes = 4 * kStPanelBytes;             // Ah | Bh | Al | Bl = 32 KiB
-constexpr int kStThreads = 640;
-constexpr int kStTransformThreads = 256;
-constexpr uint32_t kStSmemBytes = kStStages * kStStageBytes + kStTile * kStTile * 8 + 1024 + 256;
-
-struct StatsJobParams {
-    long long n_rows;          // valid rows in E
-    int d;
-    int n_tiles;               // d / 128
-    int n_pairs;               // n_tiles (n_tiles + 1) / 2
-    int n_splits;              // row splits per tile pair
-    long long rows_per_split;  // multiple of 32
-    const __half* shift;       // [d]
-    double* ws_tiles;          // [n_pairs * n_splits][128 (col)][128 (row)]
-    double* ws_sums;           // [n_tiles * n_splits][2][128]  (exact x-s sums | yh+yl sums)
-};
 
 __device__ __forceinline__ void pair_to_tiles(int pair, int n_tiles, int& ti, int& tj) {
     ti = 0;
     int rem = pair;
     while (rem >= n_tiles - ti) { rem -= n_tiles - ti; ++ti; }
     tj = ti + rem;
-}
-
-// y = x - s (exact in fp32) -> hi/lo fp16 pair
-__device__ __forceinline__ void split_hi_lo(__half2 x, __half2 s, __half2& hi, __half2& lo, float2& y) {
-    const float2 fx = __half22float2(x), fs = __half22float2(s);
-    y = make_float2(fx.x - fs.x, fx.y - fs.y);
-    hi = __floats2half2_rn(y.x, y.y);
-    const float2 fh = __half22float2(hi);
-    lo = __floats2half2_rn(y.x - fh.x, y.y - fh.y);
-}
-
-__global__ void __launch_bounds__(kStThreads, 1)
-stats_umma_kernel(const __grid_constant__ CUtensorMap map_e, const StatsJobParams p)
-{
-    using namespace sm90;
-
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    double* acc64 = reinterpret_cast<double*>(smem + kStStages * kStStageBytes);     // [col][row]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kStStages * kStStageBytes + kStTile * kStTile * 8);
-    uint64_t* full = bars;                       // TMA landed
-    uint64_t* ready = bars + kStStages;          // transform done
-    uint64_t* empty = bars + 2 * kStStages;      // MMAs retired
-    uint64_t* mma_done = bars + 3 * kStStages;   // every MMA of the job retired: stage 0 may be reused
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int job = blockIdx.x;
-    const int pair = job / p.n_splits, split = job % p.n_splits;
-    int ti, tj;
-    pair_to_tiles(pair, p.n_tiles, ti, tj);
-    const bool diag = (ti == tj);
-    const long long row_begin = (long long)split * p.rows_per_split;
-    long long row_end = row_begin + p.rows_per_split;
-    if (row_end > p.n_rows) row_end = p.n_rows;
-    const long long span = row_end > row_begin ? row_end - row_begin : 0;
-    const int n_stages_total = (int)((span + kStStageRows - 1) / kStStageRows);
-    const int n_chunks = (n_stages_total + kStStagesPerChunk - 1) / kStStagesPerChunk;
-
-    if (warp == 0 && lane == 0) tma_prefetch_desc(&map_e);
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kStStages; ++s) {
-            mbar_init(&full[s], 1); mbar_init(&ready[s], kStTransformThreads / 32); mbar_init(&empty[s], 8);
-        }
-        mbar_init(mma_done, 8);
-        mbar_fence_init();
-    }
-    for (int i = threadIdx.x; i < kStTile * kStTile; i += kStThreads) acc64[i] = 0.0;
-    __syncthreads();
-
-    if (warp == 0) {
-        if (elect_one()) {
-            int s = 0; uint32_t ph = 0;
-            for (int it = 0; it < n_stages_total; ++it) {
-                const int r0 = (int)(row_begin + (long long)it * kStStageRows);
-                mbar_wait(&empty[s], ph ^ 1);
-                mbar_expect_tx(&full[s], diag ? kStPanelBytes : 2 * kStPanelBytes);
-                uint8_t* st = smem + s * kStStageBytes;
-                tma_load_2d(st, &map_e, &full[s], ti * kStTile, r0);
-                tma_load_2d(st + kStBlockBytes, &map_e, &full[s], ti * kStTile + 64, r0);
-                if (!diag) {
-                    tma_load_2d(st + kStPanelBytes, &map_e, &full[s], tj * kStTile, r0);
-                    tma_load_2d(st + kStPanelBytes + kStBlockBytes, &map_e, &full[s], tj * kStTile + 64, r0);
-                }
-                if (++s == kStStages) { s = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp >= 4 && warp < 12) {
-        // ------------------------------------------------------- shift + hi/lo split
-        const int t = threadIdx.x - 128;              // 0..255
-        const int cg = t & 15;                        // 16-B column group inside the 128-col panel
-        const int rl = (t >> 4) & 7;                  // row lane inside an 8-row swizzle group
-        const int hf = t >> 7;                        // which half of the 32 rows
-        const int cb = cg >> 3, lc = cg & 7;
-        const uint32_t chunk_off = cb * kStBlockBytes + ((lc ^ rl) << 4);   // swizzled (row%8 == rl, lc)
-        __half2 shA[4], shB[4];
-        {
-            const uint4 a = *reinterpret_cast<const uint4*>(p.shift + ti * kStTile + cg * 8);
-            const uint4 b = *reinterpret_cast<const uint4*>(p.shift + tj * kStTile + cg * 8);
-            shA[0] = *reinterpret_cast<const __half2*>(&a.x); shA[1] = *reinterpret_cast<const __half2*>(&a.y);
-            shA[2] = *reinterpret_cast<const __half2*>(&a.z); shA[3] = *reinterpret_cast<const __half2*>(&a.w);
-            shB[0] = *reinterpret_cast<const __half2*>(&b.x); shB[1] = *reinterpret_cast<const __half2*>(&b.y);
-            shB[2] = *reinterpret_cast<const __half2*>(&b.z); shB[3] = *reinterpret_cast<const __half2*>(&b.w);
-        }
-        double sum_x[8], sum_y[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { sum_x[j] = 0.0; sum_y[j] = 0.0; }
-        int s = 0; uint32_t ph = 0;
-        for (int it = 0; it < n_stages_total; ++it) {
-            const long long r0 = row_begin + (long long)it * kStStageRows;
-            mbar_wait(&full[s], ph);
-            uint8_t* st = smem + s * kStStageBytes;
-#pragma unroll
-            for (int panel = 0; panel < 2; ++panel) {
-                if (panel == 1 && diag) break;
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    const int r = rl + 8 * (hf * 2 + i);
-                    uint4* ph_ptr = reinterpret_cast<uint4*>(st + panel * kStPanelBytes + chunk_off + r * 128);
-                    uint4* pl_ptr = reinterpret_cast<uint4*>(st + (2 + panel) * kStPanelBytes + chunk_off + r * 128);
-                    uint4 v = *ph_ptr, w = make_uint4(0, 0, 0, 0);
-                    if (r0 + r < row_end) {
-                        __half2* hx = reinterpret_cast<__half2*>(&v);
-                        __half2* hl = reinterpret_cast<__half2*>(&w);
-#pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            __half2 hi, lo; float2 y;
-                            split_hi_lo(hx[j], panel ? shB[j] : shA[j], hi, lo, y);
-                            hx[j] = hi; hl[j] = lo;
-                            if (panel == 0 && diag) {
-                                const float2 fh = __half22float2(hi), fl = __half22float2(lo);
-                                sum_x[2 * j] += (double)y.x;            sum_x[2 * j + 1] += (double)y.y;
-                                sum_y[2 * j] += (double)fh.x + (double)fl.x;
-                                sum_y[2 * j + 1] += (double)fh.y + (double)fl.y;
-                            }
-                        }
-                    } else {
-                        v = make_uint4(0, 0, 0, 0);
-                    }
-                    *ph_ptr = v;
-                    *pl_ptr = w;
-                }
-            }
-            fence_proxy_async_smem();                 // generic-proxy stores -> visible to UMMA
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&ready[s]);
-            if (++s == kStStages) { s = 0; ph ^= 1; }
-        }
-        // column sums: reduce the 16 row lanes through stage 0 once every MMA has retired
-        if (diag) {
-            mbar_wait(mma_done, 0);
-            asm volatile("bar.sync 1, 256;");
-            double* red = reinterpret_cast<double*>(smem);       // [2][16 row lanes][128 cols] = 32 KiB
-            const int lane16 = hf * 8 + rl;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-                red[lane16 * 128 + cg * 8 + j] = sum_x[j];
-                red[2048 + lane16 * 128 + cg * 8 + j] = sum_y[j];
-            }
-            asm volatile("bar.sync 1, 256;");
-            if (t < 128) {
-                double tx = 0.0, ty = 0.0;
-                for (int k = 0; k < 16; ++k) { tx += red[k * 128 + t]; ty += red[2048 + k * 128 + t]; }
-                double* wsum = p.ws_sums + ((size_t)ti * p.n_splits + split) * 2 * kStTile;
-                wsum[t] = tx;
-                wsum[kStTile + t] = ty;
-            }
-        }
-    } else if (warp >= 12) {
-        // -------------------------------------- wgmma: output rows [64 mh, 64 mh + 64) of the tile, fp32 -> fp64 smem
-        const int mh = (warp - 12) >> 2;
-        const int wq = warp & 3;
-        int s = 0; uint32_t ph = 0;
-        int it = 0;
-        float d[64];
-        for (int c = 0; c < n_chunks; ++c) {
-            const int n_st = min(kStStagesPerChunk, n_stages_total - it);
-            for (int q = 0; q < n_st; ++q, ++it) {
-                mbar_wait(&ready[s], ph);
-                const uint32_t base = smem_u32(smem + s * kStStageBytes);
-                const uint32_t ah = base + mh * kStBlockBytes, bh = diag ? base : base + kStPanelBytes;
-                const uint32_t al = base + 2 * kStPanelBytes + mh * kStBlockBytes, bl = diag ? base + 2 * kStPanelBytes : base + 3 * kStPanelBytes;
-                // MN-major SW128: 64-col blocks kStBlockBytes apart (LBO), 8-row K groups 1024 B apart (SBO)
-                const uint64_t d_ah = mnmajor_sw128_desc(ah, kStBlockBytes, 1024);
-                const uint64_t d_bh = mnmajor_sw128_desc(bh, kStBlockBytes, 1024);
-                const uint64_t d_al = mnmajor_sw128_desc(al, kStBlockBytes, 1024);
-                const uint64_t d_bl = mnmajor_sw128_desc(bl, kStBlockBytes, 1024);
-                wgmma_fence();
-#pragma unroll
-                for (int k = 0; k < kStStageRows / 16; ++k) {
-                    const uint32_t off = 128 * k;          // 16 K-rows = 2048 B = 128 x 16 B
-                    wgmma_m64n128k16_f16<1, 1>(d, d_ah + off, d_bh + off, (q | k) != 0);
-                    wgmma_m64n128k16_f16<1, 1>(d, d_ah + off, d_bl + off, 1);
-                    wgmma_m64n128k16_f16<1, 1>(d, d_al + off, d_bh + off, 1);
-                }
-                wgmma_commit();
-                wgmma_wait<0>();
-                fence_regs(d);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[s]);
-                if (++s == kStStages) { s = 0; ph ^= 1; }
-            }
-            // fragment (row 16 wq + lane / 4 + 8 i, col 8 j + 2 (lane % 4) + e) -> acc64[col][row]; one owner per element
-#pragma unroll
-            for (int j = 0; j < 16; ++j)
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-#pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int row = mh * 64 + wq * 16 + (lane >> 2) + 8 * i, col = 8 * j + 2 * (lane & 3) + e;
-                        acc64[col * kStTile + row] += (double)d[4 * j + 2 * i + e];
-                    }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(mma_done);
-    }
-    __syncthreads();
-    {
-        double* dst = p.ws_tiles + (size_t)job * kStTile * kStTile;
-        for (int i = threadIdx.x; i < kStTile * kStTile; i += kStThreads) dst[i] = acc64[i];
-    }
-}
-
-// acc += sum over row splits of the job tiles (fixed order => deterministic).
-// grid = (n_pairs), block = 256
-__global__ void stats_reduce_kernel(StatsJobParams p, double* __restrict__ acc)
-{
-    const int pair = blockIdx.x;
-    int ti, tj;
-    pair_to_tiles(pair, p.n_tiles, ti, tj);
-    const int d = p.d;
-    double* outer = acc + 1 + d;
-    for (int e = threadIdx.x; e < kStTile * kStTile; e += blockDim.x) {
-        const int col = e / kStTile, row = e % kStTile;        // workspace layout is [col][row]
-        double v = 0.0;
-        for (int s = 0; s < p.n_splits; ++s)
-            v += p.ws_tiles[((size_t)pair * p.n_splits + s) * kStTile * kStTile + e];
-        const int I = ti * kStTile + row, J = tj * kStTile + col;
-        outer[(size_t)I * d + J] += v;
-        if (ti != tj) outer[(size_t)J * d + I] += v;
-    }
-    if (ti == tj) {
-        for (int c = threadIdx.x; c < kStTile; c += blockDim.x) {
-            double vx = 0.0, vy = 0.0;
-            for (int s = 0; s < p.n_splits; ++s) {
-                const double* wsum = p.ws_sums + ((size_t)ti * p.n_splits + s) * 2 * kStTile;
-                vx += wsum[c]; vy += wsum[kStTile + c];
-            }
-            acc[1 + ti * kStTile + c] += vx;
-            acc[1 + (size_t)d + (size_t)d * d + ti * kStTile + c] += vy;
-        }
-    }
-    if (pair == 0 && threadIdx.x == 0) acc[0] += (double)p.n_rows;
 }
 
 // --------------------------------------------------------------------------------------
@@ -486,7 +218,7 @@ __global__ void __launch_bounds__(256) stats_dmma_reduce_kernel(StatsDmmaParams 
 }
 
 // --------------------------------------------------------------------------------------
-// fp64 CUDA-core version (verification path only: FADTK_STATS=simt / mode 2).  grid = (row chunks, d/64, d/64) upper tiles only.
+// fp64 CUDA-core version (verification path only: tensor_core = 2).  grid = (row chunks, d/64, d/64) upper tiles only.
 constexpr int kSimtRows = 1024;
 __global__ void __launch_bounds__(256)
 stats_simt_kernel(const __half* __restrict__ E, long long n_rows, int d,

@@ -78,12 +78,13 @@ int fad_vggish_logmel(fad_handle* h, const int16_t* pcm, const long long* ex_sta
  * loaded weights: logmel fp32 [n, 96, 64] -> fp16 NHWC [n, 48, 32, 64]. */
 int fad_vggish_conv1(fad_handle* h, const float* logmel, long long n_examples, void* out_f16, void* stream);
 /* One tensor-core layer: 3x3 conv pad 1 (taps = 9) or fully connected (taps = 1, H = W = 1) on
- * NHWC fp16 input x[NB,H,W,Cin] with fp16 weights w[Cout, taps*Cin]; fused bias, optional ReLU,
- * optional 2x2 max-pool; fp16 NHWC output (and optional fp32 copy of the un-pooled output). */
+ * NHWC fp16 input x[NB,H,W,Cin] with fp16 weights w[Cout, taps*Cin] (split_w = 0) or fp16 hi/lo tiles
+ * w[2*Cout, taps*Cin] laid out as in fad_vggish_weights.split_mask (split_w = 1); any other split_w fails and
+ * launches nothing.  Fused bias, optional ReLU, optional 2x2 max-pool; fp16 NHWC output (and optional fp32 copy of
+ * the un-pooled output). */
 int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int Cin,
                    const void* w_f16, const float* bias, int Cout, int taps, int relu, int pool,
-                   int split_w /* weights are [2*Cout, K] hi/lo tiles */,
-                   void* out_f16, float* out_f32_or_null, void* stream);
+                   int split_w, void* out_f16, float* out_f32_or_null, void* stream);
 /* The Linear / 1-D convolution GEMM every transformer and Encodec layer runs (csrc/clap_host.inc clap_gemm):
  *   C = act(A W^T + bias), act 0 none, 1 ReLU, 2 GELU (erf form), 3 ELU (alpha = 1).
  * a_f16: fp16 rows of k_cols elements, row r starting at a_f16 + r * lda (lda = 0: k_cols; lda < k_cols gives
@@ -176,7 +177,7 @@ int fad_w2v_forward(fad_handle* h, const int16_t* pcm, long long n_clips, int L,
  * _process_file / calculate_embd_statistics_online (fadtk/utils.py:13-46) ----------------
  * Packed fp64 accumulator of length fad_stats_acc_len(d):
  *   acc[0] = n, acc[1..d] = sum(x - shift) (exact), acc[1+d..1+d+d*d) = sum y y^T (d x d),
- *   acc[1+d+d*d..] = sum y,   y = x - shift (exact modes) or its fp16 hi/lo pair (mode 1)
+ *   acc[1+d+d*d..] = sum y,   y = x - shift (the same values as acc[1..d])
  * It is additive: accumulate batches into it, all-reduce (sum) it across GPUs, then finalize.
  * `shift` (fp16 [d], device) must be identical for every contribution to one accumulator. */
 size_t fad_stats_acc_len(int d);
@@ -185,9 +186,8 @@ size_t fad_stats_acc_len(int d);
  * accumulation is fp64 in a fixed order, so the result is the Gram matrix of the data to ~1e-16,
  * positive semi-definite and bit-reproducible (rank-deficient per-song sets and covariances with
  * cond ~1e9 need that, DESIGN.md section 5.4).
- * tensor_core = 1: wgmma fp16 hi/lo-split E^T E (fp32 register accumulation, ~1e-6 relative)
- * for well-conditioned, full-rank sets.
- * tensor_core = 2: the same exact arithmetic on the CUDA cores (DFMA + fp64 atomics): verification. */
+ * tensor_core = 2: the same exact arithmetic on the CUDA cores (DFMA + fp64 atomics): verification.
+ * Any other value fails and launches nothing. */
 int fad_stats_accumulate(fad_handle* h, const void* emb_f16, long long n_rows, int d,
                          const void* shift_f16, double* acc, int tensor_core, void* stream);
 /* ---- multi-GPU: the ONE exchange step of the path (SURVEY.md section 8 (e)) ----------
@@ -290,7 +290,8 @@ long long fad_launch_count(fad_handle* h);
 
 /* Stage entry (parity test / profiling): the encoder self-attention of the Whisper and wav2vec-family forwards alone.
  * qkv: fp16 [n_clips * S][3 d] (q | k | v, head i at columns i * 64), out: fp16 [n_clips * S][d], softmax(q k^T / 8) v per
- * head.  legacy = 0: wgmma kernel (csrc/attention_wgmma.cuh); 1: the mma.sync flash kernel it replaced. */
+ * head.  legacy = 0: wgmma kernel (csrc/attention_wgmma.cuh), which every model but WavLM runs; 1: the mma.sync flash
+ * kernel (csrc/whisper.cuh) WavLM runs for its gated relative position bias (here without the bias). */
 int fad_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int S, int d, void* out_f16, int legacy, void* stream);
 
 /* ---- measurement utility -------------------------------------------------------------
