@@ -24,6 +24,14 @@
 //   warpgroups 1-2  consumers: warpgroup 1 + c issues the wgmmas of tile rows [64 c, 64 c + 64) and runs
 //                   their epilogue (accumulator -> shared-memory tile -> one row per thread)
 // Pipeline: smem ring full[] (TMA -> consumers) / empty[] (consumers -> TMA).
+//
+// CTA pairs.  The kernel runs in clusters of two CTAs; the work unit is (pair of neighbouring M tiles, N tile) and
+// cluster rank r computes M tile 2 mp + r.  Both tiles need the same weight box at every k-step, so each rank loads
+// half of its rows (split weights: rank 0 the hi rows, rank 1 the lo rows) and multicasts them into the same stage of
+// both CTAs: per CTA and k-step, 16 KiB of weights come from L2 instead of 32 (16 KiB + 8 KiB instead of 16 + 16 with
+// fp16 weights).  A stage is refilled only when the consumers of BOTH CTAs are done with it.  With an odd number of M
+// tiles the last pair's rank 1 is a spare: it loads its weight half and runs the pipeline on rank 0's A rows, and its
+// epilogue stores nothing (its rows are all >= NB).  Every tile runs the same wgmma sequence as with one CTA per tile.
 #pragma once
 #include "sm90.cuh"
 
@@ -69,6 +77,7 @@ constexpr int kTileM = 128;
 constexpr int kBlockK = 64;                        // fp16 elements per 128-B swizzled row
 constexpr int kConvGemmThreads = 384;
 constexpr int kConsumers = 2;                      // consumer warpgroups, 64 tile rows each
+constexpr int kClusterCtas = 2;                    // CTAs per cluster, sharing each weight box
 constexpr int kChunkSteps = 8;                     // k-steps (of 64) per accumulation chunk
 // The tensor core truncates when it adds into its fp32 accumulator: a sum over T accumulated elements (T = K of the
 // chunk) comes out scaled by (1 - c T), c = 1.06e-9 measured on H100 with tests/diag_accum_bias.py.  Cutting K into
@@ -148,6 +157,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     using namespace sm90;
     static_assert(N_TILE == 128, "one m64n128 accumulator per consumer warpgroup");
     static_assert(WMODE == 0 || WMODE == 1, "WMODE 0: fp16 weights, 1: fp16 hi/lo pair");
+    static_assert(kClusterCtas == 2, "the work units below are M-tile pairs");
     constexpr bool SPLIT_W = WMODE == 1;
     constexpr uint32_t kStageBytes = conv_gemm_stage_bytes<N_TILE, WMODE>();
     constexpr int kBRows = (SPLIT_W ? 2 : 1) * N_TILE;              // rows of the packed weight tensor per N tile
@@ -167,27 +177,34 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
     const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;       // balanced chunks
     const int m_tiles = p.img_groups * p.tiles_h * p.tiles_w;
-    const int total_tiles = m_tiles * p.n_tiles;                    // work unit = one M tile x one N tile
+    // work unit = (M-tile pair, N tile), N fastest; this CTA computes M tile 2 * pair + rank of each unit
+    const int rank = (int)cluster_ctarank();
+    const int cluster = (int)blockIdx.x / kClusterCtas;
+    const int n_clusters = (int)gridDim.x / kClusterCtas;
+    const int total_units = (m_tiles + 1) / 2 * p.n_tiles;
 
     if (warp == 0 && lane == 0) {
         tma_prefetch_desc(&map_x);
         tma_prefetch_desc(&map_w);
     }
     if (warp == 1 && lane == 0) {
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kConsumers * 4); }
+        // empty[s]: one arrival per consumer warp of both CTAs (the partner's multicast writes into this stage too)
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kClusterCtas * kConsumers * 4); }
         mbar_fence_init();
     }
-    __syncthreads();
+    cluster_sync();                                   // both CTAs' barriers exist before any multicast or remote arrive
 
     if (warp < 4) {
         // ------------------------------------------------------------ TMA producer
         // hand the registers of this warpgroup to the two consumers, which hold 2 x 64 fp32 accumulators
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
+            constexpr int kHalfRows = kBRows / kClusterCtas;              // weight rows this rank loads per k-step
+            uint8_t* const w_half = smem + kABytes + rank * kHalfRows * 128;
             int s = 0; uint32_t ph = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int nt = tile % p.n_tiles;
-                const int m = tile / p.n_tiles;
+            for (int unit = cluster; unit < total_units; unit += n_clusters) {
+                const int nt = unit % p.n_tiles;
+                const int m = min(2 * (unit / p.n_tiles) + rank, m_tiles - 1);   // the spare reads rank 0's rows
                 const int w0 = (m % p.tiles_w) * p.box_w;
                 const int h0 = ((m / p.tiles_w) % p.tiles_h) * p.box_h;
                 const int n0 = (m / (p.tiles_w * p.tiles_h)) * p.box_n;
@@ -200,7 +217,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     uint8_t* st = smem + s * kStageBytes;
                     mbar_expect_tx(&full[s], kStageBytes);
                     tma_load_4d(st, &map_x, &full[s], cb * kBlockK, w0 + dw, h0 + dh, n0);
-                    tma_load_2d(st + kABytes, &map_w, &full[s], ks * kBlockK, nt * kBRows);
+                    tma_load_2d_multicast(w_half + s * kStageBytes, &map_w, &full[s], ks * kBlockK,
+                                          nt * kBRows + rank * kHalfRows, (1u << kClusterCtas) - 1);
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
             }
@@ -235,18 +253,26 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
             for (int cc = c0; cc < c0 + kColsPerThread && cc < p.resid_C; cc += 32)
                 asm volatile("prefetch.global.L2 [%0];" :: "l"(p.resid + tok * p.resid_C + cc));
         };
-        if ((int)blockIdx.x < total_tiles) prefetch_resid((int)blockIdx.x % p.n_tiles, (int)blockIdx.x / p.n_tiles);
+        if (cluster < total_units) prefetch_resid(cluster % p.n_tiles, 2 * (cluster / p.n_tiles) + rank);
         auto load_bias = [&](float4 (&b)[8], int col0) {
             const float4* src = reinterpret_cast<const float4*>(p.bias + col0);
 #pragma unroll
             for (int j = 0; j < 8; ++j) b[j] = __ldg(src + j);
         };
+        // a stage is free once the consumer warps of both CTAs have read it
+        auto release = [&](int st_) {
+            __syncwarp();
+            if (lane == 0) {
+#pragma unroll
+                for (int cta = 0; cta < kClusterCtas; ++cta) mbar_arrive_cluster(&empty[st_], cta);
+            }
+        };
 
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-            const int nt = tile % p.n_tiles;
-            const int m = tile / p.n_tiles;
-            if (tile + (int)gridDim.x < total_tiles)
-                prefetch_resid((tile + (int)gridDim.x) % p.n_tiles, (tile + (int)gridDim.x) / p.n_tiles);
+        for (int unit = cluster; unit < total_units; unit += n_clusters) {
+            const int nt = unit % p.n_tiles;
+            const int m = 2 * (unit / p.n_tiles) + rank;       // == m_tiles on the spare: every row is >= NB
+            if (unit + n_clusters < total_units)
+                prefetch_resid((unit + n_clusters) % p.n_tiles, 2 * ((unit + n_clusters) / p.n_tiles) + rank);
 
             // ---- main loop: chunks of <= kChunkSteps k-steps into `acc`, summed into `sum` (round-to-nearest adds,
             // undoing the expected truncation shrink of each chunk)
@@ -277,14 +303,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     }
                     wgmma_commit();
                     wgmma_wait<1>();                   // the previous k-step's wgmmas have retired: release its stage
-                    if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+                    if (prev_s >= 0) release(prev_s);
                     prev_s = s;
                     if (++s == STAGES) { s = 0; ph ^= 1; }
                 }
                 wgmma_wait<0>();
                 fence_regs(acc);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty[prev_s]);
+                release(prev_s);
 #pragma unroll
                 for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
             }
@@ -459,6 +484,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
             }
         }
     }
+    cluster_sync();                                   // the partner's last arrivals on this CTA's barriers have landed
 }
 
 }  // namespace fad

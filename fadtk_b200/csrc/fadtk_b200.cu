@@ -169,18 +169,29 @@ namespace {
 
 template <int N_TILE, int STAGES, int WMODE>
 int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const fad::ConvGemmParams& p, cudaStream_t st) {
-    static bool attr_set = false;
+    static int max_clusters = 0;                      // co-resident CTA pairs, queried once per instantiation
     constexpr uint32_t smem = fad::conv_gemm_smem_bytes<N_TILE, STAGES, WMODE>();
     static_assert(smem <= 227 * 1024, "over the per-CTA shared-memory limit");
     auto kern = fad::conv_gemm_kernel<N_TILE, STAGES, WMODE>;
-    if (!attr_set) {
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = fad::kClusterCtas; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(fad::kConvGemmThreads);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    if (max_clusters == 0) {
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set = true;
+        cfg.gridDim = dim3(fad::kClusterCtas * (unsigned)h->num_sms);
+        CK(cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg));
+        if (max_clusters <= 0) return fail("conv_gemm_kernel: no CTA pair fits on the device");
     }
-    const int total = p.img_groups * p.tiles_h * p.tiles_w * p.n_tiles;
-    if (total == 0) return 0;
-    const int grid = total < h->num_sms ? total : h->num_sms;
-    kern<<<grid, fad::kConvGemmThreads, smem, st>>>(mx, mw, p);
+    const int units = (p.img_groups * p.tiles_h * p.tiles_w + 1) / 2 * p.n_tiles;
+    if (units == 0) return 0;
+    cfg.gridDim = dim3(fad::kClusterCtas * (unsigned)std::min(units, max_clusters));
+    CK(cudaLaunchKernelEx(&cfg, kern, mx, mw, p));
     CK(cudaGetLastError());
     h->launches++;
     return 0;
@@ -202,8 +213,8 @@ int encode_layer_maps(const LayerGeom& g, const void* x, long long nb_dim, const
     const uint64_t rows_mul = g.split_w ? 2 : 1;
     const uint64_t wd[2] = {K, (uint64_t)g.Cout * rows_mul};
     const uint64_t ws[1] = {K * 2};
-    // rows per weight box: a split layer fetches hi + lo of a tile at once
-    const uint32_t wb[2] = {64, (uint32_t)(g.n_tile * rows_mul)};
+    // rows per weight box: each CTA of a pair fetches half of a tile's rows (split: the hi or the lo rows) for both
+    const uint32_t wb[2] = {64, (uint32_t)(g.n_tile * rows_mul / fad::kClusterCtas)};
     return encode_f16_map(mw, w, 2, wd, ws, wb);
 }
 

@@ -100,6 +100,25 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 
+// ------------------------------------------------------------------------- clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA in the cluster; not .aligned, so a warp may reach it diverged
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (that CTA may be this one)
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+    asm volatile(
+        "{\n\t.reg .b32 ra;\n\t"
+        "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+        "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"
+        ::"r"(smem_u32(bar)), "r"(cta) : "memory");
+}
+
 // generic-proxy writes to smem -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -116,6 +135,16 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
         " [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)),
           "r"(c0), "r"(c1) : "memory");
+}
+// the same box into the shared memory of every CTA in `cta_mask` (bit i = cluster rank i), at the same offset, each
+// completing its bytes on the mbarrier at the same offset in that CTA
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar,
+                                                      int c0, int c1, uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;"
+        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)),
+          "r"(c0), "r"(c1), "h"(cta_mask) : "memory");
 }
 __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar,
                                             int c0, int c1, int c2) {
