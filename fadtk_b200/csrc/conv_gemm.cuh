@@ -19,11 +19,18 @@
 // warpgroup accumulates at most kChunkSteps x 64 = 512 of K into its wgmma accumulator, then adds
 // the chunk into a second register array with ordinary round-to-nearest fp32 adds.
 //
-// Warp roles (384 threads, persistent over tiles):
+// Warp roles (512 threads, persistent over tiles; every role walks the same sequence of work units):
 //   warpgroup 0     TMA producer (one elected lane of warp 0)
-//   warpgroups 1-2  consumers: warpgroup 1 + c issues the wgmmas of tile rows [64 c, 64 c + 64) and runs
-//                   their epilogue (accumulator -> shared-memory tile -> one row per thread)
-// Pipeline: smem ring full[] (TMA -> consumers) / empty[] (consumers -> TMA).
+//   warpgroups 1-2  consumers: warpgroup 1 + c issues the wgmmas of tile rows [64 c, 64 c + 64), folds the chunks,
+//                   dumps the finished accumulator into its half of the fp32 shared-memory tile and starts the next
+//                   tile at once
+//   warpgroup 3     epilogue: warps 2 c and 2 c + 1 drain consumer c's half (32 rows each, one row per lane): bias,
+//                   activation, pool, stores, fused residual - overlapped with the consumers' next main loop
+// Pipeline: smem ring full[] (TMA -> consumers) / empty[] (consumers -> TMA); per consumer half, epi_full[c]
+// (consumer -> epilogue) / epi_empty[c] (epilogue -> consumer).  The handoff is per half, so one never waits for
+// the other.  Registers per thread (setmaxnreg): producer 40, epilogue kEpiRegs, consumers kConsumerRegs
+// (40 + 136 + 2 x 168 = 512 = 65536 / 128): a consumer holds sum[64] + acc[64] + addressing, nothing of the epilogue;
+// the epilogue walks its row 32 columns at a time.  ptxas -v: no spills in either instantiation.
 //
 // CTA pairs.  The kernel runs in clusters of two CTAs; the work unit is (pair of neighbouring M tiles, N tile) and
 // cluster rank r computes M tile 2 mp + r.  Both tiles need the same weight box at every k-step, so each rank loads
@@ -75,8 +82,10 @@ __device__ __forceinline__ long long window_row_to_token(long long o, int res, i
 
 constexpr int kTileM = 128;
 constexpr int kBlockK = 64;                        // fp16 elements per 128-B swizzled row
-constexpr int kConvGemmThreads = 384;
+constexpr int kConvGemmThreads = 512;
 constexpr int kConsumers = 2;                      // consumer warpgroups, 64 tile rows each
+constexpr int kConsumerRegs = 168;                 // setmaxnreg budgets: 40 + kEpiRegs + 2 x kConsumerRegs <= 512
+constexpr int kEpiRegs = 136;
 constexpr int kClusterCtas = 2;                    // CTAs per cluster, sharing each weight box
 constexpr int kChunkSteps = 8;                     // k-steps (of 64) per accumulation chunk
 // The tensor core truncates when it adds into its fp32 accumulator: a sum over T accumulated elements (T = K of the
@@ -89,7 +98,9 @@ constexpr float kAccumShrinkPerElement = 1.06e-9f;
 constexpr uint32_t kABytes = kTileM * kBlockK * 2; // 16 KiB per stage
 constexpr uint32_t kEpiRowBytes = 128 * 4;         // one fp32 row of a 128-column accumulator tile
 constexpr uint32_t kEpiBytes = 64 * kEpiRowBytes;  // per consumer: 64 rows x 128 fp32 (32 KiB)
-constexpr uint32_t kStagingBytes = 32 * 128;       // per epilogue warp: 32 rows x 128 B output staging (inside kEpiBytes)
+constexpr uint32_t kBiasBytes = 128 * 4;           // per epilogue warp: the bias of the tile's 128 columns
+static_assert(40 + kEpiRegs + kConsumers * kConsumerRegs <= 65536 / 128, "register file over-subscribed");
+static_assert(kConsumerRegs > 65536 / kConvGemmThreads, "the consumers raise their register count (setmaxnreg.inc)");
 
 // SPLIT_W: the weights are an fp16 hi/lo pair (W = Wh + Wl, 22 bits).  fp16 rounding of the
 // weights is a fixed perturbation of the model that does not average out over samples: it alone
@@ -107,7 +118,7 @@ __host__ __device__ constexpr uint32_t conv_gemm_stage_bytes() {
 template <int N_TILE, int STAGES, int WMODE>
 __host__ __device__ constexpr uint32_t conv_gemm_smem_bytes() {
     return STAGES * conv_gemm_stage_bytes<N_TILE, WMODE>() + 1024 /*align slack*/ + 256 /*barriers*/
-         + kConsumers * kEpiBytes;
+         + kConsumers * kEpiBytes + 4 * kBiasBytes;
 }
 
 __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
@@ -119,28 +130,46 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
 // q = degree-6 weighted-minimax fit of log2(erfc(z)) / z (oracle/fit_gelu.py): |erf error| <= 1.4e-7
 // in fp32, far below the fp16 rounding of the value this feeds.  One MUFU (ex2) + ~13 FMA-pipe
 // instructions per element - erff costs ~30, and two MUFUs made the fc1 epilogue MUFU-bound.
+//
+// The array forms evaluate N elements stage by stage (every element's z, then every element's next polynomial term, ...):
+// the N independent chains are then interleaved in the instruction stream.  Written element by element, ptxas kept
+// each ~100-clock dependent chain whole in the register-lean epilogue warpgroup, and a GELU tile took ~12 k clocks.
+// The arithmetic of each element is the same either way.
+template <int N>
+__device__ __forceinline__ void gelu_erf_n(float* x) {
+    float z[N], q[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) { z[i] = fminf(fabsf(x[i]) * 0.70710678118654752f, 4.3f); q[i] = 1.04899843e-04f; }
+    constexpr float kQ[6] = {-4.92790774e-04f, -2.22368206e-03f, 2.93586859e-02f, -1.48908889e-01f, -9.18342944e-01f,
+                             -1.62791250e+00f};
+#pragma unroll
+    for (int t = 0; t < 6; ++t) {
+#pragma unroll
+        for (int i = 0; i < N; ++i) q[i] = fmaf(q[i], z[i], kQ[t]);
+    }
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q[i]) : "f"(q[i] * z[i]));
+#pragma unroll
+    for (int i = 0; i < N; ++i) x[i] = 0.5f * x[i] * (1.0f + copysignf(1.0f - q[i], x[i]));
+}
 __device__ __forceinline__ float gelu_erf(float x) {
-    const float z = fminf(fabsf(x) * 0.70710678118654752f, 4.3f);
-    float q = 1.04899843e-04f;
-    q = fmaf(q, z, -4.92790774e-04f);
-    q = fmaf(q, z, -2.22368206e-03f);
-    q = fmaf(q, z, 2.93586859e-02f);
-    q = fmaf(q, z, -1.48908889e-01f);
-    q = fmaf(q, z, -9.18342944e-01f);
-    q = fmaf(q, z, -1.62791250e+00f);
-    float e;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(q * z));
-    return 0.5f * x * (1.0f + copysignf(1.0f - e, x));
+    gelu_erf_n<1>(&x);
+    return x;
 }
 
 // ELU (alpha = 1) in ~10 instructions (expm1f is ~25, in an epilogue that is issue-bound): the negative branch is
 // 2^(x log2 e) - 1 with one MUFU (absolute error 2^-22) below -1/16, and the Taylor polynomial of degree 4 above it, where
 // the subtraction would cancel (truncation < 8e-9, relative error ~1e-7 of a result that is then rounded to fp16).
-__device__ __forceinline__ float elu_ex2(float x) {
-    float e;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(fminf(x, 0.f) * 1.4426950408889634f));
-    const float t = x * fmaf(x, fmaf(x, fmaf(x, 4.16666667e-2f, 1.66666667e-1f), 0.5f), 1.0f);
-    return x > 0.f ? x : (x > -0.0625f ? t : e - 1.0f);
+// Stage by stage over N elements, as gelu_erf_n.
+template <int N>
+__device__ __forceinline__ void elu_ex2_n(float* x) {
+    float e[N], t[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e[i]) : "f"(fminf(x[i], 0.f) * 1.4426950408889634f));
+#pragma unroll
+    for (int i = 0; i < N; ++i) t[i] = x[i] * fmaf(x[i], fmaf(x[i], fmaf(x[i], 4.16666667e-2f, 1.66666667e-1f), 0.5f), 1.0f);
+#pragma unroll
+    for (int i = 0; i < N; ++i) x[i] = x[i] > 0.f ? x[i] : (x[i] > -0.0625f ? t[i] : e[i] - 1.0f);
 }
 
 __device__ __forceinline__ uint32_t hmax2_u32(uint32_t a, uint32_t b) {
@@ -161,15 +190,17 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     constexpr bool SPLIT_W = WMODE == 1;
     constexpr uint32_t kStageBytes = conv_gemm_stage_bytes<N_TILE, WMODE>();
     constexpr int kBRows = (SPLIT_W ? 2 : 1) * N_TILE;              // rows of the packed weight tensor per N tile
-    constexpr int kColsPerThread = N_TILE / 2;          // epilogue: one row, one column half per thread
-    constexpr int kGroups = kColsPerThread / 32;
+    constexpr int kGroups = N_TILE / 32;                // epilogue: one row per lane, 32 columns (one 128-B segment) per group
 
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * kStageBytes);
     uint64_t* full = bars;
     uint64_t* empty = bars + STAGES;
-    uint8_t* epi = smem + STAGES * kStageBytes + 256;                // kConsumers x kEpiBytes
+    uint64_t* epi_full = bars + 2 * STAGES;                         // [kConsumers]: consumer c's half is in the tile
+    uint64_t* epi_empty = bars + 2 * STAGES + kConsumers;           // [kConsumers]: the epilogue is done with it
+    static_assert((2 * STAGES + 2 * kConsumers) * 8 <= 256, "barriers");
+    uint8_t* epi = smem + STAGES * kStageBytes + 256;                // kConsumers x kEpiBytes, then 4 x kBiasBytes
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -177,9 +208,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
     const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;       // balanced chunks
     const int m_tiles = p.img_groups * p.tiles_h * p.tiles_w;
-    // work unit = (M-tile pair, N tile), N fastest; this CTA computes M tile 2 * pair + rank of each unit
-    const int rank = (int)cluster_ctarank();
-    const int cluster = (int)blockIdx.x / kClusterCtas;
+    // work unit = (M-tile pair, N tile), N fastest; this CTA computes M tile 2 * pair + rank of each unit.  Each role reads
+    // its cluster index and rank after its setmaxnreg: kept live across the role split, they were spilled.
     const int n_clusters = (int)gridDim.x / kClusterCtas;
     const int total_units = (m_tiles + 1) / 2 * p.n_tiles;
 
@@ -190,6 +220,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
     if (warp == 1 && lane == 0) {
         // empty[s]: one arrival per consumer warp of both CTAs (the partner's multicast writes into this stage too)
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kClusterCtas * kConsumers * 4); }
+        // epi_full[c]: every thread of consumer c; epi_empty[c]: every thread of the two epilogue warps of half c
+        for (int c = 0; c < kConsumers; ++c) { mbar_init(&epi_full[c], 128); mbar_init(&epi_empty[c], 64); }
         mbar_fence_init();
     }
     cluster_sync();                                   // both CTAs' barriers exist before any multicast or remote arrive
@@ -199,6 +231,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
         // hand the registers of this warpgroup to the two consumers, which hold 2 x 64 fp32 accumulators
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
+            const int rank = (int)cluster_ctarank();
+            const int cluster = (int)cluster_index();
             constexpr int kHalfRows = kBRows / kClusterCtas;              // weight rows this rank loads per k-step
             uint8_t* const w_half = smem + kABytes + rank * kHalfRows * 128;
             int s = 0; uint32_t ph = 0;
@@ -223,42 +257,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 }
             }
         }
-    } else {
-        // ------------------------------------------------------------ consumers: wgmma + epilogue
-        setmaxnreg_inc<232>();
+    } else if (warp < 4 + 4 * kConsumers) {
+        // ------------------------------------------------------------ consumers: wgmma + chunk fold + fragment dump
+        setmaxnreg_inc<kConsumerRegs>();
+        const int cluster = (int)cluster_index();
         const int c = (warp >> 2) - 1;                    // consumer index: tile rows [64 c, 64 c + 64)
-        const int wg_t = threadIdx.x & 127;               // thread within the warpgroup
-        const int wq = wg_t >> 5;                         // warp within the warpgroup
-        // epilogue role: row rr of this consumer's 64, column half `half`
-        const int rr = wg_t & 63;
-        const int half = wg_t >> 6;
-        const int r = c * 64 + rr;                        // row of the tile
-        const int bw = p.box_w, bh = p.box_h;
-        const int pw = r % bw;
-        const int phh = (r / bw) % bh;
-        const int pn = r / (bw * bh);
+        const int wq = warp & 3;                          // warp within the warpgroup
         const uint32_t epi_base = smem_u32(epi) + c * kEpiBytes;
-        const uint32_t bar_id = 1 + c;
-        int s = 0; uint32_t ph = 0;
-        // plain row-major GEMM (1x1 "image", 128 rows per tile): no per-tile divisions
-        const bool plain = p.tiles_w == 1 && p.tiles_h == 1 && bw == 1 && bh == 1;
-        // residual rows are read-modify-written in the epilogue: pull the NEXT tile's rows into L2
-        // while this tile is computed, so the loads do not pay HBM latency on the critical path
-        auto prefetch_resid = [&](int nt_, int m_) {
-            if (p.resid == nullptr || !plain) return;
-            const int n_ = m_ * kTileM + r;
-            if (n_ >= p.NB) return;
-            const long long tok = p.resid_res ? window_row_to_token((long long)n_, p.resid_res, p.resid_shift) : (long long)n_;
-            const int c0 = nt_ * N_TILE + half * kColsPerThread;
-            for (int cc = c0; cc < c0 + kColsPerThread && cc < p.resid_C; cc += 32)
-                asm volatile("prefetch.global.L2 [%0];" :: "l"(p.resid + tok * p.resid_C + cc));
-        };
-        if (cluster < total_units) prefetch_resid(cluster % p.n_tiles, 2 * (cluster / p.n_tiles) + rank);
-        auto load_bias = [&](float4 (&b)[8], int col0) {
-            const float4* src = reinterpret_cast<const float4*>(p.bias + col0);
-#pragma unroll
-            for (int j = 0; j < 8; ++j) b[j] = __ldg(src + j);
-        };
+        int s = 0; uint32_t ph = 0, eph = 0;
         // a stage is free once the consumer warps of both CTAs have read it
         auto release = [&](int st_) {
             __syncwarp();
@@ -269,11 +275,6 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
         };
 
         for (int unit = cluster; unit < total_units; unit += n_clusters) {
-            const int nt = unit % p.n_tiles;
-            const int m = 2 * (unit / p.n_tiles) + rank;       // == m_tiles on the spare: every row is >= NB
-            if (unit + n_clusters < total_units)
-                prefetch_resid((unit + n_clusters) % p.n_tiles, 2 * ((unit + n_clusters) / p.n_tiles) + rank);
-
             // ---- main loop: chunks of <= kChunkSteps k-steps into `acc`, summed into `sum` (round-to-nearest adds,
             // undoing the expected truncation shrink of each chunk)
             float sum[64], acc[64];
@@ -314,30 +315,79 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
             }
 
-            // ---- accumulator fragment -> fp32 tile [64 rows][128 cols] in shared memory, 16-B chunks XOR-swizzled by row
-            named_bar_sync(bar_id, 128);               // the previous tile's epilogue is done with the region
-            {
-                const int fr = wq * 16 + (lane >> 2);
+            // ---- accumulator fragment -> this consumer's half of the fp32 tile [64 rows][128 cols] in shared memory,
+            // 16-B chunks XOR-swizzled by row, once the epilogue has drained the previous tile's half; the arrive
+            // releases the stores to it
+            mbar_wait(&epi_empty[c], eph ^ 1);
+            // element (row, col) = (fr + 8 i, 8 j + 2 (lane % 4) + e) sits in 16-B chunk (col / 4) ^ (row % 8) of its row;
+            // with j = 4 jh + jl that is 8 jh + ((2 jl) ^ x), so four base registers and immediate offsets cover all 32
+            const int fr = wq * 16 + (lane >> 2);
+            const uint32_t x = ((lane & 3) >> 1) ^ (fr & 7);
+            const uint32_t row_base = epi_base + fr * kEpiRowBytes + (lane & 1) * 8;
 #pragma unroll
-                for (int j = 0; j < 16; ++j) {
+            for (int jl = 0; jl < 4; ++jl) {
+                const uint32_t a = row_base + (((2 * jl) ^ x) << 4);
+#pragma unroll
+                for (int jh = 0; jh < 4; ++jh) {
 #pragma unroll
                     for (int i = 0; i < 2; ++i) {
-                        const int row = fr + 8 * i, col = 8 * j + 2 * (lane & 3);
-                        const uint32_t addr = epi_base + row * kEpiRowBytes + ((((col >> 2) ^ (row & 7))) << 4) + (col & 3) * 4;
-                        sts64(addr, sum[4 * j + 2 * i], sum[4 * j + 2 * i + 1]);
+                        const int j = 4 * jh + jl;
+                        sts64(a + i * 8 * kEpiRowBytes + jh * 128, sum[4 * j + 2 * i], sum[4 * j + 2 * i + 1]);
                     }
                 }
             }
-            named_bar_sync(bar_id, 128);
-            float accr[kColsPerThread];
-#pragma unroll
-            for (int q4 = 0; q4 < kColsPerThread / 4; ++q4) {
-                const int ch = half * (kColsPerThread / 4) + q4;
-                const uint4 u = lds128(epi_base + rr * kEpiRowBytes + ((ch ^ (rr & 7)) << 4));
-                accr[4 * q4 + 0] = __uint_as_float(u.x); accr[4 * q4 + 1] = __uint_as_float(u.y);
-                accr[4 * q4 + 2] = __uint_as_float(u.z); accr[4 * q4 + 3] = __uint_as_float(u.w);
+            mbar_arrive(&epi_full[c]);
+            eph ^= 1;
+        }
+    } else {
+        // ------------------------------------------------------------ epilogue: one tile row per lane
+        // every warp starts at the launch allocation of 65536 / 512 = 128 registers; setmaxnreg.dec may only lower it
+        if constexpr (kEpiRegs > 65536 / kConvGemmThreads) setmaxnreg_inc<kEpiRegs>();
+        else setmaxnreg_dec<kEpiRegs>();
+        const int rank = (int)cluster_ctarank();
+        const int cluster = (int)cluster_index();
+        const int e = warp - 4 - 4 * kConsumers;         // epilogue warp 0..3
+        const int c = e >> 1;                             // it drains consumer c's half ...
+        const int rr = (e & 1) * 32 + lane;               // ... row rr of it
+        const int r = c * 64 + rr;                        // row of the tile
+        const int bw = p.box_w, bh = p.box_h;
+        const int pw = r % bw;
+        const int phh = (r / bw) % bh;
+        const int pn = r / (bw * bh);
+        // this warp's 32 rows of the tile; the 128-B segment of group g of each row doubles as its output staging once read
+        const uint32_t wrows = smem_u32(epi) + c * kEpiBytes + (e & 1) * 32 * kEpiRowBytes;
+        const uint32_t row_mine = wrows + lane * kEpiRowBytes;
+        const uint32_t bias_s = smem_u32(epi) + kConsumers * kEpiBytes + e * kBiasBytes;
+        const int sw = lane & 7;                          // == rr & 7 == r & 7: the swizzle of this lane's row
+        const int cq = lane & 7, rq = lane >> 3;          // flush role: 16-B chunk cq of rows it*4 + rq
+        uint32_t eph = 0;
+        // plain row-major GEMM (1x1 "image", 128 rows per tile): no per-tile divisions
+        const bool plain = p.tiles_w == 1 && p.tiles_h == 1 && bw == 1 && bh == 1;
+        const bool f32_path = p.out_f32 != nullptr || p.resid != nullptr;
+        // residual rows are read-modify-written here: pull the NEXT tile's rows into L2 while this one is stored,
+        // so the loads do not pay HBM latency on the critical path
+        auto prefetch_resid = [&](int nt_, int m_) {
+            if (p.resid == nullptr || !plain) return;
+            const int n_ = m_ * kTileM + r;
+            if (n_ >= p.NB) return;
+            const long long tok = p.resid_res ? window_row_to_token((long long)n_, p.resid_res, p.resid_shift) : (long long)n_;
+            for (int cc = nt_ * N_TILE; cc < nt_ * N_TILE + N_TILE && cc < p.resid_C; cc += 32)
+                asm volatile("prefetch.global.L2 [%0];" :: "l"(p.resid + tok * p.resid_C + cc));
+        };
+        if (cluster < total_units) prefetch_resid(cluster % p.n_tiles, 2 * (cluster / p.n_tiles) + rank);
+
+        for (int unit = cluster; unit < total_units; unit += n_clusters) {
+            const int nt = unit % p.n_tiles;
+            const int m = 2 * (unit / p.n_tiles) + rank;       // == m_tiles on the spare: every row is >= NB
+            if (unit + n_clusters < total_units)
+                prefetch_resid((unit + n_clusters) % p.n_tiles, 2 * ((unit + n_clusters) / p.n_tiles) + rank);
+            // the tile's bias into this warp's slice (broadcast reads below), before the wait
+            __syncwarp();                                 // the previous tile's reads of the slice are done
+            {
+                const float4 b = __ldg(reinterpret_cast<const float4*>(p.bias + nt * N_TILE) + lane);
+                sts128(bias_s + lane * 16, __float_as_uint(b.x), __float_as_uint(b.y), __float_as_uint(b.z), __float_as_uint(b.w));
             }
-            named_bar_sync(bar_id, 128);               // the tile region becomes the four warps' output staging
+            __syncwarp();
 
             int w, h, n;
             if (plain) { w = 0; h = 0; n = m * kTileM + r; }
@@ -347,11 +397,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                 n = (m / (p.tiles_w * p.tiles_h)) * p.box_n + pn;
             }
             const bool valid = n < p.NB;
-            const int ch0 = nt * N_TILE + half * kColsPerThread;
-            // Destination of this lane's row (element offsets, -1 = row beyond the batch).  Stores go
-            // through a per-warp staging tile (32 rows x 128 B, 16-B chunks XOR-swizzled by row) so a
-            // warp writes whole 128-B lines of 4 rows per instruction instead of 16 B into 32
-            // different rows.
+            const int ch0 = nt * N_TILE;
+            // Destination of this lane's row (element offsets, -1 = row beyond the batch).  Stores go through the
+            // warp's rows of the tile (16-B chunks XOR-swizzled by row) so a warp writes whole 128-B lines of 4 rows
+            // per instruction instead of 16 B into 32 different rows.
             long long out_off = -1, res_off = -1;
             if (valid && !p.pool) {
                 out_off = (long long)((size_t(n) * p.H + h) * p.W + w) * p.ld_out;
@@ -359,64 +408,65 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     res_off = (p.resid_res ? window_row_to_token((long long)n, p.resid_res, p.resid_shift) : (long long)n)
                               * p.resid_C;
             }
-            const uint32_t stg = epi_base + wq * kStagingBytes;
-            const uint32_t stg_mine = stg + lane * 128;
-            const int sw = lane & 7;
-            const int cq = lane & 7, rq = lane >> 3;      // flush role: 16-B chunk cq of rows it*4 + rq
-            const bool f32_path = p.out_f32 != nullptr || p.resid != nullptr;
-            float4 bnext[8];
-#pragma unroll
+
+            mbar_wait(&epi_full[c], eph);
+#pragma unroll 1
             for (int g = 0; g < kGroups; ++g) {
                 float f[32];
-                load_bias(bnext, ch0 + g * 32);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {
-                    const float4 b = bnext[j];
-                    f[4 * j + 0] = accr[g * 32 + 4 * j + 0] + b.x;
-                    f[4 * j + 1] = accr[g * 32 + 4 * j + 1] + b.y;
-                    f[4 * j + 2] = accr[g * 32 + 4 * j + 2] + b.z;
-                    f[4 * j + 3] = accr[g * 32 + 4 * j + 3] + b.w;
+                    const uint4 u = lds128(row_mine + g * 128 + ((j ^ sw) << 4));
+                    const uint4 b = lds128(bias_s + g * 128 + j * 16);
+                    f[4 * j + 0] = __uint_as_float(u.x) + __uint_as_float(b.x);
+                    f[4 * j + 1] = __uint_as_float(u.y) + __uint_as_float(b.y);
+                    f[4 * j + 2] = __uint_as_float(u.z) + __uint_as_float(b.z);
+                    f[4 * j + 3] = __uint_as_float(u.w) + __uint_as_float(b.w);
                 }
                 if (p.relu == 1) {
 #pragma unroll
                     for (int j = 0; j < 32; ++j) f[j] = fmaxf(f[j], 0.0f);
                 } else if (p.relu == 2) {
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = gelu_erf(f[j]);
+                    for (int j = 0; j < 32; j += 8) gelu_erf_n<8>(f + j);
                 } else if (p.relu == 3) {                           // ELU (alpha = 1): SEANet's activation
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) f[j] = elu_ex2(f[j]);
+                    for (int j = 0; j < 32; j += 8) elu_ex2_n<8>(f + j);
                 }
-                uint32_t h2[16];
-#pragma unroll
-                for (int j = 0; j < 16; ++j) h2[j] = pack_half2(f[2 * j], f[2 * j + 1]);
 
                 if (!p.pool) {
                     if (f32_path) {
-                        // fp32 outputs: this group's 32 columns = one 128-B row segment per row
+                        if (p.out != nullptr && out_off >= 0) {   // rare: both precisions; the fp16 copy direct, in 8-column pieces
+                            uint4* dst = reinterpret_cast<uint4*>(p.out + out_off + ch0 + g * 32);
+#pragma unroll
+                            for (int j = 0; j < 4; ++j)          // n_valid is a multiple of 8: a partial last group
+                                if (ch0 + g * 32 + 8 * j < p.n_valid)
+                                    dst[j] = make_uint4(pack_half2(f[8 * j], f[8 * j + 1]), pack_half2(f[8 * j + 2], f[8 * j + 3]),
+                                                        pack_half2(f[8 * j + 4], f[8 * j + 5]), pack_half2(f[8 * j + 6], f[8 * j + 7]));
+                        }
+                        // fp32 outputs: this group's 32 columns = one 128-B row segment per row, staged in place
 #pragma unroll
                         for (int j = 0; j < 8; ++j)
-                            sts128(stg_mine + ((j ^ sw) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]),
+                            sts128(row_mine + g * 128 + ((j ^ sw) << 4), __float_as_uint(f[4 * j]), __float_as_uint(f[4 * j + 1]),
                                    __float_as_uint(f[4 * j + 2]), __float_as_uint(f[4 * j + 3]));
                         __syncwarp();
-                        float4 v[8];
-#pragma unroll
-                        for (int it = 0; it < 8; ++it) {
-                            const int rr = it * 4 + rq;
-                            const uint4 u = lds128(stg + rr * 128 + ((cq ^ (rr & 7)) << 4));
-                            v[it] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
-                        }
                         const int col = ch0 + g * 32 + cq * 4;
-                        if (p.out_f32 != nullptr) {
 #pragma unroll
-                            for (int it = 0; it < 8; ++it) {
-                                const long long off = __shfl_sync(0xffffffffu, out_off, it * 4 + rq);
-                                if (off >= 0 && col < p.n_valid) *reinterpret_cast<float4*>(p.out_f32 + off + col) = v[it];
+                        for (int hf = 0; hf < 2; ++hf) {                   // 4 rows at a time: 4 loads in flight, then 4 stores
+                            float4 v[4];
+#pragma unroll
+                            for (int it = 0; it < 4; ++it) {
+                                const int x = (hf * 4 + it) * 4 + rq;
+                                const uint4 u = lds128(wrows + x * kEpiRowBytes + g * 128 + ((cq ^ (x & 7)) << 4));
+                                v[it] = make_float4(__uint_as_float(u.x), __uint_as_float(u.y), __uint_as_float(u.z), __uint_as_float(u.w));
                             }
-                        }
-                        if (p.resid != nullptr && ch0 + g * 32 < p.resid_C) {     // resid_C is a multiple of 32
+                            if (p.out_f32 != nullptr) {
 #pragma unroll
-                            for (int hf = 0; hf < 2; ++hf) {               // 4 loads in flight, then 4 stores
+                                for (int it = 0; it < 4; ++it) {
+                                    const long long off = __shfl_sync(0xffffffffu, out_off, (hf * 4 + it) * 4 + rq);
+                                    if (off >= 0 && col < p.n_valid) *reinterpret_cast<float4*>(p.out_f32 + off + col) = v[it];
+                                }
+                            }
+                            if (p.resid != nullptr && ch0 + g * 32 < p.resid_C) {     // resid_C is a multiple of 32
                                 long long offs[4];
                                 float4 xv[4];
 #pragma unroll
@@ -427,40 +477,37 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
 #pragma unroll
                                 for (int it = 0; it < 4; ++it) {
                                     if (offs[it] >= 0) {
-                                        const float4 a = v[hf * 4 + it];
+                                        const float4 a = v[it];
                                         xv[it].x += a.x; xv[it].y += a.y; xv[it].z += a.z; xv[it].w += a.w;
                                         *reinterpret_cast<float4*>(p.resid + offs[it] + col) = xv[it];
                                     }
                                 }
                             }
                         }
-                        __syncwarp();
-                        if (p.out != nullptr && out_off >= 0) {   // rare: both precisions, direct, in 8-column pieces
-                            uint4* dst = reinterpret_cast<uint4*>(p.out + out_off + ch0 + g * 32);
-#pragma unroll
-                            for (int j = 0; j < 4; ++j)          // n_valid is a multiple of 8: a partial last group
-                                if (ch0 + g * 32 + 8 * j < p.n_valid)
-                                    dst[j] = make_uint4(h2[4 * j], h2[4 * j + 1], h2[4 * j + 2], h2[4 * j + 3]);
-                        }
                     } else if (p.out != nullptr) {
-                        // fp16 output: two groups (64 columns) fill the 128-B row segment, then flush
+                        // fp16 output: groups g - 1 and g (64 columns) fill the 128-B segment of group g - 1, then flush
+                        const int seg = (g & ~1) * 128;
 #pragma unroll
                         for (int j = 0; j < 4; ++j)
-                            sts128(stg_mine + ((((g & 1) * 4 + j) ^ sw) << 4), h2[4 * j], h2[4 * j + 1], h2[4 * j + 2], h2[4 * j + 3]);
+                            sts128(row_mine + seg + ((((g & 1) * 4 + j) ^ sw) << 4),
+                                   pack_half2(f[8 * j], f[8 * j + 1]), pack_half2(f[8 * j + 2], f[8 * j + 3]),
+                                   pack_half2(f[8 * j + 4], f[8 * j + 5]), pack_half2(f[8 * j + 6], f[8 * j + 7]));
                         if (g & 1) {
                             __syncwarp();
                             const int col = ch0 + (g - 1) * 32 + cq * 8;
 #pragma unroll
                             for (int it = 0; it < 8; ++it) {
-                                const int rr = it * 4 + rq;
-                                const uint4 v = lds128(stg + rr * 128 + ((cq ^ (rr & 7)) << 4));
-                                const long long off = __shfl_sync(0xffffffffu, out_off, rr);
+                                const int x = it * 4 + rq;
+                                const uint4 v = lds128(wrows + x * kEpiRowBytes + seg + ((cq ^ (x & 7)) << 4));
+                                const long long off = __shfl_sync(0xffffffffu, out_off, x);
                                 if (off >= 0 && col < p.n_valid) *reinterpret_cast<uint4*>(p.out + off + col) = v;
                             }
-                            __syncwarp();
                         }
                     }
                 } else {
+                    uint32_t h2[16];
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) h2[j] = pack_half2(f[2 * j], f[2 * j + 1]);
                     // 2x2 max-pool: partners are lane^1 (w) and lane^box_w (h), box_w in {8,16}
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
@@ -482,6 +529,8 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap map_x,
                     }
                 }
             }
+            mbar_arrive(&epi_empty[c]);                   // this lane's reads of the half are done
+            eph ^= 1;
         }
     }
     cluster_sync();                                   // the partner's last arrivals on this CTA's barriers have landed

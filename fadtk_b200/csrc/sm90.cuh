@@ -106,6 +106,13 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
+// index of this CTA's cluster in the (1-D) grid; a volatile read, so a caller can re-read it where it needs it instead of
+// keeping one copy live through code that is short of registers
+__device__ __forceinline__ uint32_t cluster_index() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+    return r;
+}
 // every thread of every CTA in the cluster; not .aligned, so a warp may reach it diverged
 __device__ __forceinline__ void cluster_sync() {
     asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
