@@ -76,6 +76,8 @@ SIGNATURES = {
     "fad_frechet_batched": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_attention": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
     "fad_bench_dmma_peak": (C.c_int, [c_vp, C.c_int, c_vp]),
+    "fad_kad_median_sq": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_kad_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -510,6 +512,25 @@ class Engine:
         out = torch.zeros(8, dtype=torch.float64, device=mu1.device)
         _check(lib().fad_frechet(self._h, mu1.data_ptr(), cov1.data_ptr(), mu2.data_ptr(), cov2.data_ptr(),
                                  d, iters, out.data_ptr(), _stream()))
+        return out
+
+    # --------------------------------------------------------- Kernel Audio Distance
+    def kad_median_sq(self, x: torch.Tensor) -> torch.Tensor:
+        """x fp16 [m, d] (cuda, d a multiple of 8) -> fp64 [2] (cuda): the two middle squared distances of the pairs
+        i < j of x (fad_kad_median_sq; equal when m (m - 1) / 2 is odd)."""
+        assert x.dtype == torch.float16 and x.is_cuda and x.is_contiguous() and x.ndim == 2
+        out = torch.empty(2, dtype=torch.float64, device=x.device)
+        _check(lib().fad_kad_median_sq(self._h, x.data_ptr(), x.shape[0], x.shape[1], out.data_ptr(), _stream()))
+        return out
+
+    def kad_sums(self, z: torch.Tensor, m: int, sigma: torch.Tensor) -> torch.Tensor:
+        """z fp16 [m + n, d] (cuda, X rows first), sigma fp64 scalar (cuda) -> fp64 [3] (cuda): S_xx, S_yy (pairs i < j)
+        and S_xy of exp(-|a - b|^2 / (2 sigma^2)) (fad_kad_sums)."""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        out = torch.empty(3, dtype=torch.float64, device=z.device)
+        _check(lib().fad_kad_sums(self._h, z.data_ptr(), int(m), z.shape[0] - int(m), z.shape[1], sigma.data_ptr(),
+                                  out.data_ptr(), _stream()))
         return out
 
 

@@ -25,6 +25,7 @@
 #include "encodec.cuh"
 #include "wav2vec.cuh"
 #include "attention_wgmma.cuh"
+#include "kad.cuh"
 
 namespace {
 
@@ -145,6 +146,7 @@ struct fad_handle {
     size_t frb_cap = 0;
     float* rs_bank = nullptr;  size_t rs_bank_cap = 0;  int rs_in = 0, rs_out = 0;     // resampler filter bank
     float* rs_mono = nullptr;  size_t rs_mono_cap = 0;
+    unsigned char* kad_buf = nullptr;  size_t kad_cap = 0;      // fad_kad_* workspace (KadWorkspace)
     std::set<const void*> zero_lo;           // hi/lo weight tensors whose lo parts are all zero (note_split_weights)
     double* fr_scal = nullptr;   // 32 doubles
 
@@ -477,7 +479,8 @@ int fad_destroy(fad_handle* h) {
     encodec_free_state(h->encodec_state);
     w2v_free_state(h->w2v_state);
     void* ptrs[] = {h->d_twiddle, h->d_hann, h->d_melw, h->d_mel_start, h->d_mel_count, h->conv1_w, h->conv1_b,
-                    h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->fr_scal, h->frb_buf, h->rs_bank, h->rs_mono};
+                    h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->fr_scal, h->frb_buf, h->rs_bank, h->rs_mono,
+                    h->kad_buf};
     for (void* p : ptrs) if (p) cudaFree(p);
     for (int i = 0; i < 5; ++i) { if (h->conv_w[i]) cudaFree(h->conv_w[i]); if (h->conv_b[i]) cudaFree(h->conv_b[i]); }
     for (int i = 0; i < 3; ++i) { if (h->fc_w[i]) cudaFree(h->fc_w[i]); if (h->fc_b[i]) cudaFree(h->fc_b[i]); }
@@ -1098,6 +1101,132 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
         h->launches++;
     }
     prof_end(h, FAD_PROF_FRECHET, ev, st);
+    return 0;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------ Kernel Audio Distance
+namespace {
+// carve-outs of h->kad_buf for one call over N rows
+struct KadWorkspace {
+    __half *hi, *lo, *shift;
+    float* norm;
+    double *colpart, *partial;
+    unsigned long long* hist;
+    fad::KadSelectState* state;
+};
+
+int kad_check(fad_handle* h, const void* z, long long m, long long n, int d, const void* out) {
+    if (!h) return fail("null handle");
+    if (!z || !out) return fail("null argument");
+    if (m < 2 || n < 2) return fail("KAD needs at least two rows in each set");
+    if (d <= 0 || d % 8 != 0) return fail("d must be a positive multiple of 8");
+    if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(out)) & 15) return fail("pointers must be 16-byte aligned");
+    if (m + n > (1LL << 30)) return fail("too many rows");
+    return 0;
+}
+
+// shift (fp16 mean of the first m rows), hi / lo split and row norms of z [N, d]; the two TMA maps over hi / lo
+int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspace& w, CUtensorMap* map_hi,
+                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st) {
+    p.N = N; p.m = m; p.d = d;
+    p.T = (N + 127) / 128;
+    p.units = (p.T + 1) / 2;
+    const size_t rows_pad = (size_t)p.T * 128;
+    const int chunks = (m + fad::kKadColRows - 1) / fad::kKadColRows;
+    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t b_split = al(rows_pad * d * 2), b_norm = al(rows_pad * 4), b_shift = al((size_t)d * 2),
+                 b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8),
+                 b_hist = al(2 * fad::kKadHistBins * 8), b_state = al(sizeof(fad::KadSelectState));
+    if (ensure((void**)&h->kad_buf, &h->kad_cap, 2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state)) return 1;
+    unsigned char* q = h->kad_buf;
+    w.hi = reinterpret_cast<__half*>(q);            q += b_split;
+    w.lo = reinterpret_cast<__half*>(q);            q += b_split;
+    w.norm = reinterpret_cast<float*>(q);           q += b_norm;
+    w.shift = reinterpret_cast<__half*>(q);         q += b_shift;
+    w.colpart = reinterpret_cast<double*>(q);       q += b_col;
+    w.partial = reinterpret_cast<double*>(q);       q += b_part;
+    w.hist = reinterpret_cast<unsigned long long*>(q); q += b_hist;
+    w.state = reinterpret_cast<fad::KadSelectState*>(q);
+    p.norm = w.norm;
+
+    fad::kad_colsum_kernel<<<chunks, 128, 0, st>>>(z, m, d, w.colpart);
+    fad::kad_shift_kernel<<<1, 256, 0, st>>>(w.colpart, chunks, m, d, w.shift);
+    fad::kad_split_kernel<<<(unsigned)((rows_pad * 32 + 255) / 256), 256, 0, st>>>(z, N, (int)rows_pad, d, w.shift,
+                                                                                    w.hi, w.lo, w.norm);
+    CK(cudaGetLastError());
+    h->launches += 3;
+    // rows >= N and columns >= d of a box are zero-filled by the TMA unit (the kernel masks those rows by index)
+    const uint64_t dims[2] = {(uint64_t)d, (uint64_t)N};
+    const uint64_t strides[1] = {(uint64_t)d * 2};
+    const uint32_t box[2] = {64, 128};
+    if (encode_f16_map(map_hi, w.hi, 2, dims, strides, box)) return 1;
+    return encode_f16_map(map_lo, w.lo, 2, dims, strides, box);
+}
+
+template <int MODE>
+int launch_kad_tiles(fad_handle* h, const CUtensorMap& mh, const CUtensorMap& ml, const fad::KadParams& p, cudaStream_t st) {
+    static bool attr_set = false;
+    auto kern = fad::kad_tile_kernel<MODE>;
+    if (!attr_set) {
+        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kKadSmemBytes));
+        attr_set = true;
+    }
+    const int grid = std::min(p.units, h->num_sms);   // the result does not depend on it (fixed work units)
+    kern<<<grid, fad::kKadThreads, fad::kKadSmemBytes, st>>>(mh, ml, p);
+    CK(cudaGetLastError());
+    h->launches++;
+    return 0;
+}
+}  // namespace
+
+extern "C" {
+
+int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream) {
+    if (kad_check(h, x_f16, m, 2, d, out)) return 1;
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::KadParams p = {};
+    if (kad_prepare(h, reinterpret_cast<const __half*>(x_f16), (int)m, (int)m, d, w, &mh, &ml, p, st)) return 1;
+    const unsigned long long pairs = (unsigned long long)m * (unsigned long long)(m - 1) / 2;
+    fad::kad_select_init_kernel<<<1, 1, 0, st>>>(w.state, (pairs - 1) / 2, pairs / 2);
+    CK(cudaGetLastError());
+    h->launches++;
+    // radix digits of the fp32 bit pattern of q >= 0 (bit 31 is 0): 30..20, 19..10, 9..0
+    const int shifts[3] = {20, 10, 0}, bins[3] = {2048, 1024, 1024};
+    const uint32_t masks[3] = {0u, 0xFFF00000u, 0xFFFFFC00u};
+    p.prefix = reinterpret_cast<const uint32_t*>(w.state);     // KadSelectState::prefix is its first member
+    p.hist = w.hist;
+    for (int pass = 0; pass < 3; ++pass) {
+        CK(cudaMemsetAsync(w.hist, 0, 2 * fad::kKadHistBins * 8, st));
+        p.mask = masks[pass]; p.shift = shifts[pass]; p.bins = bins[pass];
+        if (launch_kad_tiles<1>(h, mh, ml, p, st)) return 1;
+        fad::kad_select_kernel<<<1, 32, 0, st>>>(w.state, w.hist, shifts[pass], bins[pass], pass == 2, out);
+        CK(cudaGetLastError());
+        h->launches++;
+    }
+    return 0;
+}
+
+int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
+                 void* stream) {
+    if (kad_check(h, z_f16, m, n, d, out)) return 1;
+    if (!sigma) return fail("null argument");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::KadParams p = {};
+    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n), (int)m, d, w, &mh, &ml, p, st)) return 1;
+    p.sigma = sigma;
+    p.partial = w.partial;
+    if (launch_kad_tiles<0>(h, mh, ml, p, st)) return 1;
+    fad::kad_reduce_kernel<<<1, 32, 0, st>>>(w.partial, p.units, out);
+    CK(cudaGetLastError());
+    h->launches++;
     return 0;
 }
 

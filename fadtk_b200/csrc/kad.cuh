@@ -1,0 +1,347 @@
+// Kernel Audio Distance (KAD): Gaussian-kernel MMD between two embedding sets on Hopper tensor cores (wgmma).
+//
+// Z = [X; Y] (fp16 [N = m + n, d], X first).  Every pair i < j of rows of Z is one of: an xx pair, a yy pair, or an xy
+// pair, each exactly once, so ONE pass over the upper-triangular 128 x 128 tiles of Z Z^T yields
+//   S_xx = sum_{i<j<m} k(z_i, z_j),  S_yy = sum_{m<=i<j} k(z_i, z_j),  S_xy = sum_{i<m<=j} k(z_i, z_j),
+//   k(a, b) = exp(-|a - b|^2 / (2 sigma^2)).
+//
+// Precision.  q = |z_i|^2 + |z_j|^2 - 2 z_i.z_j cancels: rows with a large common offset (Encodec: |mu| ~ 64 per
+// dimension, spread ~ 2) have norms ~1000 x the distances, and an fp32 dot product then leaves ~1e-4 relative error in
+// q.  So a prologue (kad_split_kernel) subtracts a shift s shared by all rows (the fp16-rounded mean of X: the same
+// for the bandwidth and the sums, and distances do not depend on it), and splits y = z - s (exact in fp32) into an
+// fp16 pair hi + lo (22 bits).  The tile kernel issues hi.hi + hi.lo + lo.hi per k-step into one fp32 accumulator
+// (lo.lo is 2^-22 of the result and dropped).  Row norms are the same three terms in fp64, rounded to fp32 once, so an
+// identical pair of rows gives q = 0 up to the accumulator's rounding; q below kQResolution * (|y_i|^2 + |y_j|^2),
+// the resolution of the expanded form, is taken as 0 (exact duplicates have q = 0: silent clips, sigma = 0 detection).
+// The accumulator uses the GEMM's chunk-and-unshrink scheme (conv_gemm.cuh), counting the three products per column.
+//
+// Work units and determinism.  T = ceil(N / 128) tile rows; unit u (u < ceil(T / 2)) is tile row u (tiles u..T-1)
+// followed by tile row T-1-u (tiles T-1-u..T-1): T + 1 tiles per unit, so units are balanced.  A CTA takes units
+// blockIdx.x, + gridDim.x, ...  Each consumer thread sums its elements of a tile in fp32 (fixed order), adds that to
+// fp64 per-thread accumulators in tile order, and at the end of the unit the 256 consumer threads are reduced in a
+// fixed tree into partial[u][3] (fp64).  kad_reduce_kernel sums the partials in unit order.  No floating-point atomic
+// anywhere: the three sums are bitwise reproducible and independent of the grid size and of timing.
+//
+// Bandwidth (MODE 1): exact selection of the two middle q values of the xx triangle by radix passes over the fp32 bit
+// pattern of q (monotone for q >= 0): bits 30..20, 19..10, 9..0.  Each pass runs the same tile loop over X alone and
+// counts the q values whose already-selected high bits match each of the two targets into shared-memory histograms,
+// flushed into 64-bit global counts with integer atomics (order-independent); kad_select_kernel picks the bin of each
+// target.  The q values are bit-for-bit the ones the sums kernel computes for the same rows.
+//
+// Warp roles (384 threads, persistent): warpgroup 0 = TMA producer (one elected lane); warpgroups 1-2 = consumers,
+// consumer c owns tile rows [64 c, 64 c + 64) x 128 columns (one m64n128 accumulator), issues the wgmmas and runs the
+// epilogue (q, ex2 or histogram, masks, class sums) on the accumulator fragment in its registers - no shared-memory
+// round trip of the tile.  Stage = {A_hi, A_lo, B_hi, B_lo} boxes of 128 rows x 64 columns (64 KiB), 3 stages.
+#pragma once
+#include "sm90.cuh"
+#include "conv_gemm.cuh"
+
+namespace fad {
+
+constexpr int kKadThreads = 384;
+constexpr int kKadStages = 3;
+constexpr int kKadConsumerRegs = 232;               // 40 x 128 + 232 x 256 <= 65536
+constexpr uint32_t kKadBox = 128 * 64 * 2;          // one 128-row x 64-column fp16 box (16 KiB)
+constexpr uint32_t kKadStageBytes = 4 * kKadBox;    // A_hi, A_lo, B_hi, B_lo
+constexpr int kKadHistBins = 2048;                  // per target; the largest radix digit has 11 bits
+constexpr uint32_t kKadHistBytes = 2 * kKadHistBins * 4;
+constexpr uint32_t kKadSmemBytes = kKadStages * kKadStageBytes + 1024 /*align slack*/ + 256 /*barriers*/
+                                 + 256 /*unit reduction*/ + kKadHistBytes;
+// q below this fraction of |y_i|^2 + |y_j|^2 is not resolved by the expanded form in fp32 (worst-case accumulator
+// rounding at d = 1024 is ~2e-5 of it) and is taken as 0
+constexpr float kQResolution = 6.103515625e-05f;    // 2^-14
+constexpr int kKadColRows = 4096;                   // rows per partial column sum of the shift prologue
+static_assert(40 * 128 + kKadConsumerRegs * 256 <= 65536, "register file over-subscribed");
+static_assert(kKadSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
+
+struct KadParams {
+    int N;                   // rows of Z (X rows first)
+    int m;                   // rows of X
+    int d;                   // columns
+    int T;                   // tile rows = ceil(N / 128)
+    int units;               // ceil(T / 2)
+    const float* norm;       // [T * 128] |y_i|^2 (zero past N)
+    // MODE 0
+    const double* sigma;     // device scalar
+    double* partial;         // [units][3]
+    // MODE 1
+    const uint32_t* prefix;  // [2] selected high bits of the two targets
+    unsigned long long* hist;// [2][kKadHistBins] global counts
+    uint32_t mask;           // bits already selected
+    int shift, bins;         // digit of this pass: (u >> shift) & (bins - 1)
+};
+
+// --------------------------------------------------------------------------------------------- prologue
+// part[chunk][col] = sum of z[r][col] over the rows of chunk (fp64, fixed order)
+__global__ void kad_colsum_kernel(const __half* __restrict__ z, int m, int d, double* __restrict__ part) {
+    const int r0 = blockIdx.x * kKadColRows;
+    const int r1 = min(m, r0 + kKadColRows);
+    for (int col = threadIdx.x; col < d; col += blockDim.x) {
+        double s = 0.0;
+        for (int r = r0; r < r1; ++r) s += (double)__half2float(z[(size_t)r * d + col]);
+        part[(size_t)blockIdx.x * d + col] = s;
+    }
+}
+// shift = fp16(mean of the first m rows), the partial sums added in chunk order
+__global__ void kad_shift_kernel(const double* __restrict__ part, int chunks, int m, int d, __half* __restrict__ shift) {
+    for (int col = threadIdx.x; col < d; col += blockDim.x) {
+        double s = 0.0;
+        for (int c = 0; c < chunks; ++c) s += part[(size_t)c * d + col];
+        shift[col] = __double2half(s / (double)m);
+    }
+}
+// one warp per row: y = z - shift (exact in fp32), hi = fp16(y), lo = fp16(y - hi); norm = sum hi^2 + 2 hi lo (fp64,
+// fixed lane order, then a fixed shuffle tree), the terms the tile kernel's dot products contain
+__global__ void kad_split_kernel(const __half* __restrict__ z, int N, int rows_pad, int d, const __half* __restrict__ shift,
+                                 __half* __restrict__ hi, __half* __restrict__ lo, float* __restrict__ norm) {
+    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (row >= rows_pad) return;
+    double acc = 0.0;
+    if (row < N) {
+        for (int col = lane; col < d; col += 32) {
+            const size_t e = (size_t)row * d + col;
+            const float y = __half2float(z[e]) - __half2float(shift[col]);
+            const __half h = __float2half_rn(y);
+            const __half l = __float2half_rn(y - __half2float(h));
+            hi[e] = h;
+            lo[e] = l;
+            const double hd = (double)__half2float(h), ld = (double)__half2float(l);
+            acc += hd * hd + 2.0 * hd * ld;
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    if (lane == 0) norm[row] = (float)acc;
+}
+
+// ------------------------------------------------------------------------------------------ tile kernel
+template <int MODE>
+__global__ void __launch_bounds__(kKadThreads, 1)
+kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const KadParams p) {
+    using namespace sm90;
+    static_assert(MODE == 0 || MODE == 1, "0: kernel sums, 1: radix histogram of q");
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
+    uint64_t* empty = full + kKadStages;
+    double* red = reinterpret_cast<double*>(smem + kKadStages * kKadStageBytes + 256);        // [8 warps][3]
+    uint32_t* hist = reinterpret_cast<uint32_t*>(smem + kKadStages * kKadStageBytes + 512);   // [2][kKadHistBins]
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int ksteps = (p.d + 63) / 64;
+    const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
+    const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;
+
+    if (warp == 0 && lane == 0) {
+        tma_prefetch_desc(&map_hi);
+        tma_prefetch_desc(&map_lo);
+        for (int s = 0; s < kKadStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
+        mbar_fence_init();
+    }
+    if (MODE == 1)
+        for (int b = threadIdx.x; b < 2 * kKadHistBins; b += kKadThreads) hist[b] = 0;
+    __syncthreads();
+
+    if (warp < 4) {
+        // ------------------------------------------------------------ TMA producer
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int s = 0; uint32_t ph = 0;
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                for (int half = 0; half < 2; ++half) {
+                    const int r = half == 0 ? u : p.T - 1 - u;
+                    if (half == 1 && r == u) break;                    // odd T: the middle row once
+                    for (int ct = r; ct < p.T; ++ct) {
+                        for (int ks = 0; ks < ksteps; ++ks) {
+                            mbar_wait(&empty[s], ph ^ 1);
+                            uint8_t* st = smem + s * kKadStageBytes;
+                            mbar_expect_tx(&full[s], kKadStageBytes);
+                            tma_load_2d(st, &map_hi, &full[s], ks * 64, r * 128);
+                            tma_load_2d(st + kKadBox, &map_lo, &full[s], ks * 64, r * 128);
+                            tma_load_2d(st + 2 * kKadBox, &map_hi, &full[s], ks * 64, ct * 128);
+                            tma_load_2d(st + 3 * kKadBox, &map_lo, &full[s], ks * 64, ct * 128);
+                            if (++s == kKadStages) { s = 0; ph ^= 1; }
+                        }
+                    }
+                }
+            }
+        }
+    } else {
+        // ------------------------------------------------------------ consumers: wgmma + epilogue in registers
+        setmaxnreg_inc<kKadConsumerRegs>();
+        const int c = (warp >> 2) - 1;                    // tile rows [64 c, 64 c + 64)
+        const int wq = warp & 3;
+        const int ct_id = threadIdx.x - 128;              // 0..255
+        int s = 0; uint32_t ph = 0;
+        float neg_coef = 0.f;
+        uint32_t pfx0 = 0, pfx1 = 0;
+        bool two = false;
+        if (MODE == 0) {
+            const double sg = *p.sigma;
+            neg_coef = (float)(-1.4426950408889634 / (2.0 * sg * sg));
+        } else {
+            pfx0 = p.prefix[0]; pfx1 = p.prefix[1];
+            two = pfx0 != pfx1;
+        }
+        const uint32_t digit_mask = (uint32_t)p.bins - 1;
+
+        for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+            double sxx = 0.0, syy = 0.0, sxy = 0.0;
+            for (int half = 0; half < 2; ++half) {
+                const int r = half == 0 ? u : p.T - 1 - u;
+                if (half == 1 && r == u) break;
+                const int row0 = r * 128 + c * 64 + wq * 16 + (lane >> 2);     // rows row0, row0 + 8
+                const float nr0 = __ldg(p.norm + row0), nr1 = __ldg(p.norm + row0 + 8);
+                for (int ct = r; ct < p.T; ++ct) {
+                    float sum[64], acc[64];
+#pragma unroll
+                    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+                    for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
+                        const int ks1 = min(ks0 + chunk_len, ksteps);
+                        // three products per real column accumulate into each element (zero-filled columns add exact
+                        // zeros, which do not truncate)
+                        const int cols = min(p.d, ks1 * 64) - ks0 * 64;
+                        const float unshrink = kAccumShrinkPerElement * (float)(3 * cols);
+                        int prev_s = -1;
+                        for (int ks = ks0; ks < ks1; ++ks) {
+                            mbar_wait(&full[s], ph);
+                            const uint32_t base = smem_u32(smem + s * kKadStageBytes);
+                            const uint64_t ah = kmajor_sw128_desc(base + c * 64 * 128);
+                            const uint64_t al = kmajor_sw128_desc(base + kKadBox + c * 64 * 128);
+                            const uint64_t bh = kmajor_sw128_desc(base + 2 * kKadBox);
+                            const uint64_t bl = kmajor_sw128_desc(base + 3 * kKadBox);
+                            wgmma_fence();
+#pragma unroll
+                            for (int k = 0; k < 4; ++k) {
+                                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bh + 2 * k, (ks > ks0) || (k > 0));
+                                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bl + 2 * k, 1);
+                                wgmma_m64n128k16_f16<0, 0>(acc, al + 2 * k, bh + 2 * k, 1);
+                            }
+                            wgmma_commit();
+                            wgmma_wait<1>();
+                            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+                            prev_s = s;
+                            if (++s == kKadStages) { s = 0; ph ^= 1; }
+                        }
+                        wgmma_wait<0>();
+                        fence_regs(acc);
+                        __syncwarp();
+                        if (lane == 0) mbar_arrive(&empty[prev_s]);
+#pragma unroll
+                        for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
+                    }
+
+                    // ---- epilogue on the fragment: element (row0 + 8 i, col0 + 8 j + e) is sum[4 j + 2 i + e]
+                    const int col0 = ct * 128 + 2 * (lane & 3);
+                    float sx[2] = {0.f, 0.f}, sy[2] = {0.f, 0.f};
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        const float2 nc = __ldg(reinterpret_cast<const float2*>(p.norm + col0 + 8 * j));
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int gi = row0 + 8 * i, gj = col0 + 8 * j + e;
+                                const float sn = (i ? nr1 : nr0) + (e ? nc.y : nc.x);
+                                float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
+                                q = q > kQResolution * sn ? q : 0.f;           // also clamps q < 0
+                                const bool valid = gj > gi && gj < p.N;        // index masks: j > i, no zero-filled row
+                                if (MODE == 0) {
+                                    float kv;
+                                    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(kv) : "f"(q * neg_coef));
+                                    kv = valid ? kv : 0.f;
+                                    if (gj < p.m) sx[i] += kv; else sy[i] += kv;
+                                } else if (valid) {
+                                    const uint32_t bits = __float_as_uint(q);
+                                    const uint32_t bin = (bits >> p.shift) & digit_mask;
+                                    if ((bits & p.mask) == pfx0) atomicAdd(&hist[bin], 1u);
+                                    else if (two && (bits & p.mask) == pfx1) atomicAdd(&hist[kKadHistBins + bin], 1u);
+                                }
+                            }
+                        }
+                    }
+                    if (MODE == 0) {
+                        // j > i: a row of Y pairs only with rows of Y
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            if (row0 + 8 * i < p.m) { sxx += (double)sx[i]; sxy += (double)sy[i]; }
+                            else syy += (double)sy[i];
+                        }
+                    }
+                }
+            }
+
+            if (MODE == 0) {
+                // fixed tree: lanes (shuffle), then the 8 consumer warps in order
+                for (int o = 16; o > 0; o >>= 1) {
+                    sxx += __shfl_xor_sync(0xffffffffu, sxx, o);
+                    syy += __shfl_xor_sync(0xffffffffu, syy, o);
+                    sxy += __shfl_xor_sync(0xffffffffu, sxy, o);
+                }
+                const int cw = ct_id >> 5;
+                if (lane == 0) { red[cw * 3 + 0] = sxx; red[cw * 3 + 1] = syy; red[cw * 3 + 2] = sxy; }
+                named_bar_sync(1, 256);
+                if (ct_id < 3) {
+                    double t = 0.0;
+                    for (int w = 0; w < 8; ++w) t += red[w * 3 + ct_id];
+                    p.partial[(size_t)u * 3 + ct_id] = t;
+                }
+                named_bar_sync(1, 256);
+            } else {
+                // per unit, so a CTA's 32-bit bins cannot overflow (a unit has (T + 1) x 16384 elements)
+                named_bar_sync(1, 256);
+                for (int b = ct_id; b < 2 * kKadHistBins; b += 256) {
+                    const uint32_t v = hist[b];
+                    if (v) { atomicAdd(p.hist + b, (unsigned long long)v); hist[b] = 0; }
+                }
+                named_bar_sync(1, 256);
+            }
+        }
+    }
+}
+
+// --------------------------------------------------------------------------------------------- epilogues
+// out[t] = sum over units, in unit order, of partial[u][t]
+__global__ void kad_reduce_kernel(const double* __restrict__ partial, int units, double* __restrict__ out) {
+    const int t = threadIdx.x;
+    if (t >= 3) return;
+    double s = 0.0;
+    for (int u = 0; u < units; ++u) s += partial[(size_t)u * 3 + t];
+    out[t] = s;
+}
+
+// state: prefix[2] (u32), then rank[2] (u64) = the rank of each target among the values that match its prefix
+struct KadSelectState {
+    uint32_t prefix[2];
+    unsigned long long rank[2];
+};
+__global__ void kad_select_init_kernel(KadSelectState* st, unsigned long long k0, unsigned long long k1) {
+    st->prefix[0] = st->prefix[1] = 0u;
+    st->rank[0] = k0;
+    st->rank[1] = k1;
+}
+// after a histogram pass: the bin of each target's rank; when both targets still shared a prefix, the pass counted
+// into histogram 0 only.  last: write the two selected q values (fp64) to out.
+__global__ void kad_select_kernel(KadSelectState* st, const unsigned long long* __restrict__ hist, int shift, int bins,
+                                  int last, double* __restrict__ out) {
+    if (threadIdx.x != 0) return;
+    const bool two = st->prefix[0] != st->prefix[1];
+    for (int t = 0; t < 2; ++t) {
+        const unsigned long long* h = hist + (two ? t : 0) * kKadHistBins;
+        unsigned long long r = st->rank[t], below = 0;
+        int b = 0;
+        for (; b < bins - 1; ++b) {
+            if (below + h[b] > r) break;
+            below += h[b];
+        }
+        st->prefix[t] |= (uint32_t)b << shift;
+        st->rank[t] = r - below;
+    }
+    if (last) {
+        out[0] = (double)__uint_as_float(st->prefix[0]);
+        out[1] = (double)__uint_as_float(st->prefix[1]);
+    }
+}
+
+}  // namespace fad

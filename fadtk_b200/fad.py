@@ -3,6 +3,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
 
     calc_embd_statistics      fad.py:42-48   -> shifted E^T E tensor-core kernel (csrc/stats.cuh)
     calc_frechet_distance     fad.py:51-120  -> Newton-Schulz GEMM chain on the PSD form (csrc/frechet.cuh)
+    calc_kernel_audio_distance  (no reference counterpart) -> wgmma pair-tile kernels (csrc/kad.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -72,6 +73,73 @@ class FADInfResults(NamedTuple):
     slope: float
     r2: float
     points: list[tuple[int, float]]
+
+
+class KADResults(NamedTuple):
+    score: float
+    bandwidth: float
+    n_baseline: int
+    n_eval: int
+
+
+def _kad_rows(a, what: str):
+    """fp16 [rows, d] numpy array or torch tensor -> contiguous fp16 torch tensor (not moved to a device yet)."""
+    t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.asarray(a))
+    if t.dtype != torch.float16:
+        raise ValueError(f"KAD needs fp16 embeddings (the cached values); the {what} set is {t.dtype}")
+    if t.ndim != 2:
+        raise ValueError(f"KAD needs [rows, d] embeddings; the {what} set has shape {tuple(t.shape)}")
+    return t
+
+
+def calc_kernel_audio_distance(emb_baseline, emb_eval) -> KADResults:
+    """Kernel Audio Distance (Chung et al., 2025) between two fp16 embedding sets X [m, d] and Y [n, d], with the fp16
+    values taken as exact reals:
+
+        q(a, b) = |a - b|^2,    k(a, b) = exp(-q(a, b) / (2 sigma^2)),
+        sigma   = median of {|x_i - x_j| : i < j} (numpy.median: the mean of the two middle distances when
+                  m (m - 1) / 2 is even) - from the baseline only, so every eval set scored against one baseline
+                  uses the same kernel,
+        MMD^2_u = 2/(m(m-1)) sum_{i<j} k(x_i, x_j) + 2/(n(n-1)) sum_{i<j} k(y_i, y_j) - 2/(mn) sum_{i,j} k(x_i, y_j),
+        KAD     = 1000 * MMD^2_u   (the paper's scaling; unbiased, so it can be slightly negative; not clamped).
+
+    The pair sums and the bandwidth selection run on the GPU (fad_kad_median_sq, fad_kad_sums); MMD^2_u is assembled
+    from the three fp64 sums.  A width that is not a multiple of 8 is zero-padded, which changes no distance.
+    Raises ValueError for fewer than two rows on either side, non-fp16 or non-2-D input, mismatched widths, and
+    sigma = 0 (more than half of the baseline pairs are identical rows)."""
+    x, y = _kad_rows(emb_baseline, "baseline"), _kad_rows(emb_eval, "eval")
+    m, n = int(x.shape[0]), int(y.shape[0])
+    if m < 2 or n < 2:
+        raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {m}, eval {n})")
+    if x.shape[1] != y.shape[1]:
+        raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
+    z = torch.cat([x, y]).contiguous()
+    pad = -z.shape[1] % 8
+    if pad:
+        z = torch.nn.functional.pad(z, (0, pad))
+    from . import _native
+    eng = _native.engine()
+    z = z.to(eng.torch_device)
+    sq = eng.kad_median_sq(z[:m]).cpu().numpy()
+    sigma = 0.5 * (float(np.sqrt(sq[0])) + float(np.sqrt(sq[1])))
+    if not sigma > 0.0:
+        raise ValueError("KAD bandwidth is 0: more than half of the baseline pairs are identical rows")
+    s_xx, s_yy, s_xy = (float(v) for v in eng.kad_sums(z, m, torch.tensor([sigma], dtype=torch.float64,
+                                                                               device=eng.torch_device)).cpu().numpy())
+    mmd2 = 2.0 * s_xx / (m * (m - 1.0)) + 2.0 * s_yy / (n * (n - 1.0)) - 2.0 * s_xy / (float(m) * n)
+    return KADResults(score=1000.0 * mmd2, bandwidth=sigma, n_baseline=m, n_eval=n)
+
+
+def kad_embedding_dir(path, model_name: str) -> Path:
+    """The embedding cache directory <path>/embeddings/<model> that KAD reads; ValueError for statistics files, named
+    statistics sets and anything else that is not a directory (they hold (mu, C), not embeddings)."""
+    named = isinstance(path, str) and _named_statistics(path) is not None
+    if named or str(path).endswith(".npz") or Path(path).is_file():
+        raise ValueError(f"KAD needs embeddings, not (mu, C) statistics: '{path}' is a statistics file or set; "
+                         "pass the audio directory instead")
+    if not Path(path).is_dir():
+        raise ValueError(f"KAD needs a directory of audio or embeddings; '{path}' is not a directory")
+    return Path(path) / "embeddings" / model_name
 
 
 def calc_embd_statistics(embd_lst: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
@@ -375,6 +443,21 @@ class FrechetAudioDistance:
         mu_bg, cov_bg = self.load_stats(baseline)
         mu_eval, cov_eval = self.load_stats(eval)
         return calc_frechet_distance(mu_bg, cov_bg, mu_eval, cov_eval)
+
+    def score_kad(self, baseline_dir: PathLike, eval_dir: PathLike) -> KADResults:
+        """Kernel Audio Distance between the cached embeddings of two directories (calc_kernel_audio_distance): all rows
+        of all <dir>/embeddings/<model>/*.npy in sorted file order, the files the directory statistics read."""
+        from . import _io_native
+        sets = []
+        for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
+            files = _sorted_npy_files(kad_embedding_dir(p, self.ml.name))
+            if not files:
+                raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
+            emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
+            if emb.dtype != np.float16:
+                raise ValueError(f"KAD needs fp16 embedding caches; {p} holds {emb.dtype}")
+            sets.append(emb)
+        return calc_kernel_audio_distance(*sets)
 
     def score_inf(self, baseline: PathLike, eval_files: list[Path], steps: int = 25, min_n=500, raw: bool = False):
         """FAD for growing sample counts and the FAD-inf extrapolation (fad.py:304-351).

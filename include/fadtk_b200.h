@@ -252,6 +252,19 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
                         const void* emb_f16, const long long* offsets, long long n_items, int d, int iters,
                         double* out, void* stream);
 
+/* ---- Kernel Audio Distance (KAD, Chung et al. 2025): the reference has no counterpart (a metric beyond fadtk).
+ * Unbiased MMD^2 between embedding sets X [m, d] and Y [n, d] under k(a, b) = exp(-|a - b|^2 / (2 sigma^2)), sigma =
+ * the median of the pairwise distances of X (DESIGN.md section 5.11).  fp16 rows (the cached embeddings), d a multiple
+ * of 8, m, n >= 2, 16-byte-aligned pointers; otherwise the call fails and launches nothing.  Workspace belongs to the
+ * handle.  Both results are bitwise reproducible (fixed work units, integer histogram counts, no float atomics).
+ *   fad_kad_median_sq  out (device fp64 [2]) = the two middle values of {|x_i - x_j|^2 : i < j} (the same value twice
+ *                      when m (m - 1) / 2 is odd), selected exactly among the fp32 values fad_kad_sums uses
+ *   fad_kad_sums       z = [X; Y] (fp16 [m + n, d], X first), sigma = device fp64 scalar;
+ *                      out (device fp64 [3]) = S_xx (i < j), S_yy (i < j), S_xy (all pairs) of k */
+int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream);
+int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
+                 void* stream);
+
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
  * sinc_interp_kaiser, beta=14.769656459379492) (:151-158), PCM16 quantisation (:160).
