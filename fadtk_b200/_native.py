@@ -75,6 +75,14 @@ SIGNATURES = {
     "fad_resample": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp]),
     "fad_frechet_batched": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_attention": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, C.c_int, c_vp]),
+    "fad_window_attention": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_attention_bias": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "fad_wavlm_gate": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_wavlm_bias_table": (C.c_int, [C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_decoder_self_attention": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_cross_attention": (C.c_int, [c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_layernorm": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                c_vp, c_vp, c_vp]),
     "fad_bench_dmma_peak": (C.c_int, [c_vp, C.c_int, c_vp]),
     "fad_kad_median_sq": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_kad_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp]),
@@ -188,6 +196,51 @@ class Engine:
         out = torch.empty((qkv.shape[0], d), dtype=torch.float16, device=qkv.device)
         _check(lib().fad_attention(self._h, qkv.data_ptr(), n_clips, S, d, out.data_ptr(), int(legacy), _stream()))
         return out
+
+    # Stage entries of the other transformer attention and LayerNorm launches: they write into the caller's cuda
+    # tensors (shapes in include/fadtk_b200.h) and raise NativeError on rejected arguments.
+    def window_attention(self, qkv, n_windows: int, C: int, heads: int, relbias, res: int, shift: int, out):
+        """fad_window_attention: CLAP Swin window attention, qkv fp16 [n_windows * 64, 3 C] -> out fp16 [.., C]"""
+        _check(lib().fad_window_attention(self._h, _ptr(qkv), int(n_windows), int(C), int(heads), _ptr(relbias),
+                                          int(res), int(shift), _ptr(out), _stream()))
+        return out
+
+    def attention_bias(self, qkv, n_clips: int, S: int, d: int, relb, gate, out):
+        """fad_attention_bias: WavLM attention with the gated relative position bias, qkv fp16 [n_clips * S, 3 d]"""
+        _check(lib().fad_attention_bias(self._h, _ptr(qkv), int(n_clips), int(S), int(d), _ptr(relb), _ptr(gate),
+                                        _ptr(out), _stream()))
+        return out
+
+    def wavlm_gate(self, x, w, b, c, rows: int, heads: int, d: int, out):
+        """fad_wavlm_gate: x fp32 [rows, d] -> out fp32 [rows, heads]"""
+        _check(lib().fad_wavlm_gate(self._h, _ptr(x), _ptr(w), _ptr(b), _ptr(c), int(rows), int(heads), int(d),
+                                    _ptr(out), _stream()))
+        return out
+
+    @staticmethod
+    def wavlm_bias_table(rel_embed: np.ndarray, S: int) -> np.ndarray:
+        """rel_embed float32 [320, heads] -> float32 [heads, 2 S - 1], the table fad_w2v_forward uploads (host only)"""
+        emb = np.ascontiguousarray(rel_embed, dtype=np.float32)
+        out = np.empty((emb.shape[1], max(2 * int(S) - 1, 0)), dtype=np.float32)
+        _check(lib().fad_wavlm_bias_table(emb.shape[1], int(S), emb.ctypes.data, out.ctypes.data))
+        return out
+
+    def decoder_self_attention(self, qkv, n_clips: int, d: int, out):
+        """fad_decoder_self_attention: Whisper decoder, qkv fp16 [n_clips * 2, 3 d] -> out fp16 [n_clips * 2, d]"""
+        _check(lib().fad_decoder_self_attention(self._h, _ptr(qkv), int(n_clips), int(d), _ptr(out), _stream()))
+        return out
+
+    def cross_attention(self, q, kv, n_clips: int, S: int, d: int, out):
+        """fad_cross_attention: q fp16 [n_clips * 2, d], kv fp16 [n_clips * S, 2 d] -> out fp16 [n_clips * 2, d]"""
+        _check(lib().fad_cross_attention(self._h, _ptr(q), _ptr(kv), int(n_clips), int(S), int(d), _ptr(out), _stream()))
+        return out
+
+    def layernorm(self, x, gamma, beta, rows: int, C: int, ld_out: int, out16, out32=None, *, res: int = 0,
+                  shift: int = 0, mode: int = 0, gelu: bool = False):
+        """fad_layernorm: x fp32 -> out16 fp16 [rows, ld_out] (and out32 fp32 [rows, width] if given)"""
+        _check(lib().fad_layernorm(self._h, _ptr(x), _ptr(gamma), _ptr(beta), int(rows), int(C), int(ld_out), int(res),
+                                   int(shift), int(mode), int(gelu), _ptr(out16), _ptr(out32), _stream()))
+        return out16
 
     def dmma_peak_tflops(self, iters: int = 0) -> float:
         """measured fp64 tensor-pipe (DMMA) rate, TFLOP/s: roofline denominator of the fp64 kernels"""

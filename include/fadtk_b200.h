@@ -307,6 +307,44 @@ long long fad_launch_count(fad_handle* h);
  * kernel (csrc/whisper.cuh) WavLM runs for its gated relative position bias (here without the bias). */
 int fad_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int S, int d, void* out_f16, int legacy, void* stream);
 
+/* Stage entries (parity tests) of the other attention and LayerNorm launches of the transformer forwards; each calls the
+ * launch code its forward calls and fails, launching nothing, on arguments that launch could not honour.
+ *
+ * fad_window_attention: Swin window attention of a CLAP block.  qkv fp16 [n_windows * 64][3 C] (q | k | v, rows in
+ * shifted-window order: 8x8 windows of res x res images), relbias fp32 [heads][64][64], out fp16 [n_windows * 64][C];
+ * per (window, head): softmax(q k^T / sqrt(C / heads) + relbias (- 100 across shift regions)) v.  C / heads is 24 or 32;
+ * res a power of two >= 8, shift 0 or (res > 8) in (0, 8), n_windows whole images.  16-byte aligned pointers. */
+int fad_window_attention(fad_handle* h, const void* qkv_f16, long long n_windows, int C, int heads, const float* relbias,
+                         int res, int shift, void* out_f16, void* stream);
+/* fad_attention_bias: WavLM self-attention, heads of 64 dims, with the gated relative position bias: score(q, k) =
+ * q.k / 8 + gate[q][head] * relb[head][k - q + S - 1].  qkv fp16 [n_clips * S][3 d], relb fp32 [d / 64][2 S - 1],
+ * gate fp32 [n_clips * S][d / 64], out fp16 [n_clips * S][d]. */
+int fad_attention_bias(fad_handle* h, const void* qkv_f16, long long n_clips, int S, int d, const float* relb,
+                       const float* gate, void* out_f16, void* stream);
+/* fad_wavlm_gate: gate[r][i] = a (b c[i] - 1) + 2 with p = w x[r][64 i : 64 i + 64] + b_lin (w [8][64], b_lin [8]),
+ * a = sigmoid(p0 + .. + p3), b = sigmoid(p4 + .. + p7).  x fp32 [rows][d], d = heads * 64; gate_out fp32 [rows][heads]. */
+int fad_wavlm_gate(fad_handle* h, const float* x, const float* w, const float* b, const float* c, long long rows, int heads,
+                   int d, float* gate_out, void* stream);
+/* fad_wavlm_bias_table (host only): the relb table fad_w2v_forward uploads for S positions, out host [heads][2 S - 1]
+ * from rel_embed host [320][heads] (bucketed key - query distance, 320 buckets, max distance 800). */
+int fad_wavlm_bias_table(int heads, int S, const float* rel_embed, float* out);
+/* fad_decoder_self_attention: Whisper decoder self-attention over the two start tokens of each clip (token 0 attends
+ * to itself, token 1 to both).  qkv fp16 [n_clips * 2][3 d], out fp16 [n_clips * 2][d]. */
+int fad_decoder_self_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int d, void* out_f16, void* stream);
+/* fad_cross_attention: Whisper decoder cross-attention of the two queries of each clip to its S encoder positions.
+ * q fp16 [n_clips * 2][d], kv fp16 [n_clips * S][2 d] (k | v), out fp16 [n_clips * 2][d]; the 2 S fp32 scores of a
+ * (clip, head) must fit in the kernel's shared memory. */
+int fad_cross_attention(fad_handle* h, const void* q_f16, const void* kv_f16, long long n_clips, int S, int d, void* out_f16,
+                        void* stream);
+/* fad_layernorm: one LayerNorm launch (eps 1e-5) as the CLAP / Whisper / wav2vec forwards issue it.  mode 0: output row
+ * o normalises token o (res = 0) or the token of window-ordered row o (res > 0, cyclic shift); mode 1: the 2x2
+ * patch-merge gather of output row o on a res x res grid, features [x(2i,2j), x(2i+1,2j), x(2i,2j+1), x(2i+1,2j+1)].
+ * width = C (mode 0) or 4 C (mode 1) must be one the kernel is built for; gelu != 0 applies exact-erf GELU after the
+ * affine.  out fp16 [rows][ld_out], columns width .. ld_out - 1 set to zero; out_f32 optional fp32 [rows][width], which
+ * may be x itself only in mode 0 with res = 0. */
+int fad_layernorm(fad_handle* h, const float* x, const float* gamma, const float* beta, long long rows, int C, int ld_out,
+                  int res, int shift, int mode, int gelu, void* out_f16, float* out_f32, void* stream);
+
 /* ---- measurement utility -------------------------------------------------------------
  * fp64 tensor-pipe (DMMA m8n8k4) rate of this GPU in TFLOP/s, measured with a register-only
  * issue loop: the roofline denominator of the exact-Gram and Newton-Schulz kernels, which

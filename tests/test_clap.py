@@ -64,6 +64,26 @@ def test_packing_shapes_and_padding():
     assert "clap-laion-audio" in names
 
 
+@pytest.mark.parametrize("variant", ["tiny", "base"])
+def test_packed_relbias_is_the_oracle_gather(variant):
+    """Every block's packed relbias [heads][64][64] is relative_position_bias_table[_rel_pos_index] of the oracle
+    (pinned to transformers by test_clap_oracle.py), query row first, bit for bit."""
+    sd = weights_clap.synthetic_clap_state(3, variant)
+    pk = weights_clap.pack_clap(sd)
+    _, depths = weights_clap.VARIANTS[variant]
+    idx = co._rel_pos_index()
+    blk = 0
+    for i, (depth, heads) in enumerate(zip(depths, weights_clap.HEADS)):
+        for j in range(depth):
+            table = sd[f"layers.{i}.blocks.{j}.attention.self.relative_position_bias_table"]
+            want = torch.stack([table[idx, hh] for hh in range(heads)])
+            got = pk[6 + 13 * blk + 4]
+            assert got.shape == (heads, 64, 64) and got.dtype == torch.float32
+            assert torch.equal(got, want), f"stage {i} block {j}"
+            blk += 1
+    assert blk == sum(depths)
+
+
 def _clips():
     return [synth.musiclike_clip(2, 10.0, 48000), synth.musiclike_clip(5, 2.5, 48000, baseline=True)]
 

@@ -38,6 +38,25 @@ def test_packing_and_registry():
     assert _native.Engine.w2v_frames(160000) == 499 and _native.Engine.w2v_frames(240000) == 749
 
 
+@pytest.mark.parametrize("heads", [12, 16])
+@pytest.mark.parametrize("S", [49, 149, 499, 1499])
+def test_wavlm_bias_table_matches_transformers(S, heads):
+    """The position-bias table fad_w2v_forward uploads (fad_wavlm_bias_table) equals WavLMAttention.compute_bias
+    (transformers' _relative_positions_bucket + rel_attn_embed gather) at every (head, query, key), bit for bit.
+    S = 1499 (30-s clips) reaches distances far past the 800 buckets' max_distance."""
+    from transformers.models.wavlm.modeling_wavlm import WavLMAttention
+    from fadtk_b200 import _native
+    torch.manual_seed(S + heads)
+    att = WavLMAttention(heads * 64, heads, num_buckets=320, max_distance=800)
+    with torch.no_grad():
+        att.rel_attn_embed.weight.copy_(torch.randn(320, heads))
+        want = att.compute_bias(S, S)                                        # [heads, S (query), S (key)]
+    got = torch.from_numpy(_native.Engine.wavlm_bias_table(att.rel_attn_embed.weight.detach().numpy(), S))
+    assert got.shape == (heads, 2 * S - 1)
+    dist = torch.arange(S)[None, :] - torch.arange(S)[:, None]               # key - query
+    assert torch.equal(got[:, dist + S - 1], want)
+
+
 def test_oracle_is_the_reference_dependency():
     sd = ww.synthetic_w2v_state(0, layers=2)
     model, fe = wo.build(sd, "hubert")
