@@ -69,6 +69,8 @@ SIGNATURES = {
     "fad_w2v_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_encodec_load": (C.c_int, [c_vp, c_vp, C.c_int, c_ll, C.c_int]),
     "fad_encodec_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_encodec_conv": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_encodec_lstm": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_resample_geometry": (C.c_int, [C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "fad_resample_length": (c_ll, [C.c_int, C.c_int, c_ll]),
     "fad_resample_bank": (C.c_int, [C.c_int, C.c_int, c_vp]),
@@ -467,6 +469,19 @@ class Engine:
             frames = -(-frames // r)
         out = torch.empty((n, frames, 128), dtype=torch.float16, device=pcm.device)
         _check(lib().fad_encodec_forward(self._h, pcm.data_ptr(), n, T, out.data_ptr(), _stream()))
+        return out
+
+    # Stage entries of the loaded encoder: they write into the caller's cuda tensors (shapes in include/fadtk_b200.h)
+    # and raise NativeError on rejected arguments.
+    def encodec_conv(self, layer: int, x, B: int, T_in: int, out, *, elu_in: bool = False, groupnorm: bool = False):
+        """fad_encodec_conv: conv `layer` (load order), x fp32 [B, T_in, Cin] -> out fp32 [B, ceil(T_in / stride), Cout]"""
+        _check(lib().fad_encodec_conv(self._h, int(layer), _ptr(x), int(B), int(T_in), int(elu_in), int(groupnorm),
+                                      _ptr(out), _stream()))
+        return out
+
+    def encodec_lstm(self, z, n_clips: int, TF: int, out):
+        """fad_encodec_lstm: z fp32 [n_clips, TF, 512] -> out fp32 [n_clips, TF, 512] = LSTM(z) + z"""
+        _check(lib().fad_encodec_lstm(self._h, _ptr(z), int(n_clips), int(TF), _ptr(out), _stream()))
         return out
 
     # -------------------------------------------------------------- audio conversion

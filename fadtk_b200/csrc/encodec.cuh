@@ -61,12 +61,21 @@ groupnorm1_apply_kernel(float* __restrict__ x, const float* __restrict__ stats, 
 // a[(b*T_out + t)][tap*C + c] = act(x[b][t*stride + tap - pad_left][c]).  Encodec's causal SConv1d pads
 // pad_left = k - stride samples on the left and completes the last window on the right, both by reflection;
 // a "valid" convolution (wav2vec2 feature encoder) passes pad_left = 0 and never leaves the signal.
+// Encodec's pad1d reflects an input no longer than its padding (T_in <= max(pad_left, pad_right)) as if it had
+// been extended with zeros to max_pad + 1 samples: the reflection runs over that length and taps past T_in read 0.
+// kShort selects that case (enc_im2col decides per launch), so the loop of every longer input stays as it was.
 // x: fp32 [B][T_in][C]; a: fp16 [B*T_out][Kpad] (columns >= k*C are zero).  One thread per 8 columns.
+template <bool kShort>
 __global__ void __launch_bounds__(256)
 encodec_im2col_kernel(const float* __restrict__ x, int T_in, int C, int k, int stride, int pad_left, int elu, int T_out, int Kpad,
                       long long n_rows, __half* __restrict__ a)
 {
     const int vecs = Kpad / 8, KC = k * C;
+    int L = T_in;                                                   // length the reflection runs over
+    if (kShort) {
+        const int pad_right = (T_out - 1) * stride + k - pad_left - T_in;
+        L = (pad_left > pad_right ? pad_left : pad_right) + 1;
+    }
     for (long long e = blockIdx.x * 256LL + threadIdx.x; e < n_rows * vecs; e += (long long)gridDim.x * 256) {
         const long long row = e / vecs;
         const int col0 = (int)(e - row * vecs) * 8;
@@ -78,10 +87,15 @@ encodec_im2col_kernel(const float* __restrict__ x, int T_in, int C, int k, int s
             const int tap = col0 / C, c = col0 - tap * C;
             int i = t * stride + tap - pad_left;
             if (i < 0) i = -i;
-            if (i >= T_in) i = 2 * (T_in - 1) - i;
-            const float4 p = *reinterpret_cast<const float4*>(xb + (long long)i * C + c);
-            const float4 q = *reinterpret_cast<const float4*>(xb + (long long)i * C + c + 4);
-            v[0] = p.x; v[1] = p.y; v[2] = p.z; v[3] = p.w; v[4] = q.x; v[5] = q.y; v[6] = q.z; v[7] = q.w;
+            if (i >= L) i = 2 * (L - 1) - i;
+            if (!kShort || i < T_in) {
+                const float4 p = *reinterpret_cast<const float4*>(xb + (long long)i * C + c);
+                const float4 q = *reinterpret_cast<const float4*>(xb + (long long)i * C + c + 4);
+                v[0] = p.x; v[1] = p.y; v[2] = p.z; v[3] = p.w; v[4] = q.x; v[5] = q.y; v[6] = q.z; v[7] = q.w;
+            } else {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[j] = 0.f;
+            }
         } else {
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
@@ -91,8 +105,8 @@ encodec_im2col_kernel(const float* __restrict__ x, int T_in, int C, int k, int s
                     const int tap = col / C, c = col - tap * C;
                     int i = t * stride + tap - pad_left;
                     if (i < 0) i = -i;
-                    if (i >= T_in) i = 2 * (T_in - 1) - i;
-                    val = xb[(long long)i * C + c];
+                    if (i >= L) i = 2 * (L - 1) - i;
+                    if (!kShort || i < T_in) val = xb[(long long)i * C + c];
                 }
                 v[j] = val;
             }

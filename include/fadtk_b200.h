@@ -162,6 +162,17 @@ int fad_encodec_load(fad_handle* h, const void* const* tensors_host, int n_tenso
 /* pcm: int16 mono 24 kHz [n_clips][T] (device), all clips of one call have the same length T.
  * emb_out: fp16 [n_clips][ceil(T/320)][128] (device). */
 int fad_encodec_forward(fad_handle* h, const int16_t* pcm, long long n_clips, int T, void* emb_out_f16, void* stream);
+/* Stage entries (parity tests) of the loaded encoder; each calls the launch code fad_encodec_forward calls and fails,
+ * launching nothing, on arguments it could not honour.  16-byte aligned device pointers.
+ * fad_encodec_conv: conv `layer` in the order of the load (0 input conv; 1 + 4 s, 2 + 4 s, 3 + 4 s, 4 + 4 s the k = 3
+ * conv, k = 1 conv, shortcut and down conv of stage s; 17 the last conv) with the variant's padding.  x fp32
+ * [B][T_in][Cin] (ELU applied to it first if elu_in) -> out fp32 [B][ceil(T_in / stride)][Cout]; groupnorm != 0 (48 kHz
+ * model only) applies the GroupNorm(1, Cout) that follows the conv.  B in [1, 4096], B * T_in <= max_chunk_samples.
+ * fad_encodec_lstm: z fp32 [n_clips][TF][512] -> out fp32 [n_clips][TF][512] = LSTM(z) + z (two layers), in groups of
+ * 512 clips; TF at most the frames of max_chunk_samples. */
+int fad_encodec_conv(fad_handle* h, int layer, const float* x_f32, long long B, int T_in, int elu_in, int groupnorm,
+                     float* out_f32, void* stream);
+int fad_encodec_lstm(fad_handle* h, const float* z_f32, long long n_clips, int TF, float* out_f32, void* stream);
 
 /* ---- wav2vec 2.0 / HuBERT / MERT: replaces W2V2Model, HuBERTModel, MERTModel load_model / _get_embedding
  * (fadtk/model_loader.py:254-288, 525-596) for the "group-norm feature encoder + post-LN transformer" checkpoints

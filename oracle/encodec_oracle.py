@@ -6,6 +6,8 @@ The ``encodec`` package (0.1.1, uv.lock) is not installed here; this restates it
 reflect-padded weight-normalised convs, ELU, residual blocks with conv shortcut, 2-layer LSTM with skip) and
 tests/test_encodec_oracle.py pins it to transformers' independent port (EncodecModel.encoder) with shared
 random weights.  Parity against the real facebook checkpoint is unpinned (no weights offline).
+``conv_layer`` and ``lstm`` run one stage of the encoder (float64 by default) for the GPU stage tests
+(tests/test_gpu_encodec_stages.py); ``encoder`` is built from them and takes a dtype too.
 """
 from __future__ import annotations
 
@@ -56,7 +58,7 @@ def _sconv(x, w, b, stride, causal=True):
     else:
         right = pad_total // 2
         x = _reflect_pad(x, pad_total - right, right + extra)
-    return F.conv1d(x, w, b, stride=stride)
+    return F.conv1d(x, w.to(x.dtype), b.to(x.dtype), stride=stride)
 
 
 def _reflect_pad(x, left, right):
@@ -70,33 +72,69 @@ def _reflect_pad(x, left, right):
     return y[..., : y.shape[-1] - extra] if extra else y
 
 
+def conv_layers(sd: dict) -> list:
+    """(state-dict prefix, stride) of every conv in the order the product loads them (weights_encodec.pack_encodec):
+    the input conv, per stage the residual block's k = 3 conv, k = 1 conv and shortcut and the down conv, the last conv"""
+    out = []
+    for idx, kind, cin, cout, k, s in conv_table():
+        if kind == "res":
+            out += [(f"layers.{idx}.block.1", 1), (f"layers.{idx}.block.3", 1), (f"layers.{idx}.shortcut", 1)]
+        else:
+            out.append((f"layers.{idx}", s))
+    return out
+
+
+def is_causal(sd: dict) -> bool:
+    return "layers.0.conv.weight" not in sd                    # 48 kHz: non-causal + GroupNorm(1, C) after every conv
+
+
 @torch.no_grad()
-def encoder(x: torch.Tensor, sd: dict) -> torch.Tensor:
-    """[B, 1, T] float32 -> [B, 128, ceil(T / 320)]"""
-    causal = "layers.0.conv.weight" not in sd                  # 48 kHz: non-causal + GroupNorm(1, C) after every conv
+def conv_layer(x: torch.Tensor, sd: dict, layer: int, elu_in: bool = False, groupnorm: bool = True,
+               dtype=torch.float64) -> torch.Tensor:
+    """conv `layer` of conv_layers(sd) on x [B, Cin, T] in `dtype`: ELU first if elu_in, then the padded conv and
+    (48 kHz model, if groupnorm) its GroupNorm(1, Cout)"""
+    prefix, stride = conv_layers(sd)[layer]
+    x = x.to(dtype)
+    if elu_in:
+        x = F.elu(x)
+    y = _sconv(x, effective_weight(sd, prefix).to(dtype), sd[prefix + ".conv.bias"], stride, is_causal(sd))
+    if groupnorm and prefix + ".norm.weight" in sd:
+        y = F.group_norm(y, 1, sd[prefix + ".norm.weight"].to(dtype), sd[prefix + ".norm.bias"].to(dtype), eps=1e-5)
+    return y
 
-    def conv(t, p, s=1):
-        y = _sconv(t, effective_weight(sd, p), sd[p + ".conv.bias"], s, causal)
-        if p + ".norm.weight" in sd:
-            y = F.group_norm(y, 1, sd[p + ".norm.weight"], sd[p + ".norm.bias"], eps=1e-5)
-        return y
 
+@torch.no_grad()
+def lstm(z: torch.Tensor, sd: dict, dtype=torch.float64) -> torch.Tensor:
+    """The encoder's two LSTM layers with the skip: z [B, T, 512] -> LSTM(z) + z in `dtype`"""
+    seq = z.to(dtype).transpose(0, 1)                          # [T, B, 512]
+    hsz = seq.shape[-1]
+    m = torch.nn.LSTM(hsz, hsz, LSTM_LAYERS)
+    m.load_state_dict({k_.split("lstm.")[1]: v for k_, v in sd.items() if ".lstm." in k_})
+    m = m.to(device=seq.device, dtype=dtype)
+    return (m(seq)[0] + seq).transpose(0, 1)
+
+
+@torch.no_grad()
+def encoder(x: torch.Tensor, sd: dict, dtype=torch.float32) -> torch.Tensor:
+    """[B, 1, T] (48 kHz: [B, 2, T]) -> [B, 128, ceil(T / 320)] in `dtype`"""
+    layer = iter(range(len(conv_layers(sd))))
+
+    def conv(t, elu_in=False):
+        return conv_layer(t, sd, next(layer), elu_in, True, dtype)
+
+    x = x.to(dtype)
     for idx, kind, cin, cout, k, s in conv_table():
         if kind == "in":
-            x = conv(x, f"layers.{idx}")
+            x = conv(x)
         elif kind == "res":
-            h = conv(F.elu(x), f"layers.{idx}.block.1")
-            h = conv(F.elu(h), f"layers.{idx}.block.3")
-            x = conv(x, f"layers.{idx}.shortcut") + h
+            h = conv(x, True)
+            h = conv(h, True)
+            x = conv(x) + h
         elif kind == "down":
-            x = conv(F.elu(x), f"layers.{idx}", s)
+            x = conv(x, True)
         else:                                                  # LSTM with skip, ELU, last conv
-            seq = x.permute(2, 0, 1)
-            hsz = seq.shape[-1]
-            lstm = torch.nn.LSTM(hsz, hsz, LSTM_LAYERS)
-            lstm.load_state_dict({k_.split("lstm.")[1]: v for k_, v in sd.items() if ".lstm." in k_})
-            y = lstm(seq)[0] + seq
-            x = conv(F.elu(y.permute(1, 2, 0)), f"layers.{idx}")
+            y = lstm(x.transpose(1, 2), sd, dtype)
+            x = conv(y.transpose(1, 2), True)
     return x
 
 

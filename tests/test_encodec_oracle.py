@@ -8,8 +8,14 @@ from fadtk_b200 import weights_encodec as we
 from oracle import encodec_oracle as eo
 
 
-@pytest.mark.parametrize("variant,length", [("24k", 24000), ("24k", 24000 * 3 + 137), ("24k", 500), ("48k", 48000), ("48k", 31337)])
+SHORT = [("24k", 1), ("24k", 100), ("24k", 1919), ("24k", 1920), ("48k", 5), ("48k", 960)]
+
+
+@pytest.mark.parametrize("variant,length", [("24k", 24000), ("24k", 24000 * 3 + 137), ("24k", 500), ("48k", 48000), ("48k", 31337)]
+                         + SHORT)
 def test_encoder_matches_independent_hf_port(variant, length):
+    """Lengths up to 1920 (24 kHz) and 960 (48 kHz) samples reach a conv whose input is no longer than its padding,
+    where Encodec's pad1d extends the input with zeros before it reflects."""
     tr = pytest.importorskip("transformers")
     sd = we.synthetic_encodec_state(3, variant)
     if variant == "24k":
@@ -28,6 +34,9 @@ def test_encoder_matches_independent_hf_port(variant, length):
     got = eo.encoder(x, sd)
     assert got.shape == want.shape == (2, 128, -(-length // 320))
     assert torch.allclose(got, want, atol=2e-5 * want.abs().max().item() + 1e-6), (got - want).abs().max()
+    got64 = eo.encoder(x, sd, torch.float64)                   # the float64 mode the GPU stage tests compare with
+    assert got64.dtype == torch.float64
+    assert torch.allclose(got64, want.double(), atol=2e-5 * want.abs().max().item() + 1e-6), (got64 - want).abs().max()
 
 
 def test_embed_shape_and_packing():
