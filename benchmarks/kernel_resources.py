@@ -19,7 +19,7 @@ for line in txt.splitlines():
 names = subprocess.run(["c++filt"] + [r[0] for r in rows], capture_output=True, text=True).stdout.splitlines()
 print("# Kernel resource audit (`cuobjdump -res-usage fadtk_b200/csrc/libfadtk_b200.so`, sm_90a)\n")
 print("Registers per thread, stack bytes (spills / local arrays), static shared memory; dynamic shared memory (conv_gemm,")
-print("attention_wgmma, logmel) is set at launch.  The fp64 tensor-pipe kernels (`dgemm_kernel`, `dgemm_strided_kernel`,")
+print("attention_wgmma, logmel) is set at launch.  The fp64 tensor-pipe kernels (`dgemm_strided_kernel`,")
 print("`stats_dmma_kernel<__half | double>`, `song_stats_dmma_kernel`) stay at <= 128 registers for two CTAs per SM.\n")
 print("| kernel | registers | stack bytes | static smem |\n|---|---|---|---|")
 for (m, r, st, sh), n in sorted(zip(rows, names), key=lambda t: t[1]):

@@ -18,7 +18,6 @@
 #include "frontend.cuh"
 #include "stats.cuh"
 #include "frechet.cuh"
-#include "frechet_batched.cuh"
 #include "clap.cuh"
 #include "resample.cuh"
 #include "whisper.cuh"
@@ -139,16 +138,11 @@ struct fad_handle {
     __half* gather_buf = nullptr;
     size_t gather_cap = 0;
 
-    // Frechet workspace (fp64 d x d matrices)
-    double* fr_buf = nullptr;
-    size_t fr_cap = 0;
-    unsigned char* frb_buf = nullptr;   // fad_frechet_batched workspace
-    size_t frb_cap = 0;
+    unsigned char* fr_buf = nullptr;  size_t fr_cap = 0;        // Frechet workspace (FrechetWorkspace)
     float* rs_bank = nullptr;  size_t rs_bank_cap = 0;  int rs_in = 0, rs_out = 0;     // resampler filter bank
     float* rs_mono = nullptr;  size_t rs_mono_cap = 0;
     unsigned char* kad_buf = nullptr;  size_t kad_cap = 0;      // fad_kad_* workspace (KadWorkspace)
     std::set<const void*> zero_lo;           // hi/lo weight tensors whose lo parts are all zero (note_split_weights)
-    double* fr_scal = nullptr;   // 32 doubles
 
     void* nccl_comm = nullptr;   // ncclComm_t created by fad_comm_init (NCCL is dlopen'ed, never linked)
 
@@ -456,7 +450,6 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(cudaMalloc(&h->d_melw, melw.size() * 8)); CK(cudaMemcpy(h->d_melw, melw.data(), melw.size() * 8, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&h->d_mel_start, ms.size() * 4)); CK(cudaMemcpy(h->d_mel_start, ms.data(), ms.size() * 4, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&h->d_mel_count, mc.size() * 4)); CK(cudaMemcpy(h->d_mel_count, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&h->fr_scal, 32 * sizeof(double)));
     CK(cudaFuncSetAttribute(fad::logmel_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)fad::logmel_smem_bytes<double>()));
     CK(cudaFuncSetAttribute(fad::logmel_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -479,7 +472,7 @@ int fad_destroy(fad_handle* h) {
     encodec_free_state(h->encodec_state);
     w2v_free_state(h->w2v_state);
     void* ptrs[] = {h->d_twiddle, h->d_hann, h->d_melw, h->d_mel_start, h->d_mel_count, h->conv1_w, h->conv1_b,
-                    h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->fr_scal, h->frb_buf, h->rs_bank, h->rs_mono,
+                    h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->rs_bank, h->rs_mono,
                     h->kad_buf};
     for (void* p : ptrs) if (p) cudaFree(p);
     for (int i = 0; i < 5; ++i) { if (h->conv_w[i]) cudaFree(h->conv_w[i]); if (h->conv_b[i]) cudaFree(h->conv_b[i]); }
@@ -735,27 +728,6 @@ int fad_stats_finalize(fad_handle* h, const double* acc, const void* shift_f16, 
     return 0;
 }
 
-// ------------------------------------------------------------------- fp64 tensor-pipe peak
-// Roofline denominator of the DMMA kernels (exact Gram, Newton-Schulz): MEASURED_PEAKS.json only
-// carries the bf16 GEMM and HBM copy rates, so the fp64 tensor-pipe rate is measured here - every warp
-// of a full grid issues independent m8n8k4 DMMAs from registers, nothing else.
-namespace {
-__global__ void __launch_bounds__(256) dmma_peak_kernel(int iters, double* sink) {
-    double c[8][2];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { c[i][0] = threadIdx.x; c[i][1] = -1.0 * threadIdx.x; }
-    const double a = 1.0 + 1e-9 * threadIdx.x, b = 1.0 - 1e-9 * threadIdx.x;
-    for (int it = 0; it < iters; ++it) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i) fad::dmma_884(c[i][0], c[i][1], a, b);
-    }
-    double s = 0.0;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
-    if (s == 12345.678) sink[0] = s;                       // keeps the chain alive, never true
-}
-}  // namespace
-
 // Stage entry (parity test): encoder self-attention of n_clips sequences of S positions, heads of 64 dims.
 // qkv fp16 [n_clips * S][3 d] (q | k | v), out fp16 [n_clips * S][d]; legacy != 0 runs the mma.sync kernel instead.
 extern "C" int fad_attention(fad_handle* h, const void* qkv_f16, long long n_clips, int S, int d, void* out_f16, int legacy, void* stream) {
@@ -771,28 +743,6 @@ extern "C" int fad_attention(fad_handle* h, const void* qkv_f16, long long n_cli
     return 0;
 }
 
-
-extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_host) {
-    if (!h || !tflops_out_host) return fail("null argument");
-    CK(cudaSetDevice(h->device));
-    if (iters <= 0) iters = 20000;
-    double* sink = h->fr_scal + 30;
-    cudaEvent_t e0, e1;
-    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
-    const int blocks = h->num_sms * 4;
-    dmma_peak_kernel<<<blocks, 256>>>(iters / 10, sink);            // warm-up
-    CK(cudaEventRecord(e0));
-    dmma_peak_kernel<<<blocks, 256>>>(iters, sink);
-    CK(cudaEventRecord(e1));
-    CK(cudaEventSynchronize(e1));
-    float ms = 0.f;
-    CK(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-    const double flop = (double)blocks * 8 /*warps*/ * (double)iters * 8 /*DMMAs*/ * 512.0;
-    *tflops_out_host = flop / (ms * 1e-3) / 1e12;
-    h->launches += 2;
-    return 0;
-}
 
 // ------------------------------------------------------------------- cross-GPU statistics merge
 // The one exchange step of the path (SURVEY.md section 8 (e)): all-reduce(sum) of the packed fp64 accumulator over
@@ -889,61 +839,112 @@ int fad_stats_allreduce(fad_handle* h, void* nccl_comm_or_null, double* acc, int
 
 // ----------------------------------------------------------------------------- Frechet
 namespace {
-int launch_dgemm2(fad_handle* h, const fad::DgemmBatch& batch, int nprob, int d, cudaStream_t st) {
-    dim3 grid((d + fad::kDgTileN - 1) / fad::kDgTileN, (d + fad::kDgTileM - 1) / fad::kDgTileM, nprob);
-    fad::dgemm_kernel<<<grid, 256, 0, st>>>(batch, d);
+// carve-outs of h->fr_buf for a group of G items of d x d problems
+struct FrechetWorkspace {
+    double *cov, *P, *M, *Y, *Z, *W, *Yn, *Zn;  // [G][d][d] each
+    double* mu;                                // [G][d]
+    double *scalC, *scalM;                     // [G][2]: {|A|_F, tr A} of C2_z and of M_z
+    float* flags;                              // [G][3]: rotating max |W - I| slots of the chain
+    int* ok;                                   // [G]: item has >= 2 rows
+    double* sqrt1;                             // [d][d]: fad_frechet's C1^(1/2)
+    double* scal1;                             // [2]: fad_frechet's {|C1|_F, tr C1}
+    double* resid;                             // [1]: |Y Y - Mn|_F^2 of one item
+    double* sink;                              // [1]: keeps dmma_peak_kernel's result alive
+};
+
+int frechet_workspace(fad_handle* h, long long G, int d, FrechetWorkspace& w) {
+    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t total = (size_t)d * d;
+    const size_t b_mat = al(G * total * 8), b_mu = al(G * d * 8), b_scal = al(G * 2 * 8), b_flags = al(G * 3 * 4),
+                 b_ok = al(G * 4), b_sqrt = al(total * 8), b_misc = al(4 * 8);
+    if (ensure((void**)&h->fr_buf, &h->fr_cap, 8 * b_mat + b_mu + 2 * b_scal + b_flags + b_ok + b_sqrt + b_misc)) return 1;
+    unsigned char* q = h->fr_buf;
+    for (double** m : {&w.cov, &w.P, &w.M, &w.Y, &w.Z, &w.W, &w.Yn, &w.Zn}) { *m = reinterpret_cast<double*>(q); q += b_mat; }
+    w.mu = reinterpret_cast<double*>(q);        q += b_mu;
+    w.scalC = reinterpret_cast<double*>(q);     q += b_scal;
+    w.scalM = reinterpret_cast<double*>(q);     q += b_scal;
+    w.flags = reinterpret_cast<float*>(q);      q += b_flags;
+    w.ok = reinterpret_cast<int*>(q);           q += b_ok;
+    w.sqrt1 = reinterpret_cast<double*>(q);     q += b_sqrt;
+    w.scal1 = reinterpret_cast<double*>(q);
+    w.resid = w.scal1 + 2;
+    w.sink = w.scal1 + 3;
+    return 0;
+}
+
+// grid of the elementwise d x d kernels: one item spreads over the whole GPU
+unsigned elem_blocks(const fad_handle* h, int d) {
+    const size_t b = ((size_t)d * d + 255) / 256;
+    return (unsigned)std::min(b, (size_t)h->num_sms * 8);
+}
+
+int launch_dgemm(fad_handle* h, const fad::DgemmStrided& p, int families, int d, cudaStream_t st) {
+    dim3 grid((d + fad::kDgTileN - 1) / fad::kDgTileN, (d + fad::kDgTileM - 1) / fad::kDgTileM, (unsigned)(p.items * families));
+    fad::dgemm_strided_kernel<<<grid, 256, 0, st>>>(p, d);
     CK(cudaGetLastError());
     h->launches++;
     return 0;
 }
-int launch_dgemm(fad_handle* h, const double* A, const double* B, double* C, int d, double alpha,
-                 double beta_diag, double* trace, cudaStream_t st) {
-    fad::DgemmBatch batch = {};
-    batch.p[0] = {A, B, C, alpha, beta_diag, trace};
-    batch.p[1] = batch.p[0];
-    return launch_dgemm2(h, batch, 1, d, st);
-}
 
-// Coupled Newton-Schulz: on return Y ~ sqrt(sym(A)/|A|_F + delta I), Z its inverse;
-// scal[0..1] = |A|_F, tr A; trY / trZ = traces of the converged iterates.
-int newton_schulz(fad_handle* h, const double* A, int d, int iters, double* Y, double* Z, double* W,
-                  double* T, double* scal, double* trY, double* trZ, float* dev /*3 floats*/, cudaStream_t st) {
-    const size_t total = (size_t)d * d;
-    unsigned eb = (unsigned)((total + 255) / 256);
-    if (eb > (unsigned)h->num_sms * 8) eb = h->num_sms * 8;
-    static const float dev_init[3] = {0.0f, 0.0f, 1.0e30f};            // slot (k-1)%3 for k = 0 is slot 2
-    CK(cudaMemcpyAsync(dev, dev_init, sizeof dev_init, cudaMemcpyHostToDevice, st));
-    fad::norm_trace_kernel<<<1, 1024, 0, st>>>(A, d, scal);
-    fad::ns_init_kernel<<<eb, 256, 0, st>>>(A, d, scal, Y, Z);
+// Coupled Newton-Schulz on the g matrices A_z: on return w.Y_z ~ sqrt(sym(A_z)/|A_z|_F + delta I), w.Z_z its
+// inverse, scal[z] = {|A_z|_F, tr A_z}.
+int newton_schulz(fad_handle* h, const FrechetWorkspace& w, const double* A, double* scal, int g, int d, int iters,
+                  cudaStream_t st) {
+    fad::norm_trace_kernel<<<g, 1024, 0, st>>>(A, d, scal);
+    fad::ns_init_kernel<<<dim3(elem_blocks(h, d), g), 256, 0, st>>>(A, d, scal, w.Y, w.Z, w.flags);
     CK(cudaGetLastError());
     h->launches += 2;
-    // (Y, Z) <-> (T, T+total) ping-pong on a fixed host schedule; an even iteration count lands the
-    // last scheduled update in (Y, Z).  If the device stops early (dev < tol) the two pairs differ by
+    // (Y, Z) <-> (Yn, Zn) ping-pong on a fixed host schedule; an even iteration count lands the
+    // last scheduled update in (Y, Z).  If an item stops early (dev < tol) the two pairs differ by
     // one factor W with |W - I| < tol, i.e. by < 1e-12 relative - either is the converged iterate.
     if (iters & 1) ++iters;
-    double* Yc = Y; double* Zc = Z; double* Yn = T; double* Zn = T + total;
-    const float tol = 1e-12f;
+    const long long T = (long long)d * d;
+    double *Yc = w.Y, *Zc = w.Z, *Yx = w.Yn, *Zx = w.Zn;
     for (int it = 0; it < iters; ++it) {
-        float* d_prev = dev + (it + 2) % 3;       // max |W - I| of iteration it-1
-        float* d_cur = dev + it % 3;
-        float* d_next = dev + (it + 1) % 3;
-        fad::DgemmBatch wb = {};
-        wb.p[0] = {Zc, Yc, W, -0.5, 1.5, nullptr};                               // W = 1.5 I - 0.5 Z Y
-        wb.p[1] = wb.p[0];
-        wb.dev_in = d_prev; wb.dev_out = d_cur; wb.dev_clear = nullptr; wb.tol = tol;
-        if (launch_dgemm2(h, wb, 1, d, st)) return 1;
-        fad::DgemmBatch yz = {};
-        yz.p[0] = {Yc, W, Yn, 1.0, 0.0, nullptr};                                // Y <- Y W
-        yz.p[1] = {W, Zc, Zn, 1.0, 0.0, nullptr};                                // Z <- W Z
-        yz.dev_in = d_prev; yz.dev_out = nullptr; yz.dev_clear = d_next; yz.tol = tol;
-        if (launch_dgemm2(h, yz, 2, d, st)) return 1;
-        double* t = Yc; Yc = Yn; Yn = t;
-        t = Zc; Zc = Zn; Zn = t;
+        fad::DgemmStrided wp = {};
+        wp.items = g; wp.flags = w.flags; wp.tol = 1e-12f;
+        wp.in_slot = (it + 2) % 3; wp.out_slot = it % 3; wp.clear_slot = -1;     // slots: iteration it-1, it, it+1
+        wp.f[0] = {Zc, Yc, w.W, T, T, T, -0.5, 1.5};                             // W = 1.5 I - 0.5 Z Y
+        if (launch_dgemm(h, wp, 1, d, st)) return 1;
+        fad::DgemmStrided yz = wp;
+        yz.out_slot = -1; yz.clear_slot = (it + 1) % 3;
+        yz.f[0] = {Yc, w.W, Yx, T, T, T, 1.0, 0.0};                              // Y <- Y W
+        yz.f[1] = {w.W, Zc, Zx, T, T, T, 1.0, 0.0};                              // Z <- W Z
+        if (launch_dgemm(h, yz, 2, d, st)) return 1;
+        std::swap(Yc, Yx);
+        std::swap(Zc, Zx);
     }
-    fad::trace_kernel<<<1, 256, 0, st>>>(Y, d, trY);
-    fad::trace_kernel<<<1, 256, 0, st>>>(Z, d, trZ);
+    return 0;
+}
+
+// FAD of g eval sets (mu2_z, C2_z) against the baseline (mu1, S = C1^(1/2), scal1 = {|C1|_F, tr C1}) into out[z][8]:
+// P = S C2_z, M_z = P S, the chain on M_z, the assembly.  out[z][3] reports `iters` as given.  With_resid (one item)
+// puts the relative residual of the square root in out[0][2]: P = Y Y, then resid_kernel.
+int frechet_items(fad_handle* h, const FrechetWorkspace& w, const double* mu1, const double* sqrt1, const double* scal1,
+                  const double* mu2, const double* cov2, int g, int d, int iters, const int* ok,
+                  const long long* offsets, bool with_resid, double* out, cudaStream_t st) {
+    const long long T = (long long)d * d;
+    fad::norm_trace_kernel<<<g, 1024, 0, st>>>(cov2, d, w.scalC);
     CK(cudaGetLastError());
-    h->launches += 2;
+    h->launches++;
+    fad::DgemmStrided p = {};
+    p.items = g; p.in_slot = p.out_slot = p.clear_slot = -1;
+    p.f[0] = {sqrt1, cov2, w.P, 0, T, T, 1.0, 0.0};                                 // P = S C2_z
+    if (launch_dgemm(h, p, 1, d, st)) return 1;
+    p.f[0] = {w.P, sqrt1, w.M, T, 0, T, 1.0, 0.0};                                  // M_z = P S
+    if (launch_dgemm(h, p, 1, d, st)) return 1;
+    if (newton_schulz(h, w, w.M, w.scalM, g, d, iters, st)) return 1;
+    if (with_resid) {
+        CK(cudaMemsetAsync(w.resid, 0, sizeof(double), st));
+        p.f[0] = {w.Y, w.Y, w.P, T, T, T, 1.0, 0.0};                                // P = Y Y
+        if (launch_dgemm(h, p, 1, d, st)) return 1;
+        fad::resid_kernel<<<elem_blocks(h, d), 256, 0, st>>>(w.P, w.M, d, w.scalM, w.resid);
+        h->launches++;
+    }
+    fad::frechet_assemble_kernel<<<g, 256, 0, st>>>(mu1, mu2, d, scal1, w.scalC, w.scalM, w.Y, w.Z,
+                                                    with_resid ? w.resid : nullptr, ok, offsets, iters, out);
+    CK(cudaGetLastError());
+    h->launches++;
     return 0;
 }
 }  // namespace
@@ -957,18 +958,13 @@ int fad_sqrt_psd(fad_handle* h, const double* cov, int d, int iters, double* sqr
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (iters <= 0) iters = 60;
-    const size_t total = (size_t)d * d;
-    if (ensure((void**)&h->fr_buf, &h->fr_cap, 8 * total * 8)) return 1;
-    double* Y = h->fr_buf;  double* Z = Y + total;  double* W = Z + total;  double* T = W + total;
-    double* scalA = h->fr_scal;  double* trS = scalA + 8;  double* trZs = scalA + 10;
-    float* devf = reinterpret_cast<float*>(scalA + 16);
-    unsigned eb = (unsigned)((total + 255) / 256);
-    if (eb > (unsigned)h->num_sms * 8) eb = h->num_sms * 8;
+    FrechetWorkspace w;
+    if (frechet_workspace(h, 1, d, w)) return 1;
     const size_t ev = prof_begin(h, st);
-    if (newton_schulz(h, cov, d, iters, Y, Z, W, T, scalA, trS, trZs, devf, st)) return 1;
-    fad::ns_unscale_kernel<<<eb, 256, 0, st>>>(Y, d, scalA, sqrt_out);
+    if (newton_schulz(h, w, cov, w.scalC, 1, d, iters, st)) return 1;
+    fad::ns_unscale_kernel<<<elem_blocks(h, d), 256, 0, st>>>(w.Y, d, w.scalC, sqrt_out);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(scal_out, scalA, 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(scal_out, w.scalC, 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
     h->launches++;
     prof_end(h, FAD_PROF_FRECHET, ev, st);
     return 0;
@@ -982,29 +978,11 @@ int fad_frechet_presqrt(fad_handle* h, const double* mu1, const double* sqrt1, c
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (iters <= 0) iters = 60;
-    const size_t total = (size_t)d * d;
-    if (ensure((void**)&h->fr_buf, &h->fr_cap, 8 * total * 8)) return 1;
-    double* Y = h->fr_buf;  double* Z = Y + total;  double* W = Z + total;  double* T = W + total;
-    double* M = T + 2 * total;  double* P = h->fr_buf + 7 * total;   // slots: Y Z W T T M S(fad_frechet) P
-    double* scalB = h->fr_scal + 2;  double* scalM = h->fr_scal + 4;
-    double* trY = h->fr_scal + 6;    double* resid = h->fr_scal + 7;  double* trZ = h->fr_scal + 9;
-    float* devf = reinterpret_cast<float*>(h->fr_scal + 16);
-    unsigned eb = (unsigned)((total + 255) / 256);
-    if (eb > (unsigned)h->num_sms * 8) eb = h->num_sms * 8;
-    const size_t ev_fr = prof_begin(h, st);
-    fad::norm_trace_kernel<<<1, 1024, 0, st>>>(cov2, d, scalB);
-    CK(cudaGetLastError());
-    h->launches++;
-    if (launch_dgemm(h, sqrt1, cov2, P, d, 1.0, 0.0, nullptr, st)) return 1;     // M = S C2 S
-    if (launch_dgemm(h, P, sqrt1, M, d, 1.0, 0.0, nullptr, st)) return 1;
-    if (newton_schulz(h, M, d, iters, Y, Z, W, T, scalM, trY, trZ, devf, st)) return 1;
-    CK(cudaMemsetAsync(resid, 0, sizeof(double), st));
-    if (launch_dgemm(h, Y, Y, P, d, 1.0, 0.0, nullptr, st)) return 1;
-    fad::resid_kernel<<<eb, 256, 0, st>>>(P, M, d, scalM, resid);
-    fad::frechet_assemble_kernel<<<1, 256, 0, st>>>(mu1, mu2, d, scal1, scalB, scalM, trY, trZ, resid, iters, out);
-    CK(cudaGetLastError());
-    h->launches += 2;
-    prof_end(h, FAD_PROF_FRECHET, ev_fr, st);
+    FrechetWorkspace w;
+    if (frechet_workspace(h, 1, d, w)) return 1;
+    const size_t ev = prof_begin(h, st);
+    if (frechet_items(h, w, mu1, sqrt1, scal1, mu2, cov2, 1, d, iters, nullptr, nullptr, true, out, st)) return 1;
+    prof_end(h, FAD_PROF_FRECHET, ev, st);
     return 0;
 }
 
@@ -1013,15 +991,14 @@ int fad_frechet(fad_handle* h, const double* mu1, const double* cov1, const doub
     if (!h) return fail("null handle");
     if (d <= 0) return fail("bad dimension");
     CK(cudaSetDevice(h->device));
-    const size_t total = (size_t)d * d;
-    if (ensure((void**)&h->fr_buf, &h->fr_cap, 8 * total * 8)) return 1;
-    double* S = h->fr_buf + 6 * total;            // scratch slot not used by the chains
-    double* scal1 = h->fr_scal + 12;
-    if (fad_sqrt_psd(h, cov1, d, iters, S, scal1, stream)) return 1;
-    return fad_frechet_presqrt(h, mu1, S, scal1, mu2, cov2, d, iters, out, stream);
+    FrechetWorkspace w;                   // the same carve-out as the two calls below: S and scal1 stay put
+    if (frechet_workspace(h, 1, d, w)) return 1;
+    if (fad_sqrt_psd(h, cov1, d, iters, w.sqrt1, w.scal1, stream)) return 1;
+    return fad_frechet_presqrt(h, mu1, w.sqrt1, w.scal1, mu2, cov2, d, iters, out, stream);
 }
 
-// Ragged-batched FAD of n_items eval sets against one cached baseline (see frechet_batched.cuh).
+// Ragged-batched FAD of n_items eval sets against one cached baseline: per-song statistics (stats.cuh), then the
+// chain over groups of up to G items.
 int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, const double* scal1,
                         const void* emb_f16, const long long* offsets, long long n_items, int d, int iters,
                         double* out, void* stream) {
@@ -1031,79 +1008,76 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (iters <= 0) iters = 60;
-    if (iters & 1) ++iters;
-    const size_t total = (size_t)d * d;
-    long long G = (long long)((size_t(1) << 31) / (64 * total));          // 8 matrices of d*d doubles per item in 2 GiB
+    if (iters & 1) ++iters;                                                // out[z][3]: the even count the chain runs
+    long long G = (long long)((size_t(1) << 31) / (64 * (size_t)d * d));  // 8 matrices of d*d doubles per item in 2 GiB
     if (G < 1) G = 1;
     if (G > 32767) G = 32767;                                              // two families share gridDim.z
     if (G > n_items) G = n_items;
-    const size_t per_item = 8 * total * 8 + (size_t)d * 8 + 4 * 8 + 3 * 4 + 4;
-    if (ensure((void**)&h->frb_buf, &h->frb_cap, per_item * (size_t)G + 256)) return 1;
-    double* cov = reinterpret_cast<double*>(h->frb_buf);
-    double* P = cov + G * total;   double* M = P + G * total;
-    double* Y = M + G * total;     double* Z = Y + G * total;   double* W = Z + G * total;
-    double* Yn = W + G * total;    double* Zn = Yn + G * total;
-    double* mu = Zn + G * total;
-    double* scalC = mu + G * d;    double* scalM = scalC + 2 * G;
-    float* flags = reinterpret_cast<float*>(scalM + 2 * G);
-    int* ok = reinterpret_cast<int*>(flags + 3 * G);
-    const int dt = (d + 31) / 32;
-    auto gemm = [&](const fad::DgemmStrided& p, int families) -> int {
-        dim3 grid((d + fad::kDgTileN - 1) / fad::kDgTileN, (d + fad::kDgTileM - 1) / fad::kDgTileM, (unsigned)(p.items * families));
-        fad::dgemm_strided_kernel<<<grid, 256, 0, st>>>(p, d);
-        CK(cudaGetLastError());
-        h->launches++;
-        return 0;
-    };
-    const float tol = 1e-12f;
+    FrechetWorkspace w;
+    if (frechet_workspace(h, G, d, w)) return 1;
+    const __half* emb = reinterpret_cast<const __half*>(emb_f16);
     const size_t ev = prof_begin(h, st);
     for (long long g0 = 0; g0 < n_items; g0 += G) {
         const int g = (int)((n_items - g0) < G ? (n_items - g0) : G);
         if (d % 64 == 0) {                                   // fp64 tensor pipe (DMMA), upper tile triangle per item
             const int nt = d / 64;
-            fad::song_stats_dmma_kernel<<<dim3(nt * (nt + 1) / 2, g), 256, 0, st>>>(reinterpret_cast<const __half*>(emb_f16), offsets + g0, d, mu, cov, ok);
+            fad::song_stats_dmma_kernel<<<dim3(nt * (nt + 1) / 2, g), 256, 0, st>>>(emb, offsets + g0, d, w.mu, w.cov, w.ok);
         } else {
-            fad::song_stats_kernel<<<dim3(dt, dt, g), 256, 0, st>>>(reinterpret_cast<const __half*>(emb_f16), offsets + g0, d, mu, cov, ok);
+            const int dt = (d + 31) / 32;
+            fad::song_stats_kernel<<<dim3(dt, dt, g), 256, 0, st>>>(emb, offsets + g0, d, w.mu, w.cov, w.ok);
         }
-        fad::norm_trace_batched_kernel<<<g, 256, 0, st>>>(cov, d, scalC);
-        CK(cudaGetLastError());
-        fad::DgemmStrided p = {};
-        p.items = g; p.flags = nullptr; p.in_slot = p.out_slot = p.clear_slot = -1; p.tol = tol;
-        p.f[0] = {sqrt1, cov, P, 0, (long long)total, (long long)total, 1.0, 0.0};          // P = S C_z
-        if (gemm(p, 1)) return 1;
-        p.f[0] = {P, sqrt1, M, (long long)total, 0, (long long)total, 1.0, 0.0};            // M = P S
-        if (gemm(p, 1)) return 1;
-        fad::norm_trace_batched_kernel<<<g, 256, 0, st>>>(M, d, scalM);
-        unsigned eb = (unsigned)((total + 255) / 256);
-        if (eb > 64) eb = 64;
-        fad::ns_init_batched_kernel<<<dim3(eb, g), 256, 0, st>>>(M, d, scalM, Y, Z, flags);
-        CK(cudaGetLastError());
-        h->launches += 4;
-        double* Yc = Y; double* Zc = Z; double* Yx = Yn; double* Zx = Zn;
-        for (int it = 0; it < iters; ++it) {
-            fad::DgemmStrided w = {};
-            w.items = g; w.flags = flags; w.tol = tol;
-            w.in_slot = (it + 2) % 3; w.out_slot = it % 3; w.clear_slot = -1;
-            w.f[0] = {Zc, Yc, W, (long long)total, (long long)total, (long long)total, -0.5, 1.5};   // W = 1.5 I - 0.5 Z Y
-            if (gemm(w, 1)) return 1;
-            fad::DgemmStrided yz = {};
-            yz.items = g; yz.flags = flags; yz.tol = tol;
-            yz.in_slot = (it + 2) % 3; yz.out_slot = -1; yz.clear_slot = (it + 1) % 3;
-            yz.f[0] = {Yc, W, Yx, (long long)total, (long long)total, (long long)total, 1.0, 0.0};   // Y <- Y W
-            yz.f[1] = {W, Zc, Zx, (long long)total, (long long)total, (long long)total, 1.0, 0.0};   // Z <- W Z
-            if (gemm(yz, 2)) return 1;
-            double* t = Yc; Yc = Yx; Yx = t;
-            t = Zc; Zc = Zx; Zx = t;
-        }
-        fad::frechet_assemble_batched_kernel<<<g, 256, 0, st>>>(mu1, mu, d, scal1, scalC, scalM, Y, Z, ok, offsets + g0,
-                                                                iters, out + g0 * 8);
         CK(cudaGetLastError());
         h->launches++;
+        if (frechet_items(h, w, mu1, sqrt1, scal1, w.mu, w.cov, g, d, iters, w.ok, offsets + g0, false, out + g0 * 8, st))
+            return 1;
     }
     prof_end(h, FAD_PROF_FRECHET, ev, st);
     return 0;
 }
 
+// ------------------------------------------------------------------- fp64 tensor-pipe peak
+// Roofline denominator of the DMMA kernels (exact Gram, Newton-Schulz): MEASURED_PEAKS.json only
+// carries the bf16 GEMM and HBM copy rates, so the fp64 tensor-pipe rate is measured here - every warp
+// of a full grid issues independent m8n8k4 DMMAs from registers, nothing else.
+namespace {
+__global__ void __launch_bounds__(256) dmma_peak_kernel(int iters, double* sink) {
+    double c[8][2];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) { c[i][0] = threadIdx.x; c[i][1] = -1.0 * threadIdx.x; }
+    const double a = 1.0 + 1e-9 * threadIdx.x, b = 1.0 - 1e-9 * threadIdx.x;
+    for (int it = 0; it < iters; ++it) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) sm90::dmma_884(c[i][0], c[i][1], a, b);
+    }
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) s += c[i][0] + c[i][1];
+    if (s == 12345.678) sink[0] = s;                       // keeps the chain alive, never true
+}
+}  // namespace
+
+extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_host) {
+    if (!h || !tflops_out_host) return fail("null argument");
+    CK(cudaSetDevice(h->device));
+    if (iters <= 0) iters = 20000;
+    FrechetWorkspace w;
+    if (frechet_workspace(h, 1, 1, w)) return 1;
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
+    const int blocks = h->num_sms * 4;
+    dmma_peak_kernel<<<blocks, 256>>>(iters / 10, w.sink);            // warm-up
+    CK(cudaEventRecord(e0));
+    dmma_peak_kernel<<<blocks, 256>>>(iters, w.sink);
+    CK(cudaEventRecord(e1));
+    CK(cudaEventSynchronize(e1));
+    float ms = 0.f;
+    CK(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    const double flop = (double)blocks * 8 /*warps*/ * (double)iters * 8 /*DMMAs*/ * 512.0;
+    *tflops_out_host = flop / (ms * 1e-3) / 1e12;
+    h->launches += 2;
+    return 0;
+}
 }  // extern "C"
 
 // ------------------------------------------------------------------------ Kernel Audio Distance

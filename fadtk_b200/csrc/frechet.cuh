@@ -12,29 +12,21 @@
 // n < d) stay exactly zero in Y, so singular inputs need no eps-regularisation branch.
 // C1^(1/2) of the baseline can be cached and reused by FAD-inf / per-song scoring.
 //
+// One chain serves every entry point: item z of a group owns the z-th d x d matrix of each operand, every stage
+// is one launch over all items, and each item carries its own convergence flags.  The single-problem entry points
+// run it with one item; fad_frechet_batched scores many eval sets (songs) against one baseline in lock-step,
+// M_z = S C_z S with S = C_base^(1/2) cached.
 // All scalars (norms, traces) stay on the device; the chain is launched without host syncs.
 #pragma once
 #include <stdint.h>
 
-namespace fad {
+#include "sm90.cuh"
 
-// C = alpha * A * B + beta_diag * I   (row-major d x d, fp64), optional trace(C) accumulation.
-// Up to two independent problems per launch (blockIdx.z): the Y <- Y W and Z <- W Z updates of
-// one Newton-Schulz iteration run side by side.  64 x 64 tile / 256 threads on DMMA (dgemm_tile below).
-//
-// Convergence control without host round trips: a launch whose `dev_in` (max |W - I| of the previous
-// iteration) is below `tol` returns immediately, so a fixed-length launch sequence costs only
-// launch latency once the iteration has converged.  `dev_out` receives max |C - I| (float bits,
-// atomicMax), `dev_clear` is zeroed for a later iteration (three rotating slots, see host code).
-struct DgemmProblem { const double* A; const double* B; double* C; double alpha, beta_diag; double* trace_out; };
-struct DgemmBatch {
-    DgemmProblem p[2];
-    const float* dev_in; float* dev_out; float* dev_clear; float tol;
-};
+namespace fad {
 
 // One 64 x 64 tile of C = alpha A B + beta_diag I per 256-thread CTA on the FP64 TENSOR pipe
 // (mma.sync m8n8k4 f64 -> SASS DMMA.8x8x4, the fp64 MMA shape of sm_90a; wgmma has no f64 kind).
-// Returns max |C - I| over this thread's outputs and its share of tr C.
+// Returns max |C - I| over this thread's outputs.
 // Layout: 8 warps as 2 (M) x 4 (N); a warp owns 32 x 16 outputs = 4 x 2 DMMA blocks (16 fp64 accumulators
 // per thread).  Per 4-wide k-step a warp issues 6 conflict-free LDS.64 (4 A + 2 B fragments) for 8 DMMAs,
 // so the tensor pipe and not shared memory is the limit (the CUDA-core tile this replaces needed 6 LDS.128
@@ -47,14 +39,9 @@ struct DgemmBatch {
 constexpr int kDgTileM = 64, kDgTileN = 64, kDgKC = 16;
 constexpr int kDgPitchA = kDgKC + 4, kDgPitchB = kDgTileN + 4;
 
-__device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
-
 __device__ __forceinline__ void dgemm_tile(const double* __restrict__ A, const double* __restrict__ B,
                                            double* __restrict__ C, int d, double alpha, double beta_diag,
-                                           float& dev, double& tr)
+                                           float& dev)
 {
     __shared__ __align__(16) double As[2][kDgTileM][kDgPitchA];
     __shared__ __align__(16) double Bs[2][kDgKC][kDgPitchB];
@@ -117,13 +104,12 @@ __device__ __forceinline__ void dgemm_tile(const double* __restrict__ A, const d
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 2; ++j) dmma_884(c[i][j][0], c[i][j][1], a[i], b[j]);
+                for (int j = 0; j < 2; ++j) sm90::dmma_884(c[i][j][0], c[i][j][1], a[i], b[j]);
         }
         if (ch + 1 < chunks) stage(buf ^ 1);
         __syncthreads();
     }
     // accumulator fragment: lane holds rows lane/4, columns 2 (lane%4) + {0, 1} of each 8 x 8 block
-    tr = 0.0;
     dev = 0.0f;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -132,8 +118,8 @@ __device__ __forceinline__ void dgemm_tile(const double* __restrict__ A, const d
             const int gi = bi + wm + i * 8 + fr, gj = bj + wn + j * 8 + 2 * fk;
             if (gi >= d) continue;
             double v0 = alpha * c[i][j][0], v1 = alpha * c[i][j][1];
-            if (gi == gj) { v0 += beta_diag; tr += v0; }
-            if (gi == gj + 1) { v1 += beta_diag; tr += v1; }
+            if (gi == gj) v0 += beta_diag;
+            if (gi == gj + 1) v1 += beta_diag;
             double* dst = C + (size_t)gi * d + gj;
             if (vec) {
                 if (gj < d) *reinterpret_cast<double2*>(dst) = make_double2(v0, v1);
@@ -146,69 +132,60 @@ __device__ __forceinline__ void dgemm_tile(const double* __restrict__ A, const d
         }
 }
 
-// grid (ceil(d / 64), ceil(d / 64), problems)
+// C_z = alpha A_z B_z + beta_diag I for two strided families of problems in one launch:
+// grid (ceil(d / 64), ceil(d / 64), families * items), blockIdx.z = item + family * items.  A stride of 0 shares the
+// operand between items (the cached baseline root).
+// Convergence control without host round trips: flags holds three rotating float slots of max |W - I| per item.  A
+// launch whose in_slot (the previous iteration) is below tol returns at once for that item, so a fixed-length launch
+// sequence costs only launch latency once an item has converged; out_slot receives max |C - I| (float bits,
+// atomicMax), clear_slot is zeroed for a later iteration.  Slot -1 or null flags = unused.
+struct DgemmFamily { const double* A; const double* B; double* C; long long sA, sB, sC; double alpha, beta_diag; };
+struct DgemmStrided {
+    DgemmFamily f[2];
+    int items;
+    float* flags;          // [items][3] or null
+    int in_slot, out_slot, clear_slot;
+    float tol;
+};
+
 __global__ void __launch_bounds__(256, 2)
-dgemm_kernel(const DgemmBatch batch, int d)
+dgemm_strided_kernel(const DgemmStrided p, int d)
 {
-    if (batch.dev_in != nullptr && *batch.dev_in < batch.tol) return;      // already converged
-    if (batch.dev_clear != nullptr && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && threadIdx.x == 0)
-        *batch.dev_clear = 0.0f;
-    const DgemmProblem pr = blockIdx.z ? batch.p[1] : batch.p[0];   // no dynamically indexed copy of the parameter block
+    const int fam = blockIdx.z >= p.items ? 1 : 0;
+    const int z = blockIdx.z - fam * p.items;
+    float* fl = p.flags ? p.flags + (size_t)z * 3 : nullptr;
+    if (fl && p.in_slot >= 0 && fl[p.in_slot] < p.tol) return;             // this item has converged
+    if (fl && p.clear_slot >= 0 && fam == 0 && blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) fl[p.clear_slot] = 0.0f;
+    const DgemmFamily f = fam ? p.f[1] : p.f[0];                          // no dynamically indexed copy of the parameter block
     float dev;
-    double tr;
-    dgemm_tile(pr.A, pr.B, pr.C, d, pr.alpha, pr.beta_diag, dev, tr);
-    if (batch.dev_out != nullptr) {
+    dgemm_tile(f.A + (size_t)z * f.sA, f.B + (size_t)z * f.sB, f.C + (size_t)z * f.sC, d, f.alpha, f.beta_diag, dev);
+    if (fl && p.out_slot >= 0) {
         for (int o = 16; o > 0; o >>= 1) dev = fmaxf(dev, __shfl_xor_sync(0xffffffffu, dev, o));
-        if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(batch.dev_out), __float_as_uint(dev));
-    }
-    if (pr.trace_out != nullptr && blockIdx.x == blockIdx.y) {
-        // tiles that meet the diagonal only; reduce inside the block, one atomic per block
-        __shared__ double red[256];
-        red[threadIdx.x] = tr;
-        __syncthreads();
-        for (int s = 128; s > 0; s >>= 1) {
-            if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
-            __syncthreads();
-        }
-        if (threadIdx.x == 0) atomicAdd(pr.trace_out, red[0]);
+        if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<unsigned int*>(fl + p.out_slot), __float_as_uint(dev));
     }
 }
 
-// out[0] = tr A      (single block)
-__global__ void trace_kernel(const double* __restrict__ A, int d, double* __restrict__ out)
-{
-    __shared__ double r[256];
-    double t = 0.0;
-    for (int i = threadIdx.x; i < d; i += 256) t += A[(size_t)i * d + i];
-    r[threadIdx.x] = t;
-    __syncthreads();
-    for (int k = 128; k > 0; k >>= 1) {
-        if (threadIdx.x < k) r[threadIdx.x] += r[threadIdx.x + k];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) out[0] = r[0];
-}
-
-// scal[0] = |A|_F, scal[1] = tr A     (single block of 1024 threads: fixed summation order)
-__global__ void __launch_bounds__(1024) norm_trace_kernel(const double* __restrict__ A, int d, double* __restrict__ scal)
+// scal[z] = {|A_z|_F, tr A_z}; one block of 1024 threads per item, fixed summation order
+__global__ void __launch_bounds__(1024) norm_trace_kernel(const double* __restrict__ A, int d, double* __restrict__ scal /*[items][2]*/)
 {
     __shared__ double r1[1024], r2[1024];
+    const double* Az = A + (size_t)blockIdx.x * d * d;
     double s0 = 0.0, s1 = 0.0, t = 0.0;
     const size_t total = (size_t)d * d;
     size_t e = threadIdx.x;
     for (; e + 1024 < total; e += 2048) {                      // two independent chains per thread
-        const double v0 = A[e], v1 = A[e + 1024];
+        const double v0 = Az[e], v1 = Az[e + 1024];
         s0 += v0 * v0; s1 += v1 * v1;
     }
-    if (e < total) { const double v = A[e]; s0 += v * v; }
-    for (int i = threadIdx.x; i < d; i += 1024) t += A[(size_t)i * d + i];
+    if (e < total) { const double v = Az[e]; s0 += v * v; }
+    for (int i = threadIdx.x; i < d; i += 1024) t += Az[(size_t)i * d + i];
     r1[threadIdx.x] = s0 + s1; r2[threadIdx.x] = t;
     __syncthreads();
     for (int k = 512; k > 0; k >>= 1) {
         if (threadIdx.x < k) { r1[threadIdx.x] += r1[threadIdx.x + k]; r2[threadIdx.x] += r2[threadIdx.x + k]; }
         __syncthreads();
     }
-    if (threadIdx.x == 0) { scal[0] = sqrt(r1[0]); scal[1] = r2[0]; }
+    if (threadIdx.x == 0) { scal[2 * blockIdx.x] = sqrt(r1[0]); scal[2 * blockIdx.x + 1] = r2[0]; }
 }
 
 // Rank-deficient covariances (n < d) have eigenvalues that are zero up to roundoff, i.e. possibly
@@ -218,18 +195,24 @@ __global__ void __launch_bounds__(1024) norm_trace_kernel(const double* __restri
 // which is exact for null directions (sqrt(d) - d/sqrt(d) = 0) and O(d) ~ 1e-13 elsewhere.
 constexpr double kNsDelta = 1e-13;
 
-// Y = (A + A^T) / (2 |A|_F) + delta I, Z = I      (|A|_F read from scal[0])
-__global__ void ns_init_kernel(const double* __restrict__ A, int d, const double* __restrict__ scal,
-                               double* __restrict__ Y, double* __restrict__ Z)
+// Y_z = sym(A_z)/|A_z|_F + delta I, Z_z = I, flags_z = {0, 0, 1e30} (slot (k-1)%3 for k = 0 is slot 2);
+// |A_z|_F read from scal[2z].  grid (blocks, items)
+__global__ void __launch_bounds__(256)
+ns_init_kernel(const double* __restrict__ A, int d, const double* __restrict__ scal,
+               double* __restrict__ Y, double* __restrict__ Z, float* __restrict__ flags)
 {
-    const double nrm = scal[0];
+    const int z = blockIdx.y;
+    const double nrm = scal[2 * z];
     const double inv = nrm > 0.0 ? 1.0 / nrm : 0.0;
-    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < (size_t)d * d;
-         e += (size_t)gridDim.x * blockDim.x) {
+    const double* Az = A + (size_t)z * d * d;
+    double* Yz = Y + (size_t)z * d * d;
+    double* Zz = Z + (size_t)z * d * d;
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < (size_t)d * d; e += (size_t)gridDim.x * blockDim.x) {
         const int i = (int)(e / d), j = (int)(e % d);
-        Y[e] = 0.5 * (A[e] + A[(size_t)j * d + i]) * inv + ((i == j) ? kNsDelta : 0.0);
-        Z[e] = (i == j) ? 1.0 : 0.0;
+        Yz[e] = 0.5 * (Az[e] + Az[(size_t)j * d + i]) * inv + ((i == j) ? kNsDelta : 0.0);
+        Zz[e] = (i == j) ? 1.0 : 0.0;
     }
+    if (blockIdx.x == 0 && threadIdx.x == 0) { flags[3 * z] = 0.0f; flags[3 * z + 1] = 0.0f; flags[3 * z + 2] = 1.0e30f; }
 }
 
 // S = sqrt(|A|_F) * Y        (un-normalise a converged square root)
@@ -241,34 +224,48 @@ __global__ void ns_unscale_kernel(const double* __restrict__ Y, int d, const dou
          e += (size_t)gridDim.x * blockDim.x) S[e] = f * Y[e];
 }
 
-// out[0] = fad, out[1] = tr sqrt(C1 C2), out[2] = relative residual |Y^2 - M/|M|_F|_F,
-// out[3] = iterations, out[4] = |mu1-mu2|^2, out[5] = tr C1, out[6] = tr C2
-__global__ void frechet_assemble_kernel(const double* __restrict__ mu1, const double* __restrict__ mu2, int d,
-                                        const double* __restrict__ scalA /*|C1|_F, trC1*/,
-                                        const double* __restrict__ trC2,
-                                        const double* __restrict__ scalM /*|M|_F, trM*/,
-                                        const double* __restrict__ trY, const double* __restrict__ trZ,
-                                        const double* __restrict__ resid,
-                                        int iters, double* __restrict__ out)
+// out[z][0] = fad, [1] = tr sqrt(C1 C2_z), [2] = relative residual |Y^2 - M/|M|_F|_F (0 without resid),
+// [3] = iterations, [4] = |mu1-mu2_z|^2, [5] = tr C1, [6] = tr C2_z, [7] = row count (left alone without offsets).
+// An item with ok[z] == 0 gets NaN in [0], [1]; null ok = every item is good.  One block per item.
+__global__ void __launch_bounds__(256)
+frechet_assemble_kernel(const double* __restrict__ mu1, const double* __restrict__ mu2 /*[items][d]*/, int d,
+                        const double* __restrict__ scal1 /*|C1|_F, tr C1*/,
+                        const double* __restrict__ scalC /*[items][2]: |C2_z|_F, tr C2_z*/,
+                        const double* __restrict__ scalM /*[items][2]*/,
+                        const double* __restrict__ Y, const double* __restrict__ Z, const double* __restrict__ resid,
+                        const int* __restrict__ ok, const long long* __restrict__ offsets,
+                        int iters, double* __restrict__ out)
 {
-    __shared__ double red[256];
-    double s = 0.0;
-    for (int i = threadIdx.x; i < d; i += 256) { const double df = mu1[i] - mu2[i]; s += df * df; }
-    red[threadIdx.x] = s;
+    __shared__ double r0[256], r1[256], r2[256];
+    const int z = blockIdx.x;
+    const double* Yz = Y + (size_t)z * d * d;
+    const double* Zz = Z + (size_t)z * d * d;
+    double s = 0.0, ty = 0.0, tz = 0.0;
+    for (int i = threadIdx.x; i < d; i += 256) {
+        const double df = mu1[i] - mu2[(size_t)z * d + i];
+        s += df * df;
+        ty += Yz[(size_t)i * d + i];
+        tz += Zz[(size_t)i * d + i];
+    }
+    r0[threadIdx.x] = s; r1[threadIdx.x] = ty; r2[threadIdx.x] = tz;
     __syncthreads();
     for (int k = 128; k > 0; k >>= 1) {
-        if (threadIdx.x < k) red[threadIdx.x] += red[threadIdx.x + k];
+        if (threadIdx.x < k) { r0[threadIdx.x] += r0[threadIdx.x + k]; r1[threadIdx.x] += r1[threadIdx.x + k]; r2[threadIdx.x] += r2[threadIdx.x + k]; }
         __syncthreads();
     }
     if (threadIdx.x == 0) {
-        const double tr_sqrt = sqrt(scalM[0]) * (trY[0] - kNsDelta * trZ[0]);
-        out[0] = red[0] + scalA[1] + trC2[1] - 2.0 * tr_sqrt;
-        out[1] = tr_sqrt;
-        out[2] = resid ? sqrt(resid[0]) : 0.0;
-        out[3] = (double)iters;
-        out[4] = red[0];
-        out[5] = scalA[1];
-        out[6] = trC2[1];
+        double* o = out + (size_t)z * 8;
+        const double nan = __longlong_as_double(0x7ff8000000000000LL);
+        const double tr_sqrt = sqrt(scalM[2 * z]) * (r1[0] - kNsDelta * r2[0]);
+        const bool good = ok == nullptr || ok[z] != 0;
+        o[0] = good ? r0[0] + scal1[1] + scalC[2 * z + 1] - 2.0 * tr_sqrt : nan;
+        o[1] = good ? tr_sqrt : nan;
+        o[2] = resid ? sqrt(resid[0]) : 0.0;
+        o[3] = (double)iters;
+        o[4] = r0[0];
+        o[5] = scal1[1];
+        o[6] = scalC[2 * z + 1];
+        if (offsets) o[7] = (double)(offsets[z + 1] - offsets[z]);
     }
 }
 

@@ -1,6 +1,6 @@
 // sm_90a device primitives used by every tensor-core kernel in this library:
 // mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async) and its shared-memory
-// matrix descriptor.
+// matrix descriptor, and the fp64 mma.sync the DMMA kernels use.
 //
 // Everything is inline PTX; nothing here depends on CUTLASS.  Bit layouts follow the PTX ISA
 // "wgmma matrix descriptor" table.
@@ -53,6 +53,14 @@ __device__ __forceinline__ uint4 lds128(uint32_t addr) {
 }
 __device__ __forceinline__ void sts64(uint32_t addr, float x, float y) {
     asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x), "f"(y) : "memory");
+}
+
+// ------------------------------------------------------------------- fp64 tensor pipe
+// {c0, c1} += a b: mma.sync m8n8k4 f64 (SASS DMMA.8x8x4), the fp64 MMA shape of sm_90a (wgmma has no f64 kind).
+// Fragments: A lane -> row lane/4, k lane%4; B k lane%4, col lane/4; C row lane/4, cols 2 (lane%4) + {0, 1}.
+__device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
+    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
 
 // ------------------------------------------------------------------------- mbarrier

@@ -17,6 +17,9 @@
 // stats_simt_kernel  (2)   fp64 CUDA-core contraction of the exact y, with atomics: the independent cross-check of
 //   the DMMA kernel (tests/test_gpu_kernels.py compares the two).
 //
+// song_stats_dmma_kernel runs the same DMMA Gram tile (gram_tile) per song for fad_frechet_batched and finishes each
+// song's mean and covariance in place; song_stats_kernel is its CUDA-core form for d not a multiple of 64.
+//
 // Packed accumulator (fp64, caller-owned, all-reduced across GPUs as-is):
 //   acc[0] = n,  acc[1 .. d] = sum(x - s) (exact),  acc[1+d .. 1+d+d*d) = sum(y y^T)
 //   (d x d, full, row-major),  acc[1+d+d*d ..] = sum y  (centring term of the covariance; the same values as
@@ -34,7 +37,7 @@ __device__ __forceinline__ void pair_to_tiles(int pair, int n_tiles, int& ti, in
 }
 
 // --------------------------------------------------------------------------------------
-// stats_dmma_kernel: the product default.  EXACT Gram matrix on the FP64 tensor pipe.
+// gram_tile / stats_dmma_kernel: the product default.  EXACT Gram matrix on the FP64 tensor pipe.
 //   y = x - s is exact in fp64 for any two fp16 values (<= 22 significant bits), every product
 //   y_a y_b is exact (<= 44 bits), and mma.sync m8n8k4 f64 (SASS DMMA.8x8x4) accumulates in fp64 in
 //   a fixed order: the result is the Gram matrix of the data to ~1e-16 - positive semi-definite, which
@@ -59,36 +62,31 @@ struct StatsDmmaParams {
     double* ws_sums;               // [n_tiles * n_splits][64]
 };
 
-__device__ __forceinline__ void stats_dmma_884(double& c0, double& c1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-                 : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
-}
+typedef double GramStage[2][2][kSdRows][kSdPitch];              // [panel i | j][buffer][row][col]
 
-// In = __half (embeddings; shift vector applied) or double (per-file mean rows of the reference's online merge, no shift)
+// The Gram tile both DMMA statistics kernels run: c += Y_i^T Y_j over rows [row_begin, row_end) of E (row pitch d),
+// Y_i / Y_j = columns [64 ti, 64 ti + 64) / [64 tj, 64 tj + 64) minus the shift row (none if shift is null).
+// In = __half (embeddings) or double (per-file mean rows, no shift).  On return c holds this thread's DMMA
+// accumulator fragments and cs_i / cs_j its loader partial column sums of Y_i / Y_j (cs_j = cs_i on the diagonal);
+// the stage buffers are free.  Called by all 256 threads.
 template <typename In>
-__global__ void __launch_bounds__(256, 2)
-stats_dmma_kernel(const In* __restrict__ E, const StatsDmmaParams p)
+__device__ __forceinline__ void gram_tile(GramStage& Ys, const In* __restrict__ E, int d, long long row_begin,
+                                          long long row_end, int ti, int tj, const __half* __restrict__ shift,
+                                          double (&c)[4][2][2], double (&cs_i)[4], double (&cs_j)[4])
 {
     constexpr bool kHalf = sizeof(In) == 2;
-    __shared__ __align__(16) double Ys[2][2][kSdRows][kSdPitch];     // [panel i | j][buffer][row][col]
-    const int job = blockIdx.x;
-    const int pair = job / p.n_splits, split = job % p.n_splits;
-    int ti, tj;
-    pair_to_tiles(pair, p.n_tiles, ti, tj);
     const bool diag = ti == tj;
-    const long long row_begin = (long long)split * p.rows_per_split;
-    const long long row_end = min(p.n_rows, row_begin + p.rows_per_split);
     const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
     const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
     const int fr = lane >> 2, fk = lane & 3;
     const int lrow = t >> 4, lcol = (t & 15) * 4;               // loader: row of the stage, first of 4 columns
 
     double si[4] = {0.0, 0.0, 0.0, 0.0}, sj[4] = {0.0, 0.0, 0.0, 0.0};
-    if (kHalf && p.shift != nullptr) {
+    if (kHalf && shift != nullptr) {
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-            si[e] = (double)__half2float(p.shift[ti * kSdTile + lcol + e]);
-            sj[e] = (double)__half2float(p.shift[tj * kSdTile + lcol + e]);
+            si[e] = (double)__half2float(shift[ti * kSdTile + lcol + e]);
+            sj[e] = (double)__half2float(shift[tj * kSdTile + lcol + e]);
         }
     }
     const In* src_i = E + (size_t)ti * kSdTile + lcol;
@@ -110,40 +108,38 @@ stats_dmma_kernel(const In* __restrict__ E, const StatsDmmaParams p)
         const long long r = r0 + lrow;
         rok = r < row_end;
         if (rok) {
-            load4(src_i + (size_t)r * p.d, ri);
-            if (!diag) load4(src_j + (size_t)r * p.d, rj);
+            load4(src_i + (size_t)r * d, ri);
+            if (!diag) load4(src_j + (size_t)r * d, rj);
         }
-    };
-    double colsum[4] = {0.0, 0.0, 0.0, 0.0};
-    auto unpack = [](const double (&v)[4], const double (&s)[4], bool ok, double (&y)[4]) {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) y[e] = ok ? v[e] - s[e] : 0.0;
     };
     auto stage = [&](int buf) {
         double y[4];
-        unpack(ri, si, rok, y);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) y[e] = rok ? ri[e] - si[e] : 0.0;
         *reinterpret_cast<double2*>(&Ys[0][buf][lrow][lcol]) = make_double2(y[0], y[1]);
         *reinterpret_cast<double2*>(&Ys[0][buf][lrow][lcol + 2]) = make_double2(y[2], y[3]);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) colsum[e] += y[e];
+        for (int e = 0; e < 4; ++e) cs_i[e] += y[e];
         if (!diag) {
-            unpack(rj, sj, rok, y);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) y[e] = rok ? rj[e] - sj[e] : 0.0;
             *reinterpret_cast<double2*>(&Ys[1][buf][lrow][lcol]) = make_double2(y[0], y[1]);
             *reinterpret_cast<double2*>(&Ys[1][buf][lrow][lcol + 2]) = make_double2(y[2], y[3]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) cs_j[e] += y[e];
         }
     };
 
-    double c[4][2][2] = {};
     const int stages = row_end > row_begin ? (int)((row_end - row_begin + kSdRows - 1) / kSdRows) : 0;
     if (stages > 0) {
         fetch(row_begin);
         stage(0);
     }
     __syncthreads();
+    const int bp = diag ? 0 : 1;
     for (int st = 0; st < stages; ++st) {
         const int buf = st & 1;
         if (st + 1 < stages) fetch(row_begin + (long long)(st + 1) * kSdRows);
-        const int bp = diag ? 0 : 1;
 #pragma unroll
         for (int kk = 0; kk < kSdRows; kk += 4) {
             double a[4], b[2];
@@ -154,11 +150,52 @@ stats_dmma_kernel(const In* __restrict__ E, const StatsDmmaParams p)
 #pragma unroll
             for (int i = 0; i < 4; ++i)
 #pragma unroll
-                for (int j = 0; j < 2; ++j) stats_dmma_884(c[i][j][0], c[i][j][1], a[i], b[j]);
+                for (int j = 0; j < 2; ++j) sm90::dmma_884(c[i][j][0], c[i][j][1], a[i], b[j]);
         }
         if (st + 1 < stages) stage(buf ^ 1);
         __syncthreads();
     }
+    if (diag) {
+#pragma unroll
+        for (int e = 0; e < 4; ++e) cs_j[e] = cs_i[e];
+    }
+}
+
+// Column sums of Y over the tile's rows: the 16 loader partials of each column added in a fixed order, through the
+// stage buffers gram_tile left free.  Thread t < 64 panels returns the sum of column t % 64 of panel t / 64 (i, j).
+__device__ __forceinline__ double gram_colsums(GramStage& Ys, const double (&cs_i)[4], const double (&cs_j)[4], int panels)
+{
+    const int t = threadIdx.x, lrow = t >> 4, lcol = (t & 15) * 4;
+    double* red = &Ys[0][0][0][0];                              // 2 x 16 x 64 doubles fit the first panel's two buffers
+    static_assert(2 * kSdRows * kSdTile <= 2 * kSdRows * kSdPitch, "reduction scratch");
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        red[lrow * kSdTile + lcol + e] = cs_i[e];
+        if (panels == 2) red[kSdRows * kSdTile + lrow * kSdTile + lcol + e] = cs_j[e];
+    }
+    __syncthreads();
+    double v = 0.0;
+    if (t < panels * kSdTile)
+        for (int k = 0; k < kSdRows; ++k) v += red[(t >> 6) * kSdRows * kSdTile + k * kSdTile + (t & 63)];
+    return v;
+}
+
+template <typename In>
+__global__ void __launch_bounds__(256, 2)
+stats_dmma_kernel(const In* __restrict__ E, const StatsDmmaParams p)
+{
+    __shared__ __align__(16) GramStage Ys;
+    const int job = blockIdx.x;
+    const int pair = job / p.n_splits, split = job % p.n_splits;
+    int ti, tj;
+    pair_to_tiles(pair, p.n_tiles, ti, tj);
+    const long long row_begin = (long long)split * p.rows_per_split;
+    const long long row_end = min(p.n_rows, row_begin + p.rows_per_split);
+    double c[4][2][2] = {}, cs_i[4] = {0.0, 0.0, 0.0, 0.0}, cs_j[4] = {0.0, 0.0, 0.0, 0.0};
+    gram_tile(Ys, E, p.d, row_begin, row_end, ti, tj, p.shift, c, cs_i, cs_j);
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+    const int fr = lane >> 2, fk = lane & 3;
     double* dst = p.ws_tiles + (size_t)job * kSdTile * kSdTile;
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -166,17 +203,9 @@ stats_dmma_kernel(const In* __restrict__ E, const StatsDmmaParams p)
         for (int j = 0; j < 2; ++j)
             *reinterpret_cast<double2*>(dst + (wm + i * 8 + fr) * kSdTile + wn + j * 8 + 2 * fk) =
                 make_double2(c[i][j][0], c[i][j][1]);
-    if (diag) {
-        // column sums: 16 loader rows per column group -> one fixed-order sum per column
-        double* red = &Ys[0][0][0][0];                          // 16 x 64 doubles, the stages are done with it
-        red[lrow * kSdTile + lcol + 0] = colsum[0]; red[lrow * kSdTile + lcol + 1] = colsum[1];
-        red[lrow * kSdTile + lcol + 2] = colsum[2]; red[lrow * kSdTile + lcol + 3] = colsum[3];
-        __syncthreads();
-        if (t < kSdTile) {
-            double v = 0.0;
-            for (int k = 0; k < 16; ++k) v += red[k * kSdTile + t];
-            p.ws_sums[((size_t)ti * p.n_splits + split) * kSdTile + t] = v;
-        }
+    if (ti == tj) {
+        const double v = gram_colsums(Ys, cs_i, cs_j, 1);
+        if (t < kSdTile) p.ws_sums[((size_t)ti * p.n_splits + split) * kSdTile + t] = v;
     }
 }
 
@@ -215,6 +244,140 @@ __global__ void __launch_bounds__(256) stats_dmma_reduce_kernel(StatsDmmaParams 
         }
     }
     if (pair == 0 && blockIdx.y == 0 && threadIdx.x == 0) acc[0] += (double)p.n_rows;
+}
+
+// --------------------------------------------------------------------------------------
+// Per-song statistics for fad_frechet_batched: item z owns rows [offsets[z], offsets[z+1]) of one fp16 [N, d] matrix.
+// mean (rounded to fp16 like np.mean of an fp16 array, returned as fp64) and covariance (ddof = 1, exact fp64 products
+// of y = x - s, s = the item's first row) of every item (fadtk/fad.py:42-48).  ok[z] = 0 for an item with fewer than 2
+// rows (the reference asserts, fad.py:46): its covariance is set to the identity so the lock-step chain stays finite,
+// and the assembly writes NaN.
+
+// CUDA-core version, any d.  grid (ceil(d/32), ceil(d/32), items), 256 threads: thread (ty, tx) owns a 2 x 2 block.
+__global__ void __launch_bounds__(256)
+song_stats_kernel(const __half* __restrict__ emb, const long long* __restrict__ offsets, int d,
+                  double* __restrict__ mu /*[items][d]*/, double* __restrict__ cov /*[items][d][d]*/,
+                  int* __restrict__ ok)
+{
+    __shared__ double Yi[32][33], Yj[32][33];
+    __shared__ double si[32], sj[32];
+    const int z = blockIdx.z;
+    const long long r0 = offsets[z], r1 = offsets[z + 1];
+    const long long n = r1 - r0;
+    const int bi = blockIdx.y * 32, bj = blockIdx.x * 32;
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    double* C = cov + (size_t)z * d * d;
+    if (n < 2) {
+        for (int e = threadIdx.x; e < 1024; e += 256) {
+            const int gi = bi + (e >> 5), gj = bj + (e & 31);
+            if (gi < d && gj < d) C[(size_t)gi * d + gj] = gi == gj ? 1.0 : 0.0;
+        }
+        if (bj == 0 && threadIdx.x < 32 && bi + threadIdx.x < d) mu[(size_t)z * d + bi + threadIdx.x] = 0.0;
+        if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) ok[z] = 0;
+        return;
+    }
+    const __half* base = emb + (size_t)r0 * d;
+    double c[2][2] = {};
+    double colsum = 0.0;                                        // threads 0..31: column bi + t; 32..63: column bj + t
+    for (long long rr = 0; rr < n; rr += 32) {
+        for (int e = threadIdx.x; e < 2048; e += 256) {
+            const int which = e >> 10, r = (e >> 5) & 31, cidx = e & 31;
+            const int gc = (which ? bj : bi) + cidx;
+            double v = 0.0;
+            if (rr + r < n && gc < d)
+                v = (double)__half2float(base[(size_t)(rr + r) * d + gc]) - (double)__half2float(base[gc]);
+            (which ? Yj : Yi)[r][cidx] = v;
+        }
+        __syncthreads();
+#pragma unroll 8
+        for (int r = 0; r < 32; ++r) {
+            const double a0 = Yi[r][ty * 2], a1 = Yi[r][ty * 2 + 1];
+            const double b0 = Yj[r][tx * 2], b1 = Yj[r][tx * 2 + 1];
+            c[0][0] = fma(a0, b0, c[0][0]); c[0][1] = fma(a0, b1, c[0][1]);
+            c[1][0] = fma(a1, b0, c[1][0]); c[1][1] = fma(a1, b1, c[1][1]);
+        }
+        if (threadIdx.x < 64) {
+            const int t = threadIdx.x & 31;
+            double s = 0.0;
+            if (threadIdx.x < 32) { for (int r = 0; r < 32; ++r) s += Yi[r][t]; }
+            else                  { for (int r = 0; r < 32; ++r) s += Yj[r][t]; }
+            colsum += s;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < 32) si[threadIdx.x] = colsum;
+    else if (threadIdx.x < 64) sj[threadIdx.x - 32] = colsum;
+    __syncthreads();
+    const double inv_n = 1.0 / (double)n, inv_n1 = 1.0 / (double)(n - 1);
+#pragma unroll
+    for (int u = 0; u < 2; ++u)
+#pragma unroll
+        for (int v = 0; v < 2; ++v) {
+            const int li = ty * 2 + u, lj = tx * 2 + v;
+            const int gi = bi + li, gj = bj + lj;
+            if (gi < d && gj < d) C[(size_t)gi * d + gj] = (c[u][v] - si[li] * sj[lj] * inv_n) * inv_n1;
+        }
+    if (bj == 0 && threadIdx.x < 32 && bi + threadIdx.x < d) {
+        const double m = (double)__half2float(base[bi + threadIdx.x]) + si[threadIdx.x] * inv_n;
+        mu[(size_t)z * d + bi + threadIdx.x] = (double)__half2float(__double2half(m));     // fp16 mean (fad.py:48)
+    }
+    if (blockIdx.x == 0 && blockIdx.y == 0 && threadIdx.x == 0) ok[z] = 1;
+}
+
+// The same statistics on the FP64 tensor pipe (d a multiple of 64): one CTA = (item, tile pair ti <= tj), the item's
+// rows streamed through gram_tile, the covariance written to both triangles from the same accumulators.
+// 5000 x [750, 128]: the CUDA-core kernel above was ~half of the whole per-song pass.  grid (n_pairs, items).
+__global__ void __launch_bounds__(256, 2)
+song_stats_dmma_kernel(const __half* __restrict__ emb, const long long* __restrict__ offsets, int d,
+                       double* __restrict__ mu, double* __restrict__ cov, int* __restrict__ ok)
+{
+    constexpr int T = kSdTile;
+    __shared__ __align__(16) GramStage Ys;
+    __shared__ double s_sum[2][T];
+    const int z = blockIdx.y;
+    const long long n = offsets[z + 1] - offsets[z];
+    int ti, tj;
+    pair_to_tiles(blockIdx.x, d / T, ti, tj);
+    const bool diag = ti == tj;
+    const int t = threadIdx.x;
+    double* C = cov + (size_t)z * d * d;
+    if (n < 2) {
+        for (int e = t; e < T * T; e += 256) {
+            const int gi = ti * T + e / T, gj = tj * T + e % T;
+            C[(size_t)gi * d + gj] = gi == gj ? 1.0 : 0.0;
+            if (!diag) C[(size_t)gj * d + gi] = 0.0;
+        }
+        if (diag && t < T) mu[(size_t)z * d + ti * T + t] = 0.0;
+        if (blockIdx.x == 0 && t == 0) ok[z] = 0;
+        return;
+    }
+    const __half* base = emb + (size_t)offsets[z] * d;
+    double c[4][2][2] = {}, cs_i[4] = {0.0, 0.0, 0.0, 0.0}, cs_j[4] = {0.0, 0.0, 0.0, 0.0};
+    gram_tile(Ys, base, d, 0, n, ti, tj, base, c, cs_i, cs_j);
+    const double sum = gram_colsums(Ys, cs_i, cs_j, 2);
+    if (t < 2 * T) s_sum[t >> 6][t & 63] = sum;
+    __syncthreads();
+    const int warp = t >> 5, lane = t & 31;
+    const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+    const int fr = lane >> 2, fk = lane & 3;
+    const double inv_n = 1.0 / (double)n, inv_n1 = 1.0 / (double)(n - 1);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int li = wm + i * 8 + fr, lj = wn + j * 8 + 2 * fk + e;
+                const double v = (c[i][j][e] - s_sum[0][li] * s_sum[1][lj] * inv_n) * inv_n1;
+                const int gi = ti * T + li, gj = tj * T + lj;
+                C[(size_t)gi * d + gj] = v;
+                if (!diag) C[(size_t)gj * d + gi] = v;
+            }
+    if (diag && t < T) {
+        const double m = (double)__half2float(base[ti * T + t]) + s_sum[0][t] * inv_n;
+        mu[(size_t)z * d + ti * T + t] = (double)__half2float(__double2half(m));      // fp16 mean (fad.py:48)
+    }
+    if (blockIdx.x == 0 && t == 0) ok[z] = 1;
 }
 
 // --------------------------------------------------------------------------------------

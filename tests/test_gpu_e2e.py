@@ -112,10 +112,12 @@ def test_score_individual_matches_reference_csv(engine, golden_dir, tmp_path):
     assert np.allclose(scores, g["scores"], rtol=1e-4)
 
 
-@pytest.mark.parametrize("d,lens", [(128, [750, 2, 1, 130, 40, 750, 333]), (512, [300, 700, 17])])
+@pytest.mark.parametrize("d,lens", [(128, [750, 2, 1, 130, 40, 750, 333]), (512, [300, 700, 17]),
+                                    (100, [300, 1, 57, 2, 160])])
 def test_frechet_batched_matches_oracle_per_item(engine, d, lens):
     """fad_frechet_batched == per-item reference arithmetic (fad.py:42-48 + :51-120), ragged items,
-    rank-deficient items (n < d), and an item with a single row (reference: AssertionError -> NaN here)."""
+    rank-deficient items (n < d), and an item with a single row (reference: AssertionError -> NaN here).
+    d = 100 takes the CUDA-core per-song statistics (d not a multiple of 64) and partial 64 x 64 GEMM tiles."""
     from fadtk_b200 import _native
     rng = np.random.default_rng(5)
     mix = rng.standard_normal((d, d)) * (1.0 / np.sqrt(d))
