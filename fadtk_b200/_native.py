@@ -88,6 +88,7 @@ SIGNATURES = {
     "fad_bench_dmma_peak": (C.c_int, [c_vp, C.c_int, c_vp]),
     "fad_kad_median_sq": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_kad_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_song_sums": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -599,6 +600,19 @@ class Engine:
         out = torch.empty(3, dtype=torch.float64, device=z.device)
         _check(lib().fad_kad_sums(self._h, z.data_ptr(), int(m), z.shape[0] - int(m), z.shape[1], sigma.data_ptr(),
                                   out.data_ptr(), _stream()))
+        return out
+
+    def kad_song_sums(self, z: torch.Tensor, m: int, offsets: torch.Tensor, sigma: torch.Tensor) -> torch.Tensor:
+        """z fp16 [m + n_total, d] (cuda, X rows first), offsets int64 [n_items + 1] (cuda, into the rows after X),
+        sigma fp64 scalar (cuda) -> fp64 [1 + 2 n_items] (cuda): S_xx, then S_yy,k and S_xy,k per song
+        (fad_kad_song_sums)."""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        n_items = offsets.shape[0] - 1
+        out = torch.empty(1 + 2 * n_items, dtype=torch.float64, device=z.device)
+        _check(lib().fad_kad_song_sums(self._h, z.data_ptr(), int(m), offsets.data_ptr(), n_items, z.shape[1],
+                                       sigma.data_ptr(), out.data_ptr(), _stream()))
         return out
 
 

@@ -1089,6 +1089,7 @@ struct KadWorkspace {
     double *colpart, *partial;
     unsigned long long* hist;
     fad::KadSelectState* state;
+    unsigned char* extra;                           // the caller's own bytes (kad_prepare's extra)
 };
 
 int kad_check(fad_handle* h, const void* z, long long m, long long n, int d, const void* out) {
@@ -1101,19 +1102,21 @@ int kad_check(fad_handle* h, const void* z, long long m, long long n, int d, con
     return 0;
 }
 
-// shift (fp16 mean of the first m rows), hi / lo split and row norms of z [N, d]; the two TMA maps over hi / lo
+// shift (fp16 mean of the first m rows), hi / lo split and row norms of z [N, d]; the two TMA maps over hi / lo.
+// norm_rows: at least this many norms (zero past N); extra: bytes of w.extra for the caller
 int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspace& w, CUtensorMap* map_hi,
-                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st) {
+                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st, size_t norm_rows = 0, size_t extra = 0) {
     p.N = N; p.m = m; p.d = d;
     p.T = (N + 127) / 128;
     p.units = (p.T + 1) / 2;
-    const size_t rows_pad = (size_t)p.T * 128;
+    const size_t rows_pad = std::max((size_t)p.T * 128, norm_rows);
     const int chunks = (m + fad::kKadColRows - 1) / fad::kKadColRows;
     auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t b_split = al(rows_pad * d * 2), b_norm = al(rows_pad * 4), b_shift = al((size_t)d * 2),
                  b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8),
                  b_hist = al(2 * fad::kKadHistBins * 8), b_state = al(sizeof(fad::KadSelectState));
-    if (ensure((void**)&h->kad_buf, &h->kad_cap, 2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state)) return 1;
+    if (ensure((void**)&h->kad_buf, &h->kad_cap,
+               2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state + al(extra))) return 1;
     unsigned char* q = h->kad_buf;
     w.hi = reinterpret_cast<__half*>(q);            q += b_split;
     w.lo = reinterpret_cast<__half*>(q);            q += b_split;
@@ -1122,7 +1125,8 @@ int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspac
     w.colpart = reinterpret_cast<double*>(q);       q += b_col;
     w.partial = reinterpret_cast<double*>(q);       q += b_part;
     w.hist = reinterpret_cast<unsigned long long*>(q); q += b_hist;
-    w.state = reinterpret_cast<fad::KadSelectState*>(q);
+    w.state = reinterpret_cast<fad::KadSelectState*>(q); q += b_state;
+    w.extra = q;
     p.norm = w.norm;
 
     fad::kad_colsum_kernel<<<chunks, 128, 0, st>>>(z, m, d, w.colpart);
@@ -1205,6 +1209,100 @@ int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int
 }
 
 }  // extern "C"
+
+namespace {
+// per-song work units: each Y tile's column tiles cut into ceil(n / G) near-equal runs of at most G tiles,
+// G = max(kKadSongMinGroup, ceil(column tiles / kKadSongUnits)): a function of the shape only, so the sums do not
+// depend on the grid; it keeps the per-unit partials (2 KiB each) to about kKadSongUnits + Ty units while giving every
+// SM many units
+constexpr long long kKadSongMinGroup = 4;
+constexpr long long kKadSongUnits = 8192;
+}  // namespace
+
+extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets,
+                                 long long n_items, int d, const double* sigma, double* out, void* stream) {
+    if (kad_check(h, z_f16, m, 2, d, out)) return 1;
+    if (!offsets || !sigma) return fail("null argument");
+    if (n_items < 0) return fail("n_items must be >= 0");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<long long> off((size_t)n_items + 1);
+    CK(cudaMemcpyAsync(off.data(), offsets, off.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (off[0] != 0) return fail("offsets[0] must be 0");
+    for (long long k = 0; k < n_items; ++k)
+        if (off[k + 1] < off[k]) return fail("offsets must be non-decreasing");
+    const long long n_total = off.back();
+    if (m + n_total > (1LL << 30)) return fail("too many rows");
+
+    // work list: per Y tile t, the column tiles X 0..Tx-1, then the band t..be(t)
+    const int Tx = (int)((m + 127) / 128), Ty = (int)((n_total + 127) / 128);
+    std::vector<int> ncols(Ty);
+    long long total = 0;
+    for (int t = 0; t < Ty; ++t) {
+        const long long last = std::min(128LL * t + 127, n_total - 1);
+        const long long k = std::upper_bound(off.begin(), off.end(), last) - off.begin() - 1;   // off[k] <= last < off[k+1]
+        ncols[t] = Tx + (int)((off[k + 1] - 1) / 128) - t + 1;
+        total += ncols[t];
+    }
+    const int G = (int)std::max(kKadSongMinGroup, (total + kKadSongUnits - 1) / kKadSongUnits);
+    std::vector<int4> work;
+    std::vector<int> unit_start(Ty + 1, 0);
+    for (int t = 0; t < Ty; ++t) {
+        // near-equal cuts: units of G tiles plus a short remainder would leave CTAs that take every other unit idle
+        const long long n = ncols[t], cuts = (n + G - 1) / G;
+        for (long long i = 0; i < cuts; ++i) work.push_back(make_int4(t, (int)(i * n / cuts), (int)((i + 1) * n / cuts), 0));
+        unit_start[t + 1] = (int)work.size();
+    }
+    const size_t units = work.size();
+
+    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t b_work = al(units * sizeof(int4)), b_start = al(unit_start.size() * 4), b_end = al((size_t)Ty * 128 * 4),
+                 b_part = al(units * 256 * 8), b_xx = al(3 * 8);
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::KadParams p = {};
+    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n_total), (int)m, d, w, &mh, &ml, p, st,
+                    (size_t)m + (size_t)Ty * 128, b_work + b_start + b_end + b_part + b_xx)) return 1;
+    unsigned char* q = w.extra;
+    int4* d_work = reinterpret_cast<int4*>(q);       q += b_work;
+    int* d_start = reinterpret_cast<int*>(q);        q += b_start;
+    int* d_end = reinterpret_cast<int*>(q);          q += b_end;
+    double* d_part = reinterpret_cast<double*>(q);   q += b_part;
+    double* d_xx = reinterpret_cast<double*>(q);
+    p.sigma = sigma;
+
+    // S_xx: the sums pass over the first m rows alone (rows >= m are masked by index: (S_xx, 0, 0))
+    fad::KadParams px = p;
+    px.N = (int)m;
+    px.T = Tx;
+    px.units = (Tx + 1) / 2;
+    px.partial = w.partial;
+    if (launch_kad_tiles<0>(h, mh, ml, px, st)) return 1;
+    fad::kad_reduce_kernel<<<1, 32, 0, st>>>(w.partial, px.units, d_xx);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, d_xx, sizeof(double), cudaMemcpyDeviceToDevice, st));
+    h->launches++;
+    if (n_items == 0) return 0;
+
+    if (units) {
+        CK(cudaMemcpyAsync(d_work, work.data(), units * sizeof(int4), cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(d_start, unit_start.data(), unit_start.size() * 4, cudaMemcpyHostToDevice, st));
+        fad::kad_row_end_kernel<<<(Ty * 128 + 255) / 256, 256, 0, st>>>(offsets, n_items, (int)m, n_total, Ty * 128, d_end);
+        CK(cudaGetLastError());
+        h->launches++;
+        p.work = d_work;
+        p.row_end = d_end;
+        p.Tx = Tx;
+        p.units = (int)units;
+        p.partial = d_part;
+        if (launch_kad_tiles<2>(h, mh, ml, p, st)) return 1;
+    }
+    fad::kad_song_reduce_kernel<<<(unsigned)n_items, fad::kKadSongReduceThreads, 0, st>>>(d_part, d_start, offsets, out);
+    CK(cudaGetLastError());
+    h->launches++;
+    return 0;
+}
 
 #include "resample_host.inc"
 #include "clap_host.inc"

@@ -22,6 +22,14 @@
 // fixed tree into partial[u][3] (fp64).  kad_reduce_kernel sums the partials in unit order.  No floating-point atomic
 // anywhere: the three sums are bitwise reproducible and independent of the grid size and of timing.
 //
+// Per-song sums (MODE 2).  Z = [X; Y_1; ...; Y_K]; S_xx comes from MODE 0 over the first m rows.  The A operand is a
+// 128-row tile of Y (rows m + 128 t, not tile-aligned in Z); the B operands are the X tiles (mask j < m), then the
+// song band: Y tiles t .. the tile holding the last row of the song that owns tile t's last row (mask i < j < end of
+// i's song).  Work unit = (Y tile, up to G consecutive column tiles), G a function of the shape only (host work list).
+// Each thread sums k over its columns per row in fp32 per tile and in fp64 over the unit's tiles; the quad's 4 lanes
+// are added by a fixed shuffle tree into partial[u][row] (S_xy and S_yy).  kad_song_reduce_kernel adds each row's
+// units in order, then each song's rows in a fixed tree: no atomics, bitwise reproducible, independent of the grid.
+//
 // Bandwidth (MODE 1): exact selection of the two middle q values of the xx triangle by radix passes over the fp32 bit
 // pattern of q (monotone for q >= 0): bits 30..20, 19..10, 9..0.  Each pass runs the same tile loop over X alone and
 // counts the q values whose already-selected high bits match each of the two targets into shared-memory histograms,
@@ -60,15 +68,20 @@ struct KadParams {
     int d;                   // columns
     int T;                   // tile rows = ceil(N / 128)
     int units;               // ceil(T / 2)
-    const float* norm;       // [T * 128] |y_i|^2 (zero past N)
-    // MODE 0
+    const float* norm;       // [T * 128] |y_i|^2 (zero past N; MODE 2: [m + Ty * 128])
+    // MODE 0 and 2
     const double* sigma;     // device scalar
-    double* partial;         // [units][3]
+    double* partial;         // MODE 0: [units][3]; MODE 2: [units][2][128] per-row S_xy, S_yy
     // MODE 1
     const uint32_t* prefix;  // [2] selected high bits of the two targets
     unsigned long long* hist;// [2][kKadHistBins] global counts
     uint32_t mask;           // bits already selected
     int shift, bins;         // digit of this pass: (u >> shift) & (bins - 1)
+    // MODE 2 (per-song sums): A = a 128-row tile of Y (rows m + 128 t ...), B = the tiles of X, then the song band
+    const int4* work;        // [units] {t, v0, v1}: virtual column tiles [v0, v1) of Y tile t; v < Tx: X tile v,
+                             // v >= Tx: Y tile t + v - Tx
+    const int* row_end;      // [Ty * 128] per Y row: the end row (in Z) of its song; 0 past the last row
+    int Tx;                  // ceil(m / 128)
 };
 
 // --------------------------------------------------------------------------------------------- prologue
@@ -115,11 +128,73 @@ __global__ void kad_split_kernel(const __half* __restrict__ z, int N, int rows_p
 }
 
 // ------------------------------------------------------------------------------------------ tile kernel
+// producer: the ksteps stages of one tile, A = rows [arow, arow + 128), B = rows [brow, brow + 128) of Z (rows past N
+// are zero-filled by the TMA unit; neither coordinate needs to be a multiple of 128)
+__device__ __forceinline__ void kad_load_tile(uint8_t* smem, uint64_t* full, uint64_t* empty, int& s, uint32_t& ph,
+                                              const CUtensorMap* map_hi, const CUtensorMap* map_lo, int ksteps,
+                                              int arow, int brow) {
+    using namespace sm90;
+    for (int ks = 0; ks < ksteps; ++ks) {
+        mbar_wait(&empty[s], ph ^ 1);
+        uint8_t* st = smem + s * kKadStageBytes;
+        mbar_expect_tx(&full[s], kKadStageBytes);
+        tma_load_2d(st, map_hi, &full[s], ks * 64, arow);
+        tma_load_2d(st + kKadBox, map_lo, &full[s], ks * 64, arow);
+        tma_load_2d(st + 2 * kKadBox, map_hi, &full[s], ks * 64, brow);
+        tma_load_2d(st + 3 * kKadBox, map_lo, &full[s], ks * 64, brow);
+        if (++s == kKadStages) { s = 0; ph ^= 1; }
+    }
+}
+
+// consumer c: sum = the fp32 dot products y_i.y_j (hi.hi + hi.lo + lo.hi) of its 64 x 128 block of one tile, in the
+// m64n128 fragment layout
+__device__ __forceinline__ void kad_mma_tile(float (&sum)[64], uint8_t* smem, uint64_t* full, uint64_t* empty, int& s,
+                                             uint32_t& ph, int c, int lane, int d, int ksteps, int chunk_len) {
+    using namespace sm90;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
+    for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
+        const int ks1 = min(ks0 + chunk_len, ksteps);
+        // three products per real column accumulate into each element (zero-filled columns add exact zeros, which do
+        // not truncate)
+        const int cols = min(d, ks1 * 64) - ks0 * 64;
+        const float unshrink = kAccumShrinkPerElement * (float)(3 * cols);
+        int prev_s = -1;
+        for (int ks = ks0; ks < ks1; ++ks) {
+            mbar_wait(&full[s], ph);
+            const uint32_t base = smem_u32(smem + s * kKadStageBytes);
+            const uint64_t ah = kmajor_sw128_desc(base + c * 64 * 128);
+            const uint64_t al = kmajor_sw128_desc(base + kKadBox + c * 64 * 128);
+            const uint64_t bh = kmajor_sw128_desc(base + 2 * kKadBox);
+            const uint64_t bl = kmajor_sw128_desc(base + 3 * kKadBox);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bh + 2 * k, (ks > ks0) || (k > 0));
+                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bl + 2 * k, 1);
+                wgmma_m64n128k16_f16<0, 0>(acc, al + 2 * k, bh + 2 * k, 1);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
+            prev_s = s;
+            if (++s == kKadStages) { s = 0; ph ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev_s]);
+#pragma unroll
+        for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
+    }
+}
+
 template <int MODE>
 __global__ void __launch_bounds__(kKadThreads, 1)
 kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const KadParams p) {
     using namespace sm90;
-    static_assert(MODE == 0 || MODE == 1, "0: kernel sums, 1: radix histogram of q");
+    static_assert(MODE == 0 || MODE == 1 || MODE == 2, "0: kernel sums, 1: radix histogram of q, 2: per-row song sums");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
@@ -148,21 +223,21 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
             int s = 0; uint32_t ph = 0;
-            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
-                for (int half = 0; half < 2; ++half) {
-                    const int r = half == 0 ? u : p.T - 1 - u;
-                    if (half == 1 && r == u) break;                    // odd T: the middle row once
-                    for (int ct = r; ct < p.T; ++ct) {
-                        for (int ks = 0; ks < ksteps; ++ks) {
-                            mbar_wait(&empty[s], ph ^ 1);
-                            uint8_t* st = smem + s * kKadStageBytes;
-                            mbar_expect_tx(&full[s], kKadStageBytes);
-                            tma_load_2d(st, &map_hi, &full[s], ks * 64, r * 128);
-                            tma_load_2d(st + kKadBox, &map_lo, &full[s], ks * 64, r * 128);
-                            tma_load_2d(st + 2 * kKadBox, &map_hi, &full[s], ks * 64, ct * 128);
-                            tma_load_2d(st + 3 * kKadBox, &map_lo, &full[s], ks * 64, ct * 128);
-                            if (++s == kKadStages) { s = 0; ph ^= 1; }
-                        }
+            if constexpr (MODE == 2) {
+                for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                    const int4 wk = p.work[u];
+                    const int arow = p.m + wk.x * 128;
+                    for (int v = wk.y; v < wk.z; ++v)
+                        kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, arow,
+                                      v < p.Tx ? v * 128 : arow + (v - p.Tx) * 128);
+                }
+            } else {
+                for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                    for (int half = 0; half < 2; ++half) {
+                        const int r = half == 0 ? u : p.T - 1 - u;
+                        if (half == 1 && r == u) break;                // odd T: the middle row once
+                        for (int ct = r; ct < p.T; ++ct)
+                            kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, r * 128, ct * 128);
                     }
                 }
             }
@@ -174,6 +249,68 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         const int wq = warp & 3;
         const int ct_id = threadIdx.x - 128;              // 0..255
         int s = 0; uint32_t ph = 0;
+        if constexpr (MODE == 2) {
+            const double sg = *p.sigma;
+            const float neg_coef = (float)(-1.4426950408889634 / (2.0 * sg * sg));
+            const int lr0 = c * 64 + wq * 16 + (lane >> 2);                    // tile rows lr0, lr0 + 8
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                const int4 wk = p.work[u];
+                const int row0 = p.m + wk.x * 128 + lr0;                       // rows of Z
+                const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
+                const int end[2] = {__ldg(p.row_end + row0 - p.m), __ldg(p.row_end + row0 + 8 - p.m)};
+                double axy[2] = {0.0, 0.0}, ayy[2] = {0.0, 0.0};
+                for (int v = wk.y; v < wk.z; ++v) {
+                    const bool xt = v < p.Tx;
+                    const int col0 = (xt ? v * 128 : p.m + (wk.x + v - p.Tx) * 128) + 2 * (lane & 3);
+                    // columns j of row i that count: X tile j < m (none for a row past the last song, end = 0);
+                    // band tile i < j < end of the song of row i
+                    int lo[2], hi[2];
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        lo[i] = xt ? -1 : row0 + 8 * i;
+                        hi[i] = xt ? (end[i] > 0 ? p.m : 0) : end[i];
+                    }
+                    float sum[64];
+                    kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                    float rs[2] = {0.f, 0.f};
+#pragma unroll
+                    for (int j = 0; j < 16; ++j) {
+                        // col0 has the parity of m in band tiles: two scalar loads, not a float2
+                        const float nc[2] = {__ldg(p.norm + col0 + 8 * j), __ldg(p.norm + col0 + 8 * j + 1)};
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                            for (int e = 0; e < 2; ++e) {
+                                const int gj = col0 + 8 * j + e;
+                                const float sn = nr[i] + nc[e];
+                                float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
+                                q = q > kQResolution * sn ? q : 0.f;
+                                float kv;
+                                asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(kv) : "f"(q * neg_coef));
+                                rs[i] += (gj > lo[i] && gj < hi[i]) ? kv : 0.f;
+                            }
+                        }
+                    }
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        if (xt) axy[i] += (double)rs[i]; else ayy[i] += (double)rs[i];
+                    }
+                }
+                // the 4 lanes of a quad hold the same two rows: fixed xor tree, then one lane writes each row
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    for (int o = 1; o < 4; o <<= 1) {
+                        axy[i] += __shfl_xor_sync(0xffffffffu, axy[i], o);
+                        ayy[i] += __shfl_xor_sync(0xffffffffu, ayy[i], o);
+                    }
+                    if ((lane & 3) == 0) {
+                        p.partial[(size_t)u * 256 + lr0 + 8 * i] = axy[i];
+                        p.partial[(size_t)u * 256 + 128 + lr0 + 8 * i] = ayy[i];
+                    }
+                }
+            }
+            return;
+        }
         float neg_coef = 0.f;
         uint32_t pfx0 = 0, pfx1 = 0;
         bool two = false;
@@ -194,43 +331,8 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                 const int row0 = r * 128 + c * 64 + wq * 16 + (lane >> 2);     // rows row0, row0 + 8
                 const float nr0 = __ldg(p.norm + row0), nr1 = __ldg(p.norm + row0 + 8);
                 for (int ct = r; ct < p.T; ++ct) {
-                    float sum[64], acc[64];
-#pragma unroll
-                    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
-                    for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
-                        const int ks1 = min(ks0 + chunk_len, ksteps);
-                        // three products per real column accumulate into each element (zero-filled columns add exact
-                        // zeros, which do not truncate)
-                        const int cols = min(p.d, ks1 * 64) - ks0 * 64;
-                        const float unshrink = kAccumShrinkPerElement * (float)(3 * cols);
-                        int prev_s = -1;
-                        for (int ks = ks0; ks < ks1; ++ks) {
-                            mbar_wait(&full[s], ph);
-                            const uint32_t base = smem_u32(smem + s * kKadStageBytes);
-                            const uint64_t ah = kmajor_sw128_desc(base + c * 64 * 128);
-                            const uint64_t al = kmajor_sw128_desc(base + kKadBox + c * 64 * 128);
-                            const uint64_t bh = kmajor_sw128_desc(base + 2 * kKadBox);
-                            const uint64_t bl = kmajor_sw128_desc(base + 3 * kKadBox);
-                            wgmma_fence();
-#pragma unroll
-                            for (int k = 0; k < 4; ++k) {
-                                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bh + 2 * k, (ks > ks0) || (k > 0));
-                                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bl + 2 * k, 1);
-                                wgmma_m64n128k16_f16<0, 0>(acc, al + 2 * k, bh + 2 * k, 1);
-                            }
-                            wgmma_commit();
-                            wgmma_wait<1>();
-                            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
-                            prev_s = s;
-                            if (++s == kKadStages) { s = 0; ph ^= 1; }
-                        }
-                        wgmma_wait<0>();
-                        fence_regs(acc);
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&empty[prev_s]);
-#pragma unroll
-                        for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
-                    }
+                    float sum[64];
+                    kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
 
                     // ---- epilogue on the fragment: element (row0 + 8 i, col0 + 8 j + e) is sum[4 j + 2 i + e]
                     const int col0 = ct * 128 + 2 * (lane & 3);
@@ -309,6 +411,54 @@ __global__ void kad_reduce_kernel(const double* __restrict__ partial, int units,
     double s = 0.0;
     for (int u = 0; u < units; ++u) s += partial[(size_t)u * 3 + t];
     out[t] = s;
+}
+
+// per-song sums, MODE 2: row_end[r] for the Y rows r < rows (Ty * 128) = m + the end row (in Y) of r's song; 0 past n_total
+__global__ void kad_row_end_kernel(const long long* __restrict__ offsets, long long n_items, int m, long long n_total,
+                                   int rows, int* __restrict__ row_end) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    if (r >= n_total) { row_end[r] = 0; return; }
+    long long lo = 0, hi = n_items;                 // offsets[lo] <= r < offsets[hi]
+    while (hi - lo > 1) {
+        const long long mid = (lo + hi) >> 1;
+        if (offsets[mid] <= r) lo = mid; else hi = mid;
+    }
+    row_end[r] = m + (int)offsets[lo + 1];
+}
+
+// one block per song: out[1 + 2k] = S_yy,k, out[2 + 2k] = S_xy,k.  Each row's partials are summed over the units of its
+// tile in unit order, a thread's rows in row order, then the block in a fixed tree - a fixed order for a given shape.
+constexpr int kKadSongReduceThreads = 128;
+__global__ void __launch_bounds__(kKadSongReduceThreads)
+kad_song_reduce_kernel(const double* __restrict__ partial, const int* __restrict__ unit_start,
+                       const long long* __restrict__ offsets, double* __restrict__ out) {
+    __shared__ double red[2][kKadSongReduceThreads / 32];
+    const int k = blockIdx.x;
+    double xy = 0.0, yy = 0.0;
+    for (long long r = offsets[k] + threadIdx.x; r < offsets[k + 1]; r += kKadSongReduceThreads) {
+        const int t = (int)(r >> 7), lr = (int)(r & 127);
+        double rx = 0.0, ry = 0.0;
+        for (int u = unit_start[t]; u < unit_start[t + 1]; ++u) {
+            rx += partial[(size_t)u * 256 + lr];
+            ry += partial[(size_t)u * 256 + 128 + lr];
+        }
+        xy += rx;
+        yy += ry;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        xy += __shfl_xor_sync(0xffffffffu, xy, o);
+        yy += __shfl_xor_sync(0xffffffffu, yy, o);
+    }
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) { red[0][w] = xy; red[1][w] = yy; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double sxy = 0.0, syy = 0.0;
+        for (int i = 0; i < kKadSongReduceThreads / 32; ++i) { sxy += red[0][i]; syy += red[1][i]; }
+        out[1 + 2 * (size_t)k] = syy;
+        out[2 + 2 * (size_t)k] = sxy;
+    }
 }
 
 // state: prefix[2] (u32), then rank[2] (u64) = the rank of each target among the values that match its prefix

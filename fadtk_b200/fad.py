@@ -4,6 +4,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_embd_statistics      fad.py:42-48   -> shifted E^T E tensor-core kernel (csrc/stats.cuh)
     calc_frechet_distance     fad.py:51-120  -> Newton-Schulz GEMM chain on the PSD form (csrc/frechet.cuh)
     calc_kernel_audio_distance  (no reference counterpart) -> wgmma pair-tile kernels (csrc/kad.cuh)
+    calc_kernel_audio_distance_songs                       -> the same, every song against one baseline in one pass
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -113,21 +114,73 @@ def calc_kernel_audio_distance(emb_baseline, emb_eval) -> KADResults:
         raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {m}, eval {n})")
     if x.shape[1] != y.shape[1]:
         raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
-    z = torch.cat([x, y]).contiguous()
+    from . import _native
+    eng = _native.engine()
+    z = _kad_device_rows(torch.cat([x, y]), eng)
+    sigma = _kad_bandwidth(eng, z, m)
+    s_xx, s_yy, s_xy = (float(v) for v in eng.kad_sums(z, m, torch.tensor([sigma], dtype=torch.float64,
+                                                                               device=eng.torch_device)).cpu().numpy())
+    return KADResults(score=_kad_score(s_xx, s_yy, s_xy, m, n), bandwidth=sigma, n_baseline=m, n_eval=n)
+
+
+def _kad_device_rows(z: torch.Tensor, eng) -> torch.Tensor:
+    """[rows, d] fp16 -> contiguous on the engine's device, the width zero-padded to a multiple of 8 (no distance
+    changes)."""
+    z = z.contiguous()
     pad = -z.shape[1] % 8
     if pad:
         z = torch.nn.functional.pad(z, (0, pad))
-    from . import _native
-    eng = _native.engine()
-    z = z.to(eng.torch_device)
+    return z.to(eng.torch_device, non_blocking=True)
+
+
+def _kad_bandwidth(eng, z: torch.Tensor, m: int) -> float:
+    """sigma from the first m rows of z (device): the numpy median of their pairwise distances; ValueError when 0."""
     sq = eng.kad_median_sq(z[:m]).cpu().numpy()
     sigma = 0.5 * (float(np.sqrt(sq[0])) + float(np.sqrt(sq[1])))
     if not sigma > 0.0:
         raise ValueError("KAD bandwidth is 0: more than half of the baseline pairs are identical rows")
-    s_xx, s_yy, s_xy = (float(v) for v in eng.kad_sums(z, m, torch.tensor([sigma], dtype=torch.float64,
-                                                                               device=eng.torch_device)).cpu().numpy())
-    mmd2 = 2.0 * s_xx / (m * (m - 1.0)) + 2.0 * s_yy / (n * (n - 1.0)) - 2.0 * s_xy / (float(m) * n)
-    return KADResults(score=1000.0 * mmd2, bandwidth=sigma, n_baseline=m, n_eval=n)
+    return sigma
+
+
+def _kad_score(s_xx: float, s_yy: float, s_xy: float, m: int, n: int) -> float:
+    """1000 * MMD^2_u from the three kernel sums"""
+    return 1000.0 * (2.0 * s_xx / (m * (m - 1.0)) + 2.0 * s_yy / (n * (n - 1.0)) - 2.0 * s_xy / (float(m) * n))
+
+
+def calc_kernel_audio_distance_songs(emb_baseline, songs) -> list[KADResults]:
+    """KAD of every song against one baseline: for each fp16 [n_k, d] array in ``songs``, the value
+    calc_kernel_audio_distance(emb_baseline, songs[k]) is defined to be (same sigma from the baseline alone, same sums),
+    with sigma and the baseline's own pair sum computed once for all songs and every song's sums in one GPU pass
+    (fad_kad_song_sums).  A song with fewer than two rows gets score NaN (n_eval still says how many rows it had).
+    Raises ValueError like calc_kernel_audio_distance: non-fp16 or non-2-D input, widths that differ from the
+    baseline's, fewer than two baseline rows, sigma = 0."""
+    x = _kad_rows(emb_baseline, "baseline")
+    ys = [_kad_rows(y, f"song {k}") for k, y in enumerate(songs)]
+    for k, y in enumerate(ys):
+        if y.shape[1] != x.shape[1]:
+            raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, song {k} {y.shape[1]})")
+    offsets = np.zeros(len(ys) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([int(y.shape[0]) for y in ys])
+    return _kad_songs(torch.cat([x, *[y.to(x.device) for y in ys]]), int(x.shape[0]), offsets)
+
+
+def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray) -> list[KADResults]:
+    """z = [X; Y_1; ...] fp16 (host or device), offsets int64 [K + 1] into the rows after X -> one KADResults per song"""
+    if m < 2:
+        raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {m})")
+    from . import _native
+    eng = _native.engine()
+    z = _kad_device_rows(z, eng)
+    sigma = _kad_bandwidth(eng, z, m)
+    dev = eng.torch_device
+    sums = eng.kad_song_sums(z, m, torch.from_numpy(offsets).to(dev),
+                             torch.tensor([sigma], dtype=torch.float64, device=dev)).cpu().numpy()
+    s_xx = float(sums[0])
+    out = []
+    for k, n in enumerate(np.diff(offsets).tolist()):
+        score = _kad_score(s_xx, float(sums[1 + 2 * k]), float(sums[2 + 2 * k]), m, n) if n >= 2 else float("nan")
+        out.append(KADResults(score=score, bandwidth=sigma, n_baseline=m, n_eval=n))
+    return out
 
 
 def kad_embedding_dir(path, model_name: str) -> Path:
@@ -458,6 +511,71 @@ class FrechetAudioDistance:
                 raise ValueError(f"KAD needs fp16 embedding caches; {p} holds {emb.dtype}")
             sets.append(emb)
         return calc_kernel_audio_distance(*sets)
+
+    def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str]) -> Path:
+        """KAD of every file in eval_dir against the embeddings of baseline_dir (calc_kernel_audio_distance_songs: the
+        bandwidth and the baseline's pair sum once, every song's sums in one GPU pass), written as score_individual
+        writes FAD: rows ``file,score`` sorted by |score|, commas in names replaced, no header; a str csv_name goes
+        under data/kad-individual/<model>/, and an existing table is returned untouched.  Files whose cache is
+        missing, unreadable or not an fp16 [rows, d] array of the baseline's width, and files with fewer than two
+        embedding rows, are logged and dropped."""
+        csv = Path(csv_name)
+        if isinstance(csv_name, str):
+            csv = Path('data') / 'kad-individual' / self.ml.name / csv_name
+        if csv.exists():
+            log.info(f"CSV file {csv} already exists, exiting...")
+            return csv
+
+        from . import _io_native
+        files = _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name))
+        if not files:
+            raise ValueError(f"no {self.ml.name} embeddings cached under {baseline_dir}: embed the baseline directory first")
+        x, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
+        if x.dtype != np.float16:
+            raise ValueError(f"KAD needs fp16 embedding caches; {baseline_dir} holds {x.dtype}")
+        kad_embedding_dir(eval_dir, self.ml.name)
+        m, d = x.shape
+
+        def _report(f, msg):
+            log.error(f"An error occurred calculating individual KAD using model {self.ml.name} on file {f}")
+            log.error(msg)
+
+        # fp16 caches read natively in one pass (libfadtk_io.so) into one pinned buffer after the baseline rows
+        all_files = sorted(Path(eval_dir).glob("*.*"))
+        caches = [get_cache_embedding_path(self.ml.name, f) for f in all_files]
+        n_rows, cols, ndim, dt, st = _io_native.npy_probe(caches, self.audio_load_worker)
+        keep = []
+        for i, f in enumerate(all_files):
+            if st[i] != _io_native.OK:
+                _report(f, f"cannot read the embedding cache {caches[i]} (status {int(st[i])})")
+            elif dt[i] != 2 or ndim[i] != 2:
+                _report(f, f"KAD needs an fp16 [rows, d] embedding cache; {caches[i]} is not one")
+            elif cols[i] != d:
+                _report(f, f"embedding widths differ (baseline {d}, {caches[i]} {int(cols[i])})")
+            elif n_rows[i] < 2:
+                _report(f, f"KAD needs at least two embedding rows, {caches[i]} has {int(n_rows[i])}"
+                           " (This probably means that your audio is too short)")
+            else:
+                keep.append(i)
+        pairs = []
+        if keep:
+            rows = n_rows[keep]
+            offs = np.zeros(len(keep) + 1, dtype=np.int64)
+            offs[1:] = np.cumsum(rows)
+            host = torch.empty((m + int(offs[-1]), d), dtype=torch.float16, pin_memory=torch.cuda.is_available())
+            host[:m] = torch.from_numpy(x)
+            _, st = _io_native.npy_read_f16([caches[i] for i in keep], rows, d, host[m:].numpy(), offs,
+                                            self.audio_load_worker)
+            for k in np.nonzero(st != _io_native.OK)[0]:     # vanished / rewritten since the probe: dropped below
+                _report(all_files[keep[k]], f"cannot read {caches[keep[k]]} (status {int(st[k])})")
+                host[m + offs[k]:m + offs[k + 1]] = 0.0
+            res = _kad_songs(host, m, offs)
+            pairs = [(all_files[i], res[k].score) for k, i in enumerate(keep) if st[k] == _io_native.OK]
+
+        pairs = sorted(pairs, key=lambda x: np.abs(x[1]))
+        csv.parent.mkdir(parents=True, exist_ok=True)
+        csv.write_text("\n".join([",".join([str(x).replace(',', '_') for x in row]) for row in pairs]))
+        return csv
 
     def score_inf(self, baseline: PathLike, eval_files: list[Path], steps: int = 25, min_n=500, raw: bool = False):
         """FAD for growing sample counts and the FAD-inf extrapolation (fad.py:304-351).

@@ -1,8 +1,10 @@
-"""``python -m fadtk_b200.kad <model> <baseline> <eval> [csv] [-w N] [-s sox]`` - Kernel Audio Distance between two
-audio directories (fad.calc_kernel_audio_distance).  Directories without embedding caches are embedded first (under
-``torchrun`` the embedding is sharded over the ranks as for ``fadtk``; rank 0 computes and reports).  With ``csv``, one
-row ``model,baseline,eval,kad,bandwidth,n_baseline,n_eval,time`` is appended; a new file gets the header first, and an
-existing file with another header is refused rather than mixed.  The ``fadtk`` command line itself is unchanged.
+"""``python -m fadtk_b200.kad <model> <baseline> <eval> [csv] [--indiv] [-w N] [-s sox]`` - Kernel Audio Distance
+between two audio directories (fad.calc_kernel_audio_distance).  Directories without embedding caches are embedded
+first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``; rank 0 computes and reports).  With
+``csv``, one row ``model,baseline,eval,kad,bandwidth,n_baseline,n_eval,time`` is appended; a new file gets the header
+first, and an existing file with another header is refused rather than mixed.  With ``--indiv``, every file of the eval
+directory is scored on its own against the baseline (FrechetAudioDistance.score_kad_individual) and ``csv`` is that
+table (default kad-individual-results.csv).  The ``fadtk`` command line itself is unchanged.
 """
 from __future__ import annotations
 
@@ -18,7 +20,9 @@ _KAD_ARGS = (
     (("model",), dict(type=str, help="embedding model (a registry name)")),
     (("baseline",), dict(type=str, help="baseline audio directory (its embeddings also set the kernel bandwidth)")),
     (("eval",), dict(type=str, help="evaluation audio directory")),
-    (("csv",), dict(type=str, nargs="?", help="append the result row here")),
+    (("csv",), dict(type=str, nargs="?", help="append the result row here; with --indiv: where the per-file table "
+                                              "goes (default kad-individual-results.csv)")),
+    (("--indiv",), dict(action="store_true", help="score every evaluation file on its own against the baseline")),
 )
 
 
@@ -48,7 +52,7 @@ def main(argv=None) -> int:
     model = registry[args.model]
     for p in (args.baseline, args.eval):            # before any embedding work: statistics cannot give a KAD
         kad_embedding_dir(p, model.name)
-    if args.csv:
+    if args.csv and not args.indiv:
         _check_csv(args.csv)
     dist.init_from_env()
     _embed_directories(model, (args.baseline, args.eval), args.workers)
@@ -57,6 +61,12 @@ def main(argv=None) -> int:
         return 0
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
+    if args.indiv:
+        table = Path(args.csv or "kad-individual-results.csv")
+        fad.score_kad_individual(args.baseline, args.eval, table)
+        log.info(f"Individual KAD scores saved to {table}")
+        dist.shutdown()
+        return 0
     res = fad.score_kad(args.baseline, args.eval)
     if args.csv:
         _append_row(args.csv, (model.name, args.baseline, args.eval, res.score, res.bandwidth, res.n_baseline,

@@ -275,6 +275,14 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
 int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream);
 int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
                  void* stream);
+/* Per-song KAD sums against one baseline: z = [X; Y_1; ...; Y_K] (fp16 [m + n_total, d], X first); offsets = device
+ * int64 [n_items + 1], song k = rows [offsets[k], offsets[k+1]) of the Y part (offsets[0] = 0, non-decreasing,
+ * n_total = offsets[n_items]; read back to the host, so the call synchronises the stream once); sigma = device fp64
+ * scalar.  out (device fp64 [1 + 2 n_items]) = S_xx, then per song S_yy,k (i < j within the song), S_xy,k (all pairs
+ * with X).  S_xx and the shift are computed once; a song of 0 or 1 rows gets S_yy,k = 0 (and S_xy,k = 0 when empty).
+ * Each value is the quantity fad_kad_sums gives for [X; Y_k], bitwise reproducible (fixed work units, no atomics). */
+int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items, int d,
+                      const double* sigma, double* out, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
