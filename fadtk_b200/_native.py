@@ -67,6 +67,10 @@ SIGNATURES = {
     "fad_whisper_logmel": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_w2v_load": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int]),
     "fad_w2v_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_w2v_normalize": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_w2v_conv": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_w2v_posconv": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_w2v_layer": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_encodec_load": (C.c_int, [c_vp, c_vp, C.c_int, c_ll, C.c_int]),
     "fad_encodec_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_encodec_conv": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, C.c_int, C.c_int, C.c_int, c_vp, c_vp]),
@@ -452,6 +456,29 @@ class Engine:
         n, L = pcm.shape
         out = torch.empty((n, self.w2v_frames(L), self._w2v_d), dtype=torch.float16, device=pcm.device)
         _check(lib().fad_w2v_forward(self._h, pcm.data_ptr(), n, L, int(layer), out.data_ptr(), _stream()))
+        return out
+
+    # Stage entries of the loaded encoder: they write into the caller's cuda tensors (shapes in include/fadtk_b200.h)
+    # and raise NativeError on rejected arguments.
+    def w2v_normalize(self, pcm, n_clips: int, L: int, out):
+        """fad_w2v_normalize: pcm int16 [n_clips, L] -> out fp32 [n_clips, L]"""
+        _check(lib().fad_w2v_normalize(self._h, _ptr(pcm), int(n_clips), int(L), _ptr(out), _stream()))
+        return out
+
+    def w2v_conv(self, c: int, x, B: int, L: int, out):
+        """fad_w2v_conv: feature-encoder conv c at the frames of L-sample clips; x [B, T_c, 512] (c = 0: fp32 [B, L])
+        -> out [B, T_c+1, 512] (fp16; c = 6: fp32)"""
+        _check(lib().fad_w2v_conv(self._h, int(c), _ptr(x), int(B), int(L), _ptr(out), _stream()))
+        return out
+
+    def w2v_posconv(self, x, B: int, S: int, out):
+        """fad_w2v_posconv: x fp32 [B, S, d] -> out fp32 [B, S, d] = x + GELU(pos_conv(x))"""
+        _check(lib().fad_w2v_posconv(self._h, _ptr(x), int(B), int(S), _ptr(out), _stream()))
+        return out
+
+    def w2v_layer(self, l: int, x, B: int, S: int, out):
+        """fad_w2v_layer: encoder layer l, x fp32 [B, S, d] (the stream entering it) -> out fp32 [B, S, d]"""
+        _check(lib().fad_w2v_layer(self._h, int(l), _ptr(x), int(B), int(S), _ptr(out), _stream()))
         return out
 
     # ------------------------------------------------------------------ Encodec

@@ -37,9 +37,12 @@ w2v_normalize_kernel(const int16_t* __restrict__ pcm, int L, float* __restrict__
 // so the fp32 [T][512] conv output never exists in HBM (it was written once and read three times before).
 // Moments and the 10 x 10 forms are evaluated in fp64.
 
-// acc[b][0..9] += sum_t x[5t + j];  acc[b][10 + j(j+1)/2 + j'] += sum_t x[5t + j] x[5t + j']  (j' <= j).  grid (slices, B).
+// Per-(clip, slice) window moments, in fixed order so that the GroupNorm coefficients are reproducible bit for bit:
+// part[b][s][0..9] = sum_t x[5t + j],  part[b][s][10 + j(j+1)/2 + j'] = sum_t x[5t + j] x[5t + j']  (j' <= j)
+// over the frames t of slice s.  grid (kW2vMomSlices, B).
+constexpr int kW2vMomSlices = 32;
 __global__ void __launch_bounds__(256)
-w2v_conv0_moments_kernel(const float* __restrict__ xn, int L, int T1, double* __restrict__ acc /*[B][65]*/)
+w2v_conv0_moments_kernel(const float* __restrict__ xn, int L, int T1, double* __restrict__ part /*[B][kW2vMomSlices][65]*/)
 {
     __shared__ double red[8][65];
     const float* x = xn + (size_t)blockIdx.y * L;
@@ -67,27 +70,32 @@ w2v_conv0_moments_kernel(const float* __restrict__ xn, int L, int T1, double* __
     if (threadIdx.x < 65) {
         double r = 0.0;
         for (int w = 0; w < 8; ++w) r += red[w][threadIdx.x];
-        atomicAdd(acc + (size_t)blockIdx.y * 65 + threadIdx.x, r);
+        part[((size_t)blockIdx.y * gridDim.x + blockIdx.x) * 65 + threadIdx.x] = r;
     }
 }
 
 // coef[b][c] = (scale, shift) with GroupNorm(y)*gamma + beta = conv_nobias(x) * scale + shift.  One thread per (b, c).
 __global__ void __launch_bounds__(256)
-w2v_conv0_coef_kernel(const double* __restrict__ acc, const float* __restrict__ w /*[512][10]*/, const float* __restrict__ bias,
+w2v_conv0_coef_kernel(const double* __restrict__ part /*[B][kW2vMomSlices][65]*/, const float* __restrict__ w /*[512][10]*/, const float* __restrict__ bias,
                       const float* __restrict__ gamma, const float* __restrict__ beta, int T1, int n /* B*512 */, float2* __restrict__ coef)
 {
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     const int b = i >> 9, c = i & 511;
-    const double* a = acc + (size_t)b * 65;
+    const double* p = part + (size_t)b * kW2vMomSlices * 65;
+    auto a = [p](int k) {                            // moment k of the clip: its slices summed in slice order
+        double r = p[k];
+        for (int s = 1; s < kW2vMomSlices; ++s) r += p[s * 65 + k];
+        return r;
+    };
     const double inv = 1.0 / (double)T1;
     double wv[10], m[10];
-    for (int j = 0; j < 10; ++j) { wv[j] = (double)w[c * 10 + j]; m[j] = a[j] * inv; }
+    for (int j = 0; j < 10; ++j) { wv[j] = (double)w[c * 10 + j]; m[j] = a(j) * inv; }
     double mean = 0.0, var = 0.0;
     for (int j = 0; j < 10; ++j) {
         mean += wv[j] * m[j];
         for (int k = 0; k <= j; ++k) {
-            const double cov = a[10 + j * (j + 1) / 2 + k] * inv - m[j] * m[k];
+            const double cov = a(10 + j * (j + 1) / 2 + k) * inv - m[j] * m[k];
             var += (k == j ? 1.0 : 2.0) * wv[j] * wv[k] * cov;
         }
     }

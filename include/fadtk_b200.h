@@ -183,6 +183,19 @@ int fad_encodec_lstm(fad_handle* h, const float* z_f32, long long n_clips, int T
 int fad_w2v_load(fad_handle* h, const int* cfg, const void* const* tensors_host, int n_tensors, int max_clips, int max_len);
 /* pcm: int16 mono [n_clips][L] (device), equal lengths; emb_out: fp16 [n_clips][frames(L)][d_model]. */
 int fad_w2v_forward(fad_handle* h, const int16_t* pcm, long long n_clips, int L, int layer, void* emb_out_f16, void* stream);
+/* Stage entries (parity tests); each calls the launch code fad_w2v_forward calls and fails, launching nothing and
+ * writing nothing, on arguments it could not honour.  B in [1, max_clips]; 16-byte aligned device pointers.
+ * fad_w2v_normalize (no load needed): pcm int16 [n_clips][L] -> out fp32 [n_clips][L], (x - mean) / sqrt(var + 1e-7).
+ * fad_w2v_conv: feature-encoder conv c in [0, 7) of the loaded variant at the frames T_c of clips of L samples
+ * (400 <= L <= max_len): c = 0 x fp32 [B][L] (normalised) -> out fp16 [B][T_1][512]; c = 1..5 x fp16 [B][T_c][512] ->
+ * out fp16 [B][T_c+1][512]; c = 6 -> out fp32 [B][T_7][512].
+ * fad_w2v_posconv: x fp32 [B][S][d] -> out = x + GELU(pos_conv(x)), S in [1, frames(max_len)].
+ * fad_w2v_layer: encoder layer l in [0, layers), x fp32 [B][S][d] the stream entering it (post-LN: the previous
+ * LayerNorm's output; pre-LN: the raw stream) -> out fp32 [B][S][d] the stream leaving it. */
+int fad_w2v_normalize(fad_handle* h, const int16_t* pcm, long long n_clips, int L, float* out_f32, void* stream);
+int fad_w2v_conv(fad_handle* h, int c, const void* x, long long B, int L, void* out, void* stream);
+int fad_w2v_posconv(fad_handle* h, const float* x_f32, long long B, int S, float* out_f32, void* stream);
+int fad_w2v_layer(fad_handle* h, int l, const float* x_f32, long long B, int S, float* out_f32, void* stream);
 
 /* ---- statistics: replaces calc_embd_statistics (fadtk/fad.py:42-48) and
  * _process_file / calculate_embd_statistics_online (fadtk/utils.py:13-46) ----------------
