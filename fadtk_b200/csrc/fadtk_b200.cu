@@ -5,6 +5,7 @@
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
+#include <cxxabi.h>
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
@@ -12,6 +13,7 @@
 #include <cstring>
 #include <set>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "conv_gemm.cuh"
@@ -110,7 +112,8 @@ struct fad_handle {
     int device = 0;
     int num_sms = 0;
     int max_examples = 0;
-    long long launches = 0;
+    long long launches = 0;          // kernels launched through `launch` (fad_launch_count)
+    int gemm_clusters[2] = {};       // co-resident CTA pairs of the wgmma GEMM, by weight mode (fad_create)
 
     // front-end tables
     double *d_twiddle = nullptr, *d_hann = nullptr, *d_melw = nullptr;
@@ -163,34 +166,81 @@ struct fad_handle {
 
 namespace {
 
-template <int N_TILE, int STAGES, int WMODE>
-int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const fad::ConvGemmParams& p, cudaStream_t st) {
-    static int max_clusters = 0;                      // co-resident CTA pairs, queried once per instantiation
-    constexpr uint32_t smem = fad::conv_gemm_smem_bytes<N_TILE, STAGES, WMODE>();
-    static_assert(smem <= 227 * 1024, "over the per-CTA shared-memory limit");
-    auto kern = fad::conv_gemm_kernel<N_TILE, STAGES, WMODE>;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = fad::kClusterCtas; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+// The kernel's demangled signature, for error messages.
+std::string kernel_name(const void* kernel) {
+    const char* mangled = nullptr;
+    if (cudaFuncGetName(&mangled, kernel) != cudaSuccess || !mangled) return "kernel launch";
+    int status = 0;
+    char* demangled = abi::__cxa_demangle(mangled, nullptr, nullptr, &status);
+    const std::string name = demangled ? demangled : mangled;
+    free(demangled);
+    return name;
+}
+
+// Every kernel launch of the library: kernel<<<grid, block, smem, st>>>(args...) with the launch attributes
+// attrs[0, n_attrs), counted in h->launches.  A grid with a zero dimension launches and counts nothing.  The arguments
+// are converted to the kernel's parameter types, and defaulted parameters must be passed too.
+template <typename... Params, typename... Args>
+int launch_attrs(fad_handle* h, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                 cudaLaunchAttribute* attrs, unsigned n_attrs, Args&&... args) {
+    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(fad::kConvGemmThreads);
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
     cfg.dynamicSmemBytes = smem;
     cfg.stream = st;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    if (max_clusters == 0) {
-        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        cfg.gridDim = dim3(fad::kClusterCtas * (unsigned)h->num_sms);
-        CK(cudaOccupancyMaxActiveClusters(&max_clusters, kern, &cfg));
-        if (max_clusters <= 0) return fail("conv_gemm_kernel: no CTA pair fits on the device");
-    }
-    const int units = (p.img_groups * p.tiles_h * p.tiles_w + 1) / 2 * p.n_tiles;
-    if (units == 0) return 0;
-    cfg.gridDim = dim3(fad::kClusterCtas * (unsigned)std::min(units, max_clusters));
-    CK(cudaLaunchKernelEx(&cfg, kern, mx, mw, p));
-    CK(cudaGetLastError());
+    cfg.attrs = attrs;
+    cfg.numAttrs = n_attrs;
+    cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+    const cudaError_t last = cudaGetLastError();     // also clears the error state a failed launch leaves behind
+    if (e == cudaSuccess) e = last;
+    if (e != cudaSuccess) return fail(kernel_name((const void*)kernel) + ": " + cudaGetErrorString(e));
     h->launches++;
     return 0;
+}
+template <typename... Params, typename... Args>
+int launch(fad_handle* h, void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+    return launch_attrs(h, kernel, grid, block, smem, st, nullptr, 0, std::forward<Args>(args)...);
+}
+
+// The wgmma GEMM (conv_gemm.cuh) by weight mode, 0: fp16, 1: fp16 hi/lo pair.  Stages: as many 32 / 48 KiB stages as
+// fit next to the two 32 KiB epilogue tiles in 227 KiB.
+template <int WMODE> struct Gemm {
+    static constexpr int kStages = WMODE ? 3 : 4;
+    static constexpr uint32_t kSmem = fad::conv_gemm_smem_bytes<128, kStages, WMODE>();
+    static_assert(kSmem <= 227 * 1024, "over the per-CTA shared-memory limit");
+    static constexpr auto kernel = fad::conv_gemm_kernel<128, kStages, WMODE>;
+};
+
+cudaLaunchAttribute cta_pair() {
+    cudaLaunchAttribute attr = {};
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = fad::kClusterCtas; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    return attr;
+}
+
+// Shared memory above the default for the GEMM, and how many of its CTA pairs fit on the device at once.
+template <int WMODE>
+int setup_gemm(fad_handle* h) {
+    CK(cudaFuncSetAttribute(Gemm<WMODE>::kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Gemm<WMODE>::kSmem));
+    cudaLaunchAttribute attr = cta_pair();
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(fad::kClusterCtas * (unsigned)h->num_sms);
+    cfg.blockDim = dim3(fad::kConvGemmThreads);
+    cfg.dynamicSmemBytes = Gemm<WMODE>::kSmem;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    CK(cudaOccupancyMaxActiveClusters(&h->gemm_clusters[WMODE], Gemm<WMODE>::kernel, &cfg));
+    if (h->gemm_clusters[WMODE] <= 0) return fail("conv_gemm_kernel: no CTA pair fits on the device");
+    return 0;
+}
+
+template <int WMODE>
+int launch_conv_gemm(fad_handle* h, const CUtensorMap& mx, const CUtensorMap& mw, const fad::ConvGemmParams& p, cudaStream_t st) {
+    const int units = (p.img_groups * p.tiles_h * p.tiles_w + 1) / 2 * p.n_tiles;
+    cudaLaunchAttribute attr = cta_pair();
+    return launch_attrs(h, Gemm<WMODE>::kernel, dim3(fad::kClusterCtas * (unsigned)std::min(units, h->gemm_clusters[WMODE])),
+                        dim3(fad::kConvGemmThreads), Gemm<WMODE>::kSmem, st, &attr, 1, mx, mw, p);
 }
 
 // a_cols: channels actually stored per pixel/row of the activation (<= g.Cin); the TMA box reads
@@ -217,11 +267,6 @@ int encode_layer_maps(const LayerGeom& g, const void* x, long long nb_dim, const
 // Encoder self-attention on wgmma (attention_wgmma.cuh).  qkv: fp16 [clips * S][3 d] (q | k | v, head h at column h * 64),
 // out: fp16 [clips * S][d].
 int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, int S, int d, int heads, __half* out, cudaStream_t st) {
-    static bool attr_set = false;
-    if (!attr_set) {
-        CK(cudaFuncSetAttribute(fad::attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kAtSmem));
-        attr_set = true;
-    }
     if (heads * 64 != d) return fail("attention_wgmma: head dimension must be 64");
     CUtensorMap map;
     const uint64_t dims[3] = {(uint64_t)3 * d, (uint64_t)S, (uint64_t)n_clips};
@@ -230,10 +275,8 @@ int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, 
     if (encode_f16_map(&map, qkv, 3, dims, strides, box)) return 1;
     fad::AttnParams p;
     p.S = S; p.d = d; p.heads = heads; p.out = out;
-    fad::attention_wgmma_kernel<<<dim3((S + 127) / 128, heads, (unsigned)n_clips), fad::kAtThreads, fad::kAtSmem, st>>>(map, p);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::attention_wgmma_kernel, dim3((S + 127) / 128, heads, (unsigned)n_clips), fad::kAtThreads, fad::kAtSmem,
+                  st, map, p);
 }
 
 // zero_lo is keyed by weight POINTER: drop the entry whenever that memory is freed or reallocated
@@ -255,9 +298,8 @@ int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CU
     p.bias = bias; p.out = reinterpret_cast<__half*>(out); p.out_f32 = out_f32;
     p.resid = resid; p.resid_C = resid_C; p.resid_res = resid_res; p.resid_shift = resid_shift;
     p.lo_adds = g.split_w == 1 && h->zero_lo.count(w) == 0;
-    // stages: as many 48 / 32 KiB stages as fit next to the two 32 KiB epilogue tiles in 227 KiB
-    if (g.split_w) return launch_conv_gemm<128, 3, 1>(h, mx, mw, p, st);
-    return launch_conv_gemm<128, 4, 0>(h, mx, mw, p, st);
+    if (g.split_w) return launch_conv_gemm<1>(h, mx, mw, p, st);
+    return launch_conv_gemm<0>(h, mx, mw, p, st);
 }
 
 // max |Wl| over the lo parts of a packed hi/lo weight tensor ([hi: 128 rows | lo: 128 rows] per tile), as float bits
@@ -280,16 +322,16 @@ int note_split_weights(fad_handle* h, const void* w, long long n_tiles, long lon
     unsigned int* d_max = nullptr;
     CK(cudaMalloc(&d_max, 4));
     unsigned int mx = 0;
-    cudaError_t e = cudaMemsetAsync(d_max, 0, 4, st);
-    if (e == cudaSuccess) {
-        const unsigned blocks = (unsigned)std::max<long long>(1, std::min<long long>((n_tiles * 128 * K + 255) / 256, (long long)h->num_sms * 16));
-        wlo_absmax_kernel<<<blocks, 256, 0, st>>>(reinterpret_cast<const __half*>(w), n_tiles, K, d_max);
-        e = cudaGetLastError();
-    }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&mx, d_max, 4, cudaMemcpyDeviceToHost, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    const unsigned blocks = (unsigned)std::max<long long>(1, std::min<long long>((n_tiles * 128 * K + 255) / 256, (long long)h->num_sms * 16));
+    const int rc = [&]() -> int {
+        CK(cudaMemsetAsync(d_max, 0, 4, st));
+        if (launch(h, wlo_absmax_kernel, blocks, 256, 0, st, reinterpret_cast<const __half*>(w), n_tiles, K, d_max)) return 1;
+        CK(cudaMemcpyAsync(&mx, d_max, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        return 0;
+    }();
     cudaFree(d_max);
-    if (e != cudaSuccess) return fail(std::string("note_split_weights: ") + cudaGetErrorString(e));
+    if (rc) return 1;
     if (mx == 0) h->zero_lo.insert(w); else h->zero_lo.erase(w);
     return 0;
 }
@@ -369,7 +411,7 @@ void prof_end(fad_handle* h, int cat, size_t e0, cudaStream_t st) {
 template <typename In>
 int launch_stats_dmma(fad_handle* h, const In* E, long long n_rows, int d, const __half* shift, double* acc, cudaStream_t st) {
     constexpr bool kProf = sizeof(In) == 2;
-    if (d % 64 != 0) return fail("d must be a multiple of 64");
+    if (d <= 0 || d % 64 != 0) return fail("d must be a positive multiple of 64");
     fad::StatsDmmaParams p;
     p.n_rows = n_rows; p.d = d; p.n_tiles = d / fad::kSdTile;
     p.n_pairs = p.n_tiles * (p.n_tiles + 1) / 2;
@@ -386,13 +428,10 @@ int launch_stats_dmma(fad_handle* h, const In* E, long long n_rows, int d, const
     if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
     p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
     size_t ev = kProf ? prof_begin(h, st) : 0;
-    fad::stats_dmma_kernel<In><<<(unsigned)jobs, 256, 0, st>>>(E, p);
-    CK(cudaGetLastError());
+    if (launch(h, fad::stats_dmma_kernel<In>, (unsigned)jobs, 256, 0, st, E, p)) return 1;
     if (kProf) { prof_end(h, FAD_PROF_STATS, ev, st); ev = prof_begin(h, st); }
-    fad::stats_dmma_reduce_kernel<<<dim3(p.n_pairs, fad::kSdTile * fad::kSdTile / 256), 256, 0, st>>>(p, acc);
-    CK(cudaGetLastError());
+    if (launch(h, fad::stats_dmma_reduce_kernel, dim3(p.n_pairs, fad::kSdTile * fad::kSdTile / 256), 256, 0, st, p, acc)) return 1;
     if (kProf) prof_end(h, FAD_PROF_STATS_REDUCE, ev, st);
-    h->launches += 2;
     return 0;
 }
 
@@ -450,10 +489,21 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(cudaMalloc(&h->d_melw, melw.size() * 8)); CK(cudaMemcpy(h->d_melw, melw.data(), melw.size() * 8, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&h->d_mel_start, ms.size() * 4)); CK(cudaMemcpy(h->d_mel_start, ms.data(), ms.size() * 4, cudaMemcpyHostToDevice));
     CK(cudaMalloc(&h->d_mel_count, mc.size() * 4)); CK(cudaMemcpy(h->d_mel_count, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
-    CK(cudaFuncSetAttribute(fad::logmel_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)fad::logmel_smem_bytes<double>()));
-    CK(cudaFuncSetAttribute(fad::logmel_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)fad::logmel_smem_bytes<float>()));
+    // one-time kernel setup, for the handle's device: the dynamic shared memory of every kernel that launches with more
+    // than the default 48 KiB, and the GEMM's co-resident CTA pairs
+    const auto smem = [](const void* kernel, size_t bytes) {
+        return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    };
+    CK(smem((const void*)fad::logmel_kernel<double>, fad::logmel_smem_bytes<double>()));
+    CK(smem((const void*)fad::logmel_kernel<float>, fad::logmel_smem_bytes<float>()));
+    CK(smem((const void*)fad::clap_logmel_kernel, fad::clap_logmel_smem_bytes()));
+    CK(smem((const void*)fad::attention_wgmma_kernel, fad::kAtSmem));
+    CK(smem((const void*)fad::clap_window_attention_kernel<24>, fad::att_smem_bytes(24, fad::kAttWarps, fad::kAttStages)));
+    CK(smem((const void*)fad::clap_window_attention_kernel<32>, fad::att_smem_bytes(32, fad::kAttWarps, fad::kAttStages)));
+    CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
+    CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
+    CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
+    if (setup_gemm<0>(h) || setup_gemm<1>(h)) return 1;
     *out = h;
     return 0;
 }
@@ -560,16 +610,11 @@ static int launch_logmel(fad_handle* h, const int16_t* pcm, const long long* ex_
     long long blocks = (frames + fad::kFeWarps - 1) / fad::kFeWarps;
     const long long cap = (long long)h->num_sms * 8;
     if (blocks > cap) blocks = cap;
-    if (blocks == 0) return 0;
     if (use_double)
-        fad::logmel_kernel<double><<<(int)blocks, fad::kFeWarps * 32, fad::logmel_smem_bytes<double>(), st>>>(
-            pcm, ex_start, (int)n, tab, out);
-    else
-        fad::logmel_kernel<float><<<(int)blocks, fad::kFeWarps * 32, fad::logmel_smem_bytes<float>(), st>>>(
-            pcm, ex_start, (int)n, tab, out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+        return launch(h, fad::logmel_kernel<double>, (int)blocks, fad::kFeWarps * 32, fad::logmel_smem_bytes<double>(), st,
+                      pcm, ex_start, (int)n, tab, out);
+    return launch(h, fad::logmel_kernel<float>, (int)blocks, fad::kFeWarps * 32, fad::logmel_smem_bytes<float>(), st,
+                  pcm, ex_start, (int)n, tab, out);
 }
 
 int fad_vggish_logmel(fad_handle* h, const int16_t* pcm, const long long* ex_start,
@@ -592,9 +637,7 @@ int fad_vggish_forward(fad_handle* h, const int16_t* pcm, const long long* ex_st
         if (launch_logmel(h, pcm, ex_start + base, nb, h->logmel, fe_double, st)) return 1;
         prof_end(h, FAD_PROF_LOGMEL, ev, st);
         ev = prof_begin(h, st);
-        fad::conv1_kernel<<<dim3(6, nb), 256, 0, st>>>(h->logmel, h->conv1_w, h->conv1_b, h->act[0]);
-        CK(cudaGetLastError());
-        h->launches++;
+        if (launch(h, fad::conv1_kernel, dim3(6, nb), 256, 0, st, h->logmel, h->conv1_w, h->conv1_b, h->act[0])) return 1;
         prof_end(h, FAD_PROF_CONV1, ev, st);
         for (int i = 0; i < 8; ++i) {
             const float* bias = i < 5 ? h->conv_b[i] : h->fc_b[i - 5];
@@ -613,11 +656,8 @@ int fad_vggish_conv1(fad_handle* h, const float* logmel, long long n_examples, v
     if (!h->vgg_loaded) return fail("fad_vggish_load has not been called");
     if (n_examples <= 0) return 0;
     CK(cudaSetDevice(h->device));
-    fad::conv1_kernel<<<dim3(6, (unsigned)n_examples), 256, 0, (cudaStream_t)stream>>>(
-        logmel, h->conv1_w, h->conv1_b, reinterpret_cast<__half*>(out_f16));
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::conv1_kernel, dim3(6, (unsigned)n_examples), 256, 0, (cudaStream_t)stream,
+                  logmel, h->conv1_w, h->conv1_b, reinterpret_cast<__half*>(out_f16));
 }
 
 int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int Cin,
@@ -651,10 +691,7 @@ int fad_stats_accumulate(fad_handle* h, const void* emb_f16, long long n_rows, i
     if (tensor_core == 0) return launch_stats_dmma(h, E, n_rows, d, shift, acc, st);
     if (d % 64 != 0) return fail("d must be a multiple of 64");
     dim3 grid((unsigned)((n_rows + fad::kSimtRows - 1) / fad::kSimtRows), d / 64, d / 64);
-    fad::stats_simt_kernel<<<grid, 256, 0, st>>>(E, n_rows, d, shift, acc);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::stats_simt_kernel, grid, 256, 0, st, E, n_rows, d, shift, acc);
 }
 
 // ---- the reference's per-file statistics semantics for equal-length files, on the device (fadtk/utils.py:13-46) ----
@@ -666,10 +703,8 @@ int fad_file_means(fad_handle* h, const void* emb_f16, long long n_files, int ro
     CK(cudaSetDevice(h->device));
     long long blocks = (n_files * d + 255) / 256;
     if (blocks > (long long)h->num_sms * 16) blocks = (long long)h->num_sms * 16;
-    fad::file_means_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const __half*>(emb_f16), n_files, rows_per_file, d, m64_out, m16_out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::file_means_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream,
+                  reinterpret_cast<const __half*>(emb_f16), n_files, rows_per_file, d, m64_out, m16_out);
 }
 
 // exact Gram statistics of fp64 rows (no shift): acc[0] += n, acc[1..d] += sum x, outer += sum x x^T (DMMA, fixed order)
@@ -688,11 +723,8 @@ int fad_stats_finalize_mirrored(fad_handle* h, const double* acc, const double* 
     const size_t total = (size_t)d * d;
     unsigned blocks = (unsigned)((total + 255) / 256);
     if (blocks > (unsigned)h->num_sms * 8) blocks = h->num_sms * 8;
-    fad::stats_finalize_mirrored_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
-        acc, acc_means64, acc_means16, reinterpret_cast<const __half*>(shift_f16), rows_per_file, d, keep, mu_out, cov_out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::stats_finalize_mirrored_kernel, blocks, 256, 0, (cudaStream_t)stream,
+                  acc, acc_means64, acc_means16, reinterpret_cast<const __half*>(shift_f16), rows_per_file, d, keep, mu_out, cov_out);
 }
 
 int fad_stats_accumulate_gather(fad_handle* h, const void* emb_f16, long long n_src_rows,
@@ -707,10 +739,8 @@ int fad_stats_accumulate_gather(fad_handle* h, const void* emb_f16, long long n_
     const long long vecs = n_idx * (d / 8);
     long long blocks = (vecs + 255) / 256;
     if (blocks > (long long)h->num_sms * 16) blocks = (long long)h->num_sms * 16;
-    fad::gather_rows_kernel<<<(unsigned)blocks, 256, 0, (cudaStream_t)stream>>>(
-        reinterpret_cast<const __half*>(emb_f16), idx, n_idx, d, h->gather_buf);
-    CK(cudaGetLastError());
-    h->launches++;
+    if (launch(h, fad::gather_rows_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream,
+               reinterpret_cast<const __half*>(emb_f16), idx, n_idx, d, h->gather_buf)) return 1;
     return launch_stats_dmma(h, h->gather_buf, n_idx, d, reinterpret_cast<const __half*>(shift_f16), acc, (cudaStream_t)stream);
 }
 
@@ -721,11 +751,8 @@ int fad_stats_finalize(fad_handle* h, const double* acc, const void* shift_f16, 
     const size_t total = (size_t)d * d;
     unsigned blocks = (unsigned)((total + 255) / 256);
     if (blocks > (unsigned)h->num_sms * 8) blocks = h->num_sms * 8;
-    fad::stats_finalize_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(
-        acc, reinterpret_cast<const __half*>(shift_f16), d, mu_out, cov_out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::stats_finalize_kernel, blocks, 256, 0, (cudaStream_t)stream,
+                  acc, reinterpret_cast<const __half*>(shift_f16), d, mu_out, cov_out);
 }
 
 // Stage entry (parity test): encoder self-attention of n_clips sequences of S positions, heads of 64 dims.
@@ -736,11 +763,8 @@ extern "C" int fad_attention(fad_handle* h, const void* qkv_f16, long long n_cli
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
     if (!legacy) return launch_attention_wgmma(h, reinterpret_cast<const __half*>(qkv_f16), n_clips, S, d, d / 64, reinterpret_cast<__half*>(out_f16), st);
-    fad::whisper_flash_attention_kernel<<<dim3((S + 63) / 64, d / 64, (unsigned)n_clips), 128, 0, st>>>(
-        reinterpret_cast<const __half*>(qkv_f16), S, d, reinterpret_cast<__half*>(out_f16));
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::whisper_flash_attention_kernel, dim3((S + 63) / 64, d / 64, (unsigned)n_clips), 128, 0, st,
+                  reinterpret_cast<const __half*>(qkv_f16), S, d, reinterpret_cast<__half*>(out_f16), nullptr, nullptr);
 }
 
 
@@ -880,20 +904,15 @@ unsigned elem_blocks(const fad_handle* h, int d) {
 
 int launch_dgemm(fad_handle* h, const fad::DgemmStrided& p, int families, int d, cudaStream_t st) {
     dim3 grid((d + fad::kDgTileN - 1) / fad::kDgTileN, (d + fad::kDgTileM - 1) / fad::kDgTileM, (unsigned)(p.items * families));
-    fad::dgemm_strided_kernel<<<grid, 256, 0, st>>>(p, d);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::dgemm_strided_kernel, grid, 256, 0, st, p, d);
 }
 
 // Coupled Newton-Schulz on the g matrices A_z: on return w.Y_z ~ sqrt(sym(A_z)/|A_z|_F + delta I), w.Z_z its
 // inverse, scal[z] = {|A_z|_F, tr A_z}.
 int newton_schulz(fad_handle* h, const FrechetWorkspace& w, const double* A, double* scal, int g, int d, int iters,
                   cudaStream_t st) {
-    fad::norm_trace_kernel<<<g, 1024, 0, st>>>(A, d, scal);
-    fad::ns_init_kernel<<<dim3(elem_blocks(h, d), g), 256, 0, st>>>(A, d, scal, w.Y, w.Z, w.flags);
-    CK(cudaGetLastError());
-    h->launches += 2;
+    if (launch(h, fad::norm_trace_kernel, g, 1024, 0, st, A, d, scal) ||
+        launch(h, fad::ns_init_kernel, dim3(elem_blocks(h, d), g), 256, 0, st, A, d, scal, w.Y, w.Z, w.flags)) return 1;
     // (Y, Z) <-> (Yn, Zn) ping-pong on a fixed host schedule; an even iteration count lands the
     // last scheduled update in (Y, Z).  If an item stops early (dev < tol) the two pairs differ by
     // one factor W with |W - I| < tol, i.e. by < 1e-12 relative - either is the converged iterate.
@@ -924,9 +943,7 @@ int frechet_items(fad_handle* h, const FrechetWorkspace& w, const double* mu1, c
                   const double* mu2, const double* cov2, int g, int d, int iters, const int* ok,
                   const long long* offsets, bool with_resid, double* out, cudaStream_t st) {
     const long long T = (long long)d * d;
-    fad::norm_trace_kernel<<<g, 1024, 0, st>>>(cov2, d, w.scalC);
-    CK(cudaGetLastError());
-    h->launches++;
+    if (launch(h, fad::norm_trace_kernel, g, 1024, 0, st, cov2, d, w.scalC)) return 1;
     fad::DgemmStrided p = {};
     p.items = g; p.in_slot = p.out_slot = p.clear_slot = -1;
     p.f[0] = {sqrt1, cov2, w.P, 0, T, T, 1.0, 0.0};                                 // P = S C2_z
@@ -938,14 +955,10 @@ int frechet_items(fad_handle* h, const FrechetWorkspace& w, const double* mu1, c
         CK(cudaMemsetAsync(w.resid, 0, sizeof(double), st));
         p.f[0] = {w.Y, w.Y, w.P, T, T, T, 1.0, 0.0};                                // P = Y Y
         if (launch_dgemm(h, p, 1, d, st)) return 1;
-        fad::resid_kernel<<<elem_blocks(h, d), 256, 0, st>>>(w.P, w.M, d, w.scalM, w.resid);
-        h->launches++;
+        if (launch(h, fad::resid_kernel, elem_blocks(h, d), 256, 0, st, w.P, w.M, d, w.scalM, w.resid)) return 1;
     }
-    fad::frechet_assemble_kernel<<<g, 256, 0, st>>>(mu1, mu2, d, scal1, w.scalC, w.scalM, w.Y, w.Z,
-                                                    with_resid ? w.resid : nullptr, ok, offsets, iters, out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::frechet_assemble_kernel, g, 256, 0, st, mu1, mu2, d, scal1, w.scalC, w.scalM, w.Y, w.Z,
+                  with_resid ? w.resid : nullptr, ok, offsets, iters, out);
 }
 }  // namespace
 
@@ -962,10 +975,8 @@ int fad_sqrt_psd(fad_handle* h, const double* cov, int d, int iters, double* sqr
     if (frechet_workspace(h, 1, d, w)) return 1;
     const size_t ev = prof_begin(h, st);
     if (newton_schulz(h, w, cov, w.scalC, 1, d, iters, st)) return 1;
-    fad::ns_unscale_kernel<<<elem_blocks(h, d), 256, 0, st>>>(w.Y, d, w.scalC, sqrt_out);
-    CK(cudaGetLastError());
+    if (launch(h, fad::ns_unscale_kernel, elem_blocks(h, d), 256, 0, st, w.Y, d, w.scalC, sqrt_out)) return 1;
     CK(cudaMemcpyAsync(scal_out, w.scalC, 2 * sizeof(double), cudaMemcpyDeviceToDevice, st));
-    h->launches++;
     prof_end(h, FAD_PROF_FRECHET, ev, st);
     return 0;
 }
@@ -1019,15 +1030,11 @@ int fad_frechet_batched(fad_handle* h, const double* mu1, const double* sqrt1, c
     const size_t ev = prof_begin(h, st);
     for (long long g0 = 0; g0 < n_items; g0 += G) {
         const int g = (int)((n_items - g0) < G ? (n_items - g0) : G);
-        if (d % 64 == 0) {                                   // fp64 tensor pipe (DMMA), upper tile triangle per item
-            const int nt = d / 64;
-            fad::song_stats_dmma_kernel<<<dim3(nt * (nt + 1) / 2, g), 256, 0, st>>>(emb, offsets + g0, d, w.mu, w.cov, w.ok);
-        } else {
-            const int dt = (d + 31) / 32;
-            fad::song_stats_kernel<<<dim3(dt, dt, g), 256, 0, st>>>(emb, offsets + g0, d, w.mu, w.cov, w.ok);
-        }
-        CK(cudaGetLastError());
-        h->launches++;
+        const int nt = d / 64, dt = (d + 31) / 32;
+        if (d % 64 == 0 ?                                    // fp64 tensor pipe (DMMA), upper tile triangle per item
+                launch(h, fad::song_stats_dmma_kernel, dim3(nt * (nt + 1) / 2, g), 256, 0, st, emb, offsets + g0, d, w.mu, w.cov, w.ok) :
+                launch(h, fad::song_stats_kernel, dim3(dt, dt, g), 256, 0, st, emb, offsets + g0, d, w.mu, w.cov, w.ok))
+            return 1;
         if (frechet_items(h, w, mu1, sqrt1, scal1, w.mu, w.cov, g, d, iters, w.ok, offsets + g0, false, out + g0 * 8, st))
             return 1;
     }
@@ -1065,9 +1072,9 @@ extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_
     cudaEvent_t e0, e1;
     CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
     const int blocks = h->num_sms * 4;
-    dmma_peak_kernel<<<blocks, 256>>>(iters / 10, w.sink);            // warm-up
+    if (launch(h, dmma_peak_kernel, blocks, 256, 0, nullptr, iters / 10, w.sink)) return 1;     // warm-up
     CK(cudaEventRecord(e0));
-    dmma_peak_kernel<<<blocks, 256>>>(iters, w.sink);
+    if (launch(h, dmma_peak_kernel, blocks, 256, 0, nullptr, iters, w.sink)) return 1;
     CK(cudaEventRecord(e1));
     CK(cudaEventSynchronize(e1));
     float ms = 0.f;
@@ -1075,7 +1082,6 @@ extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_
     cudaEventDestroy(e0); cudaEventDestroy(e1);
     const double flop = (double)blocks * 8 /*warps*/ * (double)iters * 8 /*DMMAs*/ * 512.0;
     *tflops_out_host = flop / (ms * 1e-3) / 1e12;
-    h->launches += 2;
     return 0;
 }
 }  // extern "C"
@@ -1129,12 +1135,10 @@ int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspac
     w.extra = q;
     p.norm = w.norm;
 
-    fad::kad_colsum_kernel<<<chunks, 128, 0, st>>>(z, m, d, w.colpart);
-    fad::kad_shift_kernel<<<1, 256, 0, st>>>(w.colpart, chunks, m, d, w.shift);
-    fad::kad_split_kernel<<<(unsigned)((rows_pad * 32 + 255) / 256), 256, 0, st>>>(z, N, (int)rows_pad, d, w.shift,
-                                                                                    w.hi, w.lo, w.norm);
-    CK(cudaGetLastError());
-    h->launches += 3;
+    if (launch(h, fad::kad_colsum_kernel, chunks, 128, 0, st, z, m, d, w.colpart) ||
+        launch(h, fad::kad_shift_kernel, 1, 256, 0, st, w.colpart, chunks, m, d, w.shift) ||
+        launch(h, fad::kad_split_kernel, (unsigned)((rows_pad * 32 + 255) / 256), 256, 0, st, z, N, (int)rows_pad, d, w.shift,
+               w.hi, w.lo, w.norm)) return 1;
     // rows >= N and columns >= d of a box are zero-filled by the TMA unit (the kernel masks those rows by index)
     const uint64_t dims[2] = {(uint64_t)d, (uint64_t)N};
     const uint64_t strides[1] = {(uint64_t)d * 2};
@@ -1145,17 +1149,8 @@ int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspac
 
 template <int MODE>
 int launch_kad_tiles(fad_handle* h, const CUtensorMap& mh, const CUtensorMap& ml, const fad::KadParams& p, cudaStream_t st) {
-    static bool attr_set = false;
-    auto kern = fad::kad_tile_kernel<MODE>;
-    if (!attr_set) {
-        CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fad::kKadSmemBytes));
-        attr_set = true;
-    }
     const int grid = std::min(p.units, h->num_sms);   // the result does not depend on it (fixed work units)
-    kern<<<grid, fad::kKadThreads, fad::kKadSmemBytes, st>>>(mh, ml, p);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::kad_tile_kernel<MODE>, grid, fad::kKadThreads, fad::kKadSmemBytes, st, mh, ml, p);
 }
 }  // namespace
 
@@ -1170,9 +1165,7 @@ int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, doub
     fad::KadParams p = {};
     if (kad_prepare(h, reinterpret_cast<const __half*>(x_f16), (int)m, (int)m, d, w, &mh, &ml, p, st)) return 1;
     const unsigned long long pairs = (unsigned long long)m * (unsigned long long)(m - 1) / 2;
-    fad::kad_select_init_kernel<<<1, 1, 0, st>>>(w.state, (pairs - 1) / 2, pairs / 2);
-    CK(cudaGetLastError());
-    h->launches++;
+    if (launch(h, fad::kad_select_init_kernel, 1, 1, 0, st, w.state, (pairs - 1) / 2, pairs / 2)) return 1;
     // radix digits of the fp32 bit pattern of q >= 0 (bit 31 is 0): 30..20, 19..10, 9..0
     const int shifts[3] = {20, 10, 0}, bins[3] = {2048, 1024, 1024};
     const uint32_t masks[3] = {0u, 0xFFF00000u, 0xFFFFFC00u};
@@ -1181,10 +1174,8 @@ int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, doub
     for (int pass = 0; pass < 3; ++pass) {
         CK(cudaMemsetAsync(w.hist, 0, 2 * fad::kKadHistBins * 8, st));
         p.mask = masks[pass]; p.shift = shifts[pass]; p.bins = bins[pass];
-        if (launch_kad_tiles<1>(h, mh, ml, p, st)) return 1;
-        fad::kad_select_kernel<<<1, 32, 0, st>>>(w.state, w.hist, shifts[pass], bins[pass], pass == 2, out);
-        CK(cudaGetLastError());
-        h->launches++;
+        if (launch_kad_tiles<1>(h, mh, ml, p, st) ||
+            launch(h, fad::kad_select_kernel, 1, 32, 0, st, w.state, w.hist, shifts[pass], bins[pass], pass == 2, out)) return 1;
     }
     return 0;
 }
@@ -1202,10 +1193,7 @@ int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int
     p.sigma = sigma;
     p.partial = w.partial;
     if (launch_kad_tiles<0>(h, mh, ml, p, st)) return 1;
-    fad::kad_reduce_kernel<<<1, 32, 0, st>>>(w.partial, p.units, out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, p.units, out);
 }
 
 }  // extern "C"
@@ -1278,19 +1266,16 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
     px.T = Tx;
     px.units = (Tx + 1) / 2;
     px.partial = w.partial;
-    if (launch_kad_tiles<0>(h, mh, ml, px, st)) return 1;
-    fad::kad_reduce_kernel<<<1, 32, 0, st>>>(w.partial, px.units, d_xx);
-    CK(cudaGetLastError());
+    if (launch_kad_tiles<0>(h, mh, ml, px, st) || launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, px.units, d_xx))
+        return 1;
     CK(cudaMemcpyAsync(out, d_xx, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    h->launches++;
     if (n_items == 0) return 0;
 
     if (units) {
         CK(cudaMemcpyAsync(d_work, work.data(), units * sizeof(int4), cudaMemcpyHostToDevice, st));
         CK(cudaMemcpyAsync(d_start, unit_start.data(), unit_start.size() * 4, cudaMemcpyHostToDevice, st));
-        fad::kad_row_end_kernel<<<(Ty * 128 + 255) / 256, 256, 0, st>>>(offsets, n_items, (int)m, n_total, Ty * 128, d_end);
-        CK(cudaGetLastError());
-        h->launches++;
+        if (launch(h, fad::kad_row_end_kernel, (Ty * 128 + 255) / 256, 256, 0, st, offsets, n_items, (int)m, n_total, Ty * 128, d_end))
+            return 1;
         p.work = d_work;
         p.row_end = d_end;
         p.Tx = Tx;
@@ -1298,10 +1283,7 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
         p.partial = d_part;
         if (launch_kad_tiles<2>(h, mh, ml, p, st)) return 1;
     }
-    fad::kad_song_reduce_kernel<<<(unsigned)n_items, fad::kKadSongReduceThreads, 0, st>>>(d_part, d_start, offsets, out);
-    CK(cudaGetLastError());
-    h->launches++;
-    return 0;
+    return launch(h, fad::kad_song_reduce_kernel, (unsigned)n_items, fad::kKadSongReduceThreads, 0, st, d_part, d_start, offsets, out);
 }
 
 #include "resample_host.inc"
