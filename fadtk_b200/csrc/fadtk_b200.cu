@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <set>
 #include <string>
 #include <utility>
@@ -40,6 +41,59 @@ int fail(const std::string& m) { g_err = m; return 1; }
         if (e_ != cudaSuccess)                                                            \
             return fail(std::string(#call) + ": " + cudaGetErrorString(e_));              \
     } while (0)
+
+// The one owner of device memory in the library: a block of at least size() bytes, freed by the destructor.
+class DeviceBuffer {
+public:
+    DeviceBuffer() = default;
+    DeviceBuffer(DeviceBuffer&& o) noexcept : p_(o.p_), bytes_(o.bytes_) { o.p_ = nullptr; o.bytes_ = 0; }  // no copies
+    ~DeviceBuffer() { if (p_) cudaFree(p_); }
+
+    // at least `bytes`: reallocates only when the block is smaller, and does not keep its contents
+    int grow(size_t bytes) {
+        if (bytes_ >= bytes) return 0;
+        if (p_) cudaFree(p_);
+        p_ = nullptr; bytes_ = 0;
+        CK(cudaMalloc(&p_, bytes));
+        bytes_ = bytes;
+        return 0;
+    }
+    template <typename T = void> T* get() const { return static_cast<T*>(p_); }
+    size_t size() const { return bytes_; }
+
+private:
+    void* p_ = nullptr;
+    size_t bytes_ = 0;
+};
+
+// The weights and fixed workspaces of a loaded model live in a std::vector<DeviceBuffer> of its state; the typed
+// pointers of the state are views into it.  A copy of `bytes` host bytes at *dst:
+template <typename T>
+int upload(std::vector<DeviceBuffer>& mem, T** dst, const void* src, size_t bytes) {
+    DeviceBuffer b;
+    if (b.grow(bytes)) return 1;
+    CK(cudaMemcpy(b.get(), src, bytes, cudaMemcpyHostToDevice));
+    *dst = b.get<T>();
+    mem.push_back(std::move(b));
+    return 0;
+}
+// `bytes` uninitialised (or zeroed) bytes at *dst
+template <typename T>
+int alloc(std::vector<DeviceBuffer>& mem, T** dst, size_t bytes, bool zero = false) {
+    DeviceBuffer b;
+    if (b.grow(bytes)) return 1;
+    if (zero) CK(cudaMemset(b.get(), 0, bytes));
+    *dst = b.get<T>();
+    mem.push_back(std::move(b));
+    return 0;
+}
+
+// A load checks every tensor pointer before it touches its model's slot.
+int check_tensors(const char* fn, const void* const* t, int n_tensors) {
+    for (int i = 0; i < n_tensors; ++i)
+        if (!t[i]) return fail(std::string(fn) + ": null tensor pointer");
+    return 0;
+}
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
                                   const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
@@ -106,6 +160,13 @@ int make_geom(LayerGeom& g, int H, int W, int Cin, int Cout, int taps, int relu,
     return 0;
 }
 
+// the loaded models, one slot each: set by a load that succeeded, empty after one that failed part way
+struct VggState;       // below
+struct ClapState;      // clap_host.inc
+struct WhisperState;   // whisper_host.inc
+struct EncodecState;   // encodec_host.inc
+struct W2vState;       // wav2vec_host.inc
+
 }  // namespace
 
 struct fad_handle {
@@ -116,43 +177,30 @@ struct fad_handle {
     int gemm_clusters[2] = {};       // co-resident CTA pairs of the wgmma GEMM, by weight mode (fad_create)
 
     // front-end tables
+    std::vector<DeviceBuffer> mem;
     double *d_twiddle = nullptr, *d_hann = nullptr, *d_melw = nullptr;
     int *d_mel_start = nullptr, *d_mel_count = nullptr;
 
-    // VGGish parameters (device)
-    bool vgg_loaded = false;
-    float *conv1_w = nullptr, *conv1_b = nullptr;
-    __half* conv_w[5] = {};
-    float* conv_b[5] = {};
-    __half* fc_w[3] = {};
-    float* fc_b[3] = {};
-
-    // activations (device), sized for max_examples
-    float* logmel = nullptr;
-    __half* act[9] = {};       // act[0]=conv1 out ... act[5]=conv6 out (flattened), act[6..7]=fc1, fc2 out
-
-    // per-layer cached descriptors for the fixed VGGish pipeline
-    CUtensorMap map_x[8], map_w[8];
-    LayerGeom geom[8];
-
-    // statistics workspace
-    double *ws_tiles = nullptr, *ws_sums = nullptr;
-    size_t ws_tiles_cap = 0, ws_sums_cap = 0;
-    __half* gather_buf = nullptr;
-    size_t gather_cap = 0;
-
-    unsigned char* fr_buf = nullptr;  size_t fr_cap = 0;        // Frechet workspace (FrechetWorkspace)
-    float* rs_bank = nullptr;  size_t rs_bank_cap = 0;  int rs_in = 0, rs_out = 0;     // resampler filter bank
-    float* rs_mono = nullptr;  size_t rs_mono_cap = 0;
-    unsigned char* kad_buf = nullptr;  size_t kad_cap = 0;      // fad_kad_* workspace (KadWorkspace)
-    std::set<const void*> zero_lo;           // hi/lo weight tensors whose lo parts are all zero (note_split_weights)
+    // workspaces, grown on demand
+    DeviceBuffer ws_tiles, ws_sums, gather_buf;     // statistics
+    DeviceBuffer fr_buf;                            // Frechet (FrechetWorkspace)
+    DeviceBuffer rs_bank, rs_mono;                  // resampler filter bank and mono mix
+    int rs_in = 0, rs_out = 0;                      // the rate pair of rs_bank
+    DeviceBuffer kad_buf;                           // fad_kad_* (KadWorkspace)
+    // hi/lo weight tensors whose lo parts are all zero, by address (note_split_weights).  Every hi/lo tensor is noted
+    // at its current address before any GEMM reads it: upload_split and fad_vggish_load note each one they upload,
+    // fad_umma_layer and fad_linear the caller's on every call.  An entry left behind for a freed address is
+    // therefore overwritten before it can be read.
+    std::set<const void*> zero_lo;
 
     void* nccl_comm = nullptr;   // ncclComm_t created by fad_comm_init (NCCL is dlopen'ed, never linked)
 
-    void* clap_state = nullptr;  // ClapState (clap_host.inc)
-    void* whisper_state = nullptr;   // WhisperState (whisper_host.inc)
-    void* encodec_state = nullptr;   // EncodecState (encodec_host.inc)
-    void* w2v_state = nullptr;       // W2vState (wav2vec_host.inc)
+    std::unique_ptr<VggState> vgg;
+    std::unique_ptr<ClapState> clap;
+    std::unique_ptr<WhisperState> whisper;
+    std::unique_ptr<EncodecState> encodec;
+    std::unique_ptr<W2vState> w2v;
+    ~fad_handle();      // at the end of the file, where the state types are complete
 
     // optional per-category timing with CUDA events recorded on the launching stream
     bool prof_on = false;
@@ -279,9 +327,6 @@ int launch_attention_wgmma(fad_handle* h, const __half* qkv, long long n_clips, 
                   st, map, p);
 }
 
-// zero_lo is keyed by weight POINTER: drop the entry whenever that memory is freed or reallocated
-void forget_zero_lo(fad_handle* h, const void* w) { h->zero_lo.erase(w); }
-
 int run_layer(fad_handle* h, const LayerGeom& g, const CUtensorMap& mx, const CUtensorMap& mw, const void* w,
               int NB, const float* bias, void* out, float* out_f32, cudaStream_t st,
               float* resid = nullptr, int resid_C = 0, int resid_res = 0, int resid_shift = 0, int n_valid = 0) {
@@ -317,23 +362,25 @@ __global__ void wlo_absmax_kernel(const __half* __restrict__ w, long long n_tile
 // Whether the lo parts of a hi/lo weight tensor ([2 * 128 * n_tiles, K], device) are all zero, as they are for weights
 // that are exact in fp16.  Their lo wgmmas then add exact zeros, which do not truncate the accumulator, and the GEMM's
 // unshrink counts the hi products only (ConvGemmParams::lo_adds).  Every hi/lo tensor is noted when it is uploaded;
-// caller-owned tensors (the stage entries) on every call.  Synchronous.
+// the caller's tensors (the stage entries) on every call.  Synchronous.
 int note_split_weights(fad_handle* h, const void* w, long long n_tiles, long long K, cudaStream_t st) {
-    unsigned int* d_max = nullptr;
-    CK(cudaMalloc(&d_max, 4));
+    DeviceBuffer d_max;
+    if (d_max.grow(4)) return 1;
     unsigned int mx = 0;
     const unsigned blocks = (unsigned)std::max<long long>(1, std::min<long long>((n_tiles * 128 * K + 255) / 256, (long long)h->num_sms * 16));
-    const int rc = [&]() -> int {
-        CK(cudaMemsetAsync(d_max, 0, 4, st));
-        if (launch(h, wlo_absmax_kernel, blocks, 256, 0, st, reinterpret_cast<const __half*>(w), n_tiles, K, d_max)) return 1;
-        CK(cudaMemcpyAsync(&mx, d_max, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        return 0;
-    }();
-    cudaFree(d_max);
-    if (rc) return 1;
+    CK(cudaMemsetAsync(d_max.get(), 0, 4, st));
+    if (launch(h, wlo_absmax_kernel, blocks, 256, 0, st, reinterpret_cast<const __half*>(w), n_tiles, K, d_max.get<unsigned int>()))
+        return 1;
+    CK(cudaMemcpyAsync(&mx, d_max.get(), 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     if (mx == 0) h->zero_lo.insert(w); else h->zero_lo.erase(w);
     return 0;
+}
+
+// an fp16 hi/lo weight tensor [2 n, k] (n a multiple of 128), noted for the GEMM's truncation compensation
+int upload_split(fad_handle* h, std::vector<DeviceBuffer>& mem, __half** dst, const void* src, size_t n, size_t k) {
+    if (upload(mem, dst, src, 2 * n * k * 2)) return 1;
+    return note_split_weights(h, *dst, (long long)(n / 128), (long long)k, 0);
 }
 
 // VGGish layer table: H, W are the conv's spatial size (input == un-pooled output)
@@ -351,6 +398,19 @@ const VggLayer kVgg[8] = {
 // bytes of fp16 activation per example produced by: conv1, conv2, conv3_1, conv3_2, conv4_1, conv4_2, fc1, fc2
 const size_t kActElems[8] = {48 * 32 * 64, 24 * 16 * 128, 24 * 16 * 256, 12 * 8 * 256,
                              12 * 8 * 512, 6 * 4 * 512, 4096, 4096};
+
+struct VggState {
+    std::vector<DeviceBuffer> mem;      // everything below points into it
+    float *conv1_w = nullptr, *conv1_b = nullptr;
+    __half* w[8] = {};         // the layers of kVgg: conv2 .. conv4_2, fc1 .. fc3
+    float* b[8] = {};
+    // activations, sized for max_examples
+    float* logmel = nullptr;
+    __half* act[8] = {};       // act[0]=conv1 out ... act[5]=conv6 out (flattened), act[6..7]=fc1, fc2 out
+    // per-layer cached descriptors for the fixed pipeline
+    CUtensorMap map_x[8], map_w[8];
+    LayerGeom geom[8];
+};
 
 void build_frontend_tables(std::vector<double>& tw, std::vector<double>& hann,
                            std::vector<double>& melw, std::vector<int>& mstart, std::vector<int>& mcount) {
@@ -385,15 +445,6 @@ void build_frontend_tables(std::vector<double>& tw, std::vector<double>& hann,
     }
 }
 
-int ensure(void** ptr, size_t* cap, size_t bytes) {
-    if (*cap >= bytes) return 0;
-    if (*ptr) cudaFree(*ptr);
-    *ptr = nullptr; *cap = 0;
-    CK(cudaMalloc(ptr, bytes));
-    *cap = bytes;
-    return 0;
-}
-
 size_t prof_begin(fad_handle* h, cudaStream_t st) {
     if (!h->prof_on) return 0;
     if (h->ev_used == h->ev_pool.size()) { cudaEvent_t e; cudaEventCreate(&e); h->ev_pool.push_back(e); }
@@ -424,9 +475,9 @@ int launch_stats_dmma(fad_handle* h, const In* E, long long n_rows, int d, const
     p.rows_per_split = per * fad::kSdRows;
     p.shift = shift;
     const size_t jobs = (size_t)p.n_pairs * p.n_splits;
-    if (ensure((void**)&h->ws_tiles, &h->ws_tiles_cap, jobs * fad::kSdTile * fad::kSdTile * 8)) return 1;
-    if (ensure((void**)&h->ws_sums, &h->ws_sums_cap, (size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
-    p.ws_tiles = h->ws_tiles; p.ws_sums = h->ws_sums;
+    if (h->ws_tiles.grow(jobs * fad::kSdTile * fad::kSdTile * 8)) return 1;
+    if (h->ws_sums.grow((size_t)p.n_tiles * p.n_splits * fad::kSdTile * 8)) return 1;
+    p.ws_tiles = h->ws_tiles.get<double>(); p.ws_sums = h->ws_sums.get<double>();
     size_t ev = kProf ? prof_begin(h, st) : 0;
     if (launch(h, fad::stats_dmma_kernel<In>, (unsigned)jobs, 256, 0, st, E, p)) return 1;
     if (kProf) { prof_end(h, FAD_PROF_STATS, ev, st); ev = prof_begin(h, st); }
@@ -477,18 +528,16 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
     if (prop.major != 9) return fail("fadtk_b200 kernels are built for sm_90a (Hopper H100) only");
-    fad_handle* h = new fad_handle();
+    std::unique_ptr<fad_handle> h(new fad_handle());
     h->device = device;
     h->num_sms = prop.multiProcessorCount;
     h->max_examples = max_examples > 0 ? max_examples : 2048;
 
     std::vector<double> tw, hann, melw; std::vector<int> ms, mc;
     build_frontend_tables(tw, hann, melw, ms, mc);
-    CK(cudaMalloc(&h->d_twiddle, tw.size() * 8)); CK(cudaMemcpy(h->d_twiddle, tw.data(), tw.size() * 8, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&h->d_hann, hann.size() * 8)); CK(cudaMemcpy(h->d_hann, hann.data(), hann.size() * 8, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&h->d_melw, melw.size() * 8)); CK(cudaMemcpy(h->d_melw, melw.data(), melw.size() * 8, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&h->d_mel_start, ms.size() * 4)); CK(cudaMemcpy(h->d_mel_start, ms.data(), ms.size() * 4, cudaMemcpyHostToDevice));
-    CK(cudaMalloc(&h->d_mel_count, mc.size() * 4)); CK(cudaMemcpy(h->d_mel_count, mc.data(), mc.size() * 4, cudaMemcpyHostToDevice));
+    if (upload(h->mem, &h->d_twiddle, tw.data(), tw.size() * 8) || upload(h->mem, &h->d_hann, hann.data(), hann.size() * 8) ||
+        upload(h->mem, &h->d_melw, melw.data(), melw.size() * 8) || upload(h->mem, &h->d_mel_start, ms.data(), ms.size() * 4) ||
+        upload(h->mem, &h->d_mel_count, mc.data(), mc.size() * 4)) return 1;
     // one-time kernel setup, for the handle's device: the dynamic shared memory of every kernel that launches with more
     // than the default 48 KiB, and the GEMM's co-resident CTA pairs
     const auto smem = [](const void* kernel, size_t bytes) {
@@ -503,31 +552,15 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
-    if (setup_gemm<0>(h) || setup_gemm<1>(h)) return 1;
-    *out = h;
+    if (setup_gemm<0>(h.get()) || setup_gemm<1>(h.get())) return 1;
+    *out = h.release();
     return 0;
 }
-
-static void clap_free_state(void* p);
-static void whisper_free_state(void* p);
-static void encodec_free_state(void* p);
-static void w2v_free_state(void* p);
 
 int fad_destroy(fad_handle* h) {
     if (!h) return 0;
     cudaSetDevice(h->device);
     fad_comm_destroy(h);
-    clap_free_state(h->clap_state);
-    whisper_free_state(h->whisper_state);
-    encodec_free_state(h->encodec_state);
-    w2v_free_state(h->w2v_state);
-    void* ptrs[] = {h->d_twiddle, h->d_hann, h->d_melw, h->d_mel_start, h->d_mel_count, h->conv1_w, h->conv1_b,
-                    h->logmel, h->ws_tiles, h->ws_sums, h->gather_buf, h->fr_buf, h->rs_bank, h->rs_mono,
-                    h->kad_buf};
-    for (void* p : ptrs) if (p) cudaFree(p);
-    for (int i = 0; i < 5; ++i) { if (h->conv_w[i]) cudaFree(h->conv_w[i]); if (h->conv_b[i]) cudaFree(h->conv_b[i]); }
-    for (int i = 0; i < 3; ++i) { if (h->fc_w[i]) cudaFree(h->fc_w[i]); if (h->fc_b[i]) cudaFree(h->fc_b[i]); }
-    for (int i = 0; i < 9; ++i) if (h->act[i]) cudaFree(h->act[i]);
     delete h;
     return 0;
 }
@@ -537,48 +570,41 @@ long long fad_launch_count(fad_handle* h) { return h ? h->launches : 0; }
 // ------------------------------------------------------------------------------ VGGish
 int fad_vggish_load(fad_handle* h, const fad_vggish_weights* w) {
     if (!h || !w) return fail("null argument");
+    // conv1's weight and bias, then the weights and the biases of the kVgg layers
+    const void* src[18] = {w->conv1_w_host, w->conv1_b_host,
+                           w->conv_w_host[0], w->conv_w_host[1], w->conv_w_host[2], w->conv_w_host[3], w->conv_w_host[4],
+                           w->fc_w_host[0], w->fc_w_host[1], w->fc_w_host[2],
+                           w->conv_b_host[0], w->conv_b_host[1], w->conv_b_host[2], w->conv_b_host[3], w->conv_b_host[4],
+                           w->fc_b_host[0], w->fc_b_host[1], w->fc_b_host[2]};
+    if (check_tensors("fad_vggish_load", src, 18)) return 1;
+    const void* const* wsrc = src + 2;
+    const void* const* bsrc = src + 10;
     CK(cudaSetDevice(h->device));
-    auto up = [&](void** dst, const void* src, size_t bytes) -> int {
-        if (!src) return fail("missing weight pointer");
-        if (*dst) { forget_zero_lo(h, *dst); cudaFree(*dst); *dst = nullptr; }      // sizes depend on split_mask
-        CK(cudaMalloc(dst, bytes));
-        forget_zero_lo(h, *dst);
-        CK(cudaMemcpy(*dst, src, bytes, cudaMemcpyHostToDevice));
-        return 0;
-    };
-    if (up((void**)&h->conv1_w, w->conv1_w_host, 64 * 9 * 4)) return 1;
-    if (up((void**)&h->conv1_b, w->conv1_b_host, 64 * 4)) return 1;
-    for (int i = 0; i < 5; ++i) {
+    h->vgg.reset();
+    auto vs = std::make_unique<VggState>();
+    auto& m = vs->mem;
+    if (upload(m, &vs->conv1_w, src[0], 64 * 9 * 4) || upload(m, &vs->conv1_b, src[1], 64 * 4)) return 1;
+    for (int i = 0; i < 8; ++i) {
         const VggLayer& L = kVgg[i];
-        const size_t mul = ((w->split_mask >> i) & 1) ? 2 : 1;
-        if (up((void**)&h->conv_w[i], w->conv_w_host[i], mul * L.Cout * 9 * L.Cin * 2)) return 1;
-        if (up((void**)&h->conv_b[i], w->conv_b_host[i], (size_t)L.Cout * 4)) return 1;
-    }
-    for (int i = 0; i < 3; ++i) {
-        const VggLayer& L = kVgg[5 + i];
-        const size_t mul = ((w->split_mask >> (5 + i)) & 1) ? 2 : 1;
-        if (up((void**)&h->fc_w[i], w->fc_w_host[i], mul * L.Cout * L.Cin * 2)) return 1;
-        if (up((void**)&h->fc_b[i], w->fc_b_host[i], (size_t)L.Cout * 4)) return 1;
+        const size_t mul = ((w->split_mask >> i) & 1) ? 2 : 1;      // sizes depend on split_mask
+        if (upload(m, &vs->w[i], wsrc[i], mul * L.Cout * L.taps * L.Cin * 2) || upload(m, &vs->b[i], bsrc[i], (size_t)L.Cout * 4))
+            return 1;
     }
     for (int i = 0; i < 8; ++i)
-        if ((w->split_mask >> i) & 1) {
-            const VggLayer& L = kVgg[i];
-            if (note_split_weights(h, i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5], L.Cout / 128,
-                                   (long long)L.taps * L.Cin, 0)) return 1;
-        }
+        if (((w->split_mask >> i) & 1) &&
+            note_split_weights(h, vs->w[i], kVgg[i].Cout / 128, (long long)kVgg[i].taps * kVgg[i].Cin, 0)) return 1;
     const size_t B = (size_t)h->max_examples;
-    if (!h->logmel) CK(cudaMalloc(&h->logmel, B * 96 * 64 * 4));
+    if (alloc(m, &vs->logmel, B * 96 * 64 * 4)) return 1;
     for (int i = 0; i < 8; ++i)
-        if (!h->act[i]) CK(cudaMalloc(&h->act[i], B * kActElems[i] * 2));
+        if (alloc(m, &vs->act[i], B * kActElems[i] * 2)) return 1;
     // descriptors of the fixed pipeline (batch dimension = max_examples; tiles past the live
     // batch are never scheduled and rows past it are masked in the epilogue)
     for (int i = 0; i < 8; ++i) {
         const VggLayer& L = kVgg[i];
-        if (make_geom(h->geom[i], L.H, L.W, L.Cin, L.Cout, L.taps, L.relu, L.pool, (w->split_mask >> i) & 1)) return 1;
-        const void* wptr = i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5];
-        if (encode_layer_maps(h->geom[i], h->act[i], (long long)B, wptr, &h->map_x[i], &h->map_w[i])) return 1;
+        if (make_geom(vs->geom[i], L.H, L.W, L.Cin, L.Cout, L.taps, L.relu, L.pool, (w->split_mask >> i) & 1)) return 1;
+        if (encode_layer_maps(vs->geom[i], vs->act[i], (long long)B, vs->w[i], &vs->map_x[i], &vs->map_w[i])) return 1;
     }
-    h->vgg_loaded = true;
+    h->vgg = std::move(vs);
     return 0;
 }
 
@@ -627,23 +653,23 @@ int fad_vggish_logmel(fad_handle* h, const int16_t* pcm, const long long* ex_sta
 int fad_vggish_forward(fad_handle* h, const int16_t* pcm, const long long* ex_start,
                        long long n_examples, void* emb_out_f16, void* stream) {
     if (!h) return fail("null handle");
-    if (!h->vgg_loaded) return fail("fad_vggish_load has not been called");
+    if (!h->vgg) return fail("fad_vggish_load has not been called");
     CK(cudaSetDevice(h->device));
+    const VggState& vs = *h->vgg;
     cudaStream_t st = (cudaStream_t)stream;
     static const int fe_double = []() { const char* e = getenv("FADTK_FRONTEND_FP64"); return (e && e[0] == '1') ? 1 : 0; }();
     for (long long base = 0; base < n_examples; base += h->max_examples) {
         const int nb = (int)((n_examples - base) < h->max_examples ? (n_examples - base) : h->max_examples);
         size_t ev = prof_begin(h, st);
-        if (launch_logmel(h, pcm, ex_start + base, nb, h->logmel, fe_double, st)) return 1;
+        if (launch_logmel(h, pcm, ex_start + base, nb, vs.logmel, fe_double, st)) return 1;
         prof_end(h, FAD_PROF_LOGMEL, ev, st);
         ev = prof_begin(h, st);
-        if (launch(h, fad::conv1_kernel, dim3(6, nb), 256, 0, st, h->logmel, h->conv1_w, h->conv1_b, h->act[0])) return 1;
+        if (launch(h, fad::conv1_kernel, dim3(6, nb), 256, 0, st, vs.logmel, vs.conv1_w, vs.conv1_b, vs.act[0])) return 1;
         prof_end(h, FAD_PROF_CONV1, ev, st);
         for (int i = 0; i < 8; ++i) {
-            const float* bias = i < 5 ? h->conv_b[i] : h->fc_b[i - 5];
-            void* out = (i == 7) ? (void*)((__half*)emb_out_f16 + (size_t)base * 128) : (void*)h->act[i + 1];
+            void* out = (i == 7) ? (void*)((__half*)emb_out_f16 + (size_t)base * 128) : (void*)vs.act[i + 1];
             ev = prof_begin(h, st);
-            if (run_layer(h, h->geom[i], h->map_x[i], h->map_w[i], (i < 5 ? (const void*)h->conv_w[i] : (const void*)h->fc_w[i - 5]), nb, bias, out, nullptr, st)) return 1;
+            if (run_layer(h, vs.geom[i], vs.map_x[i], vs.map_w[i], vs.w[i], nb, vs.b[i], out, nullptr, st)) return 1;
             prof_end(h, FAD_PROF_LAYER0 + i, ev, st);
         }
     }
@@ -653,11 +679,11 @@ int fad_vggish_forward(fad_handle* h, const int16_t* pcm, const long long* ex_st
 // Stage entry (parity test): conv1 (3x3, 1 -> 64, pad 1) + bias + ReLU + 2x2 max-pool on fp32 log-mel examples.
 int fad_vggish_conv1(fad_handle* h, const float* logmel, long long n_examples, void* out_f16, void* stream) {
     if (!h) return fail("null handle");
-    if (!h->vgg_loaded) return fail("fad_vggish_load has not been called");
+    if (!h->vgg) return fail("fad_vggish_load has not been called");
     if (n_examples <= 0) return 0;
     CK(cudaSetDevice(h->device));
     return launch(h, fad::conv1_kernel, dim3(6, (unsigned)n_examples), 256, 0, (cudaStream_t)stream,
-                  logmel, h->conv1_w, h->conv1_b, reinterpret_cast<__half*>(out_f16));
+                  logmel, h->vgg->conv1_w, h->vgg->conv1_b, reinterpret_cast<__half*>(out_f16));
 }
 
 int fad_umma_layer(fad_handle* h, const void* x_f16, int NB, int H, int W, int Cin,
@@ -735,13 +761,14 @@ int fad_stats_accumulate_gather(fad_handle* h, const void* emb_f16, long long n_
     if (n_idx <= 0) return 0;
     if (d % 8 != 0) return fail("d must be a multiple of 8");
     CK(cudaSetDevice(h->device));
-    if (ensure((void**)&h->gather_buf, &h->gather_cap, (size_t)n_idx * d * 2)) return 1;
+    if (h->gather_buf.grow((size_t)n_idx * d * 2)) return 1;
+    __half* rows = h->gather_buf.get<__half>();
     const long long vecs = n_idx * (d / 8);
     long long blocks = (vecs + 255) / 256;
     if (blocks > (long long)h->num_sms * 16) blocks = (long long)h->num_sms * 16;
     if (launch(h, fad::gather_rows_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream,
-               reinterpret_cast<const __half*>(emb_f16), idx, n_idx, d, h->gather_buf)) return 1;
-    return launch_stats_dmma(h, h->gather_buf, n_idx, d, reinterpret_cast<const __half*>(shift_f16), acc, (cudaStream_t)stream);
+               reinterpret_cast<const __half*>(emb_f16), idx, n_idx, d, rows)) return 1;
+    return launch_stats_dmma(h, rows, n_idx, d, reinterpret_cast<const __half*>(shift_f16), acc, (cudaStream_t)stream);
 }
 
 int fad_stats_finalize(fad_handle* h, const double* acc, const void* shift_f16, int d,
@@ -881,8 +908,8 @@ int frechet_workspace(fad_handle* h, long long G, int d, FrechetWorkspace& w) {
     const size_t total = (size_t)d * d;
     const size_t b_mat = al(G * total * 8), b_mu = al(G * d * 8), b_scal = al(G * 2 * 8), b_flags = al(G * 3 * 4),
                  b_ok = al(G * 4), b_sqrt = al(total * 8), b_misc = al(4 * 8);
-    if (ensure((void**)&h->fr_buf, &h->fr_cap, 8 * b_mat + b_mu + 2 * b_scal + b_flags + b_ok + b_sqrt + b_misc)) return 1;
-    unsigned char* q = h->fr_buf;
+    if (h->fr_buf.grow(8 * b_mat + b_mu + 2 * b_scal + b_flags + b_ok + b_sqrt + b_misc)) return 1;
+    unsigned char* q = h->fr_buf.get<unsigned char>();
     for (double** m : {&w.cov, &w.P, &w.M, &w.Y, &w.Z, &w.W, &w.Yn, &w.Zn}) { *m = reinterpret_cast<double*>(q); q += b_mat; }
     w.mu = reinterpret_cast<double*>(q);        q += b_mu;
     w.scalC = reinterpret_cast<double*>(q);     q += b_scal;
@@ -1121,9 +1148,8 @@ int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspac
     const size_t b_split = al(rows_pad * d * 2), b_norm = al(rows_pad * 4), b_shift = al((size_t)d * 2),
                  b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8),
                  b_hist = al(2 * fad::kKadHistBins * 8), b_state = al(sizeof(fad::KadSelectState));
-    if (ensure((void**)&h->kad_buf, &h->kad_cap,
-               2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state + al(extra))) return 1;
-    unsigned char* q = h->kad_buf;
+    if (h->kad_buf.grow(2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state + al(extra))) return 1;
+    unsigned char* q = h->kad_buf.get<unsigned char>();
     w.hi = reinterpret_cast<__half*>(q);            q += b_split;
     w.lo = reinterpret_cast<__half*>(q);            q += b_split;
     w.norm = reinterpret_cast<float*>(q);           q += b_norm;
@@ -1289,8 +1315,6 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
 #include "resample_host.inc"
 #include "clap_host.inc"
 
-static void clap_free_state(void* p) { clap_free(reinterpret_cast<ClapState*>(p)); }
-
 extern "C" int fad_linear(fad_handle* h, const void* a_f16, long long rows, int k_cols, long long lda, const void* w_f16,
                           int split_w, const float* bias, int n_cols, int act, void* out_f16, float* out_f32,
                           float* resid, int resid_C, int resid_res, int resid_shift, void* stream) {
@@ -1301,7 +1325,7 @@ extern "C" int fad_linear(fad_handle* h, const void* a_f16, long long rows, int 
     __half* out16 = reinterpret_cast<__half*>(out_f16);
     if (clap_gemm_check(A, rows, k_cols, W, bias, n_cols, act, out16, out_f32, resid, resid_C, resid_res, resid_shift, lda, split_w))
         return 1;
-    // caller-owned weights: whether their lo parts are zero is decided on every call, never taken from a cache
+    // the caller's weights: whether their lo parts are zero is decided on every call, never taken from a cache
     if (split_w == 1 && note_split_weights(h, W, pad_to(n_cols, 128) / 128, pad_to(k_cols, 64), (cudaStream_t)stream)) return 1;
     return clap_gemm(h, A, rows, k_cols, W, bias, n_cols, act, out16, out_f32, (cudaStream_t)stream,
                      resid, resid_C, resid_res, resid_shift, lda, split_w);
@@ -1310,3 +1334,5 @@ extern "C" int fad_linear(fad_handle* h, const void* a_f16, long long rows, int 
 #include "whisper_host.inc"
 #include "encodec_host.inc"
 #include "wav2vec_host.inc"
+
+fad_handle::~fad_handle() = default;

@@ -20,7 +20,7 @@
 // song_stats_dmma_kernel runs the same DMMA Gram tile (gram_tile) per song for fad_frechet_batched and finishes each
 // song's mean and covariance in place; song_stats_kernel is its CUDA-core form for d not a multiple of 64.
 //
-// Packed accumulator (fp64, caller-owned, all-reduced across GPUs as-is):
+// Packed accumulator (fp64, the caller's, all-reduced across GPUs as-is):
 //   acc[0] = n,  acc[1 .. d] = sum(x - s) (exact),  acc[1+d .. 1+d+d*d) = sum(y y^T)
 //   (d x d, full, row-major),  acc[1+d+d*d ..] = sum y  (centring term of the covariance; the same values as
 //   acc[1 .. d], kept so that the layout and the all-reduce length stay as they are)

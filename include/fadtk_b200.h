@@ -11,6 +11,9 @@
  *     the parameter name ends in _host; `stream` is a cudaStream_t passed as void*;
  *   - a fad_handle belongs to one device and must not be used from two threads at once;
  *     distinct handles are independent;
+ *   - a fad_*_load checks all its arguments before it frees the model loaded before: a rejected
+ *     call changes nothing.  A CUDA failure while the new model is built leaves no model loaded,
+ *     and its forward fails until a load succeeds;
  *   - there is NO CPU fallback: without a CUDA device every compute entry point fails.
  */
 #ifndef FADTK_B200_H

@@ -549,3 +549,26 @@ def test_checkpoint_files_safetensors_and_old_weight_norm_names(tmp_path, monkey
     assert len(packed) == len(ref) and all(torch.equal(a, b) for a, b in zip(packed, ref))
     raw = weights.load_checkpoint_file(tmp_path / "pytorch_model.bin")
     assert "wav2vec2.encoder.pos_conv_embed.conv.parametrizations.weight.original0" in raw
+
+
+def test_device_memory_is_allocated_and_freed_only_by_device_buffer():
+    """Every device allocation of the library has one owner: cudaMalloc and cudaFree are called inside DeviceBuffer
+    (fadtk_b200.cu) and nowhere else, so a weight or workspace cannot be leaked or freed twice by hand."""
+    csrc = ROOT / "fadtk_b200" / "csrc"
+    calls = re.compile(r"\bcuda(Malloc|Free)\(")
+    found = 0
+    for path in sorted([*csrc.glob("*.cu"), *csrc.glob("*.inc"), *csrc.glob("*.cuh")]):
+        src = path.read_text()
+        lo = hi = -1
+        m = re.search(r"\bclass DeviceBuffer\s*\{", src)
+        if m:                                                  # the class body, by brace matching
+            lo, depth = m.start(), 0
+            for i in range(m.end() - 1, len(src)):
+                depth += {"{": 1, "}": -1}.get(src[i], 0)
+                if depth == 0:
+                    hi = i
+                    break
+        for c in calls.finditer(src):
+            assert lo <= c.start() <= hi, f"{path.name}:{src.count(chr(10), 0, c.start()) + 1}: {c.group(0)} outside DeviceBuffer"
+            found += 1
+    assert found >= 2, "DeviceBuffer no longer allocates and frees"
