@@ -93,6 +93,10 @@ SIGNATURES = {
     "fad_kad_median_sq": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_kad_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp]),
     "fad_kad_song_sums": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_median_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_kad_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_song_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_shard_plan": (C.c_int, [c_vp, c_ll, C.c_int, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -641,6 +645,46 @@ class Engine:
         _check(lib().fad_kad_song_sums(self._h, z.data_ptr(), int(m), offsets.data_ptr(), n_items, z.shape[1],
                                        sigma.data_ptr(), out.data_ptr(), _stream()))
         return out
+
+    # The same three results with the tile work split into shards (include/fadtk_b200.h): local_shards = 0 is
+    # collective over the handle's communicator (comm_init), every rank getting the whole output; local_shards >= 1
+    # runs that many shards one after another on this device.  Outputs are bitwise equal to the unsharded entries.
+    def kad_median_sq_sharded(self, x: torch.Tensor, local_shards: int = 0) -> torch.Tensor:
+        """fad_kad_median_sq_sharded: kad_median_sq over shards"""
+        assert x.dtype == torch.float16 and x.is_cuda and x.is_contiguous() and x.ndim == 2
+        out = torch.empty(2, dtype=torch.float64, device=x.device)
+        _check(lib().fad_kad_median_sq_sharded(self._h, None, int(local_shards), x.data_ptr(), x.shape[0], x.shape[1],
+                                               out.data_ptr(), _stream()))
+        return out
+
+    def kad_sums_sharded(self, z: torch.Tensor, m: int, sigma: torch.Tensor, local_shards: int = 0) -> torch.Tensor:
+        """fad_kad_sums_sharded: kad_sums over shards"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        out = torch.empty(3, dtype=torch.float64, device=z.device)
+        _check(lib().fad_kad_sums_sharded(self._h, None, int(local_shards), z.data_ptr(), int(m), z.shape[0] - int(m),
+                                          z.shape[1], sigma.data_ptr(), out.data_ptr(), _stream()))
+        return out
+
+    def kad_song_sums_sharded(self, z: torch.Tensor, m: int, offsets: torch.Tensor, sigma: torch.Tensor,
+                              local_shards: int = 0) -> torch.Tensor:
+        """fad_kad_song_sums_sharded: kad_song_sums over shards"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        n_items = offsets.shape[0] - 1
+        out = torch.empty(1 + 2 * n_items, dtype=torch.float64, device=z.device)
+        _check(lib().fad_kad_song_sums_sharded(self._h, None, int(local_shards), z.data_ptr(), int(m), offsets.data_ptr(),
+                                               n_items, z.shape[1], sigma.data_ptr(), out.data_ptr(), _stream()))
+        return out
+
+    @staticmethod
+    def kad_shard_plan(unit_tiles, shards: int) -> np.ndarray:
+        """unit_tiles int64 [units] (each >= 1) -> int64 [shards + 1]: shard s = units [b[s], b[s + 1]) (host only)"""
+        t = np.ascontiguousarray(unit_tiles, dtype=np.int64)
+        bounds = np.empty(int(shards) + 1 if int(shards) >= 1 else 1, dtype=np.int64)
+        _check(lib().fad_kad_shard_plan(t.ctypes.data, t.shape[0], int(shards), bounds.ctypes.data))
+        return bounds
 
 
 class Baseline:

@@ -14,6 +14,7 @@
 #include <memory>
 #include <set>
 #include <string>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -187,6 +188,7 @@ struct fad_handle {
     DeviceBuffer rs_bank, rs_mono;                  // resampler filter bank and mono mix
     int rs_in = 0, rs_out = 0;                      // the rate pair of rs_bank
     DeviceBuffer kad_buf;                           // fad_kad_* (KadWorkspace)
+    DeviceBuffer kad_agree;                         // fad_kad_*_sharded: the ranks' argument descriptor
     // hi/lo weight tensors whose lo parts are all zero, by address (note_split_weights).  Every hi/lo tensor is noted
     // at its current address before any GEMM reads it: upload_split and fad_vggish_load note each one they upload,
     // fad_umma_layer and fad_linear the caller's on every call.  An entry left behind for a freed address is
@@ -807,6 +809,8 @@ struct NcclApi {
     int (*CommInitRank)(void**, int, NcclId, int) = nullptr;
     int (*AllReduce)(const void*, void*, size_t, int, int, void*, cudaStream_t) = nullptr;
     int (*CommDestroy)(void*) = nullptr;
+    int (*CommCount)(void*, int*) = nullptr;
+    int (*CommUserRank)(void*, int*) = nullptr;
     const char* (*GetErrorString)(int) = nullptr;
     bool ok = false;
     std::string why;
@@ -827,8 +831,11 @@ NcclApi& nccl_api() {
         a.CommInitRank = reinterpret_cast<decltype(a.CommInitRank)>(dlsym(lib, "ncclCommInitRank"));
         a.AllReduce = reinterpret_cast<decltype(a.AllReduce)>(dlsym(lib, "ncclAllReduce"));
         a.CommDestroy = reinterpret_cast<decltype(a.CommDestroy)>(dlsym(lib, "ncclCommDestroy"));
+        a.CommCount = reinterpret_cast<decltype(a.CommCount)>(dlsym(lib, "ncclCommCount"));
+        a.CommUserRank = reinterpret_cast<decltype(a.CommUserRank)>(dlsym(lib, "ncclCommUserRank"));
         a.GetErrorString = reinterpret_cast<decltype(a.GetErrorString)>(dlsym(lib, "ncclGetErrorString"));
-        a.ok = a.GetUniqueId && a.CommInitRank && a.AllReduce && a.CommDestroy && a.GetErrorString;
+        a.ok = a.GetUniqueId && a.CommInitRank && a.AllReduce && a.CommDestroy && a.CommCount && a.CommUserRank &&
+               a.GetErrorString;
         if (!a.ok) a.why = "NCCL library lacks an expected symbol";
         return a;
     }();
@@ -1119,7 +1126,7 @@ namespace {
 struct KadWorkspace {
     __half *hi, *lo, *shift;
     float* norm;
-    double *colpart, *partial;
+    double *colpart, *partial;                      // partial, hist: one copy per local shard (KadShards::copies)
     unsigned long long* hist;
     fad::KadSelectState* state;
     unsigned char* extra;                           // the caller's own bytes (kad_prepare's extra)
@@ -1136,18 +1143,20 @@ int kad_check(fad_handle* h, const void* z, long long m, long long n, int d, con
 }
 
 // shift (fp16 mean of the first m rows), hi / lo split and row norms of z [N, d]; the two TMA maps over hi / lo.
-// norm_rows: at least this many norms (zero past N); extra: bytes of w.extra for the caller
+// copies: of the partial buffer and the histogram; norm_rows: at least this many norms (zero past N); extra: bytes of
+// w.extra for the caller
 int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspace& w, CUtensorMap* map_hi,
-                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st, size_t norm_rows = 0, size_t extra = 0) {
+                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st, int copies, size_t norm_rows = 0, size_t extra = 0) {
     p.N = N; p.m = m; p.d = d;
     p.T = (N + 127) / 128;
     p.units = (p.T + 1) / 2;
+    p.unit0 = 0; p.unit1 = p.units;
     const size_t rows_pad = std::max((size_t)p.T * 128, norm_rows);
     const int chunks = (m + fad::kKadColRows - 1) / fad::kKadColRows;
     auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t b_split = al(rows_pad * d * 2), b_norm = al(rows_pad * 4), b_shift = al((size_t)d * 2),
-                 b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8),
-                 b_hist = al(2 * fad::kKadHistBins * 8), b_state = al(sizeof(fad::KadSelectState));
+                 b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8 * copies),
+                 b_hist = al(2 * fad::kKadHistBins * 8 * (size_t)copies), b_state = al(sizeof(fad::KadSelectState));
     if (h->kad_buf.grow(2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state + al(extra))) return 1;
     unsigned char* q = h->kad_buf.get<unsigned char>();
     w.hi = reinterpret_cast<__half*>(q);            q += b_split;
@@ -1173,53 +1182,212 @@ int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspac
     return encode_f16_map(map_lo, w.lo, 2, dims, strides, box);
 }
 
-template <int MODE>
-int launch_kad_tiles(fad_handle* h, const CUtensorMap& mh, const CUtensorMap& ml, const fad::KadParams& p, cudaStream_t st) {
-    const int grid = std::min(p.units, h->num_sms);   // the result does not depend on it (fixed work units)
-    return launch(h, fad::kad_tile_kernel<MODE>, grid, fad::kKadThreads, fad::kKadSmemBytes, st, mh, ml, p);
+// ---- sharding (DESIGN.md section 5.11).  A call is cut into `size` shards of contiguous work units.  Collective: this
+// process computes shard `rank` of the communicator's `size` into one zero-filled buffer, and the exchange is an NCCL
+// all-reduce.  Local: this device computes shards 0 .. size - 1 one after another, each into its own zero-filled copy,
+// and the exchange adds the copies in shard order.  Either way every exchanged value is produced by one shard and is
+// zero in the others (or is an integer count), so the sum is exact and the result equals the one-shard result bitwise.
+struct KadShards {
+    void* comm = nullptr;      // collective: the communicator; local: null
+    int rank = 0, size = 1;
+    int copies() const { return comm ? 1 : size; }
+    int first() const { return comm ? rank : 0; }
+    int last() const { return comm ? rank + 1 : size; }
+};
+
+int kad_shards(fad_handle* h, void* comm_arg, int local_shards, KadShards& sh) {
+    if (!h) return fail("null handle");
+    if (local_shards < 0) return fail("local_shards must be >= 0");
+    if (local_shards > 0) {
+        if (comm_arg) return fail("local_shards >= 1 runs without a communicator: pass NULL");
+        sh.size = local_shards;
+        return 0;
+    }
+    sh.comm = comm_arg ? comm_arg : h->nccl_comm;
+    if (!sh.comm) return fail("no communicator: call fad_comm_init or pass an ncclComm_t (or set local_shards >= 1)");
+    NcclApi& n = nccl_api();
+    if (!n.ok) return fail(n.why);
+    int rc = n.CommCount(sh.comm, &sh.size);
+    if (rc != 0) return nccl_fail("ncclCommCount", rc);
+    rc = n.CommUserRank(sh.comm, &sh.rank);
+    if (rc != 0) return nccl_fail("ncclCommUserRank", rc);
+    return 0;
+}
+
+// shard s = units [bounds[s], bounds[s + 1]): the first unit at which the running tile total reaches s / shards of
+// the whole, so a shard holds at most its ideal share plus one unit's tiles
+std::vector<long long> kad_shard_plan(const std::vector<long long>& tiles, int shards) {
+    long long total = 0;
+    for (long long t : tiles) total += t;
+    std::vector<long long> bounds(shards + 1, 0);
+    long long u = 0, acc = 0;
+    for (int s = 1; s < shards; ++s) {
+        while (u < (long long)tiles.size() && (__int128)acc * shards < (__int128)s * total) acc += tiles[u++];
+        bounds[s] = u;
+    }
+    bounds[shards] = (long long)tiles.size();
+    return bounds;
+}
+
+// tiles of the MODE 0 / 1 units over T tile rows: row u, then row T - 1 - u (once when they are the same row)
+std::vector<long long> kad_pair_unit_tiles(int T) {
+    std::vector<long long> t((T + 1) / 2);
+    for (int u = 0; u < (int)t.size(); ++u) t[u] = (T - u) + (T - 1 - u != u ? u + 1 : 0);
+    return t;
+}
+
+// the arguments of a collective call, compared across the ranks before any tile work
+constexpr int kKadArgs = 8;
+const char* const kKadArgNames[kKadArgs] = {"ok", "m", "n", "d", "n_items", "offsets", "sigma", "z"};
+enum { kArgOk, kArgM, kArgN, kArgD, kArgItems, kArgOffsets, kArgSigma, kArgZ };
+
+// bad: this rank's own checks rejected the call (g_err says why).  Local: fail with that.  Collective: every rank takes
+// part whatever its own checks said.  The digest of z (rows x d fp16) and the bits of *sigma complete args, then one
+// all-reduce (max over the values and their complements) gives each value's max and min on every rank; a rank that
+// rejected its arguments or any value that differs fails the call on every rank with the same message.
+int kad_agree(fad_handle* h, const KadShards& sh, const char* fn, bool bad, unsigned long long (&args)[kKadArgs],
+              const void* z, long long rows, int d, const double* sigma, cudaStream_t st) {
+    if (!sh.comm) return bad ? 1 : 0;
+    if (h->kad_agree.grow((2 * kKadArgs + 1) * 8)) return 1;
+    unsigned long long* dv = h->kad_agree.get<unsigned long long>();
+    if (bad) {
+        for (auto& a : args) a = 0;
+    } else {
+        args[kArgOk] = 1;
+        unsigned long long* dz = dv + 2 * kKadArgs;
+        const long long n_vec = rows * d / 8;
+        CK(cudaMemsetAsync(dz, 0, 8, st));
+        if (launch(h, fad::kad_digest_kernel, (unsigned)std::min<long long>((n_vec + 255) / 256, 4LL * h->num_sms), 256, 0,
+                   st, reinterpret_cast<const uint4*>(z), n_vec, dz)) return 1;
+        if (sigma) CK(cudaMemcpyAsync(&args[kArgSigma], sigma, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(&args[kArgZ], dz, 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+    }
+    unsigned long long v[2 * kKadArgs];
+    for (int i = 0; i < kKadArgs; ++i) { v[i] = args[i]; v[kKadArgs + i] = ~args[i]; }
+    CK(cudaMemcpyAsync(dv, v, sizeof v, cudaMemcpyHostToDevice, st));
+    const int rc = nccl_api().AllReduce(dv, dv, 2 * kKadArgs, /*ncclUint64*/ 5, /*ncclMax*/ 2, sh.comm, st);
+    if (rc != 0) return nccl_fail("ncclAllReduce", rc);
+    CK(cudaMemcpyAsync(v, dv, sizeof v, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (~v[kKadArgs + kArgOk] == 0)
+        return fail(std::string(fn) + ": a rank rejected its arguments; no rank computed anything");
+    std::string diff;
+    for (int i = 1; i < kKadArgs; ++i)
+        if (v[i] != ~v[kKadArgs + i]) diff += std::string(diff.empty() ? "" : ", ") + kKadArgNames[i];
+    if (!diff.empty()) return fail(std::string(fn) + ": the ranks' arguments differ (" + diff + "); no rank computed anything");
+    return 0;
+}
+
+unsigned long long kad_offsets_digest(const std::vector<long long>& off) {
+    unsigned long long s = 0;
+    for (size_t k = 0; k < off.size(); ++k) s += fad::kad_mix64(fad::kad_mix64(k) ^ (unsigned long long)off[k]);
+    return s;
+}
+
+// the one exchange of a pass: buf (n values of T per shard copy) summed over the shards
+template <typename T>
+int kad_exchange(fad_handle* h, const KadShards& sh, T* buf, long long n, cudaStream_t st) {
+    if (sh.size == 1) return 0;
+    if (sh.comm) {
+        const int type = std::is_same<T, double>::value ? /*ncclFloat64*/ 8 : /*ncclUint64*/ 5;
+        const int rc = nccl_api().AllReduce(buf, buf, (size_t)n, type, /*ncclSum*/ 0, sh.comm, st);
+        return rc != 0 ? nccl_fail("ncclAllReduce", rc) : 0;
+    }
+    return launch(h, fad::kad_shard_sum_kernel<T>, (unsigned)std::min<long long>((n + 255) / 256, 4LL * h->num_sms), 256,
+                  0, st, buf, n, sh.size);
+}
+
+// the tile pass of MODE over this process's shards (bounds: kad_shard_plan of the pass's units), then the exchange of
+// its output: the partials (MODE 0, 2) or the histogram (MODE 1), n values per copy at buf, zero-filled first
+template <int MODE, typename T>
+int kad_sharded_pass(fad_handle* h, const KadShards& sh, const std::vector<long long>& bounds, const CUtensorMap& mh,
+                     const CUtensorMap& ml, fad::KadParams p, T* buf, long long n, cudaStream_t st) {
+    // one shard writes every partial itself; histogram counts always start from zero
+    if (MODE == 1 || sh.size > 1) CK(cudaMemsetAsync(buf, 0, (size_t)n * sizeof(T) * sh.copies(), st));
+    for (int s = sh.first(); s < sh.last(); ++s) {
+        T* mine = buf + (size_t)(s - sh.first()) * n;
+        if constexpr (MODE == 1) p.hist = mine; else p.partial = mine;
+        p.unit0 = (int)bounds[s];
+        p.unit1 = (int)bounds[s + 1];
+        // the result does not depend on the grid (fixed work units); an empty shard launches nothing
+        if (launch(h, fad::kad_tile_kernel<MODE>, std::min(p.unit1 - p.unit0, h->num_sms), fad::kKadThreads,
+                   fad::kKadSmemBytes, st, mh, ml, p)) return 1;
+    }
+    return kad_exchange(h, sh, buf, n, st);
 }
 }  // namespace
 
 extern "C" {
 
-int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream) {
-    if (kad_check(h, x_f16, m, 2, d, out)) return 1;
+int fad_kad_shard_plan(const long long* unit_tiles, long long units, int shards, long long* bounds) {
+    if ((!unit_tiles && units > 0) || !bounds) return fail("null argument");
+    if (units < 0 || shards < 1) return fail("units must be >= 0 and shards >= 1");
+    std::vector<long long> t(unit_tiles, unit_tiles + units);
+    for (long long x : t)
+        if (x < 1) return fail("every unit has at least one tile");
+    const std::vector<long long> b = kad_shard_plan(t, shards);
+    std::copy(b.begin(), b.end(), bounds);
+    return 0;
+}
+
+int fad_kad_median_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* x_f16, long long m,
+                              int d, double* out, void* stream) {
+    KadShards sh;
+    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long args[kKadArgs] = {};
+    args[kArgM] = (unsigned long long)m; args[kArgD] = (unsigned long long)d;
+    const bool bad = kad_check(h, x_f16, m, 2, d, out) != 0;
+    if (kad_agree(h, sh, "fad_kad_median_sq_sharded", bad, args, x_f16, m, d, nullptr, st)) return 1;
     KadWorkspace w;
     CUtensorMap mh, ml;
     fad::KadParams p = {};
-    if (kad_prepare(h, reinterpret_cast<const __half*>(x_f16), (int)m, (int)m, d, w, &mh, &ml, p, st)) return 1;
+    if (kad_prepare(h, reinterpret_cast<const __half*>(x_f16), (int)m, (int)m, d, w, &mh, &ml, p, st, sh.copies())) return 1;
+    const std::vector<long long> bounds = kad_shard_plan(kad_pair_unit_tiles(p.T), sh.size);
     const unsigned long long pairs = (unsigned long long)m * (unsigned long long)(m - 1) / 2;
     if (launch(h, fad::kad_select_init_kernel, 1, 1, 0, st, w.state, (pairs - 1) / 2, pairs / 2)) return 1;
     // radix digits of the fp32 bit pattern of q >= 0 (bit 31 is 0): 30..20, 19..10, 9..0
     const int shifts[3] = {20, 10, 0}, bins[3] = {2048, 1024, 1024};
     const uint32_t masks[3] = {0u, 0xFFF00000u, 0xFFFFFC00u};
     p.prefix = reinterpret_cast<const uint32_t*>(w.state);     // KadSelectState::prefix is its first member
-    p.hist = w.hist;
     for (int pass = 0; pass < 3; ++pass) {
-        CK(cudaMemsetAsync(w.hist, 0, 2 * fad::kKadHistBins * 8, st));
         p.mask = masks[pass]; p.shift = shifts[pass]; p.bins = bins[pass];
-        if (launch_kad_tiles<1>(h, mh, ml, p, st) ||
+        if (kad_sharded_pass<1>(h, sh, bounds, mh, ml, p, w.hist, 2 * fad::kKadHistBins, st) ||
             launch(h, fad::kad_select_kernel, 1, 32, 0, st, w.state, w.hist, shifts[pass], bins[pass], pass == 2, out)) return 1;
     }
     return 0;
 }
 
-int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
-                 void* stream) {
-    if (kad_check(h, z_f16, m, n, d, out)) return 1;
-    if (!sigma) return fail("null argument");
+int fad_kad_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                         long long n, int d, const double* sigma, double* out, void* stream) {
+    KadShards sh;
+    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long args[kKadArgs] = {};
+    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
+    const bool bad = kad_check(h, z_f16, m, n, d, out) || (!sigma && fail("null argument"));
+    if (kad_agree(h, sh, "fad_kad_sums_sharded", bad, args, z_f16, m + n, d, sigma, st)) return 1;
     KadWorkspace w;
     CUtensorMap mh, ml;
     fad::KadParams p = {};
-    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n), (int)m, d, w, &mh, &ml, p, st)) return 1;
+    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n), (int)m, d, w, &mh, &ml, p, st, sh.copies()))
+        return 1;
     p.sigma = sigma;
-    p.partial = w.partial;
-    if (launch_kad_tiles<0>(h, mh, ml, p, st)) return 1;
+    if (kad_sharded_pass<0>(h, sh, kad_shard_plan(kad_pair_unit_tiles(p.T), sh.size), mh, ml, p, w.partial, 3LL * p.units, st))
+        return 1;
     return launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, p.units, out);
+}
+
+int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream) {
+    return fad_kad_median_sq_sharded(h, nullptr, 1, x_f16, m, d, out, stream);
+}
+
+int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
+                 void* stream) {
+    return fad_kad_sums_sharded(h, nullptr, 1, z_f16, m, n, d, sigma, out, stream);
 }
 
 }  // extern "C"
@@ -1231,23 +1399,40 @@ namespace {
 // SM many units
 constexpr long long kKadSongMinGroup = 4;
 constexpr long long kKadSongUnits = 8192;
-}  // namespace
 
-extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets,
-                                 long long n_items, int d, const double* sigma, double* out, void* stream) {
+// the host side of fad_kad_song_sums' checks: the offsets read back and validated (off, n_total)
+int kad_song_check(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items, int d,
+                   const double* sigma, const double* out, cudaStream_t st, std::vector<long long>& off, long long& n_total) {
     if (kad_check(h, z_f16, m, 2, d, out)) return 1;
     if (!offsets || !sigma) return fail("null argument");
     if (n_items < 0) return fail("n_items must be >= 0");
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<long long> off((size_t)n_items + 1);
+    off.resize((size_t)n_items + 1);
     CK(cudaMemcpyAsync(off.data(), offsets, off.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (off[0] != 0) return fail("offsets[0] must be 0");
     for (long long k = 0; k < n_items; ++k)
         if (off[k + 1] < off[k]) return fail("offsets must be non-decreasing");
-    const long long n_total = off.back();
+    n_total = off.back();
     if (m + n_total > (1LL << 30)) return fail("too many rows");
+    return 0;
+}
+}  // namespace
+
+extern "C" int fad_kad_song_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                         long long m, const long long* offsets, long long n_items, int d,
+                                         const double* sigma, double* out, void* stream) {
+    KadShards sh;
+    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<long long> off;
+    long long n_total = 0;
+    const bool bad = kad_song_check(h, z_f16, m, offsets, n_items, d, sigma, out, st, off, n_total) != 0;
+    unsigned long long args[kKadArgs] = {};
+    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n_total; args[kArgD] = (unsigned long long)d;
+    args[kArgItems] = (unsigned long long)n_items;
+    if (!bad) args[kArgOffsets] = kad_offsets_digest(off);
+    if (kad_agree(h, sh, "fad_kad_song_sums_sharded", bad, args, z_f16, m + n_total, d, sigma, st)) return 1;
 
     // work list: per Y tile t, the column tiles X 0..Tx-1, then the band t..be(t)
     const int Tx = (int)((m + 127) / 128), Ty = (int)((n_total + 127) / 128);
@@ -1261,23 +1446,27 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
     }
     const int G = (int)std::max(kKadSongMinGroup, (total + kKadSongUnits - 1) / kKadSongUnits);
     std::vector<int4> work;
+    std::vector<long long> work_tiles;
     std::vector<int> unit_start(Ty + 1, 0);
     for (int t = 0; t < Ty; ++t) {
         // near-equal cuts: units of G tiles plus a short remainder would leave CTAs that take every other unit idle
         const long long n = ncols[t], cuts = (n + G - 1) / G;
-        for (long long i = 0; i < cuts; ++i) work.push_back(make_int4(t, (int)(i * n / cuts), (int)((i + 1) * n / cuts), 0));
+        for (long long i = 0; i < cuts; ++i) {
+            work.push_back(make_int4(t, (int)(i * n / cuts), (int)((i + 1) * n / cuts), 0));
+            work_tiles.push_back(work.back().z - work.back().y);
+        }
         unit_start[t + 1] = (int)work.size();
     }
     const size_t units = work.size();
 
     auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
     const size_t b_work = al(units * sizeof(int4)), b_start = al(unit_start.size() * 4), b_end = al((size_t)Ty * 128 * 4),
-                 b_part = al(units * 256 * 8), b_xx = al(3 * 8);
+                 b_part = al(units * 256 * 8 * sh.copies()), b_xx = al(3 * 8);
     KadWorkspace w;
     CUtensorMap mh, ml;
     fad::KadParams p = {};
     if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n_total), (int)m, d, w, &mh, &ml, p, st,
-                    (size_t)m + (size_t)Ty * 128, b_work + b_start + b_end + b_part + b_xx)) return 1;
+                    sh.copies(), (size_t)m + (size_t)Ty * 128, b_work + b_start + b_end + b_part + b_xx)) return 1;
     unsigned char* q = w.extra;
     int4* d_work = reinterpret_cast<int4*>(q);       q += b_work;
     int* d_start = reinterpret_cast<int*>(q);        q += b_start;
@@ -1291,8 +1480,8 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
     px.N = (int)m;
     px.T = Tx;
     px.units = (Tx + 1) / 2;
-    px.partial = w.partial;
-    if (launch_kad_tiles<0>(h, mh, ml, px, st) || launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, px.units, d_xx))
+    if (kad_sharded_pass<0>(h, sh, kad_shard_plan(kad_pair_unit_tiles(Tx), sh.size), mh, ml, px, w.partial, 3LL * px.units, st) ||
+        launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, px.units, d_xx))
         return 1;
     CK(cudaMemcpyAsync(out, d_xx, sizeof(double), cudaMemcpyDeviceToDevice, st));
     if (n_items == 0) return 0;
@@ -1306,10 +1495,15 @@ extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, 
         p.row_end = d_end;
         p.Tx = Tx;
         p.units = (int)units;
-        p.partial = d_part;
-        if (launch_kad_tiles<2>(h, mh, ml, p, st)) return 1;
+        if (kad_sharded_pass<2>(h, sh, kad_shard_plan(work_tiles, sh.size), mh, ml, p, d_part, 256LL * (long long)units, st))
+            return 1;
     }
     return launch(h, fad::kad_song_reduce_kernel, (unsigned)n_items, fad::kKadSongReduceThreads, 0, st, d_part, d_start, offsets, out);
+}
+
+extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets,
+                                 long long n_items, int d, const double* sigma, double* out, void* stream) {
+    return fad_kad_song_sums_sharded(h, nullptr, 1, z_f16, m, offsets, n_items, d, sigma, out, stream);
 }
 
 #include "resample_host.inc"

@@ -16,8 +16,9 @@
 // The accumulator uses the GEMM's chunk-and-unshrink scheme (conv_gemm.cuh), counting the three products per column.
 //
 // Work units and determinism.  T = ceil(N / 128) tile rows; unit u (u < ceil(T / 2)) is tile row u (tiles u..T-1)
-// followed by tile row T-1-u (tiles T-1-u..T-1): T + 1 tiles per unit, so units are balanced.  A CTA takes units
-// blockIdx.x, + gridDim.x, ...  Each consumer thread sums its elements of a tile in fp32 (fixed order), adds that to
+// followed by tile row T-1-u (tiles T-1-u..T-1): T + 1 tiles per unit, so units are balanced.  A launch covers the
+// units [unit0, unit1) (all of them, or one shard of a sharded call), and a CTA takes units unit0 + blockIdx.x,
+// + gridDim.x, ...  Each consumer thread sums its elements of a tile in fp32 (fixed order), adds that to
 // fp64 per-thread accumulators in tile order, and at the end of the unit the 256 consumer threads are reduced in a
 // fixed tree into partial[u][3] (fp64).  kad_reduce_kernel sums the partials in unit order.  No floating-point atomic
 // anywhere: the three sums are bitwise reproducible and independent of the grid size and of timing.
@@ -67,7 +68,8 @@ struct KadParams {
     int m;                   // rows of X
     int d;                   // columns
     int T;                   // tile rows = ceil(N / 128)
-    int units;               // ceil(T / 2)
+    int units;               // ceil(T / 2) (MODE 2: the work list's length)
+    int unit0, unit1;        // this launch's units [unit0, unit1) (a shard; partials stay indexed by the global unit)
     const float* norm;       // [T * 128] |y_i|^2 (zero past N; MODE 2: [m + Ty * 128])
     // MODE 0 and 2
     const double* sigma;     // device scalar
@@ -224,7 +226,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         if (warp == 0 && elect_one()) {
             int s = 0; uint32_t ph = 0;
             if constexpr (MODE == 2) {
-                for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
                     const int4 wk = p.work[u];
                     const int arow = p.m + wk.x * 128;
                     for (int v = wk.y; v < wk.z; ++v)
@@ -232,7 +234,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                                       v < p.Tx ? v * 128 : arow + (v - p.Tx) * 128);
                 }
             } else {
-                for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
                     for (int half = 0; half < 2; ++half) {
                         const int r = half == 0 ? u : p.T - 1 - u;
                         if (half == 1 && r == u) break;                // odd T: the middle row once
@@ -253,7 +255,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
             const double sg = *p.sigma;
             const float neg_coef = (float)(-1.4426950408889634 / (2.0 * sg * sg));
             const int lr0 = c * 64 + wq * 16 + (lane >> 2);                    // tile rows lr0, lr0 + 8
-            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+            for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
                 const int4 wk = p.work[u];
                 const int row0 = p.m + wk.x * 128 + lr0;                       // rows of Z
                 const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
@@ -323,7 +325,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
         }
         const uint32_t digit_mask = (uint32_t)p.bins - 1;
 
-        for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
             double sxx = 0.0, syy = 0.0, sxy = 0.0;
             for (int half = 0; half < 2; ++half) {
                 const int r = half == 0 ? u : p.T - 1 - u;
@@ -411,6 +413,40 @@ __global__ void kad_reduce_kernel(const double* __restrict__ partial, int units,
     double s = 0.0;
     for (int u = 0; u < units; ++u) s += partial[(size_t)u * 3 + t];
     out[t] = s;
+}
+
+// sharded passes (fadtk_b200.cu, kad_exchange): buf[i] = buf[i] + buf[n + i] + ... over the shards' copies in shard
+// order.  Each value is written by one shard and zero in the others, so the sum is that value exactly.
+template <typename T>
+__global__ void kad_shard_sum_kernel(T* __restrict__ buf, long long n, int shards) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        T s = buf[i];
+        for (int c = 1; c < shards; ++c) s += buf[(size_t)c * n + i];
+        buf[i] = s;
+    }
+}
+
+// *out += the wrapping sum over the n_vec 8-element vectors of z of a 64-bit mix of (element index, fp16 bits): an
+// order-independent digest the ranks of a sharded call compare before any tile work
+__host__ __device__ __forceinline__ unsigned long long kad_mix64(unsigned long long x) {   // splitmix64 finaliser
+    x += 0x9E3779B97F4A7C15ull;
+    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+    return x ^ (x >> 31);
+}
+__global__ void kad_digest_kernel(const uint4* __restrict__ z, long long n_vec, unsigned long long* __restrict__ out) {
+    unsigned long long s = 0;
+    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n_vec; v += (long long)gridDim.x * blockDim.x) {
+        const uint4 q = z[v];
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const unsigned long long e = (unsigned long long)(8 * v + k);
+            s += kad_mix64((e << 16) | ((w[k >> 1] >> (16 * (k & 1))) & 0xFFFFu));
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) atomicAdd(out, s);
 }
 
 // per-song sums, MODE 2: row_end[r] for the Y rows r < rows (Ty * 128) = m + the end row (in Y) of r's song; 0 past n_total

@@ -93,7 +93,7 @@ def _kad_rows(a, what: str):
     return t
 
 
-def calc_kernel_audio_distance(emb_baseline, emb_eval) -> KADResults:
+def calc_kernel_audio_distance(emb_baseline, emb_eval, distributed: bool = False) -> KADResults:
     """Kernel Audio Distance (Chung et al., 2025) between two fp16 embedding sets X [m, d] and Y [n, d], with the fp16
     values taken as exact reals:
 
@@ -107,20 +107,55 @@ def calc_kernel_audio_distance(emb_baseline, emb_eval) -> KADResults:
     The pair sums and the bandwidth selection run on the GPU (fad_kad_median_sq, fad_kad_sums); MMD^2_u is assembled
     from the three fp64 sums.  A width that is not a multiple of 8 is zero-padded, which changes no distance.
     Raises ValueError for fewer than two rows on either side, non-fp16 or non-2-D input, mismatched widths, and
-    sigma = 0 (more than half of the baseline pairs are identical rows)."""
+    sigma = 0 (more than half of the baseline pairs are identical rows).
+
+    distributed=True under torchrun (world size > 1): a collective call that every rank makes with the same sets.  The
+    pair tiles are split over the ranks (fad_kad_*_sharded over the library's NCCL communicator), and every rank gets
+    the result, bitwise equal to one GPU's.  The ranks' arguments are compared first; a difference raises NativeError
+    on every rank.  RuntimeError when that communicator cannot be set up (gloo backend, FADTK_NATIVE_ALLREDUCE=0)."""
     x, y = _kad_rows(emb_baseline, "baseline"), _kad_rows(emb_eval, "eval")
     m, n = int(x.shape[0]), int(y.shape[0])
     if m < 2 or n < 2:
         raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {m}, eval {n})")
     if x.shape[1] != y.shape[1]:
         raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
-    from . import _native
-    eng = _native.engine()
+    eng, collective = _kad_engine(distributed)
     z = _kad_device_rows(torch.cat([x, y]), eng)
-    sigma = _kad_bandwidth(eng, z, m)
-    s_xx, s_yy, s_xy = (float(v) for v in eng.kad_sums(z, m, torch.tensor([sigma], dtype=torch.float64,
-                                                                               device=eng.torch_device)).cpu().numpy())
+    sigma = _kad_bandwidth(eng, z, m, collective)
+    sig = torch.tensor([sigma], dtype=torch.float64, device=eng.torch_device)
+    sums = eng.kad_sums_sharded(z, m, sig) if collective else eng.kad_sums(z, m, sig)
+    s_xx, s_yy, s_xy = (float(v) for v in sums.cpu().numpy())
     return KADResults(score=_kad_score(s_xx, s_yy, s_xy, m, n), bandwidth=sigma, n_baseline=m, n_eval=n)
+
+
+def _kad_engine(distributed: bool):
+    """-> (this process's engine, whether the KAD calls are collective over the torchrun group)"""
+    from . import _native, dist
+    eng = _native.engine()
+    if not (distributed and dist.world_size() > 1):
+        return eng, False
+    if not dist.enable_native_allreduce(eng):
+        raise RuntimeError("distributed KAD runs over the library's own NCCL communicator, which needs torch.distributed "
+                           "on the nccl backend and FADTK_NATIVE_ALLREDUCE unset or 1")
+    return eng, True
+
+
+def _on_rank0(fn, collective: bool):
+    """fn() decided on rank 0 and broadcast, so that every rank of a collective call takes the same branch; a ValueError
+    on rank 0 is raised on every rank"""
+    if not collective:
+        return fn()
+    from . import dist
+    res = None
+    if dist.rank() == 0:
+        try:
+            res = (True, fn())
+        except ValueError as e:
+            res = (False, str(e))
+    ok, val = dist.broadcast_object(res)
+    if not ok:
+        raise ValueError(val)
+    return val
 
 
 def _kad_device_rows(z: torch.Tensor, eng) -> torch.Tensor:
@@ -133,9 +168,9 @@ def _kad_device_rows(z: torch.Tensor, eng) -> torch.Tensor:
     return z.to(eng.torch_device, non_blocking=True)
 
 
-def _kad_bandwidth(eng, z: torch.Tensor, m: int) -> float:
+def _kad_bandwidth(eng, z: torch.Tensor, m: int, collective: bool = False) -> float:
     """sigma from the first m rows of z (device): the numpy median of their pairwise distances; ValueError when 0."""
-    sq = eng.kad_median_sq(z[:m]).cpu().numpy()
+    sq = (eng.kad_median_sq_sharded(z[:m]) if collective else eng.kad_median_sq(z[:m])).cpu().numpy()
     sigma = 0.5 * (float(np.sqrt(sq[0])) + float(np.sqrt(sq[1])))
     if not sigma > 0.0:
         raise ValueError("KAD bandwidth is 0: more than half of the baseline pairs are identical rows")
@@ -147,13 +182,13 @@ def _kad_score(s_xx: float, s_yy: float, s_xy: float, m: int, n: int) -> float:
     return 1000.0 * (2.0 * s_xx / (m * (m - 1.0)) + 2.0 * s_yy / (n * (n - 1.0)) - 2.0 * s_xy / (float(m) * n))
 
 
-def calc_kernel_audio_distance_songs(emb_baseline, songs) -> list[KADResults]:
+def calc_kernel_audio_distance_songs(emb_baseline, songs, distributed: bool = False) -> list[KADResults]:
     """KAD of every song against one baseline: for each fp16 [n_k, d] array in ``songs``, the value
     calc_kernel_audio_distance(emb_baseline, songs[k]) is defined to be (same sigma from the baseline alone, same sums),
     with sigma and the baseline's own pair sum computed once for all songs and every song's sums in one GPU pass
     (fad_kad_song_sums).  A song with fewer than two rows gets score NaN (n_eval still says how many rows it had).
     Raises ValueError like calc_kernel_audio_distance: non-fp16 or non-2-D input, widths that differ from the
-    baseline's, fewer than two baseline rows, sigma = 0."""
+    baseline's, fewer than two baseline rows, sigma = 0.  distributed: as for calc_kernel_audio_distance."""
     x = _kad_rows(emb_baseline, "baseline")
     ys = [_kad_rows(y, f"song {k}") for k, y in enumerate(songs)]
     for k, y in enumerate(ys):
@@ -161,20 +196,19 @@ def calc_kernel_audio_distance_songs(emb_baseline, songs) -> list[KADResults]:
             raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, song {k} {y.shape[1]})")
     offsets = np.zeros(len(ys) + 1, dtype=np.int64)
     offsets[1:] = np.cumsum([int(y.shape[0]) for y in ys])
-    return _kad_songs(torch.cat([x, *[y.to(x.device) for y in ys]]), int(x.shape[0]), offsets)
+    return _kad_songs(torch.cat([x, *[y.to(x.device) for y in ys]]), int(x.shape[0]), offsets, distributed)
 
 
-def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray) -> list[KADResults]:
+def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray, distributed: bool = False) -> list[KADResults]:
     """z = [X; Y_1; ...] fp16 (host or device), offsets int64 [K + 1] into the rows after X -> one KADResults per song"""
     if m < 2:
         raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {m})")
-    from . import _native
-    eng = _native.engine()
+    eng, collective = _kad_engine(distributed)
     z = _kad_device_rows(z, eng)
-    sigma = _kad_bandwidth(eng, z, m)
+    sigma = _kad_bandwidth(eng, z, m, collective)
     dev = eng.torch_device
-    sums = eng.kad_song_sums(z, m, torch.from_numpy(offsets).to(dev),
-                             torch.tensor([sigma], dtype=torch.float64, device=dev)).cpu().numpy()
+    args = (z, m, torch.from_numpy(offsets).to(dev), torch.tensor([sigma], dtype=torch.float64, device=dev))
+    sums = (eng.kad_song_sums_sharded(*args) if collective else eng.kad_song_sums(*args)).cpu().numpy()
     s_xx = float(sums[0])
     out = []
     for k, n in enumerate(np.diff(offsets).tolist()):
@@ -497,37 +531,47 @@ class FrechetAudioDistance:
         mu_eval, cov_eval = self.load_stats(eval)
         return calc_frechet_distance(mu_bg, cov_bg, mu_eval, cov_eval)
 
-    def score_kad(self, baseline_dir: PathLike, eval_dir: PathLike) -> KADResults:
+    def score_kad(self, baseline_dir: PathLike, eval_dir: PathLike, distributed: bool = False) -> KADResults:
         """Kernel Audio Distance between the cached embeddings of two directories (calc_kernel_audio_distance): all rows
-        of all <dir>/embeddings/<model>/*.npy in sorted file order, the files the directory statistics read."""
+        of all <dir>/embeddings/<model>/*.npy in sorted file order, the files the directory statistics read.
+        distributed=True under torchrun: a collective call; rank 0 lists the files, every rank reads them and takes its
+        share of the pair tiles, and every rank gets the result."""
         from . import _io_native
+        collective = distributed and _kad_engine(True)[1]
         sets = []
         for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
-            files = _sorted_npy_files(kad_embedding_dir(p, self.ml.name))
+            files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name)), collective)
             if not files:
                 raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
             emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
             if emb.dtype != np.float16:
                 raise ValueError(f"KAD needs fp16 embedding caches; {p} holds {emb.dtype}")
             sets.append(emb)
-        return calc_kernel_audio_distance(*sets)
+        return calc_kernel_audio_distance(*sets, distributed=distributed)
 
-    def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str]) -> Path:
+    def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
+                             distributed: bool = False) -> Path:
         """KAD of every file in eval_dir against the embeddings of baseline_dir (calc_kernel_audio_distance_songs: the
         bandwidth and the baseline's pair sum once, every song's sums in one GPU pass), written as score_individual
         writes FAD: rows ``file,score`` sorted by |score|, commas in names replaced, no header; a str csv_name goes
         under data/kad-individual/<model>/, and an existing table is returned untouched.  Files whose cache is
         missing, unreadable or not an fp16 [rows, d] array of the baseline's width, and files with fewer than two
-        embedding rows, are logged and dropped."""
+        embedding rows, are logged and dropped.  distributed=True under torchrun: a collective call; rank 0 lists the
+        directories and decides whether the table exists, every rank reads the caches and takes its share of the pair
+        tiles, and rank 0 alone logs the dropped files and writes the table."""
         csv = Path(csv_name)
         if isinstance(csv_name, str):
             csv = Path('data') / 'kad-individual' / self.ml.name / csv_name
-        if csv.exists():
-            log.info(f"CSV file {csv} already exists, exiting...")
+        collective = distributed and _kad_engine(True)[1]
+        from . import dist
+        writer = not collective or dist.rank() == 0
+        if _on_rank0(csv.exists, collective):
+            if writer:
+                log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
         from . import _io_native
-        files = _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name))
+        files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name)), collective)
         if not files:
             raise ValueError(f"no {self.ml.name} embeddings cached under {baseline_dir}: embed the baseline directory first")
         x, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
@@ -537,11 +581,12 @@ class FrechetAudioDistance:
         m, d = x.shape
 
         def _report(f, msg):
-            log.error(f"An error occurred calculating individual KAD using model {self.ml.name} on file {f}")
-            log.error(msg)
+            if writer:
+                log.error(f"An error occurred calculating individual KAD using model {self.ml.name} on file {f}")
+                log.error(msg)
 
         # fp16 caches read natively in one pass (libfadtk_io.so) into one pinned buffer after the baseline rows
-        all_files = sorted(Path(eval_dir).glob("*.*"))
+        all_files = _on_rank0(lambda: sorted(Path(eval_dir).glob("*.*")), collective)
         caches = [get_cache_embedding_path(self.ml.name, f) for f in all_files]
         n_rows, cols, ndim, dt, st = _io_native.npy_probe(caches, self.audio_load_worker)
         keep = []
@@ -569,9 +614,11 @@ class FrechetAudioDistance:
             for k in np.nonzero(st != _io_native.OK)[0]:     # vanished / rewritten since the probe: dropped below
                 _report(all_files[keep[k]], f"cannot read {caches[keep[k]]} (status {int(st[k])})")
                 host[m + offs[k]:m + offs[k + 1]] = 0.0
-            res = _kad_songs(host, m, offs)
+            res = _kad_songs(host, m, offs, distributed)
             pairs = [(all_files[i], res[k].score) for k, i in enumerate(keep) if st[k] == _io_native.OK]
 
+        if not writer:
+            return csv
         pairs = sorted(pairs, key=lambda x: np.abs(x[1]))
         csv.parent.mkdir(parents=True, exist_ok=True)
         csv.write_text("\n".join([",".join([str(x).replace(',', '_') for x in row]) for row in pairs]))

@@ -1,6 +1,8 @@
 """``python -m fadtk_b200.kad <model> <baseline> <eval> [csv] [--indiv] [-w N] [-s sox]`` - Kernel Audio Distance
 between two audio directories (fad.calc_kernel_audio_distance).  Directories without embedding caches are embedded
-first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``; rank 0 computes and reports).  With
+first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``).  Under ``torchrun`` every rank
+then takes its share of the pair tiles (``distributed=True``) when the library's NCCL communicator can be set up, and
+rank 0 scores alone otherwise; either way rank 0 alone reports and writes.  With
 ``csv``, one row ``model,baseline,eval,kad,bandwidth,n_baseline,n_eval,time`` is appended; a new file gets the header
 first, and an existing file with another header is refused rather than mixed.  With ``--indiv``, every file of the eval
 directory is scored on its own against the baseline (FrechetAudioDistance.score_kad_individual) and ``csv`` is that
@@ -56,18 +58,24 @@ def main(argv=None) -> int:
         _check_csv(args.csv)
     dist.init_from_env()
     _embed_directories(model, (args.baseline, args.eval), args.workers)
-    if dist.rank() != 0:
+    from . import _native
+    sharded = dist.is_distributed() and dist.enable_native_allreduce(_native.engine())
+    if dist.rank() != 0 and not sharded:
         dist.shutdown()
         return 0
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
     if args.indiv:
         table = Path(args.csv or "kad-individual-results.csv")
-        fad.score_kad_individual(args.baseline, args.eval, table)
-        log.info(f"Individual KAD scores saved to {table}")
+        fad.score_kad_individual(args.baseline, args.eval, table, distributed=sharded)
+        if dist.rank() == 0:
+            log.info(f"Individual KAD scores saved to {table}")
         dist.shutdown()
         return 0
-    res = fad.score_kad(args.baseline, args.eval)
+    res = fad.score_kad(args.baseline, args.eval, distributed=sharded)
+    if dist.rank() != 0:
+        dist.shutdown()
+        return 0
     if args.csv:
         _append_row(args.csv, (model.name, args.baseline, args.eval, res.score, res.bandwidth, res.n_baseline,
                                res.n_eval, time.time()))

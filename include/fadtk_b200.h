@@ -299,6 +299,28 @@ int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int
  * Each value is the quantity fad_kad_sums gives for [X; Y_k], bitwise reproducible (fixed work units, no atomics). */
 int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items, int d,
                       const double* sigma, double* out, void* stream);
+/* The same three computations split over shards of contiguous work units (DESIGN.md section 5.11, sharding); the
+ * outputs are bitwise equal to the entries above for any number of shards.
+ *   local_shards == 0  collective over nccl_comm_or_null, or the handle's own communicator (fad_comm_init) when NULL;
+ *                      rank and size come from the communicator, and every rank gets the whole output.  Every rank
+ *                      calls with its own z (the same rows), offsets and sigma.  Before any tile work the ranks compare
+ *                      m, n, d, n_items, a digest of the offsets, the bits of sigma, a digest of z and whether each
+ *                      rank accepted its arguments; any difference fails the call on every rank with the same message.
+ *                      Fails without a communicator.
+ *   local_shards >= 1  this device computes the shards 0 .. local_shards - 1 one after another and adds their outputs in
+ *                      shard order (the arithmetic of the all-reduce); nccl_comm_or_null must be NULL.  1 = the entries
+ *                      above, which are this call.
+ * fad_kad_shard_plan (host only): the cut of `units` work units of unit_tiles[u] >= 1 tiles each into `shards`
+ * contiguous ranges, shard s = [bounds[s], bounds[s + 1]) (bounds: [shards + 1]); each holds at most total / shards
+ * plus one unit's tiles, and shards may be empty when there are more shards than units. */
+int fad_kad_median_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* x_f16, long long m,
+                              int d, double* out, void* stream);
+int fad_kad_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                         long long n, int d, const double* sigma, double* out, void* stream);
+int fad_kad_song_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                              const long long* offsets, long long n_items, int d, const double* sigma, double* out,
+                              void* stream);
+int fad_kad_shard_plan(const long long* unit_tiles, long long units, int shards, long long* bounds);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
