@@ -29,6 +29,7 @@
 #include "wav2vec.cuh"
 #include "attention_wgmma.cuh"
 #include "kad.cuh"
+#include "prdc.cuh"
 
 namespace {
 
@@ -554,6 +555,8 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<0>, fad::kPrdcSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<1>, fad::kPrdcSmemBytes));
     if (setup_gemm<0>(h.get()) || setup_gemm<1>(h.get())) return 1;
     *out = h.release();
     return 0;
@@ -1504,6 +1507,83 @@ extern "C" int fad_kad_song_sums_sharded(fad_handle* h, void* nccl_comm_or_null,
 extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets,
                                  long long n_items, int d, const double* sigma, double* out, void* stream) {
     return fad_kad_song_sums_sharded(h, nullptr, 1, z_f16, m, offsets, n_items, d, sigma, out, stream);
+}
+
+// ------------------------------------------------------- precision, recall, density and coverage (DESIGN.md 5.12)
+namespace {
+// counts-pass work units: each X tile row's Y column tiles cut into `cuts` near-equal runs of about G tiles,
+// G = max(kPrdcMinRun, ceil(Tx Ty / kPrdcUnits)): a function of the shape only, enough units for every SM
+constexpr long long kPrdcMinRun = 4;
+constexpr long long kPrdcUnits = 8192;
+
+// k: the radii's (the counts pass checks with k = 1, the least any radii allow); a, b: the fp32 / int32 outputs and
+// inputs (4-byte aligned), c: the flags
+int prdc_check(fad_handle* h, const void* z, long long m, long long n, int d, int k, const void* a, const void* b,
+               const void* c) {
+    if (!h) return fail("null handle");
+    if (!z || !a || !b || !c) return fail("null argument");
+    if (k < 1 || k > fad::kPrdcMaxK) return fail("k must be in [1, 16]");
+    if (m <= k || n <= k) return fail("PRDC needs more than k rows in each set");
+    if (d <= 0 || d % 8 != 0) return fail("d must be a positive multiple of 8");
+    if ((reinterpret_cast<uintptr_t>(z) & 15) || ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 3))
+        return fail("pointers must be aligned (z to 16 bytes, the fp32 and int32 arrays to 4)");
+    if (m + n > (1LL << 30)) return fail("too many rows");
+    return 0;
+}
+
+// the shared prologue of both passes (kad_prepare: shift, split, norms, maps) and the fields of p it fixes
+int prdc_prepare(fad_handle* h, const void* z, long long m, long long n, int d, KadWorkspace& w, CUtensorMap* mh,
+                 CUtensorMap* ml, fad::PrdcParams& p, cudaStream_t st, size_t extra) {
+    p.m = (int)m; p.n = (int)n; p.d = d;
+    p.Tx = (int)((m + 127) / 128);
+    p.Ty = (int)((n + 127) / 128);
+    fad::KadParams kp = {};
+    // norms up to the last row of the last Y tile (the A operand of a Y tile starts at row m)
+    if (kad_prepare(h, reinterpret_cast<const __half*>(z), (int)(m + n), (int)m, d, w, mh, ml, kp, st, 1,
+                    (size_t)m + (size_t)p.Ty * 128, extra)) return 1;
+    p.norm = w.norm;
+    return 0;
+}
+}  // namespace
+
+extern "C" int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* radii_sq,
+                                void* stream) {
+    if (prdc_check(h, z_f16, m, n, d, k, radii_sq, radii_sq, radii_sq)) return 1;
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::PrdcParams p = {};
+    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, 0)) return 1;
+    p.k = k;
+    p.radii_sq = radii_sq;
+    p.units = p.Tx + p.Ty;
+    // every unit writes its own rows: the result does not depend on the grid
+    return launch(h, fad::prdc_tile_kernel<0>, std::min(p.units, h->num_sms), fad::kKadThreads, fad::kPrdcSmemBytes, st,
+                  mh, ml, p);
+}
+
+extern "C" int fad_prdc_counts(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* radii_sq,
+                               int* inside, unsigned char* flags, void* stream) {
+    if (prdc_check(h, z_f16, m, n, d, 1, radii_sq, inside, flags)) return 1;
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::PrdcParams p = {};
+    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, (size_t)m * 4)) return 1;
+    const long long G = std::max(kPrdcMinRun, ((long long)p.Tx * p.Ty + kPrdcUnits - 1) / kPrdcUnits);
+    p.cuts = (int)((p.Ty + G - 1) / G);
+    p.units = p.Tx * p.cuts;
+    p.radii = radii_sq;
+    p.inside = inside;
+    p.row_flags = reinterpret_cast<uint32_t*>(w.extra);
+    CK(cudaMemsetAsync(inside, 0, (size_t)n * 4, st));
+    CK(cudaMemsetAsync(p.row_flags, 0, (size_t)m * 4, st));
+    // integer atomics only: the counts do not depend on the grid or the order
+    if (launch(h, fad::prdc_tile_kernel<1>, std::min(p.units, h->num_sms), fad::kKadThreads, fad::kPrdcSmemBytes, st,
+               mh, ml, p)) return 1;
+    return launch(h, fad::prdc_flags_kernel, (unsigned)((m + 255) / 256), 256, 0, st, p.row_flags, (int)m, flags);
 }
 
 #include "resample_host.inc"

@@ -1,0 +1,233 @@
+// Precision, recall, density and coverage (PRDC) of two embedding sets on Hopper tensor cores: the k-nearest-neighbour
+// radii of each set and the ball counts between the sets (DESIGN.md section 5.12).
+//
+// Z = [X; Y] (fp16 [m + n, d], X first).  The distances are the KAD ones (kad.cuh): the same prologue (shared fp16
+// shift, hi/lo split, fp64 row norms), the same TMA + wgmma tile loop (kad_load_tile, kad_mma_tile) and the same fp32
+// q = |y_i|^2 + |y_j|^2 - 2 y_i.y_j with q below kQResolution * (|y_i|^2 + |y_j|^2) taken as 0.  Only the epilogue
+// differs, and every output is a selected fp32 value or an integer count, so both passes are bitwise reproducible and
+// independent of the grid without any partial-sum bookkeeping.
+//
+// Radii (PASS 0).  Unit u < Tx: the A operand is X tile u (rows 128 u), the B operands are every X tile; unit Tx + t:
+// the A operand is the 128-row tile of Y at row m + 128 t (as kad_tile_kernel<2>), the B operands are every Y tile.
+// Each consumer thread holds two rows and keeps, per row, the k smallest q of its columns in a sorted register list
+// (an insertion runs only when q is below the current k-th value); the columns j != i, j < the set's size of the same
+// set count (masks by index only: the rows the TMA unit zero-fills never count, duplicate rows are neighbours at 0).
+// The full square is run, not the triangle: a column-wise top-k would need a second sorted list per column of the
+// fragment, and the unit then owns whole rows.  At the end of the unit the four lanes of a quad (same rows) merge
+// their lists by a fixed xor tree, and one lane writes radii_sq[row of Z] = the k-th smallest of the set's q values.
+// Selection does not depend on order, so the value is exact and grid-independent.
+//
+// Counts (PASS 1).  Unit = (X tile tx, a run of Y column tiles [c0, c1)), runs cut by the shape only.  r_i^2 of the
+// two rows of a thread sit in registers; s_j^2 is read per column through the read-only cache, as the column norms
+// are.  Every xy pair is evaluated once, so the four metrics see one fp32 q per pair:
+//   row i:    covered |= q < r_i^2,   recalled |= q < s_j^2   (ORed over the quad, atomicOr into row_flags[i])
+//   column j: inside[j] += #{i : q < r_i^2}                    (integer shuffle tree over the 8 row groups of a warp,
+//                                                               then integer atomicAdd; order-independent)
+// No floating-point atomic anywhere.  prdc_flags_kernel packs row_flags into the uint8 flags.
+//
+// Warp roles and stages are kad_tile_kernel's: warpgroup 0 = TMA producer, warpgroups 1-2 = consumers on rows
+// [64 c, 64 c + 64) of the tile.
+#pragma once
+#include "kad.cuh"
+
+namespace fad {
+
+constexpr int kPrdcMaxK = 16;
+constexpr uint32_t kPrdcSmemBytes = kKadStages * kKadStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+static_assert(kPrdcSmemBytes <= kKadSmemBytes, "within the KAD shared-memory budget");
+
+struct PrdcParams {
+    int m, n, d;             // rows of X, rows of Y, columns
+    int Tx, Ty;              // ceil(m / 128), ceil(n / 128)
+    int units;               // PASS 0: Tx + Ty; PASS 1: Tx * cuts
+    const float* norm;       // [m + Ty * 128] |y_i|^2 of the rows of Z (zero past m + n)
+    // PASS 0
+    int k;                   // 1 .. kPrdcMaxK
+    float* radii_sq;         // [m + n] out
+    // PASS 1
+    const float* radii;      // [m + n] r_i^2 of X, then s_j^2 of Y
+    int cuts;                // column runs per X tile row: run i = Y tiles [i Ty / cuts, (i + 1) Ty / cuts)
+    int* inside;             // [n], zeroed by the host
+    uint32_t* row_flags;     // [m], zeroed by the host: bit 0 covered, bit 1 recalled
+};
+
+// the tiles of unit u: A rows from arow, B tiles [c0, c1) at rows bbase + 128 c
+struct PrdcUnit {
+    int arow, bbase, c0, c1;
+};
+template <int PASS>
+__device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
+    if constexpr (PASS == 0) {
+        if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
+        return {p.m + (u - p.Tx) * 128, p.m, 0, p.Ty};
+    } else {
+        const int tx = u / p.cuts, i = u - tx * p.cuts;
+        return {tx * 128, p.m, (int)((long long)i * p.Ty / p.cuts), (int)((long long)(i + 1) * p.Ty / p.cuts)};
+    }
+}
+
+// a[0..15] ascending, the live entries last: q < a[15] replaces the k-th value and moves down to its place (the dead
+// entries are -inf and never move, so the list keeps the k smallest values in a[16 - k .. 15])
+__device__ __forceinline__ void prdc_insert(float (&a)[kPrdcMaxK], float q) {
+    a[kPrdcMaxK - 1] = q;
+#pragma unroll
+    for (int s = kPrdcMaxK - 1; s > 0; --s) {
+        const float lo = fminf(a[s - 1], a[s]), hi = fmaxf(a[s - 1], a[s]);
+        a[s - 1] = lo;
+        a[s] = hi;
+    }
+}
+
+template <int PASS>
+__global__ void __launch_bounds__(kKadThreads, 1)
+prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
+    using namespace sm90;
+    static_assert(PASS == 0 || PASS == 1, "0: k-NN radii, 1: ball counts");
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
+    uint64_t* empty = full + kKadStages;
+
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const int ksteps = (p.d + 63) / 64;
+    const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
+    const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;
+
+    if (warp == 0 && lane == 0) {
+        tma_prefetch_desc(&map_hi);
+        tma_prefetch_desc(&map_lo);
+        for (int s = 0; s < kKadStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (warp < 4) {
+        // ------------------------------------------------------------ TMA producer
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int s = 0; uint32_t ph = 0;
+            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+                const PrdcUnit w = prdc_unit<PASS>(p, u);
+                for (int ct = w.c0; ct < w.c1; ++ct)
+                    kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, w.arow, w.bbase + ct * 128);
+            }
+        }
+        return;
+    }
+    // ---------------------------------------------------------------- consumers: wgmma + epilogue in registers
+    setmaxnreg_inc<kKadConsumerRegs>();
+    const int c = (warp >> 2) - 1;                        // tile rows [64 c, 64 c + 64)
+    const int lr0 = c * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
+    int s = 0; uint32_t ph = 0;
+    for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+        const PrdcUnit w = prdc_unit<PASS>(p, u);
+        const int row0 = w.arow + lr0;                    // rows of Z
+        const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
+        if constexpr (PASS == 0) {
+            const int set_n = w.bbase == 0 ? p.m : p.n;
+            const int ii0 = row0 - w.bbase;               // rows within the set
+            float a[2][kPrdcMaxK];
+#pragma unroll
+            for (int t = 0; t < kPrdcMaxK; ++t) {
+                a[0][t] = a[1][t] = t < kPrdcMaxK - p.k ? -INFINITY : INFINITY;
+            }
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                // element (row0 + 8 i, column jj0 + 8 j + e of the set) is sum[4 j + 2 i + e]
+                const int jj0 = ct * 128 + 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    // the Y part starts at row m, of any parity: two scalar loads, not a float2
+                    const float nc[2] = {__ldg(p.norm + w.bbase + jj0 + 8 * j), __ldg(p.norm + w.bbase + jj0 + 8 * j + 1)};
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int jj = jj0 + 8 * j + e;
+                            const float sn = nr[i] + nc[e];
+                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
+                            q = q > kQResolution * sn ? q : 0.f;     // also clamps q < 0
+                            if (jj < set_n && jj != ii0 + 8 * i && q < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], q);
+                        }
+                    }
+                }
+            }
+            // the 4 lanes of a quad hold the same two rows over disjoint columns: merge by a fixed xor tree (each lane
+            // takes a snapshot of its partner's list first, then inserts its live entries)
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    float b[kPrdcMaxK];
+#pragma unroll
+                    for (int t = 0; t < kPrdcMaxK; ++t) b[t] = __shfl_xor_sync(0xffffffffu, a[i][t], o);
+#pragma unroll
+                    for (int t = 0; t < kPrdcMaxK; ++t)
+                        if (b[t] >= 0.f && b[t] < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], b[t]);
+                }
+            }
+            if ((lane & 3) == 0) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (ii0 + 8 * i < set_n) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
+            }
+        } else {
+            // rows of X past m (the first rows of Y, or zero-filled) count nothing
+            const bool rv[2] = {row0 < p.m, row0 + 8 < p.m};
+            const float r2[2] = {rv[0] ? __ldg(p.radii + row0) : 0.f, rv[1] ? __ldg(p.radii + row0 + 8) : 0.f};
+            bool cov[2] = {false, false}, rec[2] = {false, false};
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                const int jj0 = ct * 128 + 2 * (lane & 3);    // rows of Y
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int jj = jj0 + 8 * j;
+                    const float nc[2] = {__ldg(p.norm + p.m + jj), __ldg(p.norm + p.m + jj + 1)};
+                    const float s2[2] = {jj < p.n ? __ldg(p.radii + p.m + jj) : 0.f,
+                                         jj + 1 < p.n ? __ldg(p.radii + p.m + jj + 1) : 0.f};
+                    uint32_t cj = 0;                          // column jj in bits 0-15, jj + 1 in bits 16-31
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float sn = nr[i] + nc[e];
+                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
+                            q = q > kQResolution * sn ? q : 0.f;
+                            // r2 = 0 past m and s2 = 0 past n: q < 0 is never true
+                            const bool in_r = q < r2[i] && jj + e < p.n;
+                            cov[i] |= in_r;
+                            rec[i] |= rv[i] && q < s2[e];
+                            cj += (uint32_t)in_r << (16 * e);
+                        }
+                    }
+                    // rarely taken: the 8 row groups of the warp hold the same columns, lanes l, l ^ 4, ..., l ^ 28 (at
+                    // most 16 rows per column, so the two 16-bit halves do not carry into each other)
+                    if (__any_sync(0xffffffffu, cj != 0)) {
+                        for (int o = 4; o < 32; o <<= 1) cj += __shfl_xor_sync(0xffffffffu, cj, o);
+                        if (lane < 4) {
+                            if (cj & 0xFFFFu) atomicAdd(p.inside + jj, (int)(cj & 0xFFFFu));
+                            if (cj >> 16) atomicAdd(p.inside + jj + 1, (int)(cj >> 16));
+                        }
+                    }
+                }
+            }
+            uint32_t bits[2] = {(uint32_t)cov[0] | ((uint32_t)rec[0] << 1), (uint32_t)cov[1] | ((uint32_t)rec[1] << 1)};
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                for (int o = 1; o < 4; o <<= 1) bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], o);
+                if ((lane & 3) == 0 && bits[i]) atomicOr(p.row_flags + row0 + 8 * i, bits[i]);
+            }
+        }
+    }
+}
+
+// flags[i] = row_flags[i] (bit 0 covered, bit 1 recalled)
+__global__ void prdc_flags_kernel(const uint32_t* __restrict__ row_flags, int m, unsigned char* __restrict__ flags) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < m) flags[i] = (unsigned char)row_flags[i];
+}
+
+}  // namespace fad

@@ -5,6 +5,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_frechet_distance     fad.py:51-120  -> Newton-Schulz GEMM chain on the PSD form (csrc/frechet.cuh)
     calc_kernel_audio_distance  (no reference counterpart) -> wgmma pair-tile kernels (csrc/kad.cuh)
     calc_kernel_audio_distance_songs                       -> the same, every song against one baseline in one pass
+    calc_prdc                   (no reference counterpart) -> k-NN radii and ball-count tile kernels (csrc/prdc.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -83,13 +84,23 @@ class KADResults(NamedTuple):
     n_eval: int
 
 
-def _kad_rows(a, what: str):
+class PRDCResults(NamedTuple):
+    precision: float
+    recall: float
+    density: float
+    coverage: float
+    k: int
+    n_baseline: int
+    n_eval: int
+
+
+def _kad_rows(a, what: str, metric: str = "KAD"):
     """fp16 [rows, d] numpy array or torch tensor -> contiguous fp16 torch tensor (not moved to a device yet)."""
     t = a if isinstance(a, torch.Tensor) else torch.from_numpy(np.asarray(a))
     if t.dtype != torch.float16:
-        raise ValueError(f"KAD needs fp16 embeddings (the cached values); the {what} set is {t.dtype}")
+        raise ValueError(f"{metric} needs fp16 embeddings (the cached values); the {what} set is {t.dtype}")
     if t.ndim != 2:
-        raise ValueError(f"KAD needs [rows, d] embeddings; the {what} set has shape {tuple(t.shape)}")
+        raise ValueError(f"{metric} needs [rows, d] embeddings; the {what} set has shape {tuple(t.shape)}")
     return t
 
 
@@ -217,15 +228,52 @@ def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray, distributed: bool =
     return out
 
 
-def kad_embedding_dir(path, model_name: str) -> Path:
-    """The embedding cache directory <path>/embeddings/<model> that KAD reads; ValueError for statistics files, named
-    statistics sets and anything else that is not a directory (they hold (mu, C), not embeddings)."""
+def calc_prdc(emb_baseline, emb_eval, k: int = 5) -> PRDCResults:
+    """Precision and recall (Kynkaanniemi et al., 2019), density and coverage (Naeem et al., 2020) of an eval set
+    Y [n, d] against a baseline X [m, d], both fp16 with the values taken as exact reals, q(a, b) = |a - b|^2:
+
+        r_i = distance from x_i to its k-th nearest other row of X (the self pair excluded by index, so duplicate
+              rows are neighbours at distance 0); s_j the same for y_j within Y,
+        precision = (1/n) #{j : exists i, q(x_i, y_j) < r_i^2}
+        recall    = (1/m) #{i : exists j, q(x_i, y_j) < s_j^2}
+        density   = 1/(k n) sum_j #{i : q(x_i, y_j) < r_i^2}
+        coverage  = (1/m) #{i : exists j, q(x_i, y_j) < r_i^2}
+
+    All comparisons are strict, so a row with r_i = 0 (at least k exact duplicates, e.g. silent clips) contains
+    nothing.  The radii and the ball counts run on the GPU (fad_knn_radii_sq, fad_prdc_counts) without forming a
+    distance matrix; the four values are assembled from integer counts.  A width that is not a multiple of 8 is
+    zero-padded, which changes no distance.  Raises ValueError for k outside [1, 16], m <= k or n <= k, non-fp16 or
+    non-2-D input and mismatched widths."""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 16:
+        raise ValueError(f"PRDC needs an integer k in [1, 16], not {k!r}")
+    k = int(k)
+    x, y = _kad_rows(emb_baseline, "baseline", "PRDC"), _kad_rows(emb_eval, "eval", "PRDC")
+    m, n = int(x.shape[0]), int(y.shape[0])
+    if m <= k or n <= k:
+        raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {m}, eval {n})")
+    if x.shape[1] != y.shape[1]:
+        raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
+    from . import _native
+    eng = _native.engine()
+    z = _kad_device_rows(torch.cat([x, y]), eng)
+    radii_sq = eng.knn_radii_sq(z, m, k)
+    inside, flags = (t.cpu().numpy() for t in eng.prdc_counts(z, m, radii_sq))
+    return PRDCResults(precision=float(np.count_nonzero(inside)) / n,
+                       recall=float(np.count_nonzero(flags & 2)) / m,
+                       density=float(inside.sum(dtype=np.int64)) / (k * n),
+                       coverage=float(np.count_nonzero(flags & 1)) / m,
+                       k=k, n_baseline=m, n_eval=n)
+
+
+def kad_embedding_dir(path, model_name: str, metric: str = "KAD") -> Path:
+    """The embedding cache directory <path>/embeddings/<model> that KAD (and PRDC) reads; ValueError for statistics
+    files, named statistics sets and anything else that is not a directory (they hold (mu, C), not embeddings)."""
     named = isinstance(path, str) and _named_statistics(path) is not None
     if named or str(path).endswith(".npz") or Path(path).is_file():
-        raise ValueError(f"KAD needs embeddings, not (mu, C) statistics: '{path}' is a statistics file or set; "
+        raise ValueError(f"{metric} needs embeddings, not (mu, C) statistics: '{path}' is a statistics file or set; "
                          "pass the audio directory instead")
     if not Path(path).is_dir():
-        raise ValueError(f"KAD needs a directory of audio or embeddings; '{path}' is not a directory")
+        raise ValueError(f"{metric} needs a directory of audio or embeddings; '{path}' is not a directory")
     return Path(path) / "embeddings" / model_name
 
 
@@ -548,6 +596,22 @@ class FrechetAudioDistance:
                 raise ValueError(f"KAD needs fp16 embedding caches; {p} holds {emb.dtype}")
             sets.append(emb)
         return calc_kernel_audio_distance(*sets, distributed=distributed)
+
+    def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5) -> PRDCResults:
+        """Precision, recall, density and coverage (calc_prdc) of the cached embeddings of eval_dir against those of
+        baseline_dir, read as score_kad reads them: all rows of all <dir>/embeddings/<model>/*.npy in sorted file
+        order.  Statistics files and names are refused."""
+        from . import _io_native
+        sets = []
+        for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
+            files = _sorted_npy_files(kad_embedding_dir(p, self.ml.name, "PRDC"))
+            if not files:
+                raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
+            emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
+            if emb.dtype != np.float16:
+                raise ValueError(f"PRDC needs fp16 embedding caches; {p} holds {emb.dtype}")
+            sets.append(emb)
+        return calc_prdc(*sets, k=k)
 
     def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
                              distributed: bool = False) -> Path:

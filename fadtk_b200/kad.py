@@ -28,21 +28,22 @@ _KAD_ARGS = (
 )
 
 
-def _check_csv(csv_path: str) -> None:
+def _check_csv(csv_path: str, header: str = CSV_HEADER, metric: str = "KAD") -> None:
+    """ValueError when csv_path exists with a first line other than header (shared with fadtk_b200.prdc)"""
     out = Path(csv_path)
     if out.is_file():
         with open(out) as f:
             head = f.readline()
-        if head and head != CSV_HEADER:
-            raise ValueError(f"{csv_path} has the header {head.strip()!r}, not {CSV_HEADER.strip()!r}: "
-                             "choose another file for KAD results")
+        if head and head != header:
+            raise ValueError(f"{csv_path} has the header {head.strip()!r}, not {header.strip()!r}: "
+                             f"choose another file for {metric} results")
 
 
-def _append_row(csv_path: str, row) -> None:
+def _append_row(csv_path: str, row, header: str = CSV_HEADER) -> None:
     out = Path(csv_path)
     out.parent.mkdir(parents=True, exist_ok=True)
     if not out.is_file() or out.stat().st_size == 0:
-        out.write_text(CSV_HEADER)
+        out.write_text(header)
     with open(out, "a") as f:
         f.write(",".join(str(v) for v in row) + "\n")
 

@@ -322,6 +322,23 @@ int fad_kad_song_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_
                               void* stream);
 int fad_kad_shard_plan(const long long* unit_tiles, long long units, int shards, long long* bounds);
 
+/* ---- Precision, recall, density and coverage (PRDC; Kynkaanniemi et al. 2019, Naeem et al. 2020) of an eval set
+ * Y [n, d] against a baseline X [m, d] (DESIGN.md section 5.12).  z = [X; Y] (fp16 [m + n, d], X first, 16-byte
+ * aligned), d a multiple of 8, q(a, b) = |a - b|^2 computed as for KAD (same shift, split and fp32 q).  Every argument
+ * is checked first (null or misaligned pointers, 1 <= k <= 16, m > k and n > k, d, at most 2^30 rows); a rejected call
+ * launches nothing and writes nothing.  Both outputs are bitwise reproducible (selected fp32 values, integer counts).
+ *   fad_knn_radii_sq  radii_sq (device fp32 [m + n]) = for each row of X, the k-th smallest q to the other rows of X
+ *                     (the self pair excluded by index: duplicates are neighbours at 0); then the same for each row of
+ *                     Y within Y.  The exact k-th smallest of the fp32 q values the kernel computes.
+ *   fad_prdc_counts   radii_sq (device fp32 [m + n], r_i^2 then s_j^2, e.g. from the call above; m, n >= 2) ->
+ *                     inside (device int32 [n]) = #{i : q(x_i, y_j) < r_i^2}; flags (device uint8 [m]) = bit 0 when
+ *                     some q(x_i, y_j) < r_i^2 (covered), bit 1 when some q(x_i, y_j) < s_j^2 (recalled).  Each xy pair's
+ *                     q is computed once. */
+int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* radii_sq,
+                     void* stream);
+int fad_prdc_counts(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* radii_sq, int* inside,
+                    unsigned char* flags, void* stream);
+
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
  * sinc_interp_kaiser, beta=14.769656459379492) (:151-158), PCM16 quantisation (:160).
