@@ -65,6 +65,10 @@ SIGNATURES = {
     "fad_whisper_load": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int]),
     "fad_whisper_forward": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_whisper_logmel": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp]),
+    "fad_whisper_conv": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_ll, c_vp, c_vp]),
+    "fad_whisper_enc_layer": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, c_vp, c_vp]),
+    "fad_whisper_encode": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp]),
+    "fad_whisper_dec_layer": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_w2v_load": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int]),
     "fad_w2v_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_w2v_normalize": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
@@ -438,6 +442,36 @@ class Engine:
         raw = buf[: n * 3000 * 80].view(n, 3000, 80)
         mx = buf[n * 3000 * 80:].view(n, 1, 1)
         return (torch.maximum(raw, mx - 8.0) + 4.0) / 4.0
+
+    # Stage entries of the loaded Whisper model: they write into the caller's cuda tensors (shapes in
+    # include/fadtk_b200.h) and raise NativeError on rejected arguments.
+    def whisper_logmel(self, pcm, clip_start, clip_len, n_clips: int, out):
+        """fad_whisper_logmel: out fp32 [n_clips * 3000 * 80 + n_clips], the raw log10 mel then the per-clip maxima"""
+        _check(lib().fad_whisper_logmel(self._h, _ptr(pcm), _ptr(clip_start), _ptr(clip_len), int(n_clips), _ptr(out),
+                                        _stream()))
+        return out
+
+    def whisper_conv(self, c: int, x, clip_max, B: int, out):
+        """fad_whisper_conv: c = 0 raw log10 mel fp32 [B, 3000, 80] + clip_max fp32 [B] -> out fp16 [B, 3000, d];
+        c = 1 fp16 [B, 3000, d] -> out fp32 [B, 1500, d]"""
+        _check(lib().fad_whisper_conv(self._h, int(c), _ptr(x), _ptr(clip_max), int(B), _ptr(out), _stream()))
+        return out
+
+    def whisper_enc_layer(self, l: int, x, B: int, out):
+        """fad_whisper_enc_layer: encoder layer l, x fp32 [B, 1500, d] -> out fp32 [B, 1500, d]"""
+        _check(lib().fad_whisper_enc_layer(self._h, int(l), _ptr(x), int(B), _ptr(out), _stream()))
+        return out
+
+    def whisper_encode(self, pcm, clip_start, clip_len, n_clips: int, out):
+        """fad_whisper_encode: the encoder with its final LayerNorm -> out fp16 [n_clips, 1500, d]"""
+        _check(lib().fad_whisper_encode(self._h, _ptr(pcm), _ptr(clip_start), _ptr(clip_len), int(n_clips), _ptr(out),
+                                        _stream()))
+        return out
+
+    def whisper_dec_layer(self, l: int, xd, enc_out, B: int, out):
+        """fad_whisper_dec_layer: decoder layer l, xd fp32 [B, 2, d], enc_out fp16 [B, 1500, d] -> out fp32 [B, 2, d]"""
+        _check(lib().fad_whisper_dec_layer(self._h, int(l), _ptr(xd), _ptr(enc_out), int(B), _ptr(out), _stream()))
+        return out
 
     # ------------------------------------------------------- wav2vec 2.0 / HuBERT / MERT
     def w2v_load(self, cfg: tuple, tensors: list, max_clips: int = 8, max_len: int = 16000 * 30):

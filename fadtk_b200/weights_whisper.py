@@ -23,53 +23,63 @@ N_MEL, SEQ, MAX_TARGET = 80, 1500, 448
 SYNTH_VOCAB, SYNTH_START = 64, 1          # synthetic checkpoints: tiny vocabulary, start token 1
 
 
-def synthetic_whisper_state(seed: int = 0, size: str = "small") -> dict:
+def synthetic_whisper_tensors(seed: int = 0, size: str = "small", layers: tuple | None = None):
+    """Yields the (key, tensor) pairs of ``synthetic_whisper_state`` one at a time, in generation order."""
     d, heads, n_enc, n_dec = SIZES[size]
+    if layers is not None:
+        n_enc, n_dec = (int(n) for n in layers)
+        if n_enc < 1 or n_dec < 1:
+            raise ValueError("layers must be (encoder layers >= 1, decoder layers >= 1)")
     f = 4 * d
     g = torch.Generator().manual_seed(seed)
-    sd = {}
 
     def lin(key, out_f, in_f, bias=True):
-        sd[key + ".weight"] = torch.randn((out_f, in_f), generator=g) * (1.0 / math.sqrt(in_f))
+        yield key + ".weight", torch.randn((out_f, in_f), generator=g) * (1.0 / math.sqrt(in_f))
         if bias:
-            sd[key + ".bias"] = torch.randn((out_f,), generator=g) * 0.02
+            yield key + ".bias", torch.randn((out_f,), generator=g) * 0.02
 
     def ln(key, n):
-        sd[key + ".weight"] = 1.0 + 0.1 * torch.randn((n,), generator=g)
-        sd[key + ".bias"] = 0.05 * torch.randn((n,), generator=g)
+        yield key + ".weight", 1.0 + 0.1 * torch.randn((n,), generator=g)
+        yield key + ".bias", 0.05 * torch.randn((n,), generator=g)
 
     def attn(p):
-        lin(p + "k_proj", d, d, bias=False)
-        lin(p + "v_proj", d, d)
-        lin(p + "q_proj", d, d)
-        lin(p + "out_proj", d, d)
+        yield from lin(p + "k_proj", d, d, bias=False)
+        yield from lin(p + "v_proj", d, d)
+        yield from lin(p + "q_proj", d, d)
+        yield from lin(p + "out_proj", d, d)
 
-    sd["encoder.conv1.weight"] = torch.randn((d, N_MEL, 3), generator=g) * (1.0 / math.sqrt(3 * N_MEL))
-    sd["encoder.conv1.bias"] = torch.randn((d,), generator=g) * 0.02
-    sd["encoder.conv2.weight"] = torch.randn((d, d, 3), generator=g) * (1.0 / math.sqrt(3 * d))
-    sd["encoder.conv2.bias"] = torch.randn((d,), generator=g) * 0.02
-    sd["encoder.embed_positions.weight"] = 0.1 * torch.randn((SEQ, d), generator=g)
+    yield "encoder.conv1.weight", torch.randn((d, N_MEL, 3), generator=g) * (1.0 / math.sqrt(3 * N_MEL))
+    yield "encoder.conv1.bias", torch.randn((d,), generator=g) * 0.02
+    yield "encoder.conv2.weight", torch.randn((d, d, 3), generator=g) * (1.0 / math.sqrt(3 * d))
+    yield "encoder.conv2.bias", torch.randn((d,), generator=g) * 0.02
+    yield "encoder.embed_positions.weight", 0.1 * torch.randn((SEQ, d), generator=g)
     for i in range(n_enc):
         p = f"encoder.layers.{i}."
-        attn(p + "self_attn.")
-        ln(p + "self_attn_layer_norm", d)
-        lin(p + "fc1", f, d)
-        lin(p + "fc2", d, f)
-        ln(p + "final_layer_norm", d)
-    ln("encoder.layer_norm", d)
-    sd["decoder.embed_tokens.weight"] = 0.5 * torch.randn((SYNTH_VOCAB, d), generator=g)
-    sd["decoder.embed_positions.weight"] = 0.1 * torch.randn((MAX_TARGET, d), generator=g)
+        yield from attn(p + "self_attn.")
+        yield from ln(p + "self_attn_layer_norm", d)
+        yield from lin(p + "fc1", f, d)
+        yield from lin(p + "fc2", d, f)
+        yield from ln(p + "final_layer_norm", d)
+    yield from ln("encoder.layer_norm", d)
+    yield "decoder.embed_tokens.weight", 0.5 * torch.randn((SYNTH_VOCAB, d), generator=g)
+    yield "decoder.embed_positions.weight", 0.1 * torch.randn((MAX_TARGET, d), generator=g)
     for i in range(n_dec):
         p = f"decoder.layers.{i}."
-        attn(p + "self_attn.")
-        ln(p + "self_attn_layer_norm", d)
-        attn(p + "encoder_attn.")
-        ln(p + "encoder_attn_layer_norm", d)
-        lin(p + "fc1", f, d)
-        lin(p + "fc2", d, f)
-        ln(p + "final_layer_norm", d)
-    ln("decoder.layer_norm", d)
-    return sd
+        yield from attn(p + "self_attn.")
+        yield from ln(p + "self_attn_layer_norm", d)
+        yield from attn(p + "encoder_attn.")
+        yield from ln(p + "encoder_attn_layer_norm", d)
+        yield from lin(p + "fc1", f, d)
+        yield from lin(p + "fc2", d, f)
+        yield from ln(p + "final_layer_norm", d)
+    yield from ln("decoder.layer_norm", d)
+
+
+def synthetic_whisper_state(seed: int = 0, size: str = "small", layers: tuple | None = None) -> dict:
+    """Seeded parameters of whisper-``size``.  ``layers = (n_enc, n_dec)`` generates a shortened stack of that many
+    encoder and decoder layers (same widths, its own draws after the first n_enc encoder layers); without it the
+    state has the real depth."""
+    return dict(synthetic_whisper_tensors(seed, size, layers))
 
 
 def load_whisper_state(path=None, seed: int = 0, size: str = "small"):

@@ -153,6 +153,23 @@ int fad_whisper_forward(fad_handle* h, const int16_t* pcm, const long long* clip
  * the features are (max(x, max - 8) + 4) / 4. */
 int fad_whisper_logmel(fad_handle* h, const int16_t* pcm, const long long* clip_start, const int* clip_len,
                        long long n_clips, float* out, void* stream);
+/* Stage entries of the loaded Whisper model (parity tests), each calling the launch code of fad_whisper_forward and
+ * failing, before launching or writing anything, on arguments it could not honour.  B in [1, max_clips]; 16-byte
+ * aligned device pointers.
+ * fad_whisper_conv: conv c of the stem.  c = 0: x fp32 [B][3000][80] raw log10 mel (as fad_whisper_logmel returns it)
+ * and clip_max fp32 [B] -> floor, (x + 4) / 4, conv1 + GELU -> out fp16 [B][3000][d];  c = 1: x fp16 [B][3000][d]
+ * (conv 0's output; clip_max unused) -> out fp32 [B][1500][d] = embed_positions + GELU(conv2(x)).
+ * fad_whisper_enc_layer: encoder layer l in [0, enc_layers), x fp32 [B][1500][d] -> out fp32 [B][1500][d].
+ * fad_whisper_encode: the whole encoder including encoder.layer_norm for n_clips >= 1 clips (any count, run in chunks of
+ * max_clips) -> out fp16 [n_clips][1500][d], the encoder output the decoder reads.
+ * fad_whisper_dec_layer: decoder layer l in [0, dec_layers), xd fp32 [B][2][d] and enc_out fp16 [B][1500][d] ->
+ * out fp32 [B][2][d]. */
+int fad_whisper_conv(fad_handle* h, int c, const void* x, const float* clip_max, long long B, void* out, void* stream);
+int fad_whisper_enc_layer(fad_handle* h, int l, const float* x, long long B, float* out, void* stream);
+int fad_whisper_encode(fad_handle* h, const int16_t* pcm, const long long* clip_start, const int* clip_len,
+                       long long n_clips, void* out_f16, void* stream);
+int fad_whisper_dec_layer(fad_handle* h, int l, const float* xd, const void* enc_out_f16, long long B, float* out,
+                          void* stream);
 
 /* ---- Encodec: replaces EncodecEmbModel.load_model / _get_frame for the 24 kHz variant
  * (fadtk/model_loader.py:123-130, 155-166): EncodecModel.encodec_model_24khz().encoder(audio) -> [T/320, 128].
