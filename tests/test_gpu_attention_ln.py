@@ -28,12 +28,12 @@ import torch
 
 from fadtk_b200 import _native
 from fadtk_b200 import weights_clap
+from gpu_checks import Guarded, check_bound, expect_rejected
 from oracle import clap_oracle as co
 
 pytestmark = pytest.mark.gpu
 
 GUARD = 256
-SENTINEL = {torch.float16: (torch.int16, 0x7E5A), torch.float32: (torch.int32, 0x7FC0FFEE)}   # NaN bit patterns
 U = 2.0 ** -24
 
 # rms relative error (rms |kernel - fp64| / rms |fp64|), about 3x the largest level measured per kernel on an H100 80GB
@@ -43,28 +43,6 @@ U = 2.0 ** -24
 # The largest max |err| / bound measured: window 0.81, biased 0.55, decoder 0.47, cross 0.30, gate 0.18, LayerNorm fp32
 # 0.24, LayerNorm fp16 0.997 (its half-ulp rounding term is attained; the kernel is deterministic, so this is stable).
 RMS_CEIL = {"window": 8e-4, "bias": 6.5e-4, "dec_self": 4.5e-4, "cross": 6.5e-4, "gate": 3e-7, "ln32": 5e-5, "ln16": 6.5e-4}
-
-
-class Guarded:
-    """An output tensor of `shape` inside a sentinel-filled buffer with guard regions on both sides."""
-
-    def __init__(self, shape, dtype, dev):
-        self.n = math.prod(shape)
-        self.idt, self.bits = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + self.n + GUARD, dtype=dtype, device=dev)
-        self.buf.view(self.idt).fill_(self.bits)
-        self.body = self.buf[GUARD:GUARD + self.n].view(shape)
-
-    def check(self):
-        torch.cuda.synchronize()
-        raw = self.buf.view(self.idt)
-        assert bool((raw[:GUARD] == self.bits).all()) and bool((raw[GUARD + self.n:] == self.bits).all()), \
-            "guard region overwritten"
-        assert not bool((self.body.view(self.idt) == self.bits).any()), "output elements left unwritten"
-        return self.body
-
-    def untouched(self):
-        return bool((self.buf.view(self.idt) == self.bits).all())
 
 
 @pytest.fixture(scope="module")
@@ -80,21 +58,10 @@ def _same(a, b):
     return torch.equal(a.view(torch.int16) if a.dtype == torch.float16 else a, b.view(torch.int16) if b.dtype == torch.float16 else b)
 
 
-def _rms_rel(got, ref):
-    return ((got.double() - ref).square().mean().sqrt() / ref.square().mean().sqrt()).item()
-
-
-def _check(got, ref, bound, kind, what, capsys=None):
-    err = (got.double() - ref).abs()
-    ratio = (err / bound).max().item()
-    worst = int((err / bound).flatten().argmax())
-    assert ratio <= 1.0, (f"{what}: max |err| / bound = {ratio:.3g} at flat index {worst} "
-                          f"(got {got.flatten()[worst].item()!r}, want {ref.flatten()[worst].item()!r})")
-    rms = _rms_rel(got, ref)
-    if capsys is not None:
-        with capsys.disabled():
-            print(f"\n[{kind}] {what}: rms rel err {rms:.3e}, max err / bound {ratio:.3f}")
-    assert rms <= RMS_CEIL[kind], f"{what}: rms relative error {rms:.3g} above {RMS_CEIL[kind]:.3g}"
+def _check(got, ref, bound, kind, what, capsys):
+    rms, ratio = check_bound(kind, what, got, ref, bound, {}, RMS_CEIL)
+    with capsys.disabled():
+        print(f"\n[{kind}] {what}: rms rel err {rms:.3e}, max err / bound {ratio:.3f}")
 
 
 def attention_reference(q, k, v, bias, scale, acc):
@@ -152,7 +119,7 @@ def window_reference(qkv, relbias, C, heads, res, shift):
 
 
 def run_window(engine, qkv, C, heads, relbias, res, shift):
-    out = Guarded((qkv.shape[0], C), torch.float16, qkv.device)
+    out = Guarded((qkv.shape[0], C), torch.float16, qkv.device, GUARD)
     engine.window_attention(qkv, qkv.shape[0] // 64, C, heads, relbias, res, shift, out.body)
     return out.check()
 
@@ -213,15 +180,15 @@ def test_wavlm_gate_matches_fp64(engine, dev, rows, heads, capsys):
     w = torch.randn((8, 64), generator=g, device=dev) * 0.3
     b = torch.randn((8,), generator=g, device=dev)
     c = 1.0 + torch.randn((heads,), generator=g, device=dev)
-    out = Guarded((rows, heads), torch.float32, dev)
+    out = Guarded((rows, heads), torch.float32, dev, GUARD)
     engine.wavlm_gate(x, w, b, c, rows, heads, d, out.body)
     got = out.check()
     ref, bound = gate_reference(x, w, b, c, heads)
     _check(got, ref, bound, "gate", f"rows {rows} heads {heads}", capsys)
-    again = Guarded((rows, heads), torch.float32, dev)
+    again = Guarded((rows, heads), torch.float32, dev, GUARD)
     engine.wavlm_gate(x, w, b, c, rows, heads, d, again.body)
     assert torch.equal(again.check(), got)
-    part = Guarded((101, heads), torch.float32, dev)
+    part = Guarded((101, heads), torch.float32, dev, GUARD)
     engine.wavlm_gate(x[rows - 101:].contiguous(), w, b, c, 101, heads, d, part.body)
     assert torch.equal(part.check(), got[rows - 101:])
 
@@ -251,7 +218,7 @@ def bias_reference(qkv, relb, gate, n_clips, S, d):
 
 
 def run_bias(engine, qkv, n_clips, S, d, relb, gate):
-    out = Guarded((n_clips * S, d), torch.float16, qkv.device)
+    out = Guarded((n_clips * S, d), torch.float16, qkv.device, GUARD)
     engine.attention_bias(qkv, n_clips, S, d, relb, gate, out.body)
     return out.check()
 
@@ -293,7 +260,7 @@ def test_decoder_self_attention_matches_fp64(engine, dev, d, n_clips, capsys):
     leaves (clip, head) units that do not fill the last 4-warp block."""
     heads = d // 64
     qkv = _dec_qkv(dev, d + n_clips, 2 * n_clips, d).reshape(2 * n_clips, 3 * d).half().contiguous()
-    out = Guarded((2 * n_clips, d), torch.float16, dev)
+    out = Guarded((2 * n_clips, d), torch.float16, dev, GUARD)
     engine.decoder_self_attention(qkv, n_clips, d, out.body)
     got = out.check()
     assert _same(got[0::2], qkv[0::2, 2 * d:].contiguous()), "token 0 is not v0"
@@ -302,10 +269,10 @@ def test_decoder_self_attention_matches_fp64(engine, dev, d, n_clips, capsys):
     ref, bound = attention_reference(t[0], t[1], t[2], causal, 0.125, 8 * U)
     ref, bound = (z.permute(0, 2, 1, 3).reshape(2 * n_clips, d) for z in (ref, bound))
     _check(got, ref, bound + 2.0 ** -25, "dec_self", f"d {d} clips {n_clips}", capsys)
-    again = Guarded((2 * n_clips, d), torch.float16, dev)
+    again = Guarded((2 * n_clips, d), torch.float16, dev, GUARD)
     engine.decoder_self_attention(qkv, n_clips, d, again.body)
     assert _same(again.check(), got)
-    one = Guarded((2, d), torch.float16, dev)
+    one = Guarded((2, d), torch.float16, dev, GUARD)
     engine.decoder_self_attention(qkv[-2:].contiguous(), 1, d, one.body)
     assert _same(one.check(), got[-2:]), "a clip's output depends on its batch position"
 
@@ -322,7 +289,7 @@ def test_cross_attention_matches_fp64(engine, dev, d, S, capsys):
     sig2 = torch.tensor([0.3, 1.0, 3.0, 10.0], device=dev)[torch.arange(heads, device=dev) % 4]
     q = (torch.randn((n_clips * 2, heads, 64), generator=qg, device=dev) * sig2.sqrt()[None, :, None]).reshape(n_clips * 2, d)
     q = q.half().contiguous()
-    out = Guarded((n_clips * 2, d), torch.float16, dev)
+    out = Guarded((n_clips * 2, d), torch.float16, dev, GUARD)
     engine.cross_attention(q, kv, n_clips, S, d, out.body)
     got = out.check()
     qq = q.double().view(n_clips, 2, heads, 64).permute(0, 2, 1, 3)
@@ -331,10 +298,10 @@ def test_cross_attention_matches_fp64(engine, dev, d, S, capsys):
     ref, bound = attention_reference(qq, kk[0], kk[1], zero, 0.125, (S + 4) * U)
     ref, bound = (z.permute(0, 2, 1, 3).reshape(n_clips * 2, d) for z in (ref, bound))
     _check(got, ref, bound, "cross", f"d {d} S {S}", capsys)
-    again = Guarded((n_clips * 2, d), torch.float16, dev)
+    again = Guarded((n_clips * 2, d), torch.float16, dev, GUARD)
     engine.cross_attention(q, kv, n_clips, S, d, again.body)
     assert _same(again.check(), got)
-    one = Guarded((2, d), torch.float16, dev)
+    one = Guarded((2, d), torch.float16, dev, GUARD)
     engine.cross_attention(q[2:4].contiguous(), kv[S:2 * S].contiguous(), 1, S, d, one.body)
     assert _same(one.check(), got[2:4]), "a clip's output depends on its batch position"
 
@@ -391,8 +358,8 @@ def ln_reference(xr, gamma, beta, gelu, width):
 
 def run_ln(engine, x, gamma, beta, rows, C, ld_out, res=0, shift=0, mode=0, gelu=False, want32=True, alias=False):
     width = 4 * C if mode else C
-    o16 = Guarded((rows, ld_out), torch.float16, x.device)
-    o32 = Guarded((rows, width), torch.float32, x.device) if want32 and not alias else None
+    o16 = Guarded((rows, ld_out), torch.float16, x.device, GUARD)
+    o32 = Guarded((rows, width), torch.float32, x.device, GUARD) if want32 and not alias else None
     engine.layernorm(x, gamma, beta, rows, C, ld_out, o16.body, x if alias else (o32.body if o32 else None),
                      res=res, shift=shift, mode=mode, gelu=gelu)
     out16 = o16.check()
@@ -482,12 +449,13 @@ def test_layernorm_patch_merge_gather(engine, dev, res, C, capsys):
 
 # ------------------------------------------------------------------------------------------------------- rejections
 def _window_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
+        dev = engine.torch_device
         a = dict(n_windows=4, C=96, heads=4, res=16, shift=0, offset=0)
         a.update(over)
         qkv = torch.zeros((8 * 64, 3 * 128), dtype=torch.float16, device=dev)
         relbias = torch.zeros((32, 64, 64), device=dev)
-        o = Guarded((8 * 64, 128), torch.float16, dev)
+        o = Guarded((8 * 64, 128), torch.float16, dev, GUARD)
         outs.append(o)
         engine.window_attention(qkv, a["n_windows"], a["C"], a["heads"], relbias, a["res"], a["shift"],
                                 o.buf[GUARD + a["offset"]:])
@@ -495,62 +463,67 @@ def _window_call(**over):
 
 
 def _bias_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
+        dev = engine.torch_device
         a = dict(n_clips=2, S=65, d=768)
         a.update(over)
         qkv = torch.zeros((2 * 65, 3 * 768), dtype=torch.float16, device=dev)
-        o = Guarded((2 * 65, 768), torch.float16, dev)
+        o = Guarded((2 * 65, 768), torch.float16, dev, GUARD)
         outs.append(o)
         engine.attention_bias(qkv, a["n_clips"], a["S"], a["d"], torch.zeros((12, 129), device=dev),
-                              torch.zeros((130, 12), device=dev), o.buf[GUARD:])
+                              torch.zeros((130, 12), device=dev), o.body)
     return call
 
 
 def _gate_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
+        dev = engine.torch_device
         a = dict(rows=10, heads=12, d=768)
         a.update(over)
-        o = Guarded((10, 12), torch.float32, dev)
+        o = Guarded((10, 12), torch.float32, dev, GUARD)
         outs.append(o)
         engine.wavlm_gate(torch.zeros((10, 768), device=dev), torch.zeros((8, 64), device=dev), torch.zeros(8, device=dev),
-                          torch.ones(12, device=dev), a["rows"], a["heads"], a["d"], o.buf[GUARD:])
+                          torch.ones(12, device=dev), a["rows"], a["heads"], a["d"], o.body)
     return call
 
 
-def _bias_table_s0(engine, dev, outs):
+def _bias_table_s0(engine, outs):
     _native.Engine.wavlm_bias_table(np.zeros((320, 12), np.float32), 0)
 
 
 def _dec_call(d):
-    def call(engine, dev, outs):
-        o = Guarded((4, 1024), torch.float16, dev)
+    def call(engine, outs):
+        dev = engine.torch_device
+        o = Guarded((4, 1024), torch.float16, dev, GUARD)
         outs.append(o)
-        engine.decoder_self_attention(torch.zeros((4, 3 * 1024), dtype=torch.float16, device=dev), 2, d, o.buf[GUARD:])
+        engine.decoder_self_attention(torch.zeros((4, 3 * 1024), dtype=torch.float16, device=dev), 2, d, o.body)
     return call
 
 
 def _cross_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
+        dev = engine.torch_device
         a = dict(n_clips=2, S=100, d=384)
         a.update(over)
-        o = Guarded((4, 384), torch.float16, dev)
+        o = Guarded((4, 384), torch.float16, dev, GUARD)
         outs.append(o)
         kv = torch.zeros((2 * 8000, 2 * 384), dtype=torch.float16, device=dev)
         engine.cross_attention(torch.zeros((4, 384), dtype=torch.float16, device=dev), kv, a["n_clips"], a["S"], a["d"],
-                               o.buf[GUARD:])
+                               o.body)
     return call
 
 
 def _ln_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
+        dev = engine.torch_device
         a = dict(rows=512, C=128, ld_out=128, res=16, shift=0, mode=0, out32="own", offset=0, gamma=True)
         a.update(over)
         x = torch.zeros((2048, 512), device=dev)
         gamma = torch.ones(2048, device=dev)
-        o16 = Guarded((2048, 512), torch.float16, dev)
-        o32 = Guarded((2048, 512), torch.float32, dev)
+        o16 = Guarded((2048, 512), torch.float16, dev, GUARD)
+        o32 = Guarded((2048, 512), torch.float32, dev, GUARD)
         outs += [o16, o32]
-        out32 = {"own": o32.buf[GUARD:], "x": x, "none": None}[a["out32"]]
+        out32 = {"own": o32.body, "x": x, "none": None}[a["out32"]]
         engine.layernorm(x, gamma if a["gamma"] else None, gamma, a["rows"], a["C"], a["ld_out"], o16.buf[GUARD + a["offset"]:],
                          out32, res=a["res"], shift=a["shift"], mode=a["mode"])
     return call
@@ -595,13 +568,6 @@ REJECT = [
 
 
 @pytest.mark.parametrize("call,message", [c[1:] for c in REJECT], ids=[c[0] for c in REJECT])
-def test_stage_entries_reject_invalid_arguments(engine, dev, call, message):
+def test_stage_entries_reject_invalid_arguments(engine, call, message):
     """Arguments the launch cannot honour fail with their message, launch nothing and write nothing."""
-    outs = []
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
-        call(engine, dev, outs)
-    torch.cuda.synchronize()
-    assert str(exc.value) == message
-    assert engine.launches == launches, "a rejected call launched a kernel"
-    assert all(o.untouched() for o in outs), "a rejected call wrote output"
+    expect_rejected(engine, call, message, [])

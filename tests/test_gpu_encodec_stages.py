@@ -8,36 +8,26 @@ Inputs live inside NaN-filled guard regions of at least (max padding + 2) time s
 clips of a batch differ: a tap read outside its clip shows up as NaN or as a wrong value in the output.  Outputs live
 inside sentinel-filled buffers: every element must be written and no guard touched.
 
-Conv bound, per output element y = b + sum_j w_j a_j over the K = k' Cin taps of the GEMM row (k' = k, or
-k + (P - 1) stride when P time steps share a row), a_j = ELU(x) or x at the padded index:
-  * a_j is rounded to fp16 for the GEMM:                2^-11 |a_j| (+ 2^-25 when it is fp16-subnormal)
-  * w_j is the fp16 hi/lo pair of the fp32 weight:      2^-21 |w_j| (+ 2^-25 for a subnormal lo part)
-  * fp32 accumulation of K products and the bias:       K 2^-23 sum_j |w_j a_j| + 2^-24 (|b| + |y|)
-so |got - ref| <= (2^-11 + 2^-21 + K 2^-23) S + 2^-25 (sum_j |w_j| + sum_j |a_j|) + 2^-24 (|b| + |y|), S = sum_j |w_j||a_j|,
-computed in float64 by the same padded conv on |a| and |w|.  One wrong tap moves an output by |w_j a_j|, which the
-random weights make comparable to S / sqrt(K) and so far above 2^-11 S.
-GroupNorm(1, C) after the conv (48 kHz), per sample of N values with conv errors e_i (the bound above), mean m and
-rstd r: the mean moves by mean(e), the variance by 2 mean(|x - m| e) + mean(e)^2, r by half of that relatively
-(+ 2^-23 for its fp32 copy), and the fp32 affine adds 2^-22 (|y| + |beta|):
-  |dy| <= |gamma| r (e + mean(e) + 2^-24 |m|) + |gamma| |x - m| r (dvar / (2 (var + eps)) + 2^-23) + 2^-22 (|y| + |beta|).
+Conv bound (gpu_checks.gemm_bound, 1.001 margin), per output element y = b + sum_j w_j a_j over the K = k' Cin taps of
+the GEMM row (k' = k, or k + (P - 1) stride when P time steps share a row): a_j = ELU(x) or x at the padded index, which
+the kernel rounds to fp16 (r_a = 2^-11); S and sum_j |a_j| come from the same padded conv on |a| and |w|, and on |a| and
+ones.  GroupNorm(1, C) after the conv (48 kHz): gpu_checks.ln_bound over each sample's N values, 1.001 margin.
 An rms ceiling of about 3x the level measured on the H100 sits on top (RMS_CEIL below).  The LSTM (recurrent state
 an fp16 hi/lo pair) and the whole forward are held to rms and max-abs ceilings of the same kind.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 
 import fadtk_b200 as fk
-from fadtk_b200 import _native
 from fadtk_b200 import weights_encodec as we
+from gpu_checks import (Guarded, check_bound, expect_rejected, gemm_bound, ln_bound, on_fresh_engine, report,
+                        report_stats, rms_rel)
 from oracle import encodec_oracle as eo
 
 pytestmark = pytest.mark.gpu
 
 GUARD = 256
-SENTINEL_BITS = 0x7FC0FFEE                                      # an fp32 NaN the kernels never produce themselves
 MAX_CHUNK = 8 * 48000
 
 # rms relative error (rms |kernel - fp64| / rms |fp64|), about 3x the largest level measured on an H100 80GB HBM3
@@ -85,39 +75,6 @@ def dev(engine):
     return engine.torch_device
 
 
-class Guarded:
-    """An fp32 tensor of `shape` inside a sentinel-NaN buffer with `guard` elements on both sides."""
-
-    def __init__(self, shape, dev, guard=GUARD, body=None):
-        self.n = math.prod(shape)
-        self.guard = guard
-        self.buf = torch.empty(guard + self.n + guard, dtype=torch.float32, device=dev)
-        self.buf.view(torch.int32).fill_(SENTINEL_BITS)
-        self.body = self.buf[guard:guard + self.n].view(shape)
-        if body is not None:
-            self.body.copy_(body)
-
-    def check(self):
-        torch.cuda.synchronize()
-        raw = self.buf.view(torch.int32)
-        assert bool((raw[:self.guard] == SENTINEL_BITS).all()) and bool((raw[self.guard + self.n:] == SENTINEL_BITS).all()), \
-            "guard region overwritten"
-        assert not bool((self.body.view(torch.int32) == SENTINEL_BITS).any()), "output elements left unwritten"
-        assert bool(torch.isfinite(self.body).all()), "non-finite output: a tap was read outside its clip"
-        return self.body
-
-    def untouched(self):
-        return bool((self.buf.view(torch.int32) == SENTINEL_BITS).all())
-
-
-def _rms_rel(got, ref):
-    return ((got.double() - ref).square().mean().sqrt() / ref.square().mean().sqrt()).item()
-
-
-def _report(kind, what, line):
-    print(f"\n[encodec {kind}] {what}: {line}", flush=True)
-
-
 # ------------------------------------------------------------------------------------------------------ one conv
 def conv_reference(x, sdg, layer, elu_in, groupnorm, K):
     """x fp32 [B, T_in, Cin] -> (y fp64 [B, T_out, Cout], per-element bound; see the module docstring)"""
@@ -131,21 +88,12 @@ def conv_reference(x, sdg, layer, elu_in, groupnorm, K):
     S = eo._sconv(a.abs(), w.abs(), torch.zeros_like(b), stride, causal)
     sum_a = eo._sconv(a.abs(), torch.ones_like(w), torch.zeros_like(b), stride, causal)
     sum_w = w.abs().flatten(1).sum(1)[None, :, None]
-    e = ((2.0 ** -11 + 2.0 ** -21 + K * 2.0 ** -23) * S + 2.0 ** -25 * (sum_w + sum_a)
-         + 2.0 ** -24 * (b.abs()[None, :, None] + y.abs())) * 1.001
+    e = gemm_bound(S, sum_w, sum_a, K, b, y, r_a=2.0 ** -11) * 1.001
     if groupnorm:
         g = sdg[prefix + ".norm.weight"].double()[None, :, None]
         beta = sdg[prefix + ".norm.bias"].double()[None, :, None]
-        m = y.mean((1, 2), keepdim=True)
-        yc = y - m
-        var = yc.square().mean((1, 2), keepdim=True)
-        r = 1.0 / torch.sqrt(var + 1e-5)
-        me = e.mean((1, 2), keepdim=True)
-        dvar = 2 * (yc.abs() * e).mean((1, 2), keepdim=True) + me.square()
-        yn = yc * r * g + beta
-        e = (g.abs() * r * (e + me + 2.0 ** -24 * m.abs()) + g.abs() * yc.abs() * r * (dvar / (2 * (var + 1e-5)) + 2.0 ** -23)
-             + 2.0 ** -22 * (yn.abs() + beta.abs())) * 1.001
-        y = yn
+        y, e = ln_bound(y, e, g, beta, (1, 2))
+        e = e * 1.001
     return y.transpose(1, 2), e.transpose(1, 2)
 
 
@@ -153,13 +101,11 @@ def run_conv(engine, layer, x, variant, elu_in, groupnorm):
     """x fp32 [B, T_in, Cin] copied into a NaN-guarded buffer -> the checked output [B, T_out, Cout]"""
     B, T_in, cin = x.shape
     _, cout, k, s = layer_table(variant)[layer]
-    xin = Guarded(x.shape, x.device, guard=16 * 512, body=x)   # covers the widest padding (12 steps) of 512 channels
-    out = Guarded((B, -(-T_in // s), cout), x.device)
+    xin = Guarded(x.shape, torch.float32, x.device, 16 * 512, init=x)   # covers the widest padding (12 steps) of 512 channels
+    out = Guarded((B, -(-T_in // s), cout), torch.float32, x.device, GUARD)
     engine.encodec_conv(layer, xin.body, B, T_in, out.body, elu_in=elu_in, groupnorm=groupnorm)
     got = out.check()
-    raw = xin.buf.view(torch.int32)
-    assert bool((raw[:xin.guard] == SENTINEL_BITS).all()) and bool((raw[xin.guard + xin.n:] == SENTINEL_BITS).all()) \
-        and bool(torch.equal(xin.body, x)), "the input or its guard was modified"
+    assert xin.intact_input(), "the input or its guard was modified"
     return got
 
 
@@ -180,19 +126,8 @@ def check_conv(engine, dev, variant, layer, T_in, B, elu_in, groupnorm, seed, st
     x = conv_input(dev, seed, B, T_in, cin)
     got = run_conv(engine, layer, x, variant, elu_in, groupnorm)
     ref, bound = conv_reference(x, state(variant, dev)[1], layer, elu_in, groupnorm, K)
-    err = (got.double() - ref).abs()
-    ratio = (err / bound).max().item()
-    worst = int((err / bound).flatten().argmax())
     what = f"{variant} layer {layer} T_in {T_in} B {B} elu {int(elu_in)} gn {int(groupnorm)}"
-    assert ratio <= 1.0, (f"{what}: max |err| / bound = {ratio:.3g} at flat index {worst} "
-                          f"(got {got.flatten()[worst].item()!r}, want {ref.flatten()[worst].item()!r})")
-    rms = _rms_rel(got, ref)
-    kind = "conv_gn" if groupnorm else "conv"
-    assert rms <= RMS_CEIL[kind], f"{what}: rms relative error {rms:.3g} above {RMS_CEIL[kind]:.3g}"
-    st = stats.setdefault(kind, [0.0, 0.0, ""])
-    if rms > st[0]:
-        st[0], st[2] = rms, what
-    st[1] = max(st[1], ratio)
+    check_bound("conv_gn" if groupnorm else "conv", what, got, ref, bound, stats, RMS_CEIL)
     return got, packed
 
 
@@ -222,9 +157,7 @@ def test_conv_matches_fp64(engine, dev, variant, layer, capsys):
                 paths.add(packed)
     if we.time_pack(cout) > 1:
         assert paths == {True, False}, "the lengths do not cover both the packed and the plain weights"
-    with capsys.disabled():
-        for kind, (rms, ratio, what) in stats.items():
-            _report(kind, f"{variant} layer {layer}", f"largest rms rel err {rms:.3e} ({what}), max err / bound {ratio:.3f}")
+    report_stats(capsys, "encodec", stats, f"{variant} layer {layer}")
 
 
 @pytest.mark.parametrize("variant,layer", LAYERS, ids=[f"{v}-L{l}" for v, l in LAYERS])
@@ -260,22 +193,22 @@ def test_lstm_matches_fp64(engine, dev, TF, capsys):
         n = 515
         g = torch.Generator(device=dev).manual_seed(TF)
         z = (torch.randn((n, TF, 512), generator=g, device=dev) * (0.5 + torch.rand((n, 1, 1), generator=g, device=dev))).contiguous()
-        zin = Guarded(z.shape, dev, body=z)
-        out = Guarded(z.shape, dev)
+        zin = Guarded(z.shape, torch.float32, dev, GUARD, init=z)
+        out = Guarded(z.shape, torch.float32, dev, GUARD)
         engine.encodec_lstm(zin.body, n, TF, out.body)
         got = out.check()
         ref = eo.lstm(z, state(variant, dev)[1])
-        rms = _rms_rel(got, ref)
+        rms = rms_rel(got, ref)
         mx = (got.double() - ref).abs().max().item()
-        rms_last = _rms_rel(got[512:], ref[512:])
+        rms_last = rms_rel(got[512:], ref[512:])
         with capsys.disabled():
-            _report("lstm", f"{variant} TF {TF} clips {n}", f"rms rel err {rms:.3e} (second group {rms_last:.3e}), max abs {mx:.3e}")
+            report("encodec", "lstm", f"{variant} TF {TF} clips {n}", f"rms rel err {rms:.3e} (second group {rms_last:.3e}), max abs {mx:.3e}")
         assert rms <= RMS_CEIL["lstm"] and rms_last <= RMS_CEIL["lstm"], (rms, rms_last)
         assert mx <= LSTM_MAX_ABS, mx
-        again = Guarded(z.shape, dev)
+        again = Guarded(z.shape, torch.float32, dev, GUARD)
         engine.encodec_lstm(zin.body, n, TF, again.body)
         assert torch.equal(again.check(), got), "two identical calls differ"
-        one = Guarded((1, TF, 512), dev)
+        one = Guarded((1, TF, 512), torch.float32, dev, GUARD)
         engine.encodec_lstm(z[513:514].contiguous(), 1, TF, one.body)
         assert torch.equal(one.check(), got[513:514]), "a clip's LSTM output depends on its group"
 
@@ -307,11 +240,11 @@ def check_forward(ml, variant, dev, lengths, capsys):
             ref = forward_reference(c, sdg, variant, dev)
             assert g.shape == ref.shape == (-(-T // 320), 128), (g.shape, ref.shape)
             assert bool(torch.isfinite(g).all()), f"{variant} T {T}: non-finite embedding"
-            rms = _rms_rel(g, ref)
+            rms = rms_rel(g, ref)
             mx = ((g.double() - ref).abs().max() / ref.abs().max()).item()
             worst = max(worst, rms)
             with capsys.disabled():
-                _report("forward", f"{variant} T {T}", f"rms rel err {rms:.3e}, max abs err / max |ref| {mx:.3e}")
+                report("encodec", "forward", f"{variant} T {T}", f"rms rel err {rms:.3e}, max abs err / max |ref| {mx:.3e}")
             assert rms <= RMS_CEIL["forward"], (T, rms)
             assert mx <= FORWARD_MAX_ABS_REL, (T, mx)
     return worst
@@ -349,41 +282,27 @@ def test_embedding_independent_of_batch(engine, variant):
 
 # ------------------------------------------------------------------------------------------------------- rejections
 def _conv_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
         a = dict(layer=1, B=2, T_in=16, gn=0, x="ok", out="ok")
         a.update(over)
-        x = Guarded((2, 16, 32), dev, body=torch.zeros((2, 16, 32), device=dev))
-        o = Guarded((2, 16, 32), dev)
+        dev = engine.torch_device
+        x = Guarded((2, 16, 32), torch.float32, dev, GUARD, init=torch.zeros((2, 16, 32), device=dev))
+        o = Guarded((2, 16, 32), torch.float32, dev, GUARD)
         outs.append(o)
-        xp = {"ok": x.body, "null": None, "odd": x.buf[x.guard + 1:]}[a["x"]]
-        op = {"ok": o.body, "null": None, "odd": o.buf[o.guard + 1:]}[a["out"]]
-        engine.encodec_conv(a["layer"], xp, a["B"], a["T_in"], op, groupnorm=a["gn"])
+        engine.encodec_conv(a["layer"], x.ptr(a["x"]), a["B"], a["T_in"], o.ptr(a["out"]), groupnorm=a["gn"])
     return call
 
 
 def _lstm_call(**over):
-    def call(engine, dev, outs):
+    def call(engine, outs):
         a = dict(n=2, TF=3, z="ok", out="ok")
         a.update(over)
-        z = Guarded((2, 3, 512), dev, body=torch.zeros((2, 3, 512), device=dev))
-        o = Guarded((2, 3, 512), dev)
+        dev = engine.torch_device
+        z = Guarded((2, 3, 512), torch.float32, dev, GUARD, init=torch.zeros((2, 3, 512), device=dev))
+        o = Guarded((2, 3, 512), torch.float32, dev, GUARD)
         outs.append(o)
-        zp = {"ok": z.body, "null": None, "odd": z.buf[z.guard + 1:]}[a["z"]]
-        op = {"ok": o.body, "null": None, "odd": o.buf[o.guard + 1:]}[a["out"]]
-        engine.encodec_lstm(zp, a["n"], a["TF"], op)
+        engine.encodec_lstm(z.ptr(a["z"]), a["n"], a["TF"], o.ptr(a["out"]))
     return call
-
-
-def _unloaded(call):
-    def run(engine, dev, outs):
-        fresh = _native.Engine(engine.device, 16)
-        try:
-            launches = fresh.launches
-            call(fresh, dev, outs)
-        finally:
-            assert fresh.launches == launches, "a rejected call launched a kernel"
-            fresh.close()
-    return run
 
 
 REJECT = [
@@ -399,7 +318,7 @@ REJECT = [
     ("conv null out", "24k", _conv_call(out="null"), "fad_encodec_conv: null x or out"),
     ("conv misaligned x", "24k", _conv_call(x="odd"), "fad_encodec_conv: x and out must be 16-byte aligned"),
     ("conv misaligned out", "48k", _conv_call(out="odd", gn=1), "fad_encodec_conv: x and out must be 16-byte aligned"),
-    ("conv before any load", None, _unloaded(_conv_call()), "fad_encodec_conv: fad_encodec_load has not been called"),
+    ("conv before any load", None, on_fresh_engine(_conv_call()), "fad_encodec_conv: fad_encodec_load has not been called"),
     ("lstm no clips", "24k", _lstm_call(n=0), "fad_encodec_lstm: n_clips and TF must be positive"),
     ("lstm TF 0", "48k", _lstm_call(TF=0), "fad_encodec_lstm: n_clips and TF must be positive"),
     ("lstm TF beyond the chunk", "24k", _lstm_call(TF=MAX_CHUNK // 320 + 1),
@@ -407,20 +326,13 @@ REJECT = [
     ("lstm null z", "24k", _lstm_call(z="null"), "fad_encodec_lstm: null z or out"),
     ("lstm misaligned out", "24k", _lstm_call(out="odd"), "fad_encodec_lstm: z and out must be 16-byte aligned"),
     ("lstm misaligned z", "48k", _lstm_call(z="odd"), "fad_encodec_lstm: z and out must be 16-byte aligned"),
-    ("lstm before any load", None, _unloaded(_lstm_call()), "fad_encodec_lstm: fad_encodec_load has not been called"),
+    ("lstm before any load", None, on_fresh_engine(_lstm_call()), "fad_encodec_lstm: fad_encodec_load has not been called"),
 ]
 
 
 @pytest.mark.parametrize("variant,call,message", [c[1:] for c in REJECT], ids=[c[0] for c in REJECT])
-def test_stage_entries_reject_invalid_arguments(engine, dev, variant, call, message):
+def test_stage_entries_reject_invalid_arguments(engine, variant, call, message):
     """Arguments the launch cannot honour fail with their message, launch nothing and write nothing."""
     if variant is not None:
         load(engine, variant)
-    outs = []
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
-        call(engine, dev, outs)
-    torch.cuda.synchronize()
-    assert str(exc.value) == message
-    assert engine.launches == launches, "a rejected call launched a kernel"
-    assert all(o.untouched() for o in outs), "a rejected call wrote output"
+    expect_rejected(engine, call, message, [])

@@ -15,43 +15,18 @@ import pytest
 import torch
 from scipy.special import erf
 
-from fadtk_b200 import _native
 from fadtk_b200 import weights as wts
+from gpu_checks import Guarded, expect_rejected, rms_rel
 from oracle import clap_oracle as co
 
 pytestmark = pytest.mark.gpu
 
 GUARD = 256
-SENTINEL = {torch.float16: (torch.int16, 0x7E5A), torch.float32: (torch.int32, 0x7FC0FFEE)}   # NaN bit patterns
 ACT_NONE, ACT_RELU, ACT_GELU, ACT_ELU = 0, 1, 2, 3
 
 
 def _pad(v, m):
     return (v + m - 1) // m * m
-
-
-class Guarded:
-    """[rows, cols] output view inside a sentinel-filled buffer with guard regions on both sides."""
-
-    def __init__(self, rows, cols, dtype, dev, init=None):
-        self.n = rows * cols
-        self.shape = (rows, cols)
-        self.idt, self.bits = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + self.n + 2 * cols + GUARD, dtype=dtype, device=dev)
-        self.buf.view(self.idt).fill_(self.bits)
-        self.body = self.buf[GUARD:GUARD + self.n].view(rows, cols)
-        if init is not None:
-            self.body.copy_(init)
-
-    def guards_intact(self):
-        raw = self.buf.view(self.idt)
-        return bool((raw[:GUARD] == self.bits).all()) and bool((raw[GUARD + self.n:] == self.bits).all())
-
-    def untouched(self):
-        return bool((self.buf.view(self.idt) == self.bits).all())
-
-    def fully_written(self):
-        return not bool((self.body.view(self.idt) == self.bits).any())
 
 
 @pytest.fixture(scope="module")
@@ -116,16 +91,14 @@ def check_f32(out32, ref, bound, what):
 def run_linear(engine, a, rows, k_cols, packed, bias_full, n_cols, act, split_w, lda=0, want=("16", "32"),
                resid=None, resid_C=0, resid_res=0, resid_shift=0):
     dev = a.device
-    o16 = Guarded(rows, n_cols, torch.float16, dev) if "16" in want else None
-    o32 = Guarded(rows, n_cols, torch.float32, dev) if "32" in want else None
+    o16 = Guarded((rows, n_cols), torch.float16, dev, GUARD, GUARD + 2 * n_cols) if "16" in want else None
+    o32 = Guarded((rows, n_cols), torch.float32, dev, GUARD, GUARD + 2 * n_cols) if "32" in want else None
     engine.linear(a, rows, k_cols, packed, bias_full, n_cols, act, lda=lda, split_w=split_w,
                   out16=o16.body if o16 else None, out32=o32.body if o32 else None,
                   resid=resid, resid_C=resid_C, resid_res=resid_res, resid_shift=resid_shift)
-    torch.cuda.synchronize()
     for o in (o16, o32):
         if o is not None:
-            assert o.guards_intact(), "output guard region overwritten"
-            assert o.fully_written(), "output elements left unwritten"
+            o.check()
     return (o16.body if o16 else None), (o32.body if o32 else None)
 
 
@@ -220,7 +193,7 @@ def _resid_case(engine, dev, seed, rows, k_cols, n_cols, act, resid_C, res, shif
     expect[perm] = before[perm] + out32[:, :resid_C]                     # row r adds into token perm[r]
     # the residual alone (how the transformer blocks call it), then together with both outputs
     for want in ((), ("16", "32")):
-        r = Guarded(rows, resid_C, torch.float32, dev, init=before)
+        r = Guarded((rows, resid_C), torch.float32, dev, GUARD, GUARD + 2 * resid_C, init=before)
         o16, o32 = run_linear(engine, a, rows, k_cols, packed, bias_full, n_cols, act, 1, want=want,
                               resid=r.body, resid_C=resid_C, resid_res=res, resid_shift=shift)
         assert r.guards_intact(), "residual guard region overwritten"
@@ -339,10 +312,6 @@ def test_activation_applied_to_the_same_accumulator(engine, dev, act):
 
 
 # -------------------------------------------------------------------------------------- e. weight-split precision
-def _rms_rel(out32, ref):
-    return ((out32.double() - ref).square().mean().sqrt() / ref.square().mean().sqrt()).item()
-
-
 def _split_errors(engine, dev, kind, k):
     """rms relative error of the fp32 output per weight mode against fp64 from the fp32 weights."""
     g = _gen(dev, 1000 + k)
@@ -362,12 +331,12 @@ def _split_errors(engine, dev, kind, k):
     errs = {}
     for mode in (0, 1):
         _, out32 = engine.umma_layer(x, packs[mode], b, taps, False, False, want_f32=True, split_w=mode)
-        errs[f"layer{mode}"] = _rms_rel(out32, ref)
+        errs[f"layer{mode}"] = rms_rel(out32, ref)
     if taps == 1:
         a = x.reshape(nb, cin)
         for mode in (0, 1):
             _, out32 = run_linear(engine, a, nb, cin, packs[mode], b, cout, ACT_NONE, mode, want=("32",))
-            errs[f"linear{mode}"] = _rms_rel(out32, ref.reshape(nb, cout))
+            errs[f"linear{mode}"] = rms_rel(out32, ref.reshape(nb, cout))
     return errs
 
 
@@ -484,35 +453,33 @@ def test_linear_rejects_invalid_arguments(engine, dev, case, message):
     packed = torch.randn((2 * 128, 128), generator=_gen(dev, 4), device=dev).to(torch.float16)
     bias = None if case.get("no_bias") else torch.randn((128,), generator=_gen(dev, 5), device=dev)
     want = case.get("want", ("16", "32"))
-    o16 = Guarded(rows, 128, torch.float16, dev)
-    o32 = Guarded(rows, 128, torch.float32, dev)
+    o16 = Guarded((rows, 128), torch.float16, dev, GUARD, GUARD + 256)
+    o32 = Guarded((rows, 128), torch.float32, dev, GUARD, GUARD + 256)
+    r = Guarded((rows, 128), torch.float32, dev, GUARD, GUARD + 256)
     resid_C = case.get("resid_C", 0)
-    r = Guarded(rows, 128, torch.float32, dev) if resid_C else None
-    out16 = o16.buf[GUARD:] if "16" in want else None
-    out32 = o32.buf[GUARD:] if "32" in want else None
+    out16 = o16.body if "16" in want else None
+    out32 = o32.body if "32" in want else None
     if case.get("misalign") == "out32":
-        out32 = o32.buf[GUARD + 1:]
+        out32 = o32.ptr("odd")
     if case.get("misalign") == "out16":
         out16 = o16.buf[GUARD + 4:]
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
+
+    def call(engine, outs):
         engine.linear(a, rows, k_cols, packed, bias, n_cols, case.get("act", ACT_NONE), lda=case.get("lda", 0),
-                      split_w=case.get("split_w", 1), out16=out16, out32=out32, resid=r.buf[GUARD:] if r else None,
+                      split_w=case.get("split_w", 1), out16=out16, out32=out32, resid=r.body if resid_C else None,
                       resid_C=resid_C, resid_res=case.get("resid_res", 0), resid_shift=case.get("resid_shift", 0))
-    torch.cuda.synchronize()
-    assert str(exc.value) == "clap_gemm: " + message
-    assert engine.launches == launches, "a rejected call launched a kernel"
-    assert o16.untouched() and o32.untouched() and (r is None or r.untouched()), "a rejected call wrote output"
+    expect_rejected(engine, call, "clap_gemm: " + message, [o16, o32, r])
 
 
-def _umma_layer_split_w_2(engine, dev):
+def _umma_layer_split_w_2(engine, outs):
+    dev = engine.torch_device
     x = torch.zeros((1, 1, 1, 64), dtype=torch.float16, device=dev)
     w = torch.zeros((2 * 128, 64), dtype=torch.float16, device=dev)
     engine.umma_layer(x, w, torch.zeros(128, device=dev), 1, False, False, want_f32=True, split_w=2)
 
 
-def _stats_tensor_core_1(engine, dev):
-    e = torch.zeros((16, 64), dtype=torch.float16, device=dev)
+def _stats_tensor_core_1(engine, outs):
+    e = torch.zeros((16, 64), dtype=torch.float16, device=engine.torch_device)
     engine.stats_accumulate(e, e[0], engine.stats_new(64), tensor_core=1)
 
 
@@ -525,11 +492,6 @@ MODE_REJECT = [
 
 
 @pytest.mark.parametrize("call,message", [c[1:] for c in MODE_REJECT], ids=[c[0] for c in MODE_REJECT])
-def test_stage_entries_reject_unknown_modes(engine, dev, call, message):
+def test_stage_entries_reject_unknown_modes(engine, call, message):
     """A mode the library does not have fails with its message and launches nothing."""
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
-        call(engine, dev)
-    torch.cuda.synchronize()
-    assert str(exc.value) == message
-    assert engine.launches == launches, "a rejected call launched a kernel"
+    expect_rejected(engine, call, message, [])

@@ -7,36 +7,16 @@ shifted by an odd number of M tiles (128 rows, or whole images that make an odd 
 tile to the other rank of its pair and flips the parity of the tile count: the shared rows must come out bitwise
 the same.  Outputs sit between NaN sentinels, with a trailing guard longer than a spare tile can reach.
 """
-import math
-
 import pytest
 import torch
 
 from fadtk_b200 import _native
 from fadtk_b200 import weights as wts
-from test_gpu_gemm import (ACT_ELU, ACT_GELU, ACT_NONE, ACT_RELU, GUARD, SENTINEL, _gen, check_f32, make_problem,
-                           reference)
+from gpu_checks import SENTINEL, Guarded
+from test_gpu_gemm import ACT_ELU, ACT_GELU, ACT_NONE, ACT_RELU, _gen, check_f32, make_problem, reference
 
 pytestmark = pytest.mark.gpu
-
-
-class Fenced:
-    """Output tensor of `shape` inside a sentinel-filled buffer: GUARD elements before it, `tail` after it."""
-
-    def __init__(self, shape, dtype, dev, tail, init=None):
-        self.n = math.prod(shape)
-        self.idt, self.bits = SENTINEL[dtype]
-        self.buf = torch.empty(GUARD + self.n + tail, dtype=dtype, device=dev)
-        self.buf.view(self.idt).fill_(self.bits)
-        self.body = self.buf[GUARD:GUARD + self.n].view(shape)
-        if init is not None:
-            self.body.copy_(init)
-
-    def check(self, what):
-        raw = self.buf.view(self.idt)
-        assert bool((raw[:GUARD] == self.bits).all()) and bool((raw[GUARD + self.n:] == self.bits).all()), \
-            f"{what}: a store landed outside the output"
-        assert not bool((self.body.view(self.idt) == self.bits).any()), f"{what}: output elements left unwritten"
+GUARD = 256
 
 
 # ------------------------------------------------------------------------------------------ plain geometry (Linear)
@@ -44,12 +24,11 @@ def linear(engine, a, rows, k_cols, packed, bias_full, n_cols, act, split_w, res
     """fad_linear into fenced fp16 and fp32 outputs (and the fenced residual); 256 rows of trailing guard cover the
     rows of a spare tile, which start at the next multiple of 128 at or after `rows`."""
     dev = a.device
-    o16 = Fenced((rows, n_cols), torch.float16, dev, 256 * n_cols)
-    o32 = Fenced((rows, n_cols), torch.float32, dev, 256 * n_cols)
-    r = Fenced((rows, resid_C), torch.float32, dev, 256 * resid_C, init=resid) if resid is not None else None
+    o16 = Guarded((rows, n_cols), torch.float16, dev, GUARD, 256 * n_cols)
+    o32 = Guarded((rows, n_cols), torch.float32, dev, GUARD, 256 * n_cols)
+    r = Guarded((rows, resid_C), torch.float32, dev, GUARD, 256 * resid_C, init=resid) if resid is not None else None
     engine.linear(a, rows, k_cols, packed, bias_full, n_cols, act, split_w=split_w, out16=o16.body, out32=o32.body,
                   resid=r.body if r else None, resid_C=resid_C)
-    torch.cuda.synchronize()
     for o, what in ((o16, "fp16 output"), (o32, "fp32 output"), (r, "residual")):
         if o is not None:
             o.check(what)
@@ -104,12 +83,11 @@ def umma_layer(engine, x, packed, bias, cout, relu, pool, split_w):
     nb, hh, ww, cin = x.shape
     oh, ow = (hh // 2, ww // 2) if pool else (hh, ww)
     shape, tail = (nb, oh, ow, cout), 8 * oh * ow * cout
-    o16 = Fenced(shape, torch.float16, x.device, tail)
-    o32 = None if pool else Fenced(shape, torch.float32, x.device, tail)
+    o16 = Guarded(shape, torch.float16, x.device, GUARD, tail)
+    o32 = None if pool else Guarded(shape, torch.float32, x.device, GUARD, tail)
     _native._check(_native.lib().fad_umma_layer(
         engine._h, x.data_ptr(), nb, hh, ww, cin, packed.data_ptr(), bias.data_ptr(), cout, 9, relu, int(pool),
         split_w, o16.body.data_ptr(), _native._ptr(o32.body if o32 else None), _native._stream()))
-    torch.cuda.synchronize()
     o16.check("fp16 output")
     if o32 is None:
         return o16.body

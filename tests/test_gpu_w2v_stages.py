@@ -13,36 +13,30 @@ with an fp16 NaN, so a valid output that reads one is non-finite.
 Per-element bounds (float64, 1.001 margin), S = sum_j |w_j| |a_j| over the K = k Cin taps of an output:
   * normalize: out = (x - m) inv in fp32 with m, inv the fp32 roundings of the fp64 mean and 1 / sqrt(var + 1e-7):
         |d| <= 3 2^-23 |out| + 2^-24 inv |mean|  (the fp64 moments' own error included).  A wrong eps moves the +-1-LSB clip (var ~ 6e-10 << 1e-7) by far more.
-  * GEMM conv (c >= 1, the positional conv), pre-activation:
-        e = (r_a + 2^-21 + K 2^-23) S + 2^-25 (sum_j |w_j| + sum_j |a_j|) + 2^-24 (|b| + |y|)
-    with r_a = 0 where the operand is the fp16 activation itself and 2^-11 where the kernel rounds it to fp16 (the
-    positional conv's fp32 stream; the layer variant's conv 0, whose enc_im2col rounds the normalised waveform);
-    2^-21 |w_j| is the fp16 hi/lo pair of the fp32 weight, K 2^-23 S fp32 accumulation.
+  * GEMM conv (c >= 1, the positional conv), pre-activation: gpu_checks.gemm_bound, with r_a = 0 where the operand is
+    the fp16 activation itself and 2^-11 where the kernel rounds it to fp16 (the positional conv's fp32 stream; the
+    layer variant's conv 0, whose enc_im2col rounds the normalised waveform).
   * group variant conv 0 (CUDA cores, fp32 weights hi + lo, GroupNorm folded into (scale, shift) from fp64 moments):
         e = |scale| (10 2^-24 + 2^-20) S + 2^-23 (|y| + |shift|)
     (2^-20 S |scale| covers the hi + lo weight against the original, consistently in the conv and in its GroupNorm).
-  * layer variant LayerNorm(512) over a row with conv errors e_i, mean m, rstd r (as in the Encodec GroupNorm bound):
-        |dy| <= |g| r (e + mean(e) + 2^-24 |m|) + |g| |x - m| r (dvar / (2 (var + eps)) + 2^-23) + 2^-22 (|y| + |beta|)
-  * GELU: 1.13 (its largest slope) times the error in front of it, + 2^-22 |y| for its fp32 evaluation;
-    fp16 output: + 2^-11 |y| + 2^-25;  the positional conv's fp32 residual add: + 2^-24 |out|.
+  * layer variant LayerNorm(512) over a row with conv errors e_i: gpu_checks.ln_bound.
+  * GELU, fp32 or fp16 output: gpu_checks.gelu_out;  the positional conv's fp32 residual add: + 2^-24 |out|.
 The layers (attention, two LayerNorms, two GEMMs with fp16 operands) and the whole forward are held to rms ceilings,
 about 3x the level measured on the H100 (RMS_CEIL below), and the forward's taps also to a centred ceiling: under the
 synthetic weights the hidden state is mostly a per-channel constant, and the per-frame fluctuation that FAD's covariance
 measures is what the centred metric (per-(clip, channel) mean over frames removed from error and reference) sees.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 
 import fadtk_b200 as fk
-from fadtk_b200 import _native, synth, weights_w2v as ww
+from fadtk_b200 import synth, weights_w2v as ww
+from gpu_checks import (Guarded, check_bound, expect_rejected, gelu_out, gemm_bound, layer_metrics, ln_bound,
+                        on_fresh_engine, report, report_stats, tap_metrics)
 from oracle import w2v_oracle as wo
 
 GUARD = 4096
-SENT32 = 0x7FC0FFEE                                      # fp32 NaNs the kernels never produce themselves
-SENT16 = 0x7D5A
 MAX_CLIPS = 2
 KERNEL, STRIDE = ww.CONV_KERNEL, ww.CONV_STRIDE
 
@@ -138,73 +132,6 @@ def load(engine, name, max_len, layers=2, max_clips=MAX_CLIPS):
         engine.owners["w2v"] = token
 
 
-# --------------------------------------------------------------------------------------------------- buffers
-class Guarded:
-    """A tensor of `shape` (fp32 or fp16) inside a sentinel-NaN buffer with `guard` elements on both sides."""
-
-    def __init__(self, shape, dtype=torch.float32, guard=GUARD, body=None):
-        self.n = math.prod(shape)
-        self.guard = guard
-        self.sent = SENT32 if dtype == torch.float32 else SENT16
-        self.buf = torch.empty(guard + self.n + guard, dtype=dtype, device="cuda")
-        self.raw().fill_(self.sent)
-        self.body = self.buf[guard:guard + self.n].view(shape)
-        if body is not None:
-            self.body.copy_(body)
-            self.init = self.body.clone()
-
-    def raw(self):
-        return self.buf.view(torch.int32 if self.buf.dtype == torch.float32 else torch.int16)
-
-    def guards_intact(self):
-        r = self.raw()
-        return bool((r[:self.guard] == self.sent).all()) and bool((r[self.guard + self.n:] == self.sent).all())
-
-    def check(self):
-        torch.cuda.synchronize()
-        assert self.guards_intact(), "guard region overwritten"
-        assert not bool((self.raw()[self.guard:self.guard + self.n] == self.sent).any()), "output elements left unwritten"
-        assert bool(torch.isfinite(self.body).all()), "non-finite output: a dead row or a neighbouring value was read"
-        return self.body
-
-    def intact_input(self):
-        torch.cuda.synchronize()
-        return self.guards_intact() and bool(torch.equal(self.body, self.init))
-
-    def untouched(self):
-        return bool((self.raw() == self.sent).all())
-
-
-def _rms_rel(got, ref):
-    return ((got.double() - ref).square().mean().sqrt() / ref.square().mean().sqrt()).item()
-
-
-def _report(kind, what, line):
-    print(f"\n[w2v {kind}] {what}: {line}", flush=True)
-
-
-def check_bound(kind, what, got, ref, bound, stats):
-    err = (got.double() - ref).abs()
-    r = err / bound
-    ratio = r.max().item()
-    worst = int(r.flatten().argmax())
-    assert ratio <= 1.0, (f"{what}: max |err| / bound = {ratio:.3g} at flat index {worst} "
-                          f"(got {got.flatten()[worst].item()!r}, want {ref.flatten()[worst].item()!r})")
-    rms = _rms_rel(got, ref) if bool(ref.abs().max() > 0) else err.max().item()
-    if kind in RMS_CEIL:
-        assert rms <= RMS_CEIL[kind], f"{what}: rms relative error {rms:.3g} above {RMS_CEIL[kind]:.3g}"
-    st = stats.setdefault(kind, [0.0, 0.0, ""])
-    if rms > st[0]:
-        st[0], st[2] = rms, what
-    st[1] = max(st[1], ratio)
-
-
-def report_stats(capsys, stats, what):
-    with capsys.disabled():
-        for kind, (rms, ratio, w) in stats.items():
-            _report(kind, what, f"largest rms rel err {rms:.3e} ({w}), max err / bound {ratio:.3f}")
-
-
 # ------------------------------------------------------------------------------------------------- inputs
 def sine30(n, sr):
     t = np.arange(n) / sr
@@ -245,7 +172,7 @@ def test_normalize_matches_fp64(engine, L, capsys):
              np.zeros(L, np.int16), lsb_noise(L, 4), square(L)]
     clips = [np.resize(c, L) for c in clips]
     pcm = torch.from_numpy(np.stack(clips)).cuda()
-    out = Guarded((len(clips), L))
+    out = Guarded((len(clips), L), torch.float32, "cuda", GUARD)
     engine.w2v_normalize(pcm, len(clips), L, out.body)
     got = out.check()
     ref = ref_normalize(pcm)
@@ -255,44 +182,20 @@ def test_normalize_matches_fp64(engine, L, capsys):
     bound = (3 * 2.0 ** -23 * ref.abs() + 2.0 ** -24 * inv * mean.abs()) * 1.001 + 1e-30
     stats = {}
     for i, name in enumerate(("music", "noise", "dc", "silence", "lsb", "square")):
-        check_bound("normalize", f"L {L} {name}", got[i], ref[i], bound[i], stats)
+        check_bound("normalize", f"L {L} {name}", got[i], ref[i], bound[i], stats, RMS_CEIL)
     assert bool((got[3] == 0).all())
-    report_stats(capsys, stats, f"L {L}")
+    report_stats(capsys, "w2v", stats, f"L {L}")
 
 
 # ---------------------------------------------------------------------------------------------------- convs
-def gemm_bound(a, w, b, stride, y, round_a, groups=1, padding=0, drop_last=False):
-    """pre-activation error bound of a GEMM conv (module docstring); a [B, Cin, T] float64, w [Cout, Cin/g, k]"""
-    K = w.shape[1] * w.shape[2]
+def conv_sums(a, w, stride, groups=1, padding=0, drop_last=False):
+    """(S, sum |w|, sum |a|, K) of gpu_checks.gemm_bound for a conv1d; a [B, Cin, T] float64, w [Cout, Cin/g, k]"""
     conv = lambda u, v: torch.nn.functional.conv1d(u, v, None, stride, padding, 1, groups)
     S = conv(a.abs(), w.abs())
     sa = conv(a.abs(), torch.ones_like(w))
     if drop_last:
         S, sa = S[..., :-1], sa[..., :-1]
-    sw = w.abs().flatten(1).sum(1)[None, :, None]
-    r = 2.0 ** -11 if round_a else 0.0
-    return (r + 2.0 ** -21 + K * 2.0 ** -23) * S + 2.0 ** -25 * (sw + sa) + 2.0 ** -24 * (b.abs()[None, :, None] + y.abs())
-
-
-def ln_bound(y, e, g, beta, dim):
-    """LayerNorm / GroupNorm over `dim` of y (pre-norm, float64) with errors e -> (normalised y, bound)"""
-    m = y.mean(dim, keepdim=True)
-    yc = y - m
-    var = yc.square().mean(dim, keepdim=True)
-    r = 1.0 / torch.sqrt(var + 1e-5)
-    me = e.mean(dim, keepdim=True)
-    dvar = 2 * (yc.abs() * e).mean(dim, keepdim=True) + me.square()
-    yn = yc * r * g + beta
-    return yn, (g.abs() * r * (e + me + 2.0 ** -24 * m.abs()) + g.abs() * yc.abs() * r * (dvar / (2 * (var + 1e-5)) + 2.0 ** -23)
-                + 2.0 ** -22 * (yn.abs() + beta.abs()))
-
-
-def gelu_out(y, e, fp16):
-    out = torch.nn.functional.gelu(y)
-    e = 1.13 * e + 2.0 ** -22 * out.abs()
-    if fp16:
-        e = e + 2.0 ** -11 * (out.abs() + e) + 2.0 ** -25
-    return out, e * 1.001
+    return S, w.abs().flatten(1).sum(1)[None, :, None], sa, w.shape[1] * w.shape[2]
 
 
 @torch.no_grad()
@@ -303,10 +206,9 @@ def conv_reference(model, c, x):
     y = torch.nn.functional.conv1d(x, w, b, STRIDE[c])
     layer_variant = hasattr(mod, "layer_norm") and isinstance(mod.layer_norm, torch.nn.LayerNorm)
     if layer_variant:
-        e = gemm_bound(x, w, b, STRIDE[c], y, round_a=(c == 0))
+        e = gemm_bound(*conv_sums(x, w, STRIDE[c]), b, y, r_a=2.0 ** -11 if c == 0 else 0.0)
         g, beta = mod.layer_norm.weight[None, :, None], mod.layer_norm.bias[None, :, None]
-        yn, e = ln_bound(y, e, g, beta, 1)
-        want, bound = gelu_out(yn, e, c < 6)
+        y, e = ln_bound(y, e, g, beta, 1)
     elif c == 0:
         gn = mod.layer_norm                                                # GroupNorm(512, 512)
         S = torch.nn.functional.conv1d(x.abs(), w.abs(), None, STRIDE[c])
@@ -315,10 +217,11 @@ def conv_reference(model, c, x):
         yn = yc * scale + gn.bias[None, :, None]
         shift = yn - (y - b[None, :, None]) * scale
         e = scale.abs() * (10 * 2.0 ** -24 + 2.0 ** -20) * S + 2.0 ** -23 * (yn.abs() + shift.abs())
-        want, bound = gelu_out(yn, e, True)
+        y = yn
     else:
-        e = gemm_bound(x, w, b, STRIDE[c], y, round_a=False)
-        want, bound = gelu_out(y, e, c < 6)
+        e = gemm_bound(*conv_sums(x, w, STRIDE[c]), b, y)
+    want, bound = gelu_out(y, e, c < 6)
+    bound = bound * 1.001
     ref = mod(x)
     assert (ref - want).abs().max().item() <= 1e-9 * max(1.0, want.abs().max().item()), "the bound's restatement is not the module"
     return ref.transpose(1, 2), bound.transpose(1, 2)
@@ -327,8 +230,8 @@ def conv_reference(model, c, x):
 def run_conv(engine, c, x, B, L):
     """x (conv 0: fp32 [B, L]; else fp16 [B, T_c, 512]) guarded -> the checked compact output"""
     T = frames(L)
-    xin = Guarded(x.shape, x.dtype, body=x)
-    out = Guarded((B, T[c + 1], 512), torch.float32 if c == 6 else torch.float16)
+    xin = Guarded(x.shape, x.dtype, "cuda", GUARD, init=x)
+    out = Guarded((B, T[c + 1], 512), torch.float32 if c == 6 else torch.float16, "cuda", GUARD)
     engine.w2v_conv(c, xin.body, B, L, out.body)
     got = out.check()
     assert xin.intact_input(), "the input or its guard was modified"
@@ -347,9 +250,9 @@ def check_conv_chain(engine, name, L, sr, capsys):
             got = run_conv(engine, c, x, 2, L)
             xin = x.double()[:, None] if c == 0 else x.double().transpose(1, 2)
             ref, bound = conv_reference(model, c, xin)
-            check_bound(kind, f"{name} conv {c} L {L} case {case}", got, ref, bound, stats)
+            check_bound(kind, f"{name} conv {c} L {L} case {case}", got, ref, bound, stats, RMS_CEIL)
             x = got
-    report_stats(capsys, stats, f"{name} L {L}")
+    report_stats(capsys, "w2v", stats, f"{name} L {L}")
 
 
 CONV_CASES = [("w2v2-base", L, 16000) for L in LENGTHS] + [("w2v2-base", 720000, 24000)] + \
@@ -382,8 +285,8 @@ def posconv_reference(model, x):
     w = pc.conv.weight
     xt = xd.transpose(1, 2)
     y = torch.nn.functional.conv1d(xt, w, pc.conv.bias, 1, 64, 1, 16)[..., :-1]
-    e = gemm_bound(xt, w, pc.conv.bias, 1, y, True, groups=16, padding=64, drop_last=True)
-    e = 1.13 * e + 2.0 ** -22 * torch.nn.functional.gelu(y).abs()
+    e = gemm_bound(*conv_sums(xt, w, 1, groups=16, padding=64, drop_last=True), pc.conv.bias, y, r_a=2.0 ** -11)
+    _, e = gelu_out(y, e, False)
     bound = (e.transpose(1, 2) + 2.0 ** -24 * ref.abs()) * 1.001
     return ref, bound
 
@@ -399,14 +302,14 @@ def test_posconv_matches_fp64(engine, name, capsys):
     stats = {}
     for S in (1, 2, 199, 1499):
         x = stream_input(2, S, d, S)
-        xin = Guarded(x.shape, body=x)
-        out = Guarded(x.shape)
+        xin = Guarded(x.shape, torch.float32, "cuda", GUARD, init=x)
+        out = Guarded(x.shape, torch.float32, "cuda", GUARD)
         engine.w2v_posconv(xin.body, 2, S, out.body)
         got = out.check()
         assert xin.intact_input()
         ref, bound = posconv_reference(model, x)
-        check_bound("posconv", f"{name} S {S}", got, ref, bound, stats)
-    report_stats(capsys, stats, name)
+        check_bound("posconv", f"{name} S {S}", got, ref, bound, stats, RMS_CEIL)
+    report_stats(capsys, "w2v", stats, name)
 
 
 # ------------------------------------------------------------------------------------------------- layers
@@ -424,38 +327,24 @@ def test_layers_match_fp64(engine, name, capsys):
         if not is_stable(model):                          # post-LN: the stream entering a layer is a LayerNorm's output
             x = torch.nn.functional.layer_norm(x, (d,))
         for l in range(2):
-            xin = Guarded(x.shape, body=x)
-            out = Guarded(x.shape)
+            xin = Guarded(x.shape, torch.float32, "cuda", GUARD, init=x)
+            out = Guarded(x.shape, torch.float32, "cuda", GUARD)
             engine.w2v_layer(l, xin.body, 2, S, out.body)
             got = out.check()
             assert xin.intact_input()
             with torch.no_grad():
                 ref = run_layer(model, l, x.double(), position_bias(model, 2, S) if wavlm else None)
-            rms = _rms_rel(got, ref)
-            upd = _rms_rel(got.double() - x.double(), ref - x.double())   # the layer's own contribution, not the stream
-            mx = ((got.double() - ref).abs().max() / ref.abs().max()).item()
+            rms, upd, mx = layer_metrics(got, x, ref)
             if upd > worst[0]:
                 worst = (upd, f"S {S} layer {l}, rms rel err {rms:.3e}, max |err| / max |ref| {mx:.3e}")
             assert rms <= RMS_CEIL["layer"], (name, S, l, rms)
             assert upd <= RMS_CEIL["layer_update"], (name, S, l, upd)
             assert mx <= 3 * RMS_CEIL["layer"], (name, S, l, mx)
     with capsys.disabled():
-        _report("layer", name, f"largest rms rel err of the update {worst[0]:.3e} ({worst[1]})")
+        report("w2v", "layer", name, f"largest rms rel err of the update {worst[0]:.3e} ({worst[1]})")
 
 
 # ------------------------------------------------------------------------------------------------ forward
-def tap_metrics(got, ref):
-    """(rms rel, centred rms rel, mean error / fluctuation rms) of [B, S, d] embeddings against float64"""
-    err = got.double() - ref
-    rms = (err.square().mean().sqrt() / ref.square().mean().sqrt()).item()
-    ec = err - err.mean(1, keepdim=True)
-    rc = ref - ref.mean(1, keepdim=True)
-    fl = rc.square().mean().sqrt()
-    centred = (ec.square().mean().sqrt() / fl).item()
-    mean_err = (err.mean(1).square().mean().sqrt() / fl).item()
-    return rms, centred, mean_err
-
-
 FWD_CASES = [(n, L) for n in ("w2v2-base", "hubert-large", "wavlm-base", "wavlm-large") for L in LENGTHS] + \
             [("MERT-v1-95M", L) for L in (600, 1079, 1080, 96000, 96015, 720000)]
 
@@ -483,7 +372,7 @@ def test_forward_taps_match_fp64(engine, name, L, capsys):
             assert centred <= RMS_CEIL["forward_c"], (k, centred)
             assert mean_err <= RMS_CEIL["forward_m"], (k, mean_err)
     with capsys.disabled():
-        _report("forward", f"{name} L {L}", "; ".join(lines))
+        report("w2v", "forward", f"{name} L {L}", "; ".join(lines))
 
 
 @pytest.mark.gpu
@@ -503,7 +392,7 @@ def test_long_file_reload_matches_fp64(engine, capsys):
             ref = ref_hidden_states(model, ref_normalize(pcm), False)[1]
         rms, centred, mean_err = tap_metrics(torch.as_tensor(np.asarray(g, dtype=np.float32)).cuda()[None], ref)
         with capsys.disabled():
-            _report("long", f"{len(c)} samples", f"rms {rms:.2e} centred {centred:.2e} mean/fluct {mean_err:.2e}")
+            report("w2v", "long", f"{len(c)} samples", f"rms {rms:.2e} centred {centred:.2e} mean/fluct {mean_err:.2e}")
         assert rms <= RMS_CEIL["forward"] and centred <= RMS_CEIL["forward_c"] and mean_err <= RMS_CEIL["forward_m"]
 
 
@@ -529,12 +418,10 @@ def _conv_call(**over):
     def call(engine, outs):
         a = dict(c=1, B=2, L=16000, x="ok", out="ok")
         a.update(over)
-        x = Guarded((2, 16000))
-        o = Guarded((2, 16000))
+        x = Guarded((2, 16000), torch.float32, "cuda", GUARD)
+        o = Guarded((2, 16000), torch.float32, "cuda", GUARD)
         outs.append(o)
-        xp = {"ok": x.body, "null": None, "odd": x.buf[x.guard + 1:]}[a["x"]]
-        op = {"ok": o.body, "null": None, "odd": o.buf[o.guard + 1:]}[a["out"]]
-        engine.w2v_conv(a["c"], xp, a["B"], a["L"], op)
+        engine.w2v_conv(a["c"], x.ptr(a["x"]), a["B"], a["L"], o.ptr(a["out"]))
     return call
 
 
@@ -542,15 +429,13 @@ def _stream_call(entry, **over):
     def call(engine, outs):
         a = dict(l=0, B=2, S=10, x="ok", out="ok")
         a.update(over)
-        x = Guarded((2, 10, 768), body=torch.zeros((2, 10, 768), device="cuda"))
-        o = Guarded((2, 10, 768))
+        x = Guarded((2, 10, 768), torch.float32, "cuda", GUARD, init=torch.zeros((2, 10, 768), device="cuda"))
+        o = Guarded((2, 10, 768), torch.float32, "cuda", GUARD)
         outs.append(o)
-        xp = {"ok": x.body, "null": None, "odd": x.buf[x.guard + 1:]}[a["x"]]
-        op = {"ok": o.body, "null": None, "odd": o.buf[o.guard + 1:]}[a["out"]]
         if entry == "layer":
-            engine.w2v_layer(a["l"], xp, a["B"], a["S"], op)
+            engine.w2v_layer(a["l"], x.ptr(a["x"]), a["B"], a["S"], o.ptr(a["out"]))
         else:
-            engine.w2v_posconv(xp, a["B"], a["S"], op)
+            engine.w2v_posconv(x.ptr(a["x"]), a["B"], a["S"], o.ptr(a["out"]))
     return call
 
 
@@ -559,22 +444,10 @@ def _normalize_call(**over):
         a = dict(n=2, L=400, out="ok")
         a.update(over)
         pcm = torch.zeros((2, 400), dtype=torch.int16, device="cuda")
-        o = Guarded((2, 400))
+        o = Guarded((2, 400), torch.float32, "cuda", GUARD)
         outs.append(o)
-        engine.w2v_normalize(pcm, a["n"], a["L"], o.body if a["out"] == "ok" else None)
+        engine.w2v_normalize(pcm, a["n"], a["L"], o.ptr(a["out"]))
     return call
-
-
-def _unloaded(call):
-    def run(engine, outs):
-        fresh = _native.Engine(engine.device, 16)
-        try:
-            launches = fresh.launches
-            call(fresh, outs)
-        finally:
-            assert fresh.launches == launches, "a rejected call launched a kernel"
-            fresh.close()
-    return run
 
 
 FRAMES_MAX = frames(32000)[7]
@@ -588,19 +461,19 @@ REJECT = [
     ("conv null x", _conv_call(x="null"), "fad_w2v_conv: null x or out"),
     ("conv misaligned x", _conv_call(x="odd"), "fad_w2v_conv: x and out must be 16-byte aligned"),
     ("conv misaligned out", _conv_call(c=0, out="odd"), "fad_w2v_conv: x and out must be 16-byte aligned"),
-    ("conv before any load", _unloaded(_conv_call()), "fad_w2v_conv: fad_w2v_load has not been called"),
+    ("conv before any load", on_fresh_engine(_conv_call()), "fad_w2v_conv: fad_w2v_load has not been called"),
     ("posconv S 0", _stream_call("posconv", S=0), "fad_w2v_posconv: S must be in [1, frames(max_len)]"),
     ("posconv S beyond max_len", _stream_call("posconv", S=FRAMES_MAX + 1), "fad_w2v_posconv: S must be in [1, frames(max_len)]"),
     ("posconv B beyond max_clips", _stream_call("posconv", B=MAX_CLIPS + 1), "fad_w2v_posconv: B must be in [1, max_clips]"),
     ("posconv misaligned out", _stream_call("posconv", out="odd"), "fad_w2v_posconv: x and out must be 16-byte aligned"),
-    ("posconv before any load", _unloaded(_stream_call("posconv")), "fad_w2v_posconv: fad_w2v_load has not been called"),
+    ("posconv before any load", on_fresh_engine(_stream_call("posconv")), "fad_w2v_posconv: fad_w2v_load has not been called"),
     ("layer l 2", _stream_call("layer", l=2), "fad_w2v_layer: l must be in [0, layers)"),
     ("layer l -1", _stream_call("layer", l=-1), "fad_w2v_layer: l must be in [0, layers)"),
     ("layer S beyond max_len", _stream_call("layer", S=FRAMES_MAX + 1), "fad_w2v_layer: S must be in [1, frames(max_len)]"),
     ("layer B beyond max_clips", _stream_call("layer", B=MAX_CLIPS + 1), "fad_w2v_layer: B must be in [1, max_clips]"),
     ("layer null x", _stream_call("layer", x="null"), "fad_w2v_layer: null x or out"),
     ("layer misaligned x", _stream_call("layer", x="odd"), "fad_w2v_layer: x and out must be 16-byte aligned"),
-    ("layer before any load", _unloaded(_stream_call("layer")), "fad_w2v_layer: fad_w2v_load has not been called"),
+    ("layer before any load", on_fresh_engine(_stream_call("layer")), "fad_w2v_layer: fad_w2v_load has not been called"),
     ("normalize no clips", _normalize_call(n=0), "fad_w2v_normalize: n_clips and L must be positive"),
     ("normalize L 0", _normalize_call(L=0), "fad_w2v_normalize: n_clips and L must be positive"),
     ("normalize null out", _normalize_call(out="null"), "fad_w2v_normalize: null pcm or out"),
@@ -612,14 +485,7 @@ REJECT = [
 def test_stage_entries_reject_invalid_arguments(engine, call, message):
     """Arguments the launch cannot honour fail with their message, launch nothing and write nothing."""
     load(engine, "w2v2-base", 32000)
-    outs = []
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
-        call(engine, outs)
-    torch.cuda.synchronize()
-    assert str(exc.value) == message
-    assert engine.launches == launches, "a rejected call launched a kernel"
-    assert all(o.untouched() for o in outs), "a rejected call wrote output"
+    expect_rejected(engine, call, message, [])
 
 
 # ------------------------------------------------------------------------------------------ CPU: the references

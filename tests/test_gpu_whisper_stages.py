@@ -23,13 +23,12 @@ Per-element bounds (float64, 1.001 margin; u = 2^-24):
     at -10), with m = max(mel, 1e-10) and dm = d mel + |1e-10f - 1e-10|, plus 2 ulp for log10f itself.
     The comparison is after the floor at clip_max - 8, as the model sees it: the floor is 1-Lipschitz, the clip max
     bound is the spread max(v +- b) - max(v), and an element surely under both floors is held to that spread alone.
-  * conv stem, pre-activation of a GEMM conv with K reduction columns, S = sum_j |w_j| |a_j|:
-        e = sum_j |w_j| e_a_j + (2^-21 + K 2^-23) S + 2^-25 (sum_j |w_j| + sum_j |a_j|) + 2^-24 (|b| + |y|)
-    with e_a the error of the operand the kernel reads: conv 0's features (max(x, c - 8) + 4) / 4 are fp32 (u |c - 8|
-    for the floor, u |x + 4| for the add) rounded to fp16 (2^-11 |a| + 2^-25); conv 1 reads conv 0's fp16 output
-    itself (e_a = 0).  2^-21 |w_j| is the fp16 hi/lo pair of the fp32 weight, K 2^-23 S the fp32 accumulation.
-  * GELU: 1.13 (its largest slope) times the error in front of it, + 2^-22 |y| for its fp32 evaluation; conv 0's fp16
-    output: + 2^-11 |y| + 2^-25; conv 1's fp32 add into the positional embedding: + 2^-24 |out|.
+  * conv stem, pre-activation: gpu_checks.gemm_bound (r_a = 0) + sum_j |w_j| e_a_j, with e_a the error of the operand
+    the kernel reads: conv 0's features (max(x, c - 8) + 4) / 4 are fp32 (u |c - 8| for the floor, u |x + 4| for the
+    add) rounded to fp16 (2^-11 |a| + 2^-25); conv 1 reads conv 0's fp16 output itself (e_a = 0).  K is 3 x 128 padded
+    mel channels for conv 0 and 3 d for conv 1.
+  * GELU: gpu_checks.gelu_out, conv 0 with its fp16 output; conv 1's fp32 add into the positional embedding:
+    + 2^-24 |out|.
 The layers (attention, LayerNorms, GEMMs with fp16 operands) and the taps are held to rms ceilings, about 3x the
 largest level measured on the H100 (RMS_CEIL below).  Each layer is also held on its update out - x, which the stream
 it adds to would otherwise hide.
@@ -42,12 +41,12 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from fadtk_b200 import _native, synth, weights_whisper as ww
+from fadtk_b200 import synth, weights_whisper as ww
+from gpu_checks import (Guarded, check_bound, expect_rejected, gelu_out, gemm_bound, layer_metrics, on_fresh_engine,
+                        report, report_stats, tap_metrics)
 from oracle import whisper_oracle as wo
 
 GUARD = 4096
-SENT32 = 0x7FC0FFEE                                      # fp32 NaNs the kernels never produce themselves
-SENT16 = 0x7D5A
 MAX_CLIPS = 4
 SIZES = list(ww.SIZES)
 SOT = ww.SYNTH_START
@@ -88,71 +87,6 @@ def load(engine, size, max_clips=MAX_CLIPS):
         sd = model_state(size)[0]
         engine.whisper_load(ww.config_of(sd), ww.pack_whisper(sd, SOT), max_clips)
         engine.owners["whisper"] = token
-
-
-# --------------------------------------------------------------------------------------------------- buffers
-class Guarded:
-    """A tensor of `shape` (fp32 or fp16) inside a sentinel-NaN buffer with `guard` elements on both sides."""
-
-    def __init__(self, shape, dtype=torch.float32, guard=GUARD, body=None):
-        self.n = math.prod(shape)
-        self.guard = guard
-        self.sent = SENT32 if dtype == torch.float32 else SENT16
-        self.buf = torch.empty(guard + self.n + guard, dtype=dtype, device="cuda")
-        self.raw().fill_(self.sent)
-        self.body = self.buf[guard:guard + self.n].view(shape)
-        if body is not None:
-            self.body.copy_(body)
-            self.init = self.body.clone()
-
-    def raw(self):
-        return self.buf.view(torch.int32 if self.buf.dtype == torch.float32 else torch.int16)
-
-    def guards_intact(self):
-        r = self.raw()
-        return bool((r[:self.guard] == self.sent).all()) and bool((r[self.guard + self.n:] == self.sent).all())
-
-    def check(self):
-        torch.cuda.synchronize()
-        assert self.guards_intact(), "guard region overwritten"
-        assert not bool((self.raw()[self.guard:self.guard + self.n] == self.sent).any()), "output elements left unwritten"
-        assert bool(torch.isfinite(self.body).all()), "non-finite output"
-        return self.body
-
-    def intact_input(self):
-        torch.cuda.synchronize()
-        return self.guards_intact() and bool(torch.equal(self.body, self.init))
-
-    def untouched(self):
-        return bool((self.raw() == self.sent).all())
-
-
-def _rms_rel(got, ref):
-    return ((got.double() - ref).square().mean().sqrt() / ref.square().mean().sqrt()).item()
-
-
-def _report(kind, what, line):
-    print(f"\n[whisper {kind}] {what}: {line}", flush=True)
-
-
-def check_bound(kind, what, got, ref, bound, stats):
-    err = (got.double() - ref).abs()
-    r = err / bound
-    ratio = r.max().item()
-    worst = int(r.flatten().argmax())
-    assert ratio <= 1.0, (f"{what}: max |err| / bound = {ratio:.3g} at flat index {worst} "
-                          f"(got {got.flatten()[worst].item()!r}, want {ref.flatten()[worst].item()!r})")
-    rms = _rms_rel(got, ref) if bool(ref.abs().max() > 0) else err.max().item()
-    st = stats.setdefault(kind, [0.0, 0.0, ""])
-    if rms > st[0]:
-        st[0], st[2] = rms, what
-    st[1] = max(st[1], ratio)
-
-
-def report_stats(capsys, stats, what):
-    with capsys.disabled():
-        for kind, (rms, ratio, w) in stats.items():
-            _report(kind, what, f"largest rms rel err {rms:.3e} ({w}), max err / bound {ratio:.3f}")
 
 
 # ------------------------------------------------------------------------------------------------- inputs
@@ -254,7 +188,7 @@ def features64(clips, device):
 def run_logmel(engine, clips):
     pcm, start, lens = upload(clips)
     n = len(clips)
-    out = Guarded((n * N_FRAMES * 80 + n,))
+    out = Guarded((n * N_FRAMES * 80 + n,), torch.float32, "cuda", GUARD)
     engine.whisper_logmel(pcm, start, lens, n, out.body)
     got = out.check()
     return got[:n * N_FRAMES * 80].view(n, N_FRAMES, 80), got[n * N_FRAMES * 80:]
@@ -289,8 +223,8 @@ def test_logmel_matches_fp64(engine, batch, capsys):
         assert (ck - c).abs().item() <= bc.item(), f"{what}: clip max {ck.item()!r}, want {c.item()!r} +- {bc.item():.3g}"
         fl = c - 8.0
         bound = torch.where(v - b > fl + bc, b, torch.where(v + b < fl - bc, bc.expand_as(b), torch.maximum(b, bc)))
-        check_bound("logmel", what, floored(raw[i].double(), ck), floored(v, c), bound, stats)
-    report_stats(capsys, stats, batch)
+        check_bound("logmel", what, floored(raw[i].double(), ck), floored(v, c), bound, stats, RMS_CEIL)
+    report_stats(capsys, "whisper", stats, batch)
 
 
 # ---------------------------------------------------------------------------------------------------- convs
@@ -307,24 +241,12 @@ def conv_mm(a, w, b, stride, pad):
     return y.transpose(1, 2)
 
 
-def gemm_bound(a, ea, w, b, stride, pad, y, K):
-    """pre-activation error bound of a GEMM conv (module docstring); a, ea [B, Cin, T] float64, w [Cout, Cin, k]"""
+def conv_sums(a, w, stride, pad):
+    """(S, sum |w|, sum |a|) of gpu_checks.gemm_bound for a GEMM conv; a [B, Cin, T] float64, w [Cout, Cin, k]"""
     S = conv_mm(a.abs(), w.abs(), None, stride, pad)
     ones = torch.ones((1, 1, w.shape[2]), dtype=a.dtype, device=a.device)
     sa = F.conv1d(F.pad(a.abs().sum(1, keepdim=True), (pad, pad)), ones, None, stride)
-    sw = w.abs().flatten(1).sum(1)[None, :, None]
-    e = (2.0 ** -21 + K * 2.0 ** -23) * S + 2.0 ** -25 * (sw + sa) + 2.0 ** -24 * (b.abs()[None, :, None] + y.abs())
-    if ea is not None:
-        e = e + conv_mm(ea, w.abs(), None, stride, pad)
-    return e
-
-
-def gelu_out(y, e, fp16):
-    out = F.gelu(y)
-    e = 1.13 * e + 2.0 ** -22 * out.abs()
-    if fp16:
-        e = e + 2.0 ** -11 * (out.abs() + e) + 2.0 ** -25
-    return out, e
+    return S, w.abs().flatten(1).sum(1)[None, :, None], sa
 
 
 @torch.no_grad()
@@ -336,7 +258,7 @@ def conv0_reference(model, raw, cmax):
     ea = 2.0 ** -11 * a.abs() + 2.0 ** -25 + (2.0 ** -11 + 1) * U * ((c - 8).abs() + (a * 4).abs()) / 4
     conv = model.encoder.conv1
     y = conv_mm(a, conv.weight, conv.bias, 1, 1)
-    e = gemm_bound(a, ea, conv.weight, conv.bias, 1, 1, y, 384)
+    e = gemm_bound(*conv_sums(a, conv.weight, 1, 1), 384, conv.bias, y) + conv_mm(ea, conv.weight.abs(), None, 1, 1)
     out, e = gelu_out(y, e, True)
     return out.transpose(1, 2), (e * 1.001).transpose(1, 2)
 
@@ -347,7 +269,7 @@ def conv1_reference(model, h1):
     a = h1.double().transpose(1, 2)
     conv = model.encoder.conv2
     y = conv_mm(a, conv.weight, conv.bias, 2, 1)
-    e = gemm_bound(a, None, conv.weight, conv.bias, 2, 1, y, 3 * a.shape[1])
+    e = gemm_bound(*conv_sums(a, conv.weight, 2, 1), 3 * a.shape[1], conv.bias, y)
     g, e = gelu_out(y, e, False)
     out = g.transpose(1, 2) + model.encoder.embed_positions.weight
     return out, (e.transpose(1, 2) + 2.0 ** -24 * out.abs()) * 1.001
@@ -356,13 +278,14 @@ def conv1_reference(model, h1):
 def run_stem(engine, d, raw, cmax):
     """kernel raw log-mel -> (conv 0 output fp16 [B, 3000, d], conv 1 output fp32 [B, 1500, d]), guarded"""
     B = raw.shape[0]
-    xin, cin = Guarded(raw.shape, body=raw), Guarded(cmax.shape, body=cmax)
-    h1 = Guarded((B, N_FRAMES, d), torch.float16)
+    xin = Guarded(raw.shape, torch.float32, "cuda", GUARD, init=raw)
+    cin = Guarded(cmax.shape, torch.float32, "cuda", GUARD, init=cmax)
+    h1 = Guarded((B, N_FRAMES, d), torch.float16, "cuda", GUARD)
     engine.whisper_conv(0, xin.body, cin.body, B, h1.body)
     got0 = h1.check()
     assert xin.intact_input() and cin.intact_input(), "the input or its guard was modified"
-    hin = Guarded(got0.shape, torch.float16, body=got0)
-    x = Guarded((B, SEQ, d))
+    hin = Guarded(got0.shape, torch.float16, "cuda", GUARD, init=got0)
+    x = Guarded((B, SEQ, d), torch.float32, "cuda", GUARD)
     engine.whisper_conv(1, hin.body, None, B, x.body)
     got1 = x.check()
     assert hin.intact_input(), "the input or its guard was modified"
@@ -383,9 +306,9 @@ def test_conv_stem_matches_fp64(engine, size, capsys):
     ref0, b0 = conv0_reference(model, raw, cmax)
     ref1, b1 = conv1_reference(model, h1)
     for i, (kind, n) in enumerate(STAGE_CLIPS):
-        check_bound("conv0", f"{size} {kind} {n}", h1[i], ref0[i], b0[i], stats)
-        check_bound("conv1", f"{size} {kind} {n}", x[i], ref1[i], b1[i], stats)
-    report_stats(capsys, stats, size)
+        check_bound("conv0", f"{size} {kind} {n}", h1[i], ref0[i], b0[i], stats, RMS_CEIL)
+        check_bound("conv1", f"{size} {kind} {n}", x[i], ref1[i], b1[i], stats, RMS_CEIL)
+    report_stats(capsys, "whisper", stats, size)
 
 
 # ------------------------------------------------------------------------------------------------- layers
@@ -406,14 +329,6 @@ def dec_layer_ref(model, l, xd, enc):
     return out[0] if isinstance(out, tuple) else out
 
 
-def layer_metrics(got, x, ref):
-    """(rms rel of the output, rms rel of the update out - x, max |err| / max |ref|)"""
-    rms = _rms_rel(got, ref)
-    upd = _rms_rel(got.double() - x.double(), ref - x.double())
-    mx = ((got.double() - ref).abs().max() / ref.abs().max()).item()
-    return rms, upd, mx
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("size", SIZES)
 def test_encoder_layers_match_fp64(engine, size, capsys):
@@ -426,8 +341,8 @@ def test_encoder_layers_match_fp64(engine, size, capsys):
     B = x.shape[0]
     lines = []
     for l in range(model.config.encoder_layers):
-        xin = Guarded(x.shape, body=x)
-        out = Guarded(x.shape)
+        xin = Guarded(x.shape, torch.float32, "cuda", GUARD, init=x)
+        out = Guarded(x.shape, torch.float32, "cuda", GUARD)
         engine.whisper_enc_layer(l, xin.body, B, out.body)
         got = out.check()
         assert xin.intact_input(), "the input or its guard was modified"
@@ -439,12 +354,12 @@ def test_encoder_layers_match_fp64(engine, size, capsys):
             (size, l, rms, upd, mx)
         x = got.clone()
     with capsys.disabled():
-        _report("enc_layer", size, "; ".join(lines))
+        report("whisper", "enc_layer", size, "; ".join(lines))
 
 
 def run_encode(engine, clips, d):
     pcm, start, lens = upload(clips)
-    out = Guarded((len(clips), SEQ, d), torch.float16)
+    out = Guarded((len(clips), SEQ, d), torch.float16, "cuda", GUARD)
     engine.whisper_encode(pcm, start, lens, len(clips), out.body)
     return out.check()
 
@@ -462,11 +377,11 @@ def test_decoder_layers_match_fp64(engine, size, capsys):
     enc = run_encode(engine, clips, d)
     x0 = sd["decoder.embed_tokens.weight"][SOT][None, :] + sd["decoder.embed_positions.weight"][:2]
     xd = x0.float().cuda()[None].repeat(B, 1, 1).contiguous()
-    ein = Guarded(enc.shape, torch.float16, body=enc)
+    ein = Guarded(enc.shape, torch.float16, "cuda", GUARD, init=enc)
     lines = []
     for l in range(model.config.decoder_layers):
-        xin = Guarded(xd.shape, body=xd)
-        out = Guarded(xd.shape)
+        xin = Guarded(xd.shape, torch.float32, "cuda", GUARD, init=xd)
+        out = Guarded(xd.shape, torch.float32, "cuda", GUARD)
         engine.whisper_dec_layer(l, xin.body, ein.body, B, out.body)
         got = out.check()
         assert xin.intact_input() and ein.intact_input(), "an input or its guard was modified"
@@ -478,20 +393,10 @@ def test_decoder_layers_match_fp64(engine, size, capsys):
             (size, l, rms, upd, mx)
         xd = got.clone()
     with capsys.disabled():
-        _report("dec_layer", size, "; ".join(lines))
+        report("whisper", "dec_layer", size, "; ".join(lines))
 
 
 # ------------------------------------------------------------------------------------------------ taps
-def tap_metrics(got, ref):
-    """(rms rel, centred rms rel) of [B, S, d] outputs against float64; centred: the per-(clip, channel) mean over
-    positions removed from error and reference"""
-    err = got.double() - ref
-    rms = (err.square().mean().sqrt() / ref.square().mean().sqrt()).item()
-    ec = err - err.mean(1, keepdim=True)
-    rc = ref - ref.mean(1, keepdim=True)
-    return rms, (ec.square().mean().sqrt() / rc.square().mean().sqrt()).item()
-
-
 TAP_SECONDS = [1.0, 10.0, 30.0, 31.0]
 TAP_CASES = [(s, sec) for s in SIZES for sec in TAP_SECONDS]
 
@@ -515,10 +420,10 @@ def test_encode_and_forward_match_fp64(engine, size, sec, capsys):
     fwd = engine.whisper_forward(*upload(clips))
     torch.cuda.synchronize()
     assert fwd.shape == (len(clips), 2, d) and bool(torch.isfinite(fwd).all())
-    er, ec = tap_metrics(enc, enc_ref)
-    fr, fc = tap_metrics(fwd, fwd_ref)
+    er, ec, _ = tap_metrics(enc, enc_ref)
+    fr, fc, _ = tap_metrics(fwd, fwd_ref)
     with capsys.disabled():
-        _report("taps", f"{size} {sec:g} s", f"encode rms {er:.2e} centred {ec:.2e}; forward rms {fr:.2e} centred {fc:.2e}")
+        report("whisper", "taps", f"{size} {sec:g} s", f"encode rms {er:.2e} centred {ec:.2e}; forward rms {fr:.2e} centred {fc:.2e}")
     assert er <= RMS_CEIL["encode"] and ec <= RMS_CEIL["encode_c"], (er, ec)
     assert fr <= RMS_CEIL["forward"] and fc <= RMS_CEIL["forward_c"], (fr, fc)
 
@@ -547,19 +452,15 @@ def test_outputs_independent_of_batch(engine, size):
 D_TINY = 384
 
 
-def _ptr_of(g, kind):
-    return {"ok": g.body, "null": None, "odd": g.buf[g.guard + 1:]}[kind]
-
-
 def _conv_call(**over):
     def call(engine, outs):
         a = dict(c=1, B=2, x="ok", cmax="ok", out="ok")
         a.update(over)
-        x = Guarded((2, N_FRAMES, D_TINY))
-        cm = Guarded((2,))
-        o = Guarded((2, N_FRAMES, D_TINY))
+        x = Guarded((2, N_FRAMES, D_TINY), torch.float32, "cuda", GUARD)
+        cm = Guarded((2,), torch.float32, "cuda", GUARD)
+        o = Guarded((2, N_FRAMES, D_TINY), torch.float32, "cuda", GUARD)
         outs.extend([o, cm])
-        engine.whisper_conv(a["c"], _ptr_of(x, a["x"]), _ptr_of(cm, a["cmax"]), a["B"], _ptr_of(o, a["out"]))
+        engine.whisper_conv(a["c"], x.ptr(a["x"]), cm.ptr(a["cmax"]), a["B"], o.ptr(a["out"]))
     return call
 
 
@@ -567,10 +468,10 @@ def _enc_layer_call(**over):
     def call(engine, outs):
         a = dict(l=0, B=2, x="ok", out="ok")
         a.update(over)
-        x = Guarded((2, SEQ, D_TINY), body=torch.zeros((2, SEQ, D_TINY), device="cuda"))
-        o = Guarded((2, SEQ, D_TINY))
+        x = Guarded((2, SEQ, D_TINY), torch.float32, "cuda", GUARD, init=torch.zeros((2, SEQ, D_TINY), device="cuda"))
+        o = Guarded((2, SEQ, D_TINY), torch.float32, "cuda", GUARD)
         outs.append(o)
-        engine.whisper_enc_layer(a["l"], _ptr_of(x, a["x"]), a["B"], _ptr_of(o, a["out"]))
+        engine.whisper_enc_layer(a["l"], x.ptr(a["x"]), a["B"], o.ptr(a["out"]))
     return call
 
 
@@ -578,11 +479,11 @@ def _dec_layer_call(**over):
     def call(engine, outs):
         a = dict(l=0, B=2, x="ok", enc="ok", out="ok")
         a.update(over)
-        x = Guarded((2, 2, D_TINY), body=torch.zeros((2, 2, D_TINY), device="cuda"))
-        e = Guarded((2, SEQ, D_TINY), torch.float16, body=torch.zeros((2, SEQ, D_TINY), device="cuda"))
-        o = Guarded((2, 2, D_TINY))
+        x = Guarded((2, 2, D_TINY), torch.float32, "cuda", GUARD, init=torch.zeros((2, 2, D_TINY), device="cuda"))
+        e = Guarded((2, SEQ, D_TINY), torch.float16, "cuda", GUARD, init=torch.zeros((2, SEQ, D_TINY), device="cuda"))
+        o = Guarded((2, 2, D_TINY), torch.float32, "cuda", GUARD)
         outs.append(o)
-        engine.whisper_dec_layer(a["l"], _ptr_of(x, a["x"]), _ptr_of(e, a["enc"]), a["B"], _ptr_of(o, a["out"]))
+        engine.whisper_dec_layer(a["l"], x.ptr(a["x"]), e.ptr(a["enc"]), a["B"], o.ptr(a["out"]))
     return call
 
 
@@ -592,27 +493,15 @@ def _clips_call(entry, **over):
         a.update(over)
         pcm, start, lens = upload([make_clip("noise", 1600), make_clip("noise", 800)])
         if entry == "encode":
-            o = Guarded((2, SEQ, D_TINY), torch.float16)
+            o = Guarded((2, SEQ, D_TINY), torch.float16, "cuda", GUARD)
             fn = engine.whisper_encode
         else:
-            o = Guarded((2 * N_FRAMES * 80 + 2,))
+            o = Guarded((2 * N_FRAMES * 80 + 2,), torch.float32, "cuda", GUARD)
             fn = engine.whisper_logmel
         outs.append(o)
         fn(pcm if a["pcm"] == "ok" else None, start if a["start"] == "ok" else None, lens, a["n"],
-           o.body if a["out"] == "ok" else None)
+           o.ptr(a["out"]))
     return call
-
-
-def _unloaded(call):
-    def run(engine, outs):
-        fresh = _native.Engine(engine.device, 16)
-        try:
-            launches = fresh.launches
-            call(fresh, outs)
-        finally:
-            assert fresh.launches == launches, "a rejected call launched a kernel"
-            fresh.close()
-    return run
 
 
 REJECT = [
@@ -625,28 +514,28 @@ REJECT = [
     ("conv misaligned x", _conv_call(x="odd"), "fad_whisper_conv: x and out must be 16-byte aligned"),
     ("conv misaligned out", _conv_call(c=0, out="odd"), "fad_whisper_conv: x and out must be 16-byte aligned"),
     ("conv 0 null clip_max", _conv_call(c=0, cmax="null"), "fad_whisper_conv: c = 0 needs a 4-byte aligned clip_max"),
-    ("conv before any load", _unloaded(_conv_call()), "fad_whisper_conv: fad_whisper_load has not been called"),
+    ("conv before any load", on_fresh_engine(_conv_call()), "fad_whisper_conv: fad_whisper_load has not been called"),
     ("enc layer l 4", _enc_layer_call(l=4), "fad_whisper_enc_layer: l must be in [0, enc_layers)"),
     ("enc layer l -1", _enc_layer_call(l=-1), "fad_whisper_enc_layer: l must be in [0, enc_layers)"),
     ("enc layer B beyond max_clips", _enc_layer_call(B=MAX_CLIPS + 1), "fad_whisper_enc_layer: B must be in [1, max_clips]"),
     ("enc layer null out", _enc_layer_call(out="null"), "fad_whisper_enc_layer: null x or out"),
     ("enc layer misaligned x", _enc_layer_call(x="odd"), "fad_whisper_enc_layer: x and out must be 16-byte aligned"),
-    ("enc layer before any load", _unloaded(_enc_layer_call()), "fad_whisper_enc_layer: fad_whisper_load has not been called"),
+    ("enc layer before any load", on_fresh_engine(_enc_layer_call()), "fad_whisper_enc_layer: fad_whisper_load has not been called"),
     ("dec layer l 4", _dec_layer_call(l=4), "fad_whisper_dec_layer: l must be in [0, dec_layers)"),
     ("dec layer B 0", _dec_layer_call(B=0), "fad_whisper_dec_layer: B must be in [1, max_clips]"),
     ("dec layer null x", _dec_layer_call(x="null"), "fad_whisper_dec_layer: null x or out"),
     ("dec layer misaligned out", _dec_layer_call(out="odd"), "fad_whisper_dec_layer: x and out must be 16-byte aligned"),
     ("dec layer null enc_out", _dec_layer_call(enc="null"), "fad_whisper_dec_layer: enc_out must be a 16-byte aligned pointer"),
     ("dec layer misaligned enc_out", _dec_layer_call(enc="odd"), "fad_whisper_dec_layer: enc_out must be a 16-byte aligned pointer"),
-    ("dec layer before any load", _unloaded(_dec_layer_call()), "fad_whisper_dec_layer: fad_whisper_load has not been called"),
+    ("dec layer before any load", on_fresh_engine(_dec_layer_call()), "fad_whisper_dec_layer: fad_whisper_load has not been called"),
     ("encode no clips", _clips_call("encode", n=0), "fad_whisper_encode: n_clips must be positive"),
     ("encode null pcm", _clips_call("encode", pcm="null"), "fad_whisper_encode: null pcm, clip_start, clip_len or out"),
     ("encode null out", _clips_call("encode", out="null"), "fad_whisper_encode: null pcm, clip_start, clip_len or out"),
-    ("encode before any load", _unloaded(_clips_call("encode")), "fad_whisper_encode: fad_whisper_load has not been called"),
+    ("encode before any load", on_fresh_engine(_clips_call("encode")), "fad_whisper_encode: fad_whisper_load has not been called"),
     ("logmel no clips", _clips_call("logmel", n=0), "fad_whisper_logmel: n_clips must be positive"),
     ("logmel null clip_start", _clips_call("logmel", start="null"), "fad_whisper_logmel: null pcm, clip_start, clip_len or out"),
     ("logmel null out", _clips_call("logmel", out="null"), "fad_whisper_logmel: null pcm, clip_start, clip_len or out"),
-    ("logmel before any load", _unloaded(_clips_call("logmel")), "fad_whisper_logmel: fad_whisper_load has not been called"),
+    ("logmel before any load", on_fresh_engine(_clips_call("logmel")), "fad_whisper_logmel: fad_whisper_load has not been called"),
 ]
 
 
@@ -655,14 +544,7 @@ REJECT = [
 def test_stage_entries_reject_invalid_arguments(engine, call, message):
     """Arguments the launch cannot honour fail with their message, launch nothing and write nothing."""
     load(engine, "tiny")
-    outs = []
-    launches = engine.launches
-    with pytest.raises(_native.NativeError) as exc:
-        call(engine, outs)
-    torch.cuda.synchronize()
-    assert str(exc.value) == message
-    assert engine.launches == launches, "a rejected call launched a kernel"
-    assert all(o.untouched() for o in outs), "a rejected call wrote output"
+    expect_rejected(engine, call, message, [])
 
 
 # ------------------------------------------------------------------------------------------ CPU: the references
