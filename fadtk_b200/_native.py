@@ -52,6 +52,10 @@ SIGNATURES = {
     "fad_clap_plan_frames": (c_ll, [c_vp, c_ll, c_vp, c_vp, c_vp, c_ll, c_vp]),
     "fad_clap_forward": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_ll, c_vp, c_vp]),
     "fad_clap_logmel": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, c_vp, c_vp]),
+    "fad_clap_patch_embed": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, c_vp, c_vp]),
+    "fad_clap_block": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, c_vp, c_vp]),
+    "fad_clap_merge": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, c_vp, c_vp]),
+    "fad_clap_head": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_stats_acc_len": (C.c_size_t, [C.c_int]),
     "fad_stats_accumulate": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp, C.c_int, c_vp]),
     "fad_stats_accumulate_gather": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
@@ -413,6 +417,41 @@ class Engine:
                                      plan_dev["pool_valid"].data_ptr(), plan_dev["pool_frame"].data_ptr(), n_pool,
                                      pool.data_ptr(), _stream()))
         return pool[plan_dev["frame_index"].long()]
+
+    # Stage entries of the loaded CLAP model: they write into the caller's cuda tensors (shapes in
+    # include/fadtk_b200.h) and raise NativeError on rejected arguments.
+    def clap_pool(self, pcm, pool_start, pool_valid, pool_frame, n_pool: int, out):
+        """fad_clap_logmel: out fp32 [n_pool, 64], the BatchNorm-ed log-mel row of every frame-pool entry"""
+        _check(lib().fad_clap_logmel(self._h, _ptr(pcm), _ptr(pool_start), _ptr(pool_valid), _ptr(pool_frame),
+                                     int(n_pool), _ptr(out), _stream()))
+        return out
+
+    def clap_patch_embed(self, pool, n_pool: int, frame_index, B: int, out):
+        """fad_clap_patch_embed: pool fp32 [n_pool, 64], frame_index int32 [B, 1001] -> out fp32 [B, 4096, E]"""
+        _check(lib().fad_clap_patch_embed(self._h, _ptr(pool), int(n_pool), _ptr(frame_index), int(B), _ptr(out),
+                                          _stream()))
+        return out
+
+    def clap_block(self, blk: int, x, B: int, out):
+        """fad_clap_block: Swin block blk, x fp32 [B, res^2, C] -> out fp32 [B, res^2, C]"""
+        _check(lib().fad_clap_block(self._h, int(blk), _ptr(x), int(B), _ptr(out), _stream()))
+        return out
+
+    def clap_merge(self, s: int, x, B: int, out):
+        """fad_clap_merge: patch merge s, x fp32 [B, res^2, C] -> out fp32 [B, res^2 / 4, 2 C]"""
+        _check(lib().fad_clap_merge(self._h, int(s), _ptr(x), int(B), _ptr(out), _stream()))
+        return out
+
+    def clap_head(self, x, B: int, out):
+        """fad_clap_head: x fp32 [B, 64, 8 E] -> out fp16 [B, 512]"""
+        _check(lib().fad_clap_head(self._h, _ptr(x), int(B), _ptr(out), _stream()))
+        return out
+
+    def clap_forward_raw(self, pcm, pool_start, pool_valid, pool_frame, n_pool: int, frame_index, n_chunks: int, out):
+        """fad_clap_forward with every pointer and count as given (None -> NULL)"""
+        _check(lib().fad_clap_forward(self._h, _ptr(pcm), _ptr(pool_start), _ptr(pool_valid), _ptr(pool_frame),
+                                      int(n_pool), _ptr(frame_index), int(n_chunks), _ptr(out), _stream()))
+        return out
 
     # ------------------------------------------------------------------ Whisper
     def whisper_load(self, cfg: tuple, tensors: list, max_clips: int = 16):

@@ -136,6 +136,22 @@ int fad_clap_forward(fad_handle* h, const int16_t* pcm, const long long* pool_st
 /* stage entry point: BatchNorm-ed log-mel rows [n_pool, 64] fp32 */
 int fad_clap_logmel(fad_handle* h, const int16_t* pcm, const long long* pool_start, const int* pool_valid,
                     const int* pool_frame, long long n_pool, float* out, void* stream);
+/* Stage entries of the loaded CLAP model (parity tests), each calling the launch code of fad_clap_forward and
+ * failing, before launching or writing anything, on arguments it could not honour; so do fad_clap_logmel and
+ * fad_clap_forward (n_pool, n_chunks >= 0; a pointer may be NULL only when its count is 0).  B in [1, max_chunks];
+ * device pointers the kernels read or write aligned to their element size (the streams x / out are only copied and
+ * may have any alignment).  E = 96 (HTSAT-tiny) or 128 (HTSAT-base); the stream entering
+ * stage s is [B][res^2][C] with res = 64 >> s, C = E << s.
+ * fad_clap_patch_embed: pool fp32 [n_pool][64] (fad_clap_logmel's rows), frame_index [B][1001] with every value in
+ * [0, n_pool) (not checked: it lives on the device) -> x_out fp32 [B][4096][E].
+ * fad_clap_block: Swin block blk in [0, 12 | 18) (stage-major), x fp32 [B][res^2][C] -> out fp32 [B][res^2][C].
+ * fad_clap_merge: patch merge s in {0, 1, 2}, x fp32 [B][res^2][C] -> out fp32 [B][res^2 / 4][2 C].
+ * fad_clap_head: x fp32 [B][64][8 E] -> out fp16 [B][512], L2-normalised. */
+int fad_clap_patch_embed(fad_handle* h, const float* pool, long long n_pool, const int* frame_index, long long B,
+                         float* x_out, void* stream);
+int fad_clap_block(fad_handle* h, int blk, const float* x, long long B, float* out, void* stream);
+int fad_clap_merge(fad_handle* h, int s, const float* x, long long B, float* out, void* stream);
+int fad_clap_head(fad_handle* h, const float* x, long long B, void* out_f16, void* stream);
 
 /* ---- Whisper: replaces WhisperModel.load_model / _get_embedding (fadtk/model_loader.py:657-669):
  * WhisperFeatureExtractor (clip padded / truncated to 30 s, log-mel 80 x 3000) and

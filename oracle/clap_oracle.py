@@ -111,8 +111,9 @@ def log_mel(chunks: torch.Tensor) -> torch.Tensor:
 
 
 # ------------------------------------------------------------------------------- network
-def _rel_pos_index(ws: int = WINDOW) -> torch.Tensor:
-    coords = torch.stack(torch.meshgrid(torch.arange(ws), torch.arange(ws), indexing="ij")).flatten(1)
+def _rel_pos_index(ws: int = WINDOW, device=None) -> torch.Tensor:
+    ar = torch.arange(ws, device=device)
+    coords = torch.stack(torch.meshgrid(ar, ar, indexing="ij")).flatten(1)
     rel = (coords[:, :, None] - coords[:, None, :]).permute(1, 2, 0).contiguous()
     rel[:, :, 0] += ws - 1
     rel[:, :, 1] += ws - 1
@@ -120,8 +121,8 @@ def _rel_pos_index(ws: int = WINDOW) -> torch.Tensor:
     return rel.sum(-1)                                                # [64, 64]
 
 
-def _shift_mask(h: int, w: int, ws: int, shift: int) -> torch.Tensor:
-    img = torch.zeros((1, h, w, 1))
+def _shift_mask(h: int, w: int, ws: int, shift: int, device=None, dtype=torch.float32) -> torch.Tensor:
+    img = torch.zeros((1, h, w, 1), device=device, dtype=dtype)
     cnt = 0
     for hs in (slice(0, -ws), slice(-ws, -shift), slice(-shift, None)):
         for wsl in (slice(0, -ws), slice(-ws, -shift), slice(-shift, None)):
@@ -167,10 +168,10 @@ def swin_block(x, sd, pre, res, heads, shift):
     k = _lin(win, sd, pre + "attention.self.key").view(-1, ws * ws, heads, hd).transpose(1, 2)
     v = _lin(win, sd, pre + "attention.self.value").view(-1, ws * ws, heads, hd).transpose(1, 2)
     att = q @ k.transpose(-1, -2) / math.sqrt(hd)
-    bias = sd[pre + "attention.self.relative_position_bias_table"][_rel_pos_index().view(-1)]
+    bias = sd[pre + "attention.self.relative_position_bias_table"][_rel_pos_index(device=x.device).view(-1)]
     att = att + bias.view(ws * ws, ws * ws, heads).permute(2, 0, 1).unsqueeze(0)
     if shift:
-        mask = _shift_mask(h, w, ws, shift)
+        mask = _shift_mask(h, w, ws, shift, x.device, x.dtype)
         att = att.view(-1, mask.shape[0], heads, ws * ws, ws * ws) + mask.unsqueeze(1).unsqueeze(0)
         att = att.view(-1, heads, ws * ws, ws * ws)
     ctx = (att.softmax(-1) @ v).permute(0, 2, 1, 3).reshape(-1, ws * ws, c)
@@ -191,11 +192,15 @@ def patch_merge(x, sd, pre, res):
     return F.linear(x, sd[pre + "reduction.weight"])
 
 
-def mel_to_image(lm: torch.Tensor, sd: dict) -> torch.Tensor:
-    """[B, 1001, 64] log-mel -> BatchNorm over mel bins -> bicubic time resize to 1024 ->
-    fold four 256-frame blocks along frequency -> [B, 1, 256, 256]."""
+def batch_norm(lm: torch.Tensor, sd: dict) -> torch.Tensor:
+    """[B, 1001, 64] log-mel -> BatchNorm (eval) over mel bins"""
     x = (lm - sd["batch_norm.running_mean"]) / torch.sqrt(sd["batch_norm.running_var"] + 1e-5)
-    x = x * sd["batch_norm.weight"] + sd["batch_norm.bias"]
+    return x * sd["batch_norm.weight"] + sd["batch_norm.bias"]
+
+
+def fold_image(x: torch.Tensor) -> torch.Tensor:
+    """[B, 1001, 64] BatchNorm-ed log-mel -> bicubic time resize to 1024 -> fold four 256-frame blocks along
+    frequency -> [B, 1, 256, 256]."""
     x = x[:, None]                                                     # [B,1,T,F]
     x = F.interpolate(x, (SPEC * 4, N_MEL), mode="bicubic", align_corners=True)
     b = x.shape[0]
@@ -203,12 +208,29 @@ def mel_to_image(lm: torch.Tensor, sd: dict) -> torch.Tensor:
     return x.reshape(b, 1, 4 * N_MEL, SPEC)
 
 
+def mel_to_image(lm: torch.Tensor, sd: dict) -> torch.Tensor:
+    """[B, 1001, 64] log-mel -> BatchNorm over mel bins -> bicubic time resize to 1024 ->
+    fold four 256-frame blocks along frequency -> [B, 1, 256, 256]."""
+    return fold_image(batch_norm(lm, sd))
+
+
+def image_tokens(img: torch.Tensor, sd: dict) -> torch.Tensor:
+    """[B, 1, 256, 256] -> 4x4/4 conv -> LayerNorm -> the residual stream entering block 0 [B, 4096, E]"""
+    x = F.conv2d(img, sd["patch_embed.proj.weight"], sd["patch_embed.proj.bias"], stride=4)
+    return _ln(x.flatten(2).transpose(1, 2), sd, "patch_embed.norm")
+
+
+def head(x: torch.Tensor, sd: dict) -> torch.Tensor:
+    """the stream leaving the last block [B, 64, 8 E] -> final LayerNorm, token mean, projection, L2 norm [B, 512]"""
+    x = _ln(x, sd, "norm").mean(1)                                     # token average -> [B, 8 E]
+    x = _lin(F.relu(_lin(x, sd, "audio_projection.linear1")), sd, "audio_projection.linear2")
+    return F.normalize(x, dim=-1)
+
+
 @torch.no_grad()
 def network(lm: torch.Tensor, sd: dict) -> torch.Tensor:
-    """[B, 1001, 64] float32 log-mel -> [B, 512] L2-normalised embedding (float32, CPU)."""
-    img = mel_to_image(lm, sd)
-    x = F.conv2d(img, sd["patch_embed.proj.weight"], sd["patch_embed.proj.bias"], stride=4)
-    x = _ln(x.flatten(2).transpose(1, 2), sd, "patch_embed.norm")      # [B, 4096, 96]
+    """[B, 1001, 64] log-mel -> [B, 512] L2-normalised embedding, in the dtype and on the device of lm and sd."""
+    x = image_tokens(mel_to_image(lm, sd), sd)                         # [B, 4096, 96]
     res = SPEC // 4
     _, depths = config_of(sd)
     for i, (depth, heads) in enumerate(zip(depths, HEADS)):
@@ -217,9 +239,7 @@ def network(lm: torch.Tensor, sd: dict) -> torch.Tensor:
         if i < len(depths) - 1:
             x = patch_merge(x, sd, f"layers.{i}.downsample.", res)
             res //= 2
-    x = _ln(x, sd, "norm").mean(1)                                     # token average -> [B, 768]
-    x = _lin(F.relu(_lin(x, sd, "audio_projection.linear1")), sd, "audio_projection.linear2")
-    return F.normalize(x, dim=-1)
+    return head(x, sd)
 
 
 @torch.no_grad()
