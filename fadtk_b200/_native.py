@@ -107,6 +107,8 @@ SIGNATURES = {
     "fad_kad_shard_plan": (C.c_int, [c_vp, c_ll, C.c_int, c_vp]),
     "fad_knn_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_prdc_counts": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "fad_knn_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_prdc_counts_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -771,6 +773,14 @@ class Engine:
                                       out.data_ptr(), _stream()))
         return out
 
+    def knn_radii_sq_sharded(self, z: torch.Tensor, m: int, k: int, local_shards: int = 0) -> torch.Tensor:
+        """fad_knn_radii_sq_sharded: knn_radii_sq over shards (local_shards as for kad_sums_sharded)"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
+        _check(lib().fad_knn_radii_sq_sharded(self._h, None, int(local_shards), z.data_ptr(), int(m), z.shape[0] - int(m),
+                                              z.shape[1], int(k), out.data_ptr(), _stream()))
+        return out
+
     def prdc_counts(self, z: torch.Tensor, m: int, radii_sq: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
         """z fp16 [m + n, d] (cuda, X rows first), radii_sq fp32 [m + n] (cuda) -> (inside int32 [n], flags uint8 [m])
         (cuda): the number of baseline balls that contain each y_j, and per x_i bit 0 = covered, bit 1 = recalled
@@ -783,6 +793,19 @@ class Engine:
         flags = torch.empty(max(int(m), 0), dtype=torch.uint8, device=z.device)
         _check(lib().fad_prdc_counts(self._h, z.data_ptr(), int(m), n, z.shape[1], radii_sq.data_ptr(),
                                      inside.data_ptr(), flags.data_ptr(), _stream()))
+        return inside, flags
+
+    def prdc_counts_sharded(self, z: torch.Tensor, m: int, radii_sq: torch.Tensor,
+                            local_shards: int = 0) -> tuple[torch.Tensor, torch.Tensor]:
+        """fad_prdc_counts_sharded: prdc_counts over shards (local_shards as for kad_sums_sharded)"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert radii_sq.dtype == torch.float32 and radii_sq.is_cuda and radii_sq.is_contiguous()
+        assert radii_sq.shape == (z.shape[0],)
+        n = z.shape[0] - int(m)
+        inside = torch.empty(max(n, 0), dtype=torch.int32, device=z.device)
+        flags = torch.empty(max(int(m), 0), dtype=torch.uint8, device=z.device)
+        _check(lib().fad_prdc_counts_sharded(self._h, None, int(local_shards), z.data_ptr(), int(m), n, z.shape[1],
+                                             radii_sq.data_ptr(), inside.data_ptr(), flags.data_ptr(), _stream()))
         return inside, flags
 
 

@@ -1239,31 +1239,40 @@ std::vector<long long> kad_pair_unit_tiles(int T) {
     return t;
 }
 
-// the arguments of a collective call, compared across the ranks before any tile work
-constexpr int kKadArgs = 8;
-const char* const kKadArgNames[kKadArgs] = {"ok", "m", "n", "d", "n_items", "offsets", "sigma", "z"};
-enum { kArgOk, kArgM, kArgN, kArgD, kArgItems, kArgOffsets, kArgSigma, kArgZ };
+// the arguments of a collective call, compared across the ranks before any tile work (k and radii: PRDC's; 0 in KAD)
+constexpr int kKadArgs = 10;
+const char* const kKadArgNames[kKadArgs] = {"ok", "m", "n", "d", "n_items", "offsets", "sigma", "z", "k", "radii"};
+enum { kArgOk, kArgM, kArgN, kArgD, kArgItems, kArgOffsets, kArgSigma, kArgZ, kArgK, kArgRadii };
+
+// *out = the digest (kad_digest_kernel) of n_vec words W at x
+template <typename W>
+int kad_digest(fad_handle* h, const W* x, long long n_vec, unsigned long long* out, cudaStream_t st) {
+    CK(cudaMemsetAsync(out, 0, 8, st));
+    return launch(h, fad::kad_digest_kernel<W>, (unsigned)std::min<long long>((n_vec + 255) / 256, 4LL * h->num_sms), 256,
+                  0, st, x, n_vec, out);
+}
 
 // bad: this rank's own checks rejected the call (g_err says why).  Local: fail with that.  Collective: every rank takes
-// part whatever its own checks said.  The digest of z (rows x d fp16) and the bits of *sigma complete args, then one
-// all-reduce (max over the values and their complements) gives each value's max and min on every rank; a rank that
-// rejected its arguments or any value that differs fails the call on every rank with the same message.
+// part whatever its own checks said.  The digest of z (rows x d fp16), the bits of *sigma and the digest of radii
+// (n_radii fp32, when given) complete args, then one all-reduce (max over the values and their complements) gives each
+// value's max and min on every rank; a rank that rejected its arguments or any value that differs fails the call on
+// every rank with the same message.
 int kad_agree(fad_handle* h, const KadShards& sh, const char* fn, bool bad, unsigned long long (&args)[kKadArgs],
-              const void* z, long long rows, int d, const double* sigma, cudaStream_t st) {
+              const void* z, long long rows, int d, const double* sigma, cudaStream_t st, const float* radii = nullptr,
+              long long n_radii = 0) {
     if (!sh.comm) return bad ? 1 : 0;
-    if (h->kad_agree.grow((2 * kKadArgs + 1) * 8)) return 1;
+    if (h->kad_agree.grow((2 * kKadArgs + 2) * 8)) return 1;
     unsigned long long* dv = h->kad_agree.get<unsigned long long>();
     if (bad) {
         for (auto& a : args) a = 0;
     } else {
         args[kArgOk] = 1;
         unsigned long long* dz = dv + 2 * kKadArgs;
-        const long long n_vec = rows * d / 8;
-        CK(cudaMemsetAsync(dz, 0, 8, st));
-        if (launch(h, fad::kad_digest_kernel, (unsigned)std::min<long long>((n_vec + 255) / 256, 4LL * h->num_sms), 256, 0,
-                   st, reinterpret_cast<const uint4*>(z), n_vec, dz)) return 1;
+        if (kad_digest(h, reinterpret_cast<const uint4*>(z), rows * d / 8, dz, st)) return 1;
+        if (radii && kad_digest(h, reinterpret_cast<const uint32_t*>(radii), n_radii, dz + 1, st)) return 1;
         if (sigma) CK(cudaMemcpyAsync(&args[kArgSigma], sigma, 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(&args[kArgZ], dz, 8, cudaMemcpyDeviceToHost, st));
+        if (radii) CK(cudaMemcpyAsync(&args[kArgRadii], dz + 1, 8, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
     }
     unsigned long long v[2 * kKadArgs];
@@ -1291,9 +1300,12 @@ unsigned long long kad_offsets_digest(const std::vector<long long>& off) {
 // the one exchange of a pass: buf (n values of T per shard copy) summed over the shards
 template <typename T>
 int kad_exchange(fad_handle* h, const KadShards& sh, T* buf, long long n, cudaStream_t st) {
+    static_assert(std::is_same<T, double>::value || std::is_same<T, unsigned long long>::value ||
+                  std::is_same<T, uint32_t>::value || std::is_same<T, int>::value, "an exchanged type");
     if (sh.size == 1) return 0;
     if (sh.comm) {
-        const int type = std::is_same<T, double>::value ? /*ncclFloat64*/ 8 : /*ncclUint64*/ 5;
+        const int type = std::is_same<T, double>::value ? /*ncclFloat64*/ 8 : std::is_same<T, unsigned long long>::value
+                         ? /*ncclUint64*/ 5 : std::is_same<T, uint32_t>::value ? /*ncclUint32*/ 3 : /*ncclInt32*/ 2;
         const int rc = nccl_api().AllReduce(buf, buf, (size_t)n, type, /*ncclSum*/ 0, sh.comm, st);
         return rc != 0 ? nccl_fail("ncclAllReduce", rc) : 0;
     }
@@ -1301,23 +1313,33 @@ int kad_exchange(fad_handle* h, const KadShards& sh, T* buf, long long n, cudaSt
                   0, st, buf, n, sh.size);
 }
 
-// the tile pass of MODE over this process's shards (bounds: kad_shard_plan of the pass's units), then the exchange of
-// its output: the partials (MODE 0, 2) or the histogram (MODE 1), n values per copy at buf, zero-filled first
+// the tile pass of `kernel` (a KAD or PRDC tile kernel, params P with unit0 / unit1) over this process's shards
+// (bounds: kad_shard_plan of the pass's units), then the exchange of its output: n values of T per copy at buf,
+// zero-filled first when `zero`; bind(p, copy) points p's outputs at one shard's copy
+template <typename P, typename T, typename Bind>
+int sharded_tile_pass(fad_handle* h, const KadShards& sh, const std::vector<long long>& bounds,
+                      void (*kernel)(const CUtensorMap, const CUtensorMap, const P), uint32_t smem, const CUtensorMap& mh,
+                      const CUtensorMap& ml, P p, bool zero, T* buf, long long n, cudaStream_t st, Bind bind) {
+    if (zero) CK(cudaMemsetAsync(buf, 0, (size_t)n * sizeof(T) * sh.copies(), st));
+    for (int s = sh.first(); s < sh.last(); ++s) {
+        bind(p, buf + (size_t)(s - sh.first()) * n);
+        p.unit0 = (int)bounds[s];
+        p.unit1 = (int)bounds[s + 1];
+        // the result does not depend on the grid (fixed work units); an empty shard launches nothing
+        if (launch(h, kernel, std::min(p.unit1 - p.unit0, h->num_sms), fad::kKadThreads, smem, st, mh, ml, p)) return 1;
+    }
+    return kad_exchange(h, sh, buf, n, st);
+}
+
+// sharded_tile_pass of kad_tile_kernel<MODE>: the partials (MODE 0, 2) or the histogram (MODE 1)
 template <int MODE, typename T>
 int kad_sharded_pass(fad_handle* h, const KadShards& sh, const std::vector<long long>& bounds, const CUtensorMap& mh,
                      const CUtensorMap& ml, fad::KadParams p, T* buf, long long n, cudaStream_t st) {
     // one shard writes every partial itself; histogram counts always start from zero
-    if (MODE == 1 || sh.size > 1) CK(cudaMemsetAsync(buf, 0, (size_t)n * sizeof(T) * sh.copies(), st));
-    for (int s = sh.first(); s < sh.last(); ++s) {
-        T* mine = buf + (size_t)(s - sh.first()) * n;
-        if constexpr (MODE == 1) p.hist = mine; else p.partial = mine;
-        p.unit0 = (int)bounds[s];
-        p.unit1 = (int)bounds[s + 1];
-        // the result does not depend on the grid (fixed work units); an empty shard launches nothing
-        if (launch(h, fad::kad_tile_kernel<MODE>, std::min(p.unit1 - p.unit0, h->num_sms), fad::kKadThreads,
-                   fad::kKadSmemBytes, st, mh, ml, p)) return 1;
-    }
-    return kad_exchange(h, sh, buf, n, st);
+    return sharded_tile_pass(h, sh, bounds, fad::kad_tile_kernel<MODE>, fad::kKadSmemBytes, mh, ml, p, MODE == 1 || sh.size > 1,
+                             buf, n, st, [](fad::KadParams& q, T* mine) {
+                                 if constexpr (MODE == 1) q.hist = mine; else q.partial = mine;
+                             });
 }
 }  // namespace
 
@@ -1546,44 +1568,84 @@ int prdc_prepare(fad_handle* h, const void* z, long long m, long long n, int d, 
 }
 }  // namespace
 
-extern "C" int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* radii_sq,
-                                void* stream) {
-    if (prdc_check(h, z_f16, m, n, d, k, radii_sq, radii_sq, radii_sq)) return 1;
+extern "C" int fad_knn_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                        long long m, long long n, int d, int k, float* radii_sq, void* stream) {
+    KadShards sh;
+    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
     CK(cudaSetDevice(h->device));
     cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long args[kKadArgs] = {};
+    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
+    args[kArgK] = (unsigned long long)k;
+    const bool bad = prdc_check(h, z_f16, m, n, d, k, radii_sq, radii_sq, radii_sq) != 0;
+    if (kad_agree(h, sh, "fad_knn_radii_sq_sharded", bad, args, z_f16, m + n, d, nullptr, st)) return 1;
+    // local shards: one radii copy each in the workspace, added into the first and copied out; otherwise radii_sq
+    const long long rows = m + n;
+    const bool staged = sh.copies() > 1;
     KadWorkspace w;
     CUtensorMap mh, ml;
     fad::PrdcParams p = {};
-    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, 0)) return 1;
+    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, staged ? (size_t)rows * 4 * sh.copies() : 0)) return 1;
     p.k = k;
-    p.radii_sq = radii_sq;
-    p.units = p.Tx + p.Ty;
-    // every unit writes its own rows: the result does not depend on the grid
-    return launch(h, fad::prdc_tile_kernel<0>, std::min(p.units, h->num_sms), fad::kKadThreads, fad::kPrdcSmemBytes, st,
-                  mh, ml, p);
+    // Tx units of Tx tiles (the rows of X), then Ty units of Ty tiles (the rows of Y)
+    std::vector<long long> tiles(p.Tx, p.Tx);
+    tiles.resize(p.Tx + p.Ty, p.Ty);
+    uint32_t* buf = reinterpret_cast<uint32_t*>(staged ? (void*)w.extra : (void*)radii_sq);
+    // every unit writes its own rows, so one shard leaves no radius unwritten and the result does not depend on the
+    // grid; the shards' copies are added as integer bit patterns (exactly one copy holds a row's word)
+    if (sharded_tile_pass(h, sh, kad_shard_plan(tiles, sh.size), fad::prdc_tile_kernel<0>, fad::kPrdcSmemBytes, mh, ml, p,
+                          sh.size > 1, buf, rows, st,
+                          [](fad::PrdcParams& q, uint32_t* mine) { q.radii_sq = reinterpret_cast<float*>(mine); }))
+        return 1;
+    if (staged) CK(cudaMemcpyAsync(radii_sq, buf, (size_t)rows * 4, cudaMemcpyDeviceToDevice, st));
+    return 0;
+}
+
+extern "C" int fad_prdc_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                       long long m, long long n, int d, const float* radii_sq, int* inside,
+                                       unsigned char* flags, void* stream) {
+    KadShards sh;
+    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = (cudaStream_t)stream;
+    unsigned long long args[kKadArgs] = {};
+    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
+    const bool bad = prdc_check(h, z_f16, m, n, d, 1, radii_sq, inside, flags) != 0;
+    if (kad_agree(h, sh, "fad_prdc_counts_sharded", bad, args, z_f16, m + n, d, nullptr, st, radii_sq, m + n)) return 1;
+    // per shard copy (int32): inside [n], then the covered and recalled planes [2][m]
+    const long long per = n + 2 * m;
+    KadWorkspace w;
+    CUtensorMap mh, ml;
+    fad::PrdcParams p = {};
+    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, (size_t)per * 4 * sh.copies())) return 1;
+    const long long G = std::max(kPrdcMinRun, ((long long)p.Tx * p.Ty + kPrdcUnits - 1) / kPrdcUnits);
+    p.cuts = (int)((p.Ty + G - 1) / G);
+    p.radii = radii_sq;
+    std::vector<long long> tiles((size_t)p.Tx * p.cuts);
+    for (size_t u = 0; u < tiles.size(); ++u) {
+        const long long i = (long long)(u % p.cuts);
+        tiles[u] = (i + 1) * p.Ty / p.cuts - i * p.Ty / p.cuts;
+    }
+    int* buf = reinterpret_cast<int*>(w.extra);
+    // integer atomics only: the counts do not depend on the grid or the order, and the shards' copies add exactly
+    if (sharded_tile_pass(h, sh, kad_shard_plan(tiles, sh.size), fad::prdc_tile_kernel<1>, fad::kPrdcSmemBytes, mh, ml, p,
+                          true, buf, per, st, [](fad::PrdcParams& q, int* mine) {
+                              q.inside = mine;
+                              q.row_flags = mine + q.n;
+                          }))
+        return 1;
+    CK(cudaMemcpyAsync(inside, buf, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
+    return launch(h, fad::prdc_flags_kernel, (unsigned)((m + 255) / 256), 256, 0, st, buf + n, (int)m, flags);
+}
+
+extern "C" int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* radii_sq,
+                                void* stream) {
+    return fad_knn_radii_sq_sharded(h, nullptr, 1, z_f16, m, n, d, k, radii_sq, stream);
 }
 
 extern "C" int fad_prdc_counts(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* radii_sq,
                                int* inside, unsigned char* flags, void* stream) {
-    if (prdc_check(h, z_f16, m, n, d, 1, radii_sq, inside, flags)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::PrdcParams p = {};
-    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, (size_t)m * 4)) return 1;
-    const long long G = std::max(kPrdcMinRun, ((long long)p.Tx * p.Ty + kPrdcUnits - 1) / kPrdcUnits);
-    p.cuts = (int)((p.Ty + G - 1) / G);
-    p.units = p.Tx * p.cuts;
-    p.radii = radii_sq;
-    p.inside = inside;
-    p.row_flags = reinterpret_cast<uint32_t*>(w.extra);
-    CK(cudaMemsetAsync(inside, 0, (size_t)n * 4, st));
-    CK(cudaMemsetAsync(p.row_flags, 0, (size_t)m * 4, st));
-    // integer atomics only: the counts do not depend on the grid or the order
-    if (launch(h, fad::prdc_tile_kernel<1>, std::min(p.units, h->num_sms), fad::kKadThreads, fad::kPrdcSmemBytes, st,
-               mh, ml, p)) return 1;
-    return launch(h, fad::prdc_flags_kernel, (unsigned)((m + 255) / 256), 256, 0, st, p.row_flags, (int)m, flags);
+    return fad_prdc_counts_sharded(h, nullptr, 1, z_f16, m, n, d, radii_sq, inside, flags, stream);
 }
 
 #include "resample_host.inc"

@@ -426,22 +426,26 @@ __global__ void kad_shard_sum_kernel(T* __restrict__ buf, long long n, int shard
     }
 }
 
-// *out += the wrapping sum over the n_vec 8-element vectors of z of a 64-bit mix of (element index, fp16 bits): an
-// order-independent digest the ranks of a sharded call compare before any tile work
+// *out += the wrapping sum over the 16-bit elements of z, read as n_vec words W (uint4: 8 elements, uint32_t: 2), of a
+// 64-bit mix of (element index, element bits): an order-independent digest the ranks of a sharded call compare before
+// any tile work.  uint4 for the fp16 rows; uint32_t for fp32 arrays, which are only 4-byte aligned and need not fill
+// a whole number of uint4.
 __host__ __device__ __forceinline__ unsigned long long kad_mix64(unsigned long long x) {   // splitmix64 finaliser
     x += 0x9E3779B97F4A7C15ull;
     x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
     x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
     return x ^ (x >> 31);
 }
-__global__ void kad_digest_kernel(const uint4* __restrict__ z, long long n_vec, unsigned long long* __restrict__ out) {
+template <typename W>
+__global__ void kad_digest_kernel(const W* __restrict__ z, long long n_vec, unsigned long long* __restrict__ out) {
+    constexpr int kElems = sizeof(W) / 2;
     unsigned long long s = 0;
     for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n_vec; v += (long long)gridDim.x * blockDim.x) {
-        const uint4 q = z[v];
-        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+        const W q = z[v];
+        const uint32_t* w = reinterpret_cast<const uint32_t*>(&q);
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-            const unsigned long long e = (unsigned long long)(8 * v + k);
+        for (int k = 0; k < kElems; ++k) {
+            const unsigned long long e = (unsigned long long)(kElems * v + k);
             s += kad_mix64((e << 16) | ((w[k >> 1] >> (16 * (k & 1))) & 0xFFFFu));
         }
     }

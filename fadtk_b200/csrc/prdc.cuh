@@ -20,10 +20,15 @@
 // Counts (PASS 1).  Unit = (X tile tx, a run of Y column tiles [c0, c1)), runs cut by the shape only.  r_i^2 of the
 // two rows of a thread sit in registers; s_j^2 is read per column through the read-only cache, as the column norms
 // are.  Every xy pair is evaluated once, so the four metrics see one fp32 q per pair:
-//   row i:    covered |= q < r_i^2,   recalled |= q < s_j^2   (ORed over the quad, atomicOr into row_flags[i])
+//   row i:    covered |= q < r_i^2,   recalled |= q < s_j^2   (ORed over the quad, then atomicOr of 1 into the
+//                                                               covered and recalled planes of row_flags at row i)
 //   column j: inside[j] += #{i : q < r_i^2}                    (integer shuffle tree over the 8 row groups of a warp,
 //                                                               then integer atomicAdd; order-independent)
-// No floating-point atomic anywhere.  prdc_flags_kernel packs row_flags into the uint8 flags.
+// No floating-point atomic anywhere.  prdc_flags_kernel packs the two planes into the uint8 flags.
+//
+// Shards (fadtk_b200.cu, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
+// shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
+// one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
 //
 // Warp roles and stages are kad_tile_kernel's: warpgroup 0 = TMA producer, warpgroups 1-2 = consumers on rows
 // [64 c, 64 c + 64) of the tile.
@@ -39,7 +44,8 @@ static_assert(kPrdcSmemBytes <= kKadSmemBytes, "within the KAD shared-memory bud
 struct PrdcParams {
     int m, n, d;             // rows of X, rows of Y, columns
     int Tx, Ty;              // ceil(m / 128), ceil(n / 128)
-    int units;               // PASS 0: Tx + Ty; PASS 1: Tx * cuts
+    int unit0, unit1;        // this launch's units [unit0, unit1) of Tx + Ty (PASS 0) or Tx * cuts (PASS 1): all of
+                             // them, or one shard of a sharded call; outputs stay indexed by the global row / column
     const float* norm;       // [m + Ty * 128] |y_i|^2 of the rows of Z (zero past m + n)
     // PASS 0
     int k;                   // 1 .. kPrdcMaxK
@@ -48,7 +54,7 @@ struct PrdcParams {
     const float* radii;      // [m + n] r_i^2 of X, then s_j^2 of Y
     int cuts;                // column runs per X tile row: run i = Y tiles [i Ty / cuts, (i + 1) Ty / cuts)
     int* inside;             // [n], zeroed by the host
-    uint32_t* row_flags;     // [m], zeroed by the host: bit 0 covered, bit 1 recalled
+    int* row_flags;          // [2][m], zeroed by the host: plane 0 covered, plane 1 recalled (1 where set)
 };
 
 // the tiles of unit u: A rows from arow, B tiles [c0, c1) at rows bbase + 128 c
@@ -107,7 +113,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
         setmaxnreg_dec<40>();
         if (warp == 0 && elect_one()) {
             int s = 0; uint32_t ph = 0;
-            for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+            for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
                 const PrdcUnit w = prdc_unit<PASS>(p, u);
                 for (int ct = w.c0; ct < w.c1; ++ct)
                     kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, w.arow, w.bbase + ct * 128);
@@ -120,7 +126,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
     const int c = (warp >> 2) - 1;                        // tile rows [64 c, 64 c + 64)
     const int lr0 = c * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
     int s = 0; uint32_t ph = 0;
-    for (int u = blockIdx.x; u < p.units; u += gridDim.x) {
+    for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
         const PrdcUnit w = prdc_unit<PASS>(p, u);
         const int row0 = w.arow + lr0;                    // rows of Z
         const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
@@ -218,16 +224,20 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
 #pragma unroll
             for (int i = 0; i < 2; ++i) {
                 for (int o = 1; o < 4; o <<= 1) bits[i] |= __shfl_xor_sync(0xffffffffu, bits[i], o);
-                if ((lane & 3) == 0 && bits[i]) atomicOr(p.row_flags + row0 + 8 * i, bits[i]);
+                if ((lane & 3) == 0) {
+                    if (bits[i] & 1u) atomicOr(p.row_flags + row0 + 8 * i, 1);
+                    if (bits[i] & 2u) atomicOr(p.row_flags + p.m + row0 + 8 * i, 1);
+                }
             }
         }
     }
 }
 
-// flags[i] = row_flags[i] (bit 0 covered, bit 1 recalled)
-__global__ void prdc_flags_kernel(const uint32_t* __restrict__ row_flags, int m, unsigned char* __restrict__ flags) {
+// flags[i] = bit 0 covered, bit 1 recalled: a plane entry is the number of shards that set it (1 unsharded), so a
+// nonzero entry is the OR over the shards
+__global__ void prdc_flags_kernel(const int* __restrict__ row_flags, int m, unsigned char* __restrict__ flags) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < m) flags[i] = (unsigned char)row_flags[i];
+    if (i < m) flags[i] = (unsigned char)((row_flags[i] != 0) | ((row_flags[m + i] != 0) << 1));
 }
 
 }  // namespace fad

@@ -139,15 +139,15 @@ def calc_kernel_audio_distance(emb_baseline, emb_eval, distributed: bool = False
     return KADResults(score=_kad_score(s_xx, s_yy, s_xy, m, n), bandwidth=sigma, n_baseline=m, n_eval=n)
 
 
-def _kad_engine(distributed: bool):
-    """-> (this process's engine, whether the KAD calls are collective over the torchrun group)"""
+def _kad_engine(distributed: bool, metric: str = "KAD"):
+    """-> (this process's engine, whether the KAD (or PRDC) calls are collective over the torchrun group)"""
     from . import _native, dist
     eng = _native.engine()
     if not (distributed and dist.world_size() > 1):
         return eng, False
     if not dist.enable_native_allreduce(eng):
-        raise RuntimeError("distributed KAD runs over the library's own NCCL communicator, which needs torch.distributed "
-                           "on the nccl backend and FADTK_NATIVE_ALLREDUCE unset or 1")
+        raise RuntimeError(f"distributed {metric} runs over the library's own NCCL communicator, which needs "
+                           "torch.distributed on the nccl backend and FADTK_NATIVE_ALLREDUCE unset or 1")
     return eng, True
 
 
@@ -228,7 +228,7 @@ def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray, distributed: bool =
     return out
 
 
-def calc_prdc(emb_baseline, emb_eval, k: int = 5) -> PRDCResults:
+def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> PRDCResults:
     """Precision and recall (Kynkaanniemi et al., 2019), density and coverage (Naeem et al., 2020) of an eval set
     Y [n, d] against a baseline X [m, d], both fp16 with the values taken as exact reals, q(a, b) = |a - b|^2:
 
@@ -243,7 +243,13 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5) -> PRDCResults:
     nothing.  The radii and the ball counts run on the GPU (fad_knn_radii_sq, fad_prdc_counts) without forming a
     distance matrix; the four values are assembled from integer counts.  A width that is not a multiple of 8 is
     zero-padded, which changes no distance.  Raises ValueError for k outside [1, 16], m <= k or n <= k, non-fp16 or
-    non-2-D input and mismatched widths."""
+    non-2-D input and mismatched widths.
+
+    distributed=True under torchrun (world size > 1): a collective call that every rank makes with the same sets and k.
+    The radii and ball-count tiles are split over the ranks (fad_knn_radii_sq_sharded, fad_prdc_counts_sharded over the
+    library's NCCL communicator), and every rank gets the result, bitwise equal to one GPU's.  The ranks' arguments are
+    compared first; a difference raises NativeError on every rank.  RuntimeError when that communicator cannot be set
+    up, as for calc_kernel_audio_distance."""
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 16:
         raise ValueError(f"PRDC needs an integer k in [1, 16], not {k!r}")
     k = int(k)
@@ -253,11 +259,11 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5) -> PRDCResults:
         raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {m}, eval {n})")
     if x.shape[1] != y.shape[1]:
         raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
-    from . import _native
-    eng = _native.engine()
+    eng, collective = _kad_engine(distributed, "PRDC")
     z = _kad_device_rows(torch.cat([x, y]), eng)
-    radii_sq = eng.knn_radii_sq(z, m, k)
-    inside, flags = (t.cpu().numpy() for t in eng.prdc_counts(z, m, radii_sq))
+    radii_sq = eng.knn_radii_sq_sharded(z, m, k) if collective else eng.knn_radii_sq(z, m, k)
+    counts = eng.prdc_counts_sharded(z, m, radii_sq) if collective else eng.prdc_counts(z, m, radii_sq)
+    inside, flags = (t.cpu().numpy() for t in counts)
     return PRDCResults(precision=float(np.count_nonzero(inside)) / n,
                        recall=float(np.count_nonzero(flags & 2)) / m,
                        density=float(inside.sum(dtype=np.int64)) / (k * n),
@@ -597,21 +603,24 @@ class FrechetAudioDistance:
             sets.append(emb)
         return calc_kernel_audio_distance(*sets, distributed=distributed)
 
-    def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5) -> PRDCResults:
+    def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5, distributed: bool = False) -> PRDCResults:
         """Precision, recall, density and coverage (calc_prdc) of the cached embeddings of eval_dir against those of
         baseline_dir, read as score_kad reads them: all rows of all <dir>/embeddings/<model>/*.npy in sorted file
-        order.  Statistics files and names are refused."""
+        order.  Statistics files and names are refused.  distributed=True under torchrun: a collective call; rank 0
+        lists the files, every rank reads them and takes its share of the radii and ball-count tiles, and every rank
+        gets the result."""
         from . import _io_native
+        collective = distributed and _kad_engine(True, "PRDC")[1]
         sets = []
         for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
-            files = _sorted_npy_files(kad_embedding_dir(p, self.ml.name, "PRDC"))
+            files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name, "PRDC")), collective)
             if not files:
                 raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
             emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
             if emb.dtype != np.float16:
                 raise ValueError(f"PRDC needs fp16 embedding caches; {p} holds {emb.dtype}")
             sets.append(emb)
-        return calc_prdc(*sets, k=k)
+        return calc_prdc(*sets, k=k, distributed=distributed)
 
     def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
                              distributed: bool = False) -> Path:

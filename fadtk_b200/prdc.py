@@ -1,7 +1,9 @@
 """``python -m fadtk_b200.prdc <model> <baseline> <eval> [csv] [-k K] [-w N] [-s sox]`` - precision, recall, density
 and coverage of an eval directory against a baseline directory (fad.calc_prdc on the cached embeddings).  Directories
 without embedding caches are embedded first (under ``torchrun`` the embedding is sharded over the ranks as for
-``fadtk``, and rank 0 then scores alone).  With ``csv``, one row
+``fadtk``).  Under ``torchrun`` every rank then takes its share of the radii and ball-count tiles
+(``distributed=True``) when the library's NCCL communicator can be set up, and rank 0 scores alone otherwise; either
+way rank 0 alone reports and writes.  With ``csv``, one row
 ``model,baseline,eval,k,precision,recall,density,coverage,n_baseline,n_eval,time`` is appended; a new file gets the
 header first, and an existing file with another header is refused rather than mixed.
 """
@@ -37,12 +39,17 @@ def main(argv=None) -> int:
         _check_csv(args.csv, CSV_HEADER, "PRDC")
     dist.init_from_env()
     _embed_directories(model, (args.baseline, args.eval), args.workers)
-    if dist.rank() != 0:
+    from . import _native
+    sharded = dist.is_distributed() and dist.enable_native_allreduce(_native.engine())
+    if dist.rank() != 0 and not sharded:
         dist.shutdown()
         return 0
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
-    res = fad.score_prdc(args.baseline, args.eval, k=args.k)
+    res = fad.score_prdc(args.baseline, args.eval, k=args.k, distributed=sharded)
+    if dist.rank() != 0:
+        dist.shutdown()
+        return 0
     if args.csv:
         _append_row(args.csv, (model.name, args.baseline, args.eval, res.k, res.precision, res.recall, res.density,
                                res.coverage, res.n_baseline, res.n_eval, time.time()), CSV_HEADER)

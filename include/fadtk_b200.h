@@ -371,6 +371,15 @@ int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n,
                      void* stream);
 int fad_prdc_counts(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* radii_sq, int* inside,
                     unsigned char* flags, void* stream);
+/* The same two passes split over shards of contiguous work units (DESIGN.md section 5.12, sharding over GPUs);
+ * local_shards means what it means for fad_kad_*_sharded, and the outputs are bitwise equal to the entries above
+ * (which are the local_shards = 1 case) for any number of shards.  Collective calls compare, before any tile work, m, n,
+ * d, a digest of z, whether each rank accepted its arguments, and k (radii) or a digest of radii_sq (counts); any
+ * difference fails the call on every rank with the same message. */
+int fad_knn_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                             long long n, int d, int k, float* radii_sq, void* stream);
+int fad_prdc_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                            long long n, int d, const float* radii_sq, int* inside, unsigned char* flags, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
