@@ -90,6 +90,19 @@ int alloc(std::vector<DeviceBuffer>& mem, T** dst, size_t bytes, bool zero = fal
     return 0;
 }
 
+// One buffer of a workspace: n elements of T (rounded up to 256 bytes), whose address carve() stores in p
+template <typename T> struct Slot { T** p; size_t bytes; };
+template <typename T> Slot<T> slot(T*& p, size_t n) { return {&p, (n * sizeof(T) + 255) & ~size_t(255)}; }
+
+// A workspace laid out in buf: the slots in the order given.  Grows buf to the total and points every slot at its place.
+template <typename... T>
+int carve(DeviceBuffer& buf, Slot<T>... s) {
+    if (buf.grow((s.bytes + ... + size_t(0)))) return 1;
+    unsigned char* q = buf.get<unsigned char>();
+    ((*s.p = reinterpret_cast<T*>(q), q += s.bytes), ...);
+    return 0;
+}
+
 // A load checks every tensor pointer before it touches its model's slot.
 int check_tensors(const char* fn, const void* const* t, int n_tensors) {
     for (int i = 0; i < n_tensors; ++i)
@@ -188,8 +201,8 @@ struct fad_handle {
     DeviceBuffer fr_buf;                            // Frechet (FrechetWorkspace)
     DeviceBuffer rs_bank, rs_mono;                  // resampler filter bank and mono mix
     int rs_in = 0, rs_out = 0;                      // the rate pair of rs_bank
-    DeviceBuffer kad_buf;                           // fad_kad_* (KadWorkspace)
-    DeviceBuffer kad_agree;                         // fad_kad_*_sharded: the ranks' argument descriptor
+    DeviceBuffer pair_buf;                          // fad_kad_*, fad_knn_radii_sq, fad_prdc_counts (pair_prepare)
+    DeviceBuffer agree_buf;                         // the sharded entries: the ranks' argument descriptor (agree)
     // hi/lo weight tensors whose lo parts are all zero, by address (note_split_weights).  Every hi/lo tensor is noted
     // at its current address before any GEMM reads it: upload_split and fad_vggish_load note each one they upload,
     // fad_umma_layer and fad_linear the caller's on every call.  An entry left behind for a freed address is
@@ -914,20 +927,10 @@ struct FrechetWorkspace {
 };
 
 int frechet_workspace(fad_handle* h, long long G, int d, FrechetWorkspace& w) {
-    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t total = (size_t)d * d;
-    const size_t b_mat = al(G * total * 8), b_mu = al(G * d * 8), b_scal = al(G * 2 * 8), b_flags = al(G * 3 * 4),
-                 b_ok = al(G * 4), b_sqrt = al(total * 8), b_misc = al(4 * 8);
-    if (h->fr_buf.grow(8 * b_mat + b_mu + 2 * b_scal + b_flags + b_ok + b_sqrt + b_misc)) return 1;
-    unsigned char* q = h->fr_buf.get<unsigned char>();
-    for (double** m : {&w.cov, &w.P, &w.M, &w.Y, &w.Z, &w.W, &w.Yn, &w.Zn}) { *m = reinterpret_cast<double*>(q); q += b_mat; }
-    w.mu = reinterpret_cast<double*>(q);        q += b_mu;
-    w.scalC = reinterpret_cast<double*>(q);     q += b_scal;
-    w.scalM = reinterpret_cast<double*>(q);     q += b_scal;
-    w.flags = reinterpret_cast<float*>(q);      q += b_flags;
-    w.ok = reinterpret_cast<int*>(q);           q += b_ok;
-    w.sqrt1 = reinterpret_cast<double*>(q);     q += b_sqrt;
-    w.scal1 = reinterpret_cast<double*>(q);
+    const size_t mat = G * (size_t)d * d;
+    if (carve(h->fr_buf, slot(w.cov, mat), slot(w.P, mat), slot(w.M, mat), slot(w.Y, mat), slot(w.Z, mat), slot(w.W, mat),
+              slot(w.Yn, mat), slot(w.Zn, mat), slot(w.mu, G * d), slot(w.scalC, G * 2), slot(w.scalM, G * 2),
+              slot(w.flags, G * 3), slot(w.ok, G), slot(w.sqrt1, (size_t)d * d), slot(w.scal1, 4))) return 1;
     w.resid = w.scal1 + 2;
     w.sink = w.scal1 + 3;
     return 0;
@@ -1123,530 +1126,7 @@ extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_
 }
 }  // extern "C"
 
-// ------------------------------------------------------------------------ Kernel Audio Distance
-namespace {
-// carve-outs of h->kad_buf for one call over N rows
-struct KadWorkspace {
-    __half *hi, *lo, *shift;
-    float* norm;
-    double *colpart, *partial;                      // partial, hist: one copy per local shard (KadShards::copies)
-    unsigned long long* hist;
-    fad::KadSelectState* state;
-    unsigned char* extra;                           // the caller's own bytes (kad_prepare's extra)
-};
-
-int kad_check(fad_handle* h, const void* z, long long m, long long n, int d, const void* out) {
-    if (!h) return fail("null handle");
-    if (!z || !out) return fail("null argument");
-    if (m < 2 || n < 2) return fail("KAD needs at least two rows in each set");
-    if (d <= 0 || d % 8 != 0) return fail("d must be a positive multiple of 8");
-    if ((reinterpret_cast<uintptr_t>(z) | reinterpret_cast<uintptr_t>(out)) & 15) return fail("pointers must be 16-byte aligned");
-    if (m + n > (1LL << 30)) return fail("too many rows");
-    return 0;
-}
-
-// shift (fp16 mean of the first m rows), hi / lo split and row norms of z [N, d]; the two TMA maps over hi / lo.
-// copies: of the partial buffer and the histogram; norm_rows: at least this many norms (zero past N); extra: bytes of
-// w.extra for the caller
-int kad_prepare(fad_handle* h, const __half* z, int N, int m, int d, KadWorkspace& w, CUtensorMap* map_hi,
-                CUtensorMap* map_lo, fad::KadParams& p, cudaStream_t st, int copies, size_t norm_rows = 0, size_t extra = 0) {
-    p.N = N; p.m = m; p.d = d;
-    p.T = (N + 127) / 128;
-    p.units = (p.T + 1) / 2;
-    p.unit0 = 0; p.unit1 = p.units;
-    const size_t rows_pad = std::max((size_t)p.T * 128, norm_rows);
-    const int chunks = (m + fad::kKadColRows - 1) / fad::kKadColRows;
-    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t b_split = al(rows_pad * d * 2), b_norm = al(rows_pad * 4), b_shift = al((size_t)d * 2),
-                 b_col = al((size_t)chunks * d * 8), b_part = al((size_t)p.units * 3 * 8 * copies),
-                 b_hist = al(2 * fad::kKadHistBins * 8 * (size_t)copies), b_state = al(sizeof(fad::KadSelectState));
-    if (h->kad_buf.grow(2 * b_split + b_norm + b_shift + b_col + b_part + b_hist + b_state + al(extra))) return 1;
-    unsigned char* q = h->kad_buf.get<unsigned char>();
-    w.hi = reinterpret_cast<__half*>(q);            q += b_split;
-    w.lo = reinterpret_cast<__half*>(q);            q += b_split;
-    w.norm = reinterpret_cast<float*>(q);           q += b_norm;
-    w.shift = reinterpret_cast<__half*>(q);         q += b_shift;
-    w.colpart = reinterpret_cast<double*>(q);       q += b_col;
-    w.partial = reinterpret_cast<double*>(q);       q += b_part;
-    w.hist = reinterpret_cast<unsigned long long*>(q); q += b_hist;
-    w.state = reinterpret_cast<fad::KadSelectState*>(q); q += b_state;
-    w.extra = q;
-    p.norm = w.norm;
-
-    if (launch(h, fad::kad_colsum_kernel, chunks, 128, 0, st, z, m, d, w.colpart) ||
-        launch(h, fad::kad_shift_kernel, 1, 256, 0, st, w.colpart, chunks, m, d, w.shift) ||
-        launch(h, fad::kad_split_kernel, (unsigned)((rows_pad * 32 + 255) / 256), 256, 0, st, z, N, (int)rows_pad, d, w.shift,
-               w.hi, w.lo, w.norm)) return 1;
-    // rows >= N and columns >= d of a box are zero-filled by the TMA unit (the kernel masks those rows by index)
-    const uint64_t dims[2] = {(uint64_t)d, (uint64_t)N};
-    const uint64_t strides[1] = {(uint64_t)d * 2};
-    const uint32_t box[2] = {64, 128};
-    if (encode_f16_map(map_hi, w.hi, 2, dims, strides, box)) return 1;
-    return encode_f16_map(map_lo, w.lo, 2, dims, strides, box);
-}
-
-// ---- sharding (DESIGN.md section 5.11).  A call is cut into `size` shards of contiguous work units.  Collective: this
-// process computes shard `rank` of the communicator's `size` into one zero-filled buffer, and the exchange is an NCCL
-// all-reduce.  Local: this device computes shards 0 .. size - 1 one after another, each into its own zero-filled copy,
-// and the exchange adds the copies in shard order.  Either way every exchanged value is produced by one shard and is
-// zero in the others (or is an integer count), so the sum is exact and the result equals the one-shard result bitwise.
-struct KadShards {
-    void* comm = nullptr;      // collective: the communicator; local: null
-    int rank = 0, size = 1;
-    int copies() const { return comm ? 1 : size; }
-    int first() const { return comm ? rank : 0; }
-    int last() const { return comm ? rank + 1 : size; }
-};
-
-int kad_shards(fad_handle* h, void* comm_arg, int local_shards, KadShards& sh) {
-    if (!h) return fail("null handle");
-    if (local_shards < 0) return fail("local_shards must be >= 0");
-    if (local_shards > 0) {
-        if (comm_arg) return fail("local_shards >= 1 runs without a communicator: pass NULL");
-        sh.size = local_shards;
-        return 0;
-    }
-    sh.comm = comm_arg ? comm_arg : h->nccl_comm;
-    if (!sh.comm) return fail("no communicator: call fad_comm_init or pass an ncclComm_t (or set local_shards >= 1)");
-    NcclApi& n = nccl_api();
-    if (!n.ok) return fail(n.why);
-    int rc = n.CommCount(sh.comm, &sh.size);
-    if (rc != 0) return nccl_fail("ncclCommCount", rc);
-    rc = n.CommUserRank(sh.comm, &sh.rank);
-    if (rc != 0) return nccl_fail("ncclCommUserRank", rc);
-    return 0;
-}
-
-// shard s = units [bounds[s], bounds[s + 1]): the first unit at which the running tile total reaches s / shards of
-// the whole, so a shard holds at most its ideal share plus one unit's tiles
-std::vector<long long> kad_shard_plan(const std::vector<long long>& tiles, int shards) {
-    long long total = 0;
-    for (long long t : tiles) total += t;
-    std::vector<long long> bounds(shards + 1, 0);
-    long long u = 0, acc = 0;
-    for (int s = 1; s < shards; ++s) {
-        while (u < (long long)tiles.size() && (__int128)acc * shards < (__int128)s * total) acc += tiles[u++];
-        bounds[s] = u;
-    }
-    bounds[shards] = (long long)tiles.size();
-    return bounds;
-}
-
-// tiles of the MODE 0 / 1 units over T tile rows: row u, then row T - 1 - u (once when they are the same row)
-std::vector<long long> kad_pair_unit_tiles(int T) {
-    std::vector<long long> t((T + 1) / 2);
-    for (int u = 0; u < (int)t.size(); ++u) t[u] = (T - u) + (T - 1 - u != u ? u + 1 : 0);
-    return t;
-}
-
-// the arguments of a collective call, compared across the ranks before any tile work (k and radii: PRDC's; 0 in KAD)
-constexpr int kKadArgs = 10;
-const char* const kKadArgNames[kKadArgs] = {"ok", "m", "n", "d", "n_items", "offsets", "sigma", "z", "k", "radii"};
-enum { kArgOk, kArgM, kArgN, kArgD, kArgItems, kArgOffsets, kArgSigma, kArgZ, kArgK, kArgRadii };
-
-// *out = the digest (kad_digest_kernel) of n_vec words W at x
-template <typename W>
-int kad_digest(fad_handle* h, const W* x, long long n_vec, unsigned long long* out, cudaStream_t st) {
-    CK(cudaMemsetAsync(out, 0, 8, st));
-    return launch(h, fad::kad_digest_kernel<W>, (unsigned)std::min<long long>((n_vec + 255) / 256, 4LL * h->num_sms), 256,
-                  0, st, x, n_vec, out);
-}
-
-// bad: this rank's own checks rejected the call (g_err says why).  Local: fail with that.  Collective: every rank takes
-// part whatever its own checks said.  The digest of z (rows x d fp16), the bits of *sigma and the digest of radii
-// (n_radii fp32, when given) complete args, then one all-reduce (max over the values and their complements) gives each
-// value's max and min on every rank; a rank that rejected its arguments or any value that differs fails the call on
-// every rank with the same message.
-int kad_agree(fad_handle* h, const KadShards& sh, const char* fn, bool bad, unsigned long long (&args)[kKadArgs],
-              const void* z, long long rows, int d, const double* sigma, cudaStream_t st, const float* radii = nullptr,
-              long long n_radii = 0) {
-    if (!sh.comm) return bad ? 1 : 0;
-    if (h->kad_agree.grow((2 * kKadArgs + 2) * 8)) return 1;
-    unsigned long long* dv = h->kad_agree.get<unsigned long long>();
-    if (bad) {
-        for (auto& a : args) a = 0;
-    } else {
-        args[kArgOk] = 1;
-        unsigned long long* dz = dv + 2 * kKadArgs;
-        if (kad_digest(h, reinterpret_cast<const uint4*>(z), rows * d / 8, dz, st)) return 1;
-        if (radii && kad_digest(h, reinterpret_cast<const uint32_t*>(radii), n_radii, dz + 1, st)) return 1;
-        if (sigma) CK(cudaMemcpyAsync(&args[kArgSigma], sigma, 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&args[kArgZ], dz, 8, cudaMemcpyDeviceToHost, st));
-        if (radii) CK(cudaMemcpyAsync(&args[kArgRadii], dz + 1, 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
-    unsigned long long v[2 * kKadArgs];
-    for (int i = 0; i < kKadArgs; ++i) { v[i] = args[i]; v[kKadArgs + i] = ~args[i]; }
-    CK(cudaMemcpyAsync(dv, v, sizeof v, cudaMemcpyHostToDevice, st));
-    const int rc = nccl_api().AllReduce(dv, dv, 2 * kKadArgs, /*ncclUint64*/ 5, /*ncclMax*/ 2, sh.comm, st);
-    if (rc != 0) return nccl_fail("ncclAllReduce", rc);
-    CK(cudaMemcpyAsync(v, dv, sizeof v, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (~v[kKadArgs + kArgOk] == 0)
-        return fail(std::string(fn) + ": a rank rejected its arguments; no rank computed anything");
-    std::string diff;
-    for (int i = 1; i < kKadArgs; ++i)
-        if (v[i] != ~v[kKadArgs + i]) diff += std::string(diff.empty() ? "" : ", ") + kKadArgNames[i];
-    if (!diff.empty()) return fail(std::string(fn) + ": the ranks' arguments differ (" + diff + "); no rank computed anything");
-    return 0;
-}
-
-unsigned long long kad_offsets_digest(const std::vector<long long>& off) {
-    unsigned long long s = 0;
-    for (size_t k = 0; k < off.size(); ++k) s += fad::kad_mix64(fad::kad_mix64(k) ^ (unsigned long long)off[k]);
-    return s;
-}
-
-// the one exchange of a pass: buf (n values of T per shard copy) summed over the shards
-template <typename T>
-int kad_exchange(fad_handle* h, const KadShards& sh, T* buf, long long n, cudaStream_t st) {
-    static_assert(std::is_same<T, double>::value || std::is_same<T, unsigned long long>::value ||
-                  std::is_same<T, uint32_t>::value || std::is_same<T, int>::value, "an exchanged type");
-    if (sh.size == 1) return 0;
-    if (sh.comm) {
-        const int type = std::is_same<T, double>::value ? /*ncclFloat64*/ 8 : std::is_same<T, unsigned long long>::value
-                         ? /*ncclUint64*/ 5 : std::is_same<T, uint32_t>::value ? /*ncclUint32*/ 3 : /*ncclInt32*/ 2;
-        const int rc = nccl_api().AllReduce(buf, buf, (size_t)n, type, /*ncclSum*/ 0, sh.comm, st);
-        return rc != 0 ? nccl_fail("ncclAllReduce", rc) : 0;
-    }
-    return launch(h, fad::kad_shard_sum_kernel<T>, (unsigned)std::min<long long>((n + 255) / 256, 4LL * h->num_sms), 256,
-                  0, st, buf, n, sh.size);
-}
-
-// the tile pass of `kernel` (a KAD or PRDC tile kernel, params P with unit0 / unit1) over this process's shards
-// (bounds: kad_shard_plan of the pass's units), then the exchange of its output: n values of T per copy at buf,
-// zero-filled first when `zero`; bind(p, copy) points p's outputs at one shard's copy
-template <typename P, typename T, typename Bind>
-int sharded_tile_pass(fad_handle* h, const KadShards& sh, const std::vector<long long>& bounds,
-                      void (*kernel)(const CUtensorMap, const CUtensorMap, const P), uint32_t smem, const CUtensorMap& mh,
-                      const CUtensorMap& ml, P p, bool zero, T* buf, long long n, cudaStream_t st, Bind bind) {
-    if (zero) CK(cudaMemsetAsync(buf, 0, (size_t)n * sizeof(T) * sh.copies(), st));
-    for (int s = sh.first(); s < sh.last(); ++s) {
-        bind(p, buf + (size_t)(s - sh.first()) * n);
-        p.unit0 = (int)bounds[s];
-        p.unit1 = (int)bounds[s + 1];
-        // the result does not depend on the grid (fixed work units); an empty shard launches nothing
-        if (launch(h, kernel, std::min(p.unit1 - p.unit0, h->num_sms), fad::kKadThreads, smem, st, mh, ml, p)) return 1;
-    }
-    return kad_exchange(h, sh, buf, n, st);
-}
-
-// sharded_tile_pass of kad_tile_kernel<MODE>: the partials (MODE 0, 2) or the histogram (MODE 1)
-template <int MODE, typename T>
-int kad_sharded_pass(fad_handle* h, const KadShards& sh, const std::vector<long long>& bounds, const CUtensorMap& mh,
-                     const CUtensorMap& ml, fad::KadParams p, T* buf, long long n, cudaStream_t st) {
-    // one shard writes every partial itself; histogram counts always start from zero
-    return sharded_tile_pass(h, sh, bounds, fad::kad_tile_kernel<MODE>, fad::kKadSmemBytes, mh, ml, p, MODE == 1 || sh.size > 1,
-                             buf, n, st, [](fad::KadParams& q, T* mine) {
-                                 if constexpr (MODE == 1) q.hist = mine; else q.partial = mine;
-                             });
-}
-}  // namespace
-
-extern "C" {
-
-int fad_kad_shard_plan(const long long* unit_tiles, long long units, int shards, long long* bounds) {
-    if ((!unit_tiles && units > 0) || !bounds) return fail("null argument");
-    if (units < 0 || shards < 1) return fail("units must be >= 0 and shards >= 1");
-    std::vector<long long> t(unit_tiles, unit_tiles + units);
-    for (long long x : t)
-        if (x < 1) return fail("every unit has at least one tile");
-    const std::vector<long long> b = kad_shard_plan(t, shards);
-    std::copy(b.begin(), b.end(), bounds);
-    return 0;
-}
-
-int fad_kad_median_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* x_f16, long long m,
-                              int d, double* out, void* stream) {
-    KadShards sh;
-    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long args[kKadArgs] = {};
-    args[kArgM] = (unsigned long long)m; args[kArgD] = (unsigned long long)d;
-    const bool bad = kad_check(h, x_f16, m, 2, d, out) != 0;
-    if (kad_agree(h, sh, "fad_kad_median_sq_sharded", bad, args, x_f16, m, d, nullptr, st)) return 1;
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::KadParams p = {};
-    if (kad_prepare(h, reinterpret_cast<const __half*>(x_f16), (int)m, (int)m, d, w, &mh, &ml, p, st, sh.copies())) return 1;
-    const std::vector<long long> bounds = kad_shard_plan(kad_pair_unit_tiles(p.T), sh.size);
-    const unsigned long long pairs = (unsigned long long)m * (unsigned long long)(m - 1) / 2;
-    if (launch(h, fad::kad_select_init_kernel, 1, 1, 0, st, w.state, (pairs - 1) / 2, pairs / 2)) return 1;
-    // radix digits of the fp32 bit pattern of q >= 0 (bit 31 is 0): 30..20, 19..10, 9..0
-    const int shifts[3] = {20, 10, 0}, bins[3] = {2048, 1024, 1024};
-    const uint32_t masks[3] = {0u, 0xFFF00000u, 0xFFFFFC00u};
-    p.prefix = reinterpret_cast<const uint32_t*>(w.state);     // KadSelectState::prefix is its first member
-    for (int pass = 0; pass < 3; ++pass) {
-        p.mask = masks[pass]; p.shift = shifts[pass]; p.bins = bins[pass];
-        if (kad_sharded_pass<1>(h, sh, bounds, mh, ml, p, w.hist, 2 * fad::kKadHistBins, st) ||
-            launch(h, fad::kad_select_kernel, 1, 32, 0, st, w.state, w.hist, shifts[pass], bins[pass], pass == 2, out)) return 1;
-    }
-    return 0;
-}
-
-int fad_kad_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
-                         long long n, int d, const double* sigma, double* out, void* stream) {
-    KadShards sh;
-    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long args[kKadArgs] = {};
-    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
-    const bool bad = kad_check(h, z_f16, m, n, d, out) || (!sigma && fail("null argument"));
-    if (kad_agree(h, sh, "fad_kad_sums_sharded", bad, args, z_f16, m + n, d, sigma, st)) return 1;
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::KadParams p = {};
-    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n), (int)m, d, w, &mh, &ml, p, st, sh.copies()))
-        return 1;
-    p.sigma = sigma;
-    if (kad_sharded_pass<0>(h, sh, kad_shard_plan(kad_pair_unit_tiles(p.T), sh.size), mh, ml, p, w.partial, 3LL * p.units, st))
-        return 1;
-    return launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, p.units, out);
-}
-
-int fad_kad_median_sq(fad_handle* h, const void* x_f16, long long m, int d, double* out, void* stream) {
-    return fad_kad_median_sq_sharded(h, nullptr, 1, x_f16, m, d, out, stream);
-}
-
-int fad_kad_sums(fad_handle* h, const void* z_f16, long long m, long long n, int d, const double* sigma, double* out,
-                 void* stream) {
-    return fad_kad_sums_sharded(h, nullptr, 1, z_f16, m, n, d, sigma, out, stream);
-}
-
-}  // extern "C"
-
-namespace {
-// per-song work units: each Y tile's column tiles cut into ceil(n / G) near-equal runs of at most G tiles,
-// G = max(kKadSongMinGroup, ceil(column tiles / kKadSongUnits)): a function of the shape only, so the sums do not
-// depend on the grid; it keeps the per-unit partials (2 KiB each) to about kKadSongUnits + Ty units while giving every
-// SM many units
-constexpr long long kKadSongMinGroup = 4;
-constexpr long long kKadSongUnits = 8192;
-
-// the host side of fad_kad_song_sums' checks: the offsets read back and validated (off, n_total)
-int kad_song_check(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items, int d,
-                   const double* sigma, const double* out, cudaStream_t st, std::vector<long long>& off, long long& n_total) {
-    if (kad_check(h, z_f16, m, 2, d, out)) return 1;
-    if (!offsets || !sigma) return fail("null argument");
-    if (n_items < 0) return fail("n_items must be >= 0");
-    off.resize((size_t)n_items + 1);
-    CK(cudaMemcpyAsync(off.data(), offsets, off.size() * sizeof(long long), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (off[0] != 0) return fail("offsets[0] must be 0");
-    for (long long k = 0; k < n_items; ++k)
-        if (off[k + 1] < off[k]) return fail("offsets must be non-decreasing");
-    n_total = off.back();
-    if (m + n_total > (1LL << 30)) return fail("too many rows");
-    return 0;
-}
-}  // namespace
-
-extern "C" int fad_kad_song_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
-                                         long long m, const long long* offsets, long long n_items, int d,
-                                         const double* sigma, double* out, void* stream) {
-    KadShards sh;
-    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<long long> off;
-    long long n_total = 0;
-    const bool bad = kad_song_check(h, z_f16, m, offsets, n_items, d, sigma, out, st, off, n_total) != 0;
-    unsigned long long args[kKadArgs] = {};
-    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n_total; args[kArgD] = (unsigned long long)d;
-    args[kArgItems] = (unsigned long long)n_items;
-    if (!bad) args[kArgOffsets] = kad_offsets_digest(off);
-    if (kad_agree(h, sh, "fad_kad_song_sums_sharded", bad, args, z_f16, m + n_total, d, sigma, st)) return 1;
-
-    // work list: per Y tile t, the column tiles X 0..Tx-1, then the band t..be(t)
-    const int Tx = (int)((m + 127) / 128), Ty = (int)((n_total + 127) / 128);
-    std::vector<int> ncols(Ty);
-    long long total = 0;
-    for (int t = 0; t < Ty; ++t) {
-        const long long last = std::min(128LL * t + 127, n_total - 1);
-        const long long k = std::upper_bound(off.begin(), off.end(), last) - off.begin() - 1;   // off[k] <= last < off[k+1]
-        ncols[t] = Tx + (int)((off[k + 1] - 1) / 128) - t + 1;
-        total += ncols[t];
-    }
-    const int G = (int)std::max(kKadSongMinGroup, (total + kKadSongUnits - 1) / kKadSongUnits);
-    std::vector<int4> work;
-    std::vector<long long> work_tiles;
-    std::vector<int> unit_start(Ty + 1, 0);
-    for (int t = 0; t < Ty; ++t) {
-        // near-equal cuts: units of G tiles plus a short remainder would leave CTAs that take every other unit idle
-        const long long n = ncols[t], cuts = (n + G - 1) / G;
-        for (long long i = 0; i < cuts; ++i) {
-            work.push_back(make_int4(t, (int)(i * n / cuts), (int)((i + 1) * n / cuts), 0));
-            work_tiles.push_back(work.back().z - work.back().y);
-        }
-        unit_start[t + 1] = (int)work.size();
-    }
-    const size_t units = work.size();
-
-    auto al = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t b_work = al(units * sizeof(int4)), b_start = al(unit_start.size() * 4), b_end = al((size_t)Ty * 128 * 4),
-                 b_part = al(units * 256 * 8 * sh.copies()), b_xx = al(3 * 8);
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::KadParams p = {};
-    if (kad_prepare(h, reinterpret_cast<const __half*>(z_f16), (int)(m + n_total), (int)m, d, w, &mh, &ml, p, st,
-                    sh.copies(), (size_t)m + (size_t)Ty * 128, b_work + b_start + b_end + b_part + b_xx)) return 1;
-    unsigned char* q = w.extra;
-    int4* d_work = reinterpret_cast<int4*>(q);       q += b_work;
-    int* d_start = reinterpret_cast<int*>(q);        q += b_start;
-    int* d_end = reinterpret_cast<int*>(q);          q += b_end;
-    double* d_part = reinterpret_cast<double*>(q);   q += b_part;
-    double* d_xx = reinterpret_cast<double*>(q);
-    p.sigma = sigma;
-
-    // S_xx: the sums pass over the first m rows alone (rows >= m are masked by index: (S_xx, 0, 0))
-    fad::KadParams px = p;
-    px.N = (int)m;
-    px.T = Tx;
-    px.units = (Tx + 1) / 2;
-    if (kad_sharded_pass<0>(h, sh, kad_shard_plan(kad_pair_unit_tiles(Tx), sh.size), mh, ml, px, w.partial, 3LL * px.units, st) ||
-        launch(h, fad::kad_reduce_kernel, 1, 32, 0, st, w.partial, px.units, d_xx))
-        return 1;
-    CK(cudaMemcpyAsync(out, d_xx, sizeof(double), cudaMemcpyDeviceToDevice, st));
-    if (n_items == 0) return 0;
-
-    if (units) {
-        CK(cudaMemcpyAsync(d_work, work.data(), units * sizeof(int4), cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(d_start, unit_start.data(), unit_start.size() * 4, cudaMemcpyHostToDevice, st));
-        if (launch(h, fad::kad_row_end_kernel, (Ty * 128 + 255) / 256, 256, 0, st, offsets, n_items, (int)m, n_total, Ty * 128, d_end))
-            return 1;
-        p.work = d_work;
-        p.row_end = d_end;
-        p.Tx = Tx;
-        p.units = (int)units;
-        if (kad_sharded_pass<2>(h, sh, kad_shard_plan(work_tiles, sh.size), mh, ml, p, d_part, 256LL * (long long)units, st))
-            return 1;
-    }
-    return launch(h, fad::kad_song_reduce_kernel, (unsigned)n_items, fad::kKadSongReduceThreads, 0, st, d_part, d_start, offsets, out);
-}
-
-extern "C" int fad_kad_song_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets,
-                                 long long n_items, int d, const double* sigma, double* out, void* stream) {
-    return fad_kad_song_sums_sharded(h, nullptr, 1, z_f16, m, offsets, n_items, d, sigma, out, stream);
-}
-
-// ------------------------------------------------------- precision, recall, density and coverage (DESIGN.md 5.12)
-namespace {
-// counts-pass work units: each X tile row's Y column tiles cut into `cuts` near-equal runs of about G tiles,
-// G = max(kPrdcMinRun, ceil(Tx Ty / kPrdcUnits)): a function of the shape only, enough units for every SM
-constexpr long long kPrdcMinRun = 4;
-constexpr long long kPrdcUnits = 8192;
-
-// k: the radii's (the counts pass checks with k = 1, the least any radii allow); a, b: the fp32 / int32 outputs and
-// inputs (4-byte aligned), c: the flags
-int prdc_check(fad_handle* h, const void* z, long long m, long long n, int d, int k, const void* a, const void* b,
-               const void* c) {
-    if (!h) return fail("null handle");
-    if (!z || !a || !b || !c) return fail("null argument");
-    if (k < 1 || k > fad::kPrdcMaxK) return fail("k must be in [1, 16]");
-    if (m <= k || n <= k) return fail("PRDC needs more than k rows in each set");
-    if (d <= 0 || d % 8 != 0) return fail("d must be a positive multiple of 8");
-    if ((reinterpret_cast<uintptr_t>(z) & 15) || ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 3))
-        return fail("pointers must be aligned (z to 16 bytes, the fp32 and int32 arrays to 4)");
-    if (m + n > (1LL << 30)) return fail("too many rows");
-    return 0;
-}
-
-// the shared prologue of both passes (kad_prepare: shift, split, norms, maps) and the fields of p it fixes
-int prdc_prepare(fad_handle* h, const void* z, long long m, long long n, int d, KadWorkspace& w, CUtensorMap* mh,
-                 CUtensorMap* ml, fad::PrdcParams& p, cudaStream_t st, size_t extra) {
-    p.m = (int)m; p.n = (int)n; p.d = d;
-    p.Tx = (int)((m + 127) / 128);
-    p.Ty = (int)((n + 127) / 128);
-    fad::KadParams kp = {};
-    // norms up to the last row of the last Y tile (the A operand of a Y tile starts at row m)
-    if (kad_prepare(h, reinterpret_cast<const __half*>(z), (int)(m + n), (int)m, d, w, mh, ml, kp, st, 1,
-                    (size_t)m + (size_t)p.Ty * 128, extra)) return 1;
-    p.norm = w.norm;
-    return 0;
-}
-}  // namespace
-
-extern "C" int fad_knn_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
-                                        long long m, long long n, int d, int k, float* radii_sq, void* stream) {
-    KadShards sh;
-    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long args[kKadArgs] = {};
-    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
-    args[kArgK] = (unsigned long long)k;
-    const bool bad = prdc_check(h, z_f16, m, n, d, k, radii_sq, radii_sq, radii_sq) != 0;
-    if (kad_agree(h, sh, "fad_knn_radii_sq_sharded", bad, args, z_f16, m + n, d, nullptr, st)) return 1;
-    // local shards: one radii copy each in the workspace, added into the first and copied out; otherwise radii_sq
-    const long long rows = m + n;
-    const bool staged = sh.copies() > 1;
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::PrdcParams p = {};
-    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, staged ? (size_t)rows * 4 * sh.copies() : 0)) return 1;
-    p.k = k;
-    // Tx units of Tx tiles (the rows of X), then Ty units of Ty tiles (the rows of Y)
-    std::vector<long long> tiles(p.Tx, p.Tx);
-    tiles.resize(p.Tx + p.Ty, p.Ty);
-    uint32_t* buf = reinterpret_cast<uint32_t*>(staged ? (void*)w.extra : (void*)radii_sq);
-    // every unit writes its own rows, so one shard leaves no radius unwritten and the result does not depend on the
-    // grid; the shards' copies are added as integer bit patterns (exactly one copy holds a row's word)
-    if (sharded_tile_pass(h, sh, kad_shard_plan(tiles, sh.size), fad::prdc_tile_kernel<0>, fad::kPrdcSmemBytes, mh, ml, p,
-                          sh.size > 1, buf, rows, st,
-                          [](fad::PrdcParams& q, uint32_t* mine) { q.radii_sq = reinterpret_cast<float*>(mine); }))
-        return 1;
-    if (staged) CK(cudaMemcpyAsync(radii_sq, buf, (size_t)rows * 4, cudaMemcpyDeviceToDevice, st));
-    return 0;
-}
-
-extern "C" int fad_prdc_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
-                                       long long m, long long n, int d, const float* radii_sq, int* inside,
-                                       unsigned char* flags, void* stream) {
-    KadShards sh;
-    if (kad_shards(h, nccl_comm_or_null, local_shards, sh)) return 1;
-    CK(cudaSetDevice(h->device));
-    cudaStream_t st = (cudaStream_t)stream;
-    unsigned long long args[kKadArgs] = {};
-    args[kArgM] = (unsigned long long)m; args[kArgN] = (unsigned long long)n; args[kArgD] = (unsigned long long)d;
-    const bool bad = prdc_check(h, z_f16, m, n, d, 1, radii_sq, inside, flags) != 0;
-    if (kad_agree(h, sh, "fad_prdc_counts_sharded", bad, args, z_f16, m + n, d, nullptr, st, radii_sq, m + n)) return 1;
-    // per shard copy (int32): inside [n], then the covered and recalled planes [2][m]
-    const long long per = n + 2 * m;
-    KadWorkspace w;
-    CUtensorMap mh, ml;
-    fad::PrdcParams p = {};
-    if (prdc_prepare(h, z_f16, m, n, d, w, &mh, &ml, p, st, (size_t)per * 4 * sh.copies())) return 1;
-    const long long G = std::max(kPrdcMinRun, ((long long)p.Tx * p.Ty + kPrdcUnits - 1) / kPrdcUnits);
-    p.cuts = (int)((p.Ty + G - 1) / G);
-    p.radii = radii_sq;
-    std::vector<long long> tiles((size_t)p.Tx * p.cuts);
-    for (size_t u = 0; u < tiles.size(); ++u) {
-        const long long i = (long long)(u % p.cuts);
-        tiles[u] = (i + 1) * p.Ty / p.cuts - i * p.Ty / p.cuts;
-    }
-    int* buf = reinterpret_cast<int*>(w.extra);
-    // integer atomics only: the counts do not depend on the grid or the order, and the shards' copies add exactly
-    if (sharded_tile_pass(h, sh, kad_shard_plan(tiles, sh.size), fad::prdc_tile_kernel<1>, fad::kPrdcSmemBytes, mh, ml, p,
-                          true, buf, per, st, [](fad::PrdcParams& q, int* mine) {
-                              q.inside = mine;
-                              q.row_flags = mine + q.n;
-                          }))
-        return 1;
-    CK(cudaMemcpyAsync(inside, buf, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-    return launch(h, fad::prdc_flags_kernel, (unsigned)((m + 255) / 256), 256, 0, st, buf + n, (int)m, flags);
-}
-
-extern "C" int fad_knn_radii_sq(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* radii_sq,
-                                void* stream) {
-    return fad_knn_radii_sq_sharded(h, nullptr, 1, z_f16, m, n, d, k, radii_sq, stream);
-}
-
-extern "C" int fad_prdc_counts(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* radii_sq,
-                               int* inside, unsigned char* flags, void* stream) {
-    return fad_prdc_counts_sharded(h, nullptr, 1, z_f16, m, n, d, radii_sq, inside, flags, stream);
-}
+#include "pairwise_host.inc"
 
 #include "resample_host.inc"
 #include "clap_host.inc"

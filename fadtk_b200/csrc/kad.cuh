@@ -415,7 +415,7 @@ __global__ void kad_reduce_kernel(const double* __restrict__ partial, int units,
     out[t] = s;
 }
 
-// sharded passes (fadtk_b200.cu, kad_exchange): buf[i] = buf[i] + buf[n + i] + ... over the shards' copies in shard
+// sharded passes (pairwise_host.inc, exchange): buf[i] = buf[i] + buf[n + i] + ... over the shards' copies in shard
 // order.  Each value is written by one shard and zero in the others, so the sum is that value exactly.
 template <typename T>
 __global__ void kad_shard_sum_kernel(T* __restrict__ buf, long long n, int shards) {

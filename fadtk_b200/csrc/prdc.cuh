@@ -26,7 +26,7 @@
 //                                                               then integer atomicAdd; order-independent)
 // No floating-point atomic anywhere.  prdc_flags_kernel packs the two planes into the uint8 flags.
 //
-// Shards (fadtk_b200.cu, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
+// Shards (pairwise_host.inc, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
 // shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
 // one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
 //

@@ -590,18 +590,8 @@ class FrechetAudioDistance:
         of all <dir>/embeddings/<model>/*.npy in sorted file order, the files the directory statistics read.
         distributed=True under torchrun: a collective call; rank 0 lists the files, every rank reads them and takes its
         share of the pair tiles, and every rank gets the result."""
-        from . import _io_native
-        collective = distributed and _kad_engine(True)[1]
-        sets = []
-        for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
-            files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name)), collective)
-            if not files:
-                raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
-            emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
-            if emb.dtype != np.float16:
-                raise ValueError(f"KAD needs fp16 embedding caches; {p} holds {emb.dtype}")
-            sets.append(emb)
-        return calc_kernel_audio_distance(*sets, distributed=distributed)
+        return calc_kernel_audio_distance(*self._cached_sets(baseline_dir, eval_dir, "KAD", distributed),
+                                          distributed=distributed)
 
     def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5, distributed: bool = False) -> PRDCResults:
         """Precision, recall, density and coverage (calc_prdc) of the cached embeddings of eval_dir against those of
@@ -609,18 +599,23 @@ class FrechetAudioDistance:
         order.  Statistics files and names are refused.  distributed=True under torchrun: a collective call; rank 0
         lists the files, every rank reads them and takes its share of the radii and ball-count tiles, and every rank
         gets the result."""
+        return calc_prdc(*self._cached_sets(baseline_dir, eval_dir, "PRDC", distributed), k=k, distributed=distributed)
+
+    def _cached_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, distributed: bool) -> list:
+        """The fp16 embeddings of the two directories that score_kad and score_prdc score, for `metric` (named in the
+        errors).  Collective under distributed=True: rank 0 lists the files, every rank reads them."""
         from . import _io_native
-        collective = distributed and _kad_engine(True, "PRDC")[1]
+        collective = distributed and _kad_engine(True, metric)[1]
         sets = []
         for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
-            files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name, "PRDC")), collective)
+            files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name, metric)), collective)
             if not files:
                 raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")
             emb, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
             if emb.dtype != np.float16:
-                raise ValueError(f"PRDC needs fp16 embedding caches; {p} holds {emb.dtype}")
+                raise ValueError(f"{metric} needs fp16 embedding caches; {p} holds {emb.dtype}")
             sets.append(emb)
-        return calc_prdc(*sets, k=k, distributed=distributed)
+        return sets
 
     def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
                              distributed: bool = False) -> Path:
