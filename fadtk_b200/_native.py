@@ -109,6 +109,13 @@ SIGNATURES = {
     "fad_prdc_counts": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp]),
     "fad_knn_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_prdc_counts_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "fad_knn_song_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_prdc_song_counts": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp]),
+    "fad_knn_song_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp,
+                                                c_vp]),
+    "fad_prdc_song_counts_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp,
+                                               c_vp]),
+    "fad_prdc_song_spans": (C.c_int, [c_vp, c_ll, c_ll, c_vp, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -807,6 +814,61 @@ class Engine:
         _check(lib().fad_prdc_counts_sharded(self._h, None, int(local_shards), z.data_ptr(), int(m), n, z.shape[1],
                                              radii_sq.data_ptr(), inside.data_ptr(), flags.data_ptr(), _stream()))
         return inside, flags
+
+    # Per-song PRDC (include/fadtk_b200.h): z = [X; Y_1; ...] fp16 (cuda), offsets int64 [n_items + 1] (cuda, into the
+    # rows after X)
+    def knn_song_radii_sq(self, z: torch.Tensor, m: int, offsets: torch.Tensor, k: int) -> torch.Tensor:
+        """-> fp32 [m + n_total] (cuda): r_i^2 within X, then s_j^2 of each row of Y within its own song
+        (fad_knn_song_radii_sq)"""
+        return self._song_radii(lib().fad_knn_song_radii_sq, (), z, m, offsets, k)
+
+    def knn_song_radii_sq_sharded(self, z: torch.Tensor, m: int, offsets: torch.Tensor, k: int,
+                                  local_shards: int = 0) -> torch.Tensor:
+        """fad_knn_song_radii_sq_sharded: knn_song_radii_sq over shards (local_shards as for kad_sums_sharded)"""
+        return self._song_radii(lib().fad_knn_song_radii_sq_sharded, (None, int(local_shards)), z, m, offsets, k)
+
+    def _song_radii(self, fn, shard_args, z, m, offsets, k):
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        out = torch.empty(z.shape[0], dtype=torch.float32, device=z.device)
+        _check(fn(self._h, *shard_args, z.data_ptr(), int(m), offsets.data_ptr(), offsets.shape[0] - 1, z.shape[1],
+                  int(k), out.data_ptr(), _stream()))
+        return out
+
+    def prdc_song_counts(self, z: torch.Tensor, m: int, offsets: torch.Tensor,
+                         radii_sq: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor]:
+        """radii_sq fp32 [m + n_total] (cuda) -> (inside int32 [n_total], song_counts int32 [n_items, 2]) (cuda): the
+        baseline balls that contain each y_j, and per song the covered and recalled baseline rows
+        (fad_prdc_song_counts)"""
+        return self._song_counts(lib().fad_prdc_song_counts, (), z, m, offsets, radii_sq)
+
+    def prdc_song_counts_sharded(self, z: torch.Tensor, m: int, offsets: torch.Tensor, radii_sq: torch.Tensor,
+                                 local_shards: int = 0) -> tuple[torch.Tensor, torch.Tensor]:
+        """fad_prdc_song_counts_sharded: prdc_song_counts over shards (local_shards as for kad_sums_sharded)"""
+        return self._song_counts(lib().fad_prdc_song_counts_sharded, (None, int(local_shards)), z, m, offsets, radii_sq)
+
+    def _song_counts(self, fn, shard_args, z, m, offsets, radii_sq):
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert radii_sq.dtype == torch.float32 and radii_sq.is_cuda and radii_sq.is_contiguous()
+        assert radii_sq.shape == (z.shape[0],)
+        n_items = offsets.shape[0] - 1
+        inside = torch.empty(max(z.shape[0] - int(m), 0), dtype=torch.int32, device=z.device)
+        counts = torch.empty((max(n_items, 0), 2), dtype=torch.int32, device=z.device)
+        _check(fn(self._h, *shard_args, z.data_ptr(), int(m), offsets.data_ptr(), n_items, z.shape[1],
+                  radii_sq.data_ptr(), inside.data_ptr(), counts.data_ptr(), _stream()))
+        return inside, counts
+
+    @staticmethod
+    def prdc_song_spans(offsets, m: int) -> np.ndarray:
+        """offsets int64 [n_items + 1] (host) -> int64 [spans, 4]: {first row, end row, first song, songs} of each span
+        of the per-song counts pass against m baseline rows (fad_prdc_song_spans, host only)"""
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        n_items = max(off.shape[0] - 1, 0)
+        spans = np.empty((max(n_items, 1), 4), dtype=np.int64)
+        n = np.zeros(1, dtype=np.int64)
+        _check(lib().fad_prdc_song_spans(off.ctypes.data, n_items, int(m), spans.ctypes.data, n.ctypes.data))
+        return spans[:int(n[0])]
 
 
 class Baseline:

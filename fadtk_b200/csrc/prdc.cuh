@@ -26,6 +26,22 @@
 //                                                               then integer atomicAdd; order-independent)
 // No floating-point atomic anywhere.  prdc_flags_kernel packs the two planes into the uint8 flags.
 //
+// Per-song radii (PASS 2).  Z = [X; Y_1; ...; Y_K]; song_of[r] = the song of Y row r (-1 past the last row).  Units
+// u < Tx are PASS 0's X units; unit Tx + t has the A operand at row m + 128 t as in PASS 0, and its B operands are the
+// song band: 128-row boxes from the first row of the song that owns the tile's first row up to the end of the song that
+// owns its last row (boxes need not be tile-aligned).  A row counts the columns of its own
+// song other than itself (song_of[j] == song_of[i], j != i, applied as the row's song range [offsets[s], offsets[s+1])),
+// so s_j is the radius calc_prdc(X, Y_k) computes for y_j: the same operand orientation and chunking, only the tile
+// position differs.
+//
+// Per-song counts (PASS 3).  Unit = (X tile row, span): a span is a run of whole songs cut by the host (spans[]); the B
+// boxes start at the span's first row and count the columns of its songs.  inside[j] as in PASS 1.  Per (baseline row,
+// song) the covered / recalled decisions are ORed over the song's columns: each thread walks its columns in ascending
+// order, so the songs arrive in monotone order; it carries a running (song, flags) pair and, when the song changes,
+// atomicOrs nonzero flags into a shared-memory bitmap [songs][128 rows / 32][2 planes].  At the end of the unit the 256
+// consumers popcount each song's words into song_counts[song][covered | recalled] (integer atomicAdd) and clear the
+// bitmap.  Each (X tile, song) pair belongs to one unit, so no (row, song) pair is counted twice.
+//
 // Shards (pairwise_host.inc, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
 // shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
 // one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
@@ -40,6 +56,11 @@ namespace fad {
 constexpr int kPrdcMaxK = 16;
 constexpr uint32_t kPrdcSmemBytes = kKadStages * kKadStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 static_assert(kPrdcSmemBytes <= kKadSmemBytes, "within the KAD shared-memory budget");
+// PASS 3: at most kPrdcSpanSongs songs per span, a bitmap of [songs][128 / 32 words][2 planes] after the barriers
+constexpr int kPrdcSpanSongs = 512;
+constexpr uint32_t kPrdcBitmapWords = kPrdcSpanSongs * 4 * 2;
+constexpr uint32_t kPrdcSongSmemBytes = kPrdcSmemBytes + kPrdcBitmapWords * 4;
+static_assert(kPrdcSongSmemBytes <= kKadSmemBytes, "the bitmap takes the histogram's share of the KAD budget");
 
 struct PrdcParams {
     int m, n, d;             // rows of X, rows of Y, columns
@@ -55,6 +76,11 @@ struct PrdcParams {
     int cuts;                // column runs per X tile row: run i = Y tiles [i Ty / cuts, (i + 1) Ty / cuts)
     int* inside;             // [n], zeroed by the host
     int* row_flags;          // [2][m], zeroed by the host: plane 0 covered, plane 1 recalled (1 where set)
+    // PASS 2 and 3 (per song): n = n_total, the rows of all songs; PASS 3: cuts = the number of spans
+    const int* song_of;      // [Ty * 128 + 128] the song of each Y row, -1 past the last row
+    const long long* offsets;// [songs + 1] song s = Y rows [offsets[s], offsets[s + 1])
+    const int4* spans;       // PASS 3: [cuts] {first Y row, end Y row, first song, songs}
+    int* song_counts;        // PASS 3: [songs][2] covered, recalled baseline rows, zeroed by the host
 };
 
 // the tiles of unit u: A rows from arow, B tiles [c0, c1) at rows bbase + 128 c
@@ -66,9 +92,20 @@ __device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
     if constexpr (PASS == 0) {
         if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
         return {p.m + (u - p.Tx) * 128, p.m, 0, p.Ty};
-    } else {
+    } else if constexpr (PASS == 1) {
         const int tx = u / p.cuts, i = u - tx * p.cuts;
         return {tx * 128, p.m, (int)((long long)i * p.Ty / p.cuts), (int)((long long)(i + 1) * p.Ty / p.cuts)};
+    } else if constexpr (PASS == 2) {
+        // Y tile t: the band from the first row of the song of row 128 t to the end of the song of its last row
+        if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
+        const int t = u - p.Tx;
+        const int first = (int)__ldg(p.offsets + __ldg(p.song_of + 128 * t));
+        const int end = (int)__ldg(p.offsets + __ldg(p.song_of + min(128 * t + 127, p.n - 1)) + 1);
+        return {p.m + 128 * t, p.m + first, 0, (end - first + 127) / 128};
+    } else {
+        const int tx = u / p.cuts;
+        const int4 sp = p.spans[u - tx * p.cuts];
+        return {tx * 128, p.m + sp.x, 0, (sp.y - sp.x + 127) / 128};
     }
 }
 
@@ -84,11 +121,38 @@ __device__ __forceinline__ void prdc_insert(float (&a)[kPrdcMaxK], float q) {
     }
 }
 
+// the 4 lanes of a quad hold the same two rows over disjoint columns: merge by a fixed xor tree (each lane takes a
+// snapshot of its partner's list first, then inserts its live entries)
+__device__ __forceinline__ void prdc_topk_merge(float (&a)[2][kPrdcMaxK]) {
+#pragma unroll
+    for (int o = 1; o < 4; o <<= 1) {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            float b[kPrdcMaxK];
+#pragma unroll
+            for (int t = 0; t < kPrdcMaxK; ++t) b[t] = __shfl_xor_sync(0xffffffffu, a[i][t], o);
+#pragma unroll
+            for (int t = 0; t < kPrdcMaxK; ++t)
+                if (b[t] >= 0.f && b[t] < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], b[t]);
+        }
+    }
+}
+
+// counts: the decisions of one xy pair from its dot product and norms, bit 0 q < r2 (where the column counts), bit 1
+// q < s2 (where the row counts).  r2 = 0 for a row past m and s2 = 0 for a column that does not count: q < 0 is never
+// true
+__device__ __forceinline__ uint32_t prdc_pair(float dot, float nr, float nc, float r2, float s2, bool col_ok, bool row_ok) {
+    const float sn = nr + nc;
+    float q = fmaf(-2.f, dot, sn);
+    q = q > kQResolution * sn ? q : 0.f;
+    return (uint32_t)(q < r2 && col_ok) | ((uint32_t)(row_ok && q < s2) << 1);
+}
+
 template <int PASS>
 __global__ void __launch_bounds__(kKadThreads, 1)
 prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
     using namespace sm90;
-    static_assert(PASS == 0 || PASS == 1, "0: k-NN radii, 1: ball counts");
+    static_assert(PASS >= 0 && PASS <= 3, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts");
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
@@ -106,6 +170,9 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
         for (int s = 0; s < kKadStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
         mbar_fence_init();
     }
+    uint32_t* bitmap = reinterpret_cast<uint32_t*>(smem + kKadStages * kKadStageBytes + 256);   // PASS 3
+    if constexpr (PASS == 3)
+        for (int b = threadIdx.x; b < (int)kPrdcBitmapWords; b += kKadThreads) bitmap[b] = 0;
     __syncthreads();
 
     if (warp < 4) {
@@ -160,26 +227,60 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                     }
                 }
             }
-            // the 4 lanes of a quad hold the same two rows over disjoint columns: merge by a fixed xor tree (each lane
-            // takes a snapshot of its partner's list first, then inserts its live entries)
-#pragma unroll
-            for (int o = 1; o < 4; o <<= 1) {
-#pragma unroll
-                for (int i = 0; i < 2; ++i) {
-                    float b[kPrdcMaxK];
-#pragma unroll
-                    for (int t = 0; t < kPrdcMaxK; ++t) b[t] = __shfl_xor_sync(0xffffffffu, a[i][t], o);
-#pragma unroll
-                    for (int t = 0; t < kPrdcMaxK; ++t)
-                        if (b[t] >= 0.f && b[t] < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], b[t]);
-                }
-            }
+            prdc_topk_merge(a);
             if ((lane & 3) == 0) {
 #pragma unroll
                 for (int i = 0; i < 2; ++i)
                     if (ii0 + 8 * i < set_n) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
             }
-        } else {
+        } else if constexpr (PASS == 2) {
+            // each row's set as a range [lo, hi) of rows of Z: X for the X units; for the Y units the row's song, and
+            // empty past the last row (song_of = -1)
+            int lo[2], hi[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                if (w.bbase == 0) {
+                    lo[i] = 0;
+                    hi[i] = p.m;
+                } else {
+                    const int sg = __ldg(p.song_of + row0 + 8 * i - p.m);
+                    lo[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg);
+                    hi[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg + 1);
+                }
+            }
+            float a[2][kPrdcMaxK];
+#pragma unroll
+            for (int t = 0; t < kPrdcMaxK; ++t) {
+                a[0][t] = a[1][t] = t < kPrdcMaxK - p.k ? -INFINITY : INFINITY;
+            }
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                // element (row0 + 8 i, column j0 + 8 j + e of Z) is sum[4 j + 2 i + e]
+                const int j0 = w.bbase + ct * 128 + 2 * (lane & 3);
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const float nc[2] = {__ldg(p.norm + j0 + 8 * j), __ldg(p.norm + j0 + 8 * j + 1)};
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int jz = j0 + 8 * j + e;
+                            const float sn = nr[i] + nc[e];
+                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
+                            q = q > kQResolution * sn ? q : 0.f;
+                            if (jz >= lo[i] && jz < hi[i] && jz != row0 + 8 * i && q < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], q);
+                        }
+                    }
+                }
+            }
+            prdc_topk_merge(a);
+            if ((lane & 3) == 0) {
+#pragma unroll
+                for (int i = 0; i < 2; ++i)
+                    if (row0 + 8 * i >= lo[i] && row0 + 8 * i < hi[i]) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
+            }
+        } else if constexpr (PASS == 1) {
             // rows of X past m (the first rows of Y, or zero-filled) count nothing
             const bool rv[2] = {row0 < p.m, row0 + 8 < p.m};
             const float r2[2] = {rv[0] ? __ldg(p.radii + row0) : 0.f, rv[1] ? __ldg(p.radii + row0 + 8) : 0.f};
@@ -199,14 +300,10 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                     for (int i = 0; i < 2; ++i) {
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
-                            const float sn = nr[i] + nc[e];
-                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
-                            q = q > kQResolution * sn ? q : 0.f;
-                            // r2 = 0 past m and s2 = 0 past n: q < 0 is never true
-                            const bool in_r = q < r2[i] && jj + e < p.n;
-                            cov[i] |= in_r;
-                            rec[i] |= rv[i] && q < s2[e];
-                            cj += (uint32_t)in_r << (16 * e);
+                            const uint32_t b = prdc_pair(sum[4 * j + 2 * i + e], nr[i], nc[e], r2[i], s2[e], jj + e < p.n, rv[i]);
+                            cov[i] |= b & 1u;
+                            rec[i] |= b >> 1;
+                            cj += (b & 1u) << (16 * e);
                         }
                     }
                     // rarely taken: the 8 row groups of the warp hold the same columns, lanes l, l ^ 4, ..., l ^ 28 (at
@@ -229,8 +326,91 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                     if (bits[i] & 2u) atomicOr(p.row_flags + p.m + row0 + 8 * i, 1);
                 }
             }
+        } else {
+            const int4 sp = p.spans[u % p.cuts];             // Y rows [sp.x, sp.y), songs [sp.z, sp.z + sp.w)
+            const bool rv[2] = {row0 < p.m, row0 + 8 < p.m};
+            const float r2[2] = {rv[0] ? __ldg(p.radii + row0) : 0.f, rv[1] ? __ldg(p.radii + row0 + 8) : 0.f};
+            // the running (song, flags) pair; flags per row: bit 0 covered, bit 1 recalled
+            int cur = -1;
+            uint32_t fl[2] = {0u, 0u};
+            const auto flush = [&]() {
+                if (cur >= 0 && (fl[0] | fl[1])) {
+                    uint32_t* b = bitmap + (cur - sp.z) * 8;
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        const int lr = lr0 + 8 * i;
+                        if (fl[i] & 1u) atomicOr(b + (lr >> 5) * 2, 1u << (lr & 31));
+                        if (fl[i] & 2u) atomicOr(b + (lr >> 5) * 2 + 1, 1u << (lr & 31));
+                    }
+                }
+            };
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                const int jj0 = sp.x + ct * 128 + 2 * (lane & 3);   // rows of Y
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int jj = jj0 + 8 * j;
+                    const float nc[2] = {__ldg(p.norm + p.m + jj), __ldg(p.norm + p.m + jj + 1)};
+                    // the columns of the span's songs count (song_of = -1 past the last row)
+                    const int sg[2] = {__ldg(p.song_of + jj), __ldg(p.song_of + jj + 1)};
+                    const bool ok[2] = {sg[0] >= sp.z && sg[0] < sp.z + sp.w, sg[1] >= sp.z && sg[1] < sp.z + sp.w};
+                    const float s2[2] = {ok[0] ? __ldg(p.radii + p.m + jj) : 0.f, ok[1] ? __ldg(p.radii + p.m + jj + 1) : 0.f};
+                    uint32_t cj = 0;                          // as in PASS 1
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        uint32_t b[2];
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            b[i] = prdc_pair(sum[4 * j + 2 * i + e], nr[i], nc[e], r2[i], s2[e], ok[e], rv[i]);
+                            cj += (b[i] & 1u) << (16 * e);
+                        }
+                        if (ok[e]) {
+                            if (sg[e] != cur) {
+                                flush();
+                                cur = sg[e];
+                                fl[0] = fl[1] = 0u;
+                            }
+                            fl[0] |= b[0];
+                            fl[1] |= b[1];
+                        }
+                    }
+                    if (__any_sync(0xffffffffu, cj != 0)) {
+                        for (int o = 4; o < 32; o <<= 1) cj += __shfl_xor_sync(0xffffffffu, cj, o);
+                        if (lane < 4) {
+                            if (cj & 0xFFFFu) atomicAdd(p.inside + jj, (int)(cj & 0xFFFFu));
+                            if (cj >> 16) atomicAdd(p.inside + jj + 1, (int)(cj >> 16));
+                        }
+                    }
+                }
+            }
+            flush();
+            // every consumer's flags are in the bitmap: count each (song, plane), then clear it for the next unit
+            const int ct_id = threadIdx.x - 128;
+            named_bar_sync(1, 256);
+            for (int e = ct_id; e < 2 * sp.w; e += 256) {
+                uint32_t* b = bitmap + (e >> 1) * 8 + (e & 1);
+                const int cnt = __popc(b[0]) + __popc(b[2]) + __popc(b[4]) + __popc(b[6]);
+                b[0] = b[2] = b[4] = b[6] = 0u;
+                if (cnt) atomicAdd(p.song_counts + 2 * (sp.z + (e >> 1)) + (e & 1), cnt);
+            }
+            named_bar_sync(1, 256);
         }
     }
+}
+
+// per-song passes: song_of[r] for the Y rows r < rows = the song s with offsets[s] <= r < offsets[s + 1]; -1 from n_total
+__global__ void prdc_song_of_kernel(const long long* __restrict__ offsets, long long n_items, long long n_total, int rows,
+                                    int* __restrict__ song_of) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= rows) return;
+    if (r >= n_total) { song_of[r] = -1; return; }
+    long long lo = 0, hi = n_items;                 // offsets[lo] <= r < offsets[hi]
+    while (hi - lo > 1) {
+        const long long mid = (lo + hi) >> 1;
+        if (offsets[mid] <= r) lo = mid; else hi = mid;
+    }
+    song_of[r] = (int)lo;
 }
 
 // flags[i] = bit 0 covered, bit 1 recalled: a plane entry is the number of shards that set it (1 unsharded), so a

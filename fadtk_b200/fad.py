@@ -6,6 +6,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_kernel_audio_distance  (no reference counterpart) -> wgmma pair-tile kernels (csrc/kad.cuh)
     calc_kernel_audio_distance_songs                       -> the same, every song against one baseline in one pass
     calc_prdc                   (no reference counterpart) -> k-NN radii and ball-count tile kernels (csrc/prdc.cuh)
+    calc_prdc_songs                                        -> the same, every song against one baseline in one pass
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -250,9 +251,7 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> 
     library's NCCL communicator), and every rank gets the result, bitwise equal to one GPU's.  The ranks' arguments are
     compared first; a difference raises NativeError on every rank.  RuntimeError when that communicator cannot be set
     up, as for calc_kernel_audio_distance."""
-    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 16:
-        raise ValueError(f"PRDC needs an integer k in [1, 16], not {k!r}")
-    k = int(k)
+    k = _prdc_k(k)
     x, y = _kad_rows(emb_baseline, "baseline", "PRDC"), _kad_rows(emb_eval, "eval", "PRDC")
     m, n = int(x.shape[0]), int(y.shape[0])
     if m <= k or n <= k:
@@ -269,6 +268,60 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> 
                        density=float(inside.sum(dtype=np.int64)) / (k * n),
                        coverage=float(np.count_nonzero(flags & 1)) / m,
                        k=k, n_baseline=m, n_eval=n)
+
+
+def _prdc_k(k) -> int:
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 16:
+        raise ValueError(f"PRDC needs an integer k in [1, 16], not {k!r}")
+    return int(k)
+
+
+def calc_prdc_songs(emb_baseline, songs, k: int = 5, distributed: bool = False) -> list[PRDCResults]:
+    """Precision, recall, density and coverage of every song against one baseline: for each fp16 [n_k, d] array in
+    ``songs`` with more than k rows, exactly the values calc_prdc(emb_baseline, songs[k], k) gives - the same r_i, s_j
+    the k-NN radius of y_j within its own song, the same fp32 q and strict comparisons, so equal as floats, not merely
+    close.  The baseline radii are computed once, and every song's radii and counts in one GPU pass each
+    (fad_knn_song_radii_sq, fad_prdc_song_counts).  A song with at most k rows (empty ones included) gets NaN for all
+    four values, n_eval still saying how many rows it had, and is never sent to the GPU.  Coverage and recall of a short
+    song against a large baseline are small by definition.  Raises ValueError like calc_prdc: k outside [1, 16],
+    m <= k, non-fp16 or non-2-D input, widths that differ from the baseline's.  distributed: as for calc_prdc."""
+    k = _prdc_k(k)
+    x = _kad_rows(emb_baseline, "baseline", "PRDC")
+    ys = [_kad_rows(y, f"song {i}", "PRDC") for i, y in enumerate(songs)]
+    for i, y in enumerate(ys):
+        if y.shape[1] != x.shape[1]:
+            raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, song {i} {y.shape[1]})")
+    kept = [y.to(x.device) for y in ys if y.shape[0] > k]
+    return _prdc_songs(torch.cat([x, *kept]), int(x.shape[0]), [int(y.shape[0]) for y in ys], k, distributed)
+
+
+def _prdc_songs(z: torch.Tensor, m: int, rows: list, k: int, distributed: bool = False) -> list[PRDCResults]:
+    """z = [X; the songs of more than k rows, in order] fp16 (host or device), rows = the row counts of all songs ->
+    one PRDCResults per song (NaN for the songs not in z)"""
+    if m <= k:
+        raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {m})")
+    nan = float("nan")
+    out = [PRDCResults(nan, nan, nan, nan, k=k, n_baseline=m, n_eval=n) for n in rows]
+    kept = [i for i, n in enumerate(rows) if n > k]
+    if not kept:
+        return out
+    offsets = np.zeros(len(kept) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([rows[i] for i in kept])
+    eng, collective = _kad_engine(distributed, "PRDC")
+    z = _kad_device_rows(z, eng)
+    off = torch.from_numpy(offsets).to(eng.torch_device)
+    radii_sq = (eng.knn_song_radii_sq_sharded(z, m, off, k) if collective else eng.knn_song_radii_sq(z, m, off, k))
+    counts = (eng.prdc_song_counts_sharded(z, m, off, radii_sq) if collective
+              else eng.prdc_song_counts(z, m, off, radii_sq))
+    inside, per_song = (t.cpu().numpy() for t in counts)
+    for s, i in enumerate(kept):
+        ins, n = inside[offsets[s]:offsets[s + 1]], rows[i]
+        out[i] = PRDCResults(precision=float(np.count_nonzero(ins)) / n,
+                             recall=float(per_song[s, 1]) / m,
+                             density=float(ins.sum(dtype=np.int64)) / (k * n),
+                             coverage=float(per_song[s, 0]) / m,
+                             k=k, n_baseline=m, n_eval=n)
+    return out
 
 
 def kad_embedding_dir(path, model_name: str, metric: str = "KAD") -> Path:
@@ -638,19 +691,82 @@ class FrechetAudioDistance:
                 log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
+        x, host, offs, names = self._individual_sets(baseline_dir, eval_dir, "KAD", 2, "at least two embedding rows",
+                                                     collective, writer)
+        pairs = []
+        if names:
+            res = _kad_songs(host, x.shape[0], offs, distributed)
+            pairs = [(f, r.score) for f, r in zip(names, res) if f is not None]
+
+        if not writer:
+            return csv
+        pairs = sorted(pairs, key=lambda x: np.abs(x[1]))
+        csv.parent.mkdir(parents=True, exist_ok=True)
+        csv.write_text("\n".join([",".join([str(x).replace(',', '_') for x in row]) for row in pairs]))
+        return csv
+
+    def score_prdc_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
+                              k: int = 5, distributed: bool = False) -> Path:
+        """Precision, recall, density and coverage of every file in eval_dir against the embeddings of baseline_dir
+        (calc_prdc_songs: the baseline radii once, every file's radii and counts in one GPU pass each).  The table has
+        the header ``file,precision,recall,density,coverage,n_eval`` and one row per file, sorted by density, highest
+        (most baseline-like) first, ties by path; commas in names are replaced.  A str csv_name goes under
+        data/prdc-individual/<model>/, and an existing table is returned untouched.  Files whose cache is missing,
+        unreadable or not an fp16 [rows, d] array of the baseline's width, and files with at most k embedding rows,
+        are logged and dropped.  distributed=True under torchrun: as for score_kad_individual, over the radii and
+        ball-count tiles."""
+        k = _prdc_k(k)
+        csv = Path(csv_name)
+        if isinstance(csv_name, str):
+            csv = Path('data') / 'prdc-individual' / self.ml.name / csv_name
+        collective = distributed and _kad_engine(True, "PRDC")[1]
+        from . import dist
+        writer = not collective or dist.rank() == 0
+        if _on_rank0(csv.exists, collective):
+            if writer:
+                log.info(f"CSV file {csv} already exists, exiting...")
+            return csv
+
+        x, host, offs, names = self._individual_sets(baseline_dir, eval_dir, "PRDC", k + 1,
+                                                     f"more than k = {k} embedding rows", collective, writer)
+        rows = []
+        if names:
+            res = _prdc_songs(host, x.shape[0], np.diff(offs).tolist(), k, distributed)
+            rows = [(f, r) for f, r in zip(names, res) if f is not None]
+        elif x.shape[0] <= k:
+            raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {x.shape[0]})")
+
+        if not writer:
+            return csv
+        rows.sort(key=lambda t: (-t[1].density, str(t[0])))
+        csv.parent.mkdir(parents=True, exist_ok=True)
+        lines = ["file,precision,recall,density,coverage,n_eval"]
+        lines += [",".join([str(f).replace(',', '_'), *(str(v) for v in (r.precision, r.recall, r.density, r.coverage,
+                                                                              r.n_eval))]) for f, r in rows]
+        csv.write_text("\n".join(lines) + "\n")
+        return csv
+
+    def _individual_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, min_rows: int, need: str,
+                         collective: bool, writer: bool):
+        """The embeddings score_kad_individual and score_prdc_individual score -> (x, host, offs, names): x the
+        baseline's fp16 rows; host = [x; the kept files' rows] fp16 (pinned when there is a GPU), offs their int64
+        offsets after x, names[k] the file of kept song k, or None when its cache could not be read (its rows are
+        zeros: score it and drop it).  A file is kept when its cache is an fp16 [rows, d] array of the baseline's width
+        with at least min_rows rows (`need` says so in the log); the others are logged (by the writer) and dropped.
+        Collective: rank 0 lists the directories, every rank reads the caches."""
         from . import _io_native
-        files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name)), collective)
+        files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name, metric)), collective)
         if not files:
             raise ValueError(f"no {self.ml.name} embeddings cached under {baseline_dir}: embed the baseline directory first")
         x, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
         if x.dtype != np.float16:
-            raise ValueError(f"KAD needs fp16 embedding caches; {baseline_dir} holds {x.dtype}")
-        kad_embedding_dir(eval_dir, self.ml.name)
+            raise ValueError(f"{metric} needs fp16 embedding caches; {baseline_dir} holds {x.dtype}")
+        kad_embedding_dir(eval_dir, self.ml.name, metric)
         m, d = x.shape
 
         def _report(f, msg):
             if writer:
-                log.error(f"An error occurred calculating individual KAD using model {self.ml.name} on file {f}")
+                log.error(f"An error occurred calculating individual {metric} using model {self.ml.name} on file {f}")
                 log.error(msg)
 
         # fp16 caches read natively in one pass (libfadtk_io.so) into one pinned buffer after the baseline rows
@@ -662,35 +778,27 @@ class FrechetAudioDistance:
             if st[i] != _io_native.OK:
                 _report(f, f"cannot read the embedding cache {caches[i]} (status {int(st[i])})")
             elif dt[i] != 2 or ndim[i] != 2:
-                _report(f, f"KAD needs an fp16 [rows, d] embedding cache; {caches[i]} is not one")
+                _report(f, f"{metric} needs an fp16 [rows, d] embedding cache; {caches[i]} is not one")
             elif cols[i] != d:
                 _report(f, f"embedding widths differ (baseline {d}, {caches[i]} {int(cols[i])})")
-            elif n_rows[i] < 2:
-                _report(f, f"KAD needs at least two embedding rows, {caches[i]} has {int(n_rows[i])}"
+            elif n_rows[i] < min_rows:
+                _report(f, f"{metric} needs {need}, {caches[i]} has {int(n_rows[i])}"
                            " (This probably means that your audio is too short)")
             else:
                 keep.append(i)
-        pairs = []
-        if keep:
-            rows = n_rows[keep]
-            offs = np.zeros(len(keep) + 1, dtype=np.int64)
-            offs[1:] = np.cumsum(rows)
-            host = torch.empty((m + int(offs[-1]), d), dtype=torch.float16, pin_memory=torch.cuda.is_available())
-            host[:m] = torch.from_numpy(x)
-            _, st = _io_native.npy_read_f16([caches[i] for i in keep], rows, d, host[m:].numpy(), offs,
-                                            self.audio_load_worker)
-            for k in np.nonzero(st != _io_native.OK)[0]:     # vanished / rewritten since the probe: dropped below
-                _report(all_files[keep[k]], f"cannot read {caches[keep[k]]} (status {int(st[k])})")
-                host[m + offs[k]:m + offs[k + 1]] = 0.0
-            res = _kad_songs(host, m, offs, distributed)
-            pairs = [(all_files[i], res[k].score) for k, i in enumerate(keep) if st[k] == _io_native.OK]
-
-        if not writer:
-            return csv
-        pairs = sorted(pairs, key=lambda x: np.abs(x[1]))
-        csv.parent.mkdir(parents=True, exist_ok=True)
-        csv.write_text("\n".join([",".join([str(x).replace(',', '_') for x in row]) for row in pairs]))
-        return csv
+        if not keep:
+            return x, None, None, []
+        rows = n_rows[keep]
+        offs = np.zeros(len(keep) + 1, dtype=np.int64)
+        offs[1:] = np.cumsum(rows)
+        host = torch.empty((m + int(offs[-1]), d), dtype=torch.float16, pin_memory=torch.cuda.is_available())
+        host[:m] = torch.from_numpy(x)
+        _, st = _io_native.npy_read_f16([caches[i] for i in keep], rows, d, host[m:].numpy(), offs,
+                                        self.audio_load_worker)
+        for k in np.nonzero(st != _io_native.OK)[0]:     # vanished / rewritten since the probe: dropped by the caller
+            _report(all_files[keep[k]], f"cannot read {caches[keep[k]]} (status {int(st[k])})")
+            host[m + offs[k]:m + offs[k + 1]] = 0.0
+        return x, host, offs, [all_files[i] if st[k] == _io_native.OK else None for k, i in enumerate(keep)]
 
     def score_inf(self, baseline: PathLike, eval_files: list[Path], steps: int = 25, min_n=500, raw: bool = False):
         """FAD for growing sample counts and the FAD-inf extrapolation (fad.py:304-351).

@@ -1,16 +1,19 @@
-"""``python -m fadtk_b200.prdc <model> <baseline> <eval> [csv] [-k K] [-w N] [-s sox]`` - precision, recall, density
-and coverage of an eval directory against a baseline directory (fad.calc_prdc on the cached embeddings).  Directories
-without embedding caches are embedded first (under ``torchrun`` the embedding is sharded over the ranks as for
-``fadtk``).  Under ``torchrun`` every rank then takes its share of the radii and ball-count tiles
+"""``python -m fadtk_b200.prdc <model> <baseline> <eval> [csv] [-k K] [--indiv] [-w N] [-s sox]`` - precision, recall,
+density and coverage of an eval directory against a baseline directory (fad.calc_prdc on the cached embeddings).
+Directories without embedding caches are embedded first (under ``torchrun`` the embedding is sharded over the ranks as
+for ``fadtk``).  Under ``torchrun`` every rank then takes its share of the radii and ball-count tiles
 (``distributed=True``) when the library's NCCL communicator can be set up, and rank 0 scores alone otherwise; either
 way rank 0 alone reports and writes.  With ``csv``, one row
 ``model,baseline,eval,k,precision,recall,density,coverage,n_baseline,n_eval,time`` is appended; a new file gets the
-header first, and an existing file with another header is refused rather than mixed.
+header first, and an existing file with another header is refused rather than mixed.  With ``--indiv``, every file of
+the eval directory is scored on its own against the baseline (FrechetAudioDistance.score_prdc_individual) and ``csv``
+is that table (default prdc-individual-results.csv).
 """
 from __future__ import annotations
 
 import sys
 import time
+from pathlib import Path
 
 from . import dist
 from .cli import _embed_directories, _parser, _registry
@@ -21,8 +24,10 @@ _PRDC_ARGS = (
     (("model",), dict(type=str, help="embedding model (a registry name)")),
     (("baseline",), dict(type=str, help="baseline audio directory (the real distribution)")),
     (("eval",), dict(type=str, help="evaluation audio directory")),
-    (("csv",), dict(type=str, nargs="?", help="append the result row here")),
+    (("csv",), dict(type=str, nargs="?", help="append the result row here; with --indiv: where the per-file table "
+                                              "goes (default prdc-individual-results.csv)")),
     (("-k",), dict(type=int, default=5, help="nearest neighbour that sets each ball's radius, 1 to 16 (default 5)")),
+    (("--indiv",), dict(action="store_true", help="score every evaluation file on its own against the baseline")),
 )
 
 
@@ -35,7 +40,7 @@ def main(argv=None) -> int:
     model = registry[args.model]
     for p in (args.baseline, args.eval):            # statistics cannot give nearest neighbours
         kad_embedding_dir(p, model.name, "PRDC")
-    if args.csv:
+    if args.csv and not args.indiv:
         _check_csv(args.csv, CSV_HEADER, "PRDC")
     dist.init_from_env()
     _embed_directories(model, (args.baseline, args.eval), args.workers)
@@ -46,6 +51,13 @@ def main(argv=None) -> int:
         return 0
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
+    if args.indiv:
+        table = Path(args.csv or "prdc-individual-results.csv")
+        fad.score_prdc_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded)
+        if dist.rank() == 0:
+            log.info(f"Individual PRDC values saved to {table}")
+        dist.shutdown()
+        return 0
     res = fad.score_prdc(args.baseline, args.eval, k=args.k, distributed=sharded)
     if dist.rank() != 0:
         dist.shutdown()

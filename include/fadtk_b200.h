@@ -380,6 +380,36 @@ int fad_knn_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_s
                              long long n, int d, int k, float* radii_sq, void* stream);
 int fad_prdc_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
                             long long n, int d, const float* radii_sq, int* inside, unsigned char* flags, void* stream);
+/* Per-song PRDC against one baseline (DESIGN.md section 5.12, per-song PRDC): z = [X; Y_1; ...; Y_K] (fp16
+ * [m + n_total, d], X first); offsets = device int64 [n_items + 1], song s = rows [offsets[s], offsets[s+1]) of the Y
+ * part (offsets[0] = 0, non-decreasing, n_items >= 1, n_total = offsets[n_items]; read back to the host, so the call
+ * synchronises the stream once).  Every song must have more than k rows (the counts: at least 2).  The other checks are
+ * fad_knn_radii_sq's (m > k), and int32 outputs are 4-byte aligned; a rejected call launches nothing and writes nothing.
+ * Song s's values are the ones fad_knn_radii_sq / fad_prdc_counts give for [X; Y_s], bitwise.
+ *   fad_knn_song_radii_sq  radii_sq (device fp32 [m + n_total]) = r_i^2 of X as fad_knn_radii_sq, then for each row of Y
+ *                          the k-th smallest q to the other rows of its own song
+ *   fad_prdc_song_counts   radii_sq (device fp32 [m + n_total], e.g. from the call above) -> inside (device int32
+ *                          [n_total]) = #{i : q(x_i, y_j) < r_i^2}; song_counts (device int32 [n_items][2]) = per song
+ *                          #{i : some y_j of the song has q(x_i, y_j) < r_i^2} (covered), then the same with s_j^2
+ *                          (recalled)
+ * The _sharded forms split the tile work as fad_knn_radii_sq_sharded / fad_prdc_counts_sharded do, bitwise equal for
+ * any number of shards; collective calls also compare n_items and a digest of the offsets.  The unsharded entries are
+ * the local_shards = 1 case.
+ * fad_prdc_song_spans (host only): the counts pass's cut of the songs (host int64 offsets [n_items + 1], every song at
+ * least one row) for a baseline of m rows into spans, runs of whole songs in order of at most G * 128 rows (G as
+ * fad_prdc_counts chooses its column runs) and at most 512 songs, a longer song alone; spans (host int64
+ * [n_items][4]) = {first row, end row, first song, songs} per span, *n_spans = their number. */
+int fad_knn_song_radii_sq(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items,
+                          int d, int k, float* radii_sq, void* stream);
+int fad_prdc_song_counts(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items,
+                         int d, const float* radii_sq, int* inside, int* song_counts, void* stream);
+int fad_knn_song_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                  long long m, const long long* offsets, long long n_items, int d, int k,
+                                  float* radii_sq, void* stream);
+int fad_prdc_song_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                 long long m, const long long* offsets, long long n_items, int d,
+                                 const float* radii_sq, int* inside, int* song_counts, void* stream);
+int fad_prdc_song_spans(const long long* offsets, long long n_items, long long m, long long* spans, long long* n_spans);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
