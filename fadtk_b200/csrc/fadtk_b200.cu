@@ -568,9 +568,9 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
-    CK(smem((const void*)fad::prdc_tile_kernel<0>, fad::kPrdcSmemBytes));
-    CK(smem((const void*)fad::prdc_tile_kernel<1>, fad::kPrdcSmemBytes));
-    CK(smem((const void*)fad::prdc_tile_kernel<2>, fad::kPrdcSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<0>, fad::kPairSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<1>, fad::kPairSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<2>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<3>, fad::kPrdcSongSmemBytes));
     if (setup_gemm<0>(h.get()) || setup_gemm<1>(h.get())) return 1;
     *out = h.release();

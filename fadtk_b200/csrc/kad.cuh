@@ -5,15 +5,9 @@
 //   S_xx = sum_{i<j<m} k(z_i, z_j),  S_yy = sum_{m<=i<j} k(z_i, z_j),  S_xy = sum_{i<m<=j} k(z_i, z_j),
 //   k(a, b) = exp(-|a - b|^2 / (2 sigma^2)).
 //
-// Precision.  q = |z_i|^2 + |z_j|^2 - 2 z_i.z_j cancels: rows with a large common offset (Encodec: |mu| ~ 64 per
-// dimension, spread ~ 2) have norms ~1000 x the distances, and an fp32 dot product then leaves ~1e-4 relative error in
-// q.  So a prologue (kad_split_kernel) subtracts a shift s shared by all rows (the fp16-rounded mean of X: the same
-// for the bandwidth and the sums, and distances do not depend on it), and splits y = z - s (exact in fp32) into an
-// fp16 pair hi + lo (22 bits).  The tile kernel issues hi.hi + hi.lo + lo.hi per k-step into one fp32 accumulator
-// (lo.lo is 2^-22 of the result and dropped).  Row norms are the same three terms in fp64, rounded to fp32 once, so an
-// identical pair of rows gives q = 0 up to the accumulator's rounding; q below kQResolution * (|y_i|^2 + |y_j|^2),
-// the resolution of the expanded form, is taken as 0 (exact duplicates have q = 0: silent clips, sigma = 0 detection).
-// The accumulator uses the GEMM's chunk-and-unshrink scheme (conv_gemm.cuh), counting the three products per column.
+// The distances, the prologue (shift, hi/lo split, row norms), the tile loop and the warp roles are the pair-tile code
+// both pairwise metrics run (pair_tile.cuh); this file holds what KAD alone runs: the tile kernel's three epilogues
+// (q, ex2 or histogram, masks, class sums) and the reductions and selection after it.
 //
 // Work units and determinism.  T = ceil(N / 128) tile rows; unit u (u < ceil(T / 2)) is tile row u (tiles u..T-1)
 // followed by tile row T-1-u (tiles T-1-u..T-1): T + 1 tiles per unit, so units are balanced.  A launch covers the
@@ -26,41 +20,25 @@
 // Per-song sums (MODE 2).  Z = [X; Y_1; ...; Y_K]; S_xx comes from MODE 0 over the first m rows.  The A operand is a
 // 128-row tile of Y (rows m + 128 t, not tile-aligned in Z); the B operands are the X tiles (mask j < m), then the
 // song band: Y tiles t .. the tile holding the last row of the song that owns tile t's last row (mask i < j < end of
-// i's song).  Work unit = (Y tile, up to G consecutive column tiles), G a function of the shape only (host work list).
-// Each thread sums k over its columns per row in fp32 per tile and in fp64 over the unit's tiles; the quad's 4 lanes
-// are added by a fixed shuffle tree into partial[u][row] (S_xy and S_yy).  kad_song_reduce_kernel adds each row's
-// units in order, then each song's rows in a fixed tree: no atomics, bitwise reproducible, independent of the grid.
+// i's song, read from song_of and offsets as the per-song PRDC passes read them).  Work unit = (Y tile, up to G
+// consecutive column tiles), G a function of the shape only (host work list).  Each thread sums k over its columns per
+// row in fp32 per tile and in fp64 over the unit's tiles; the quad's 4 lanes are added by a fixed shuffle tree into
+// partial[u][row] (S_xy and S_yy).  kad_song_reduce_kernel adds each row's units in order, then each song's rows in a
+// fixed tree: no atomics, bitwise reproducible, independent of the grid.
 //
 // Bandwidth (MODE 1): exact selection of the two middle q values of the xx triangle by radix passes over the fp32 bit
 // pattern of q (monotone for q >= 0): bits 30..20, 19..10, 9..0.  Each pass runs the same tile loop over X alone and
 // counts the q values whose already-selected high bits match each of the two targets into shared-memory histograms,
 // flushed into 64-bit global counts with integer atomics (order-independent); kad_select_kernel picks the bin of each
 // target.  The q values are bit-for-bit the ones the sums kernel computes for the same rows.
-//
-// Warp roles (384 threads, persistent): warpgroup 0 = TMA producer (one elected lane); warpgroups 1-2 = consumers,
-// consumer c owns tile rows [64 c, 64 c + 64) x 128 columns (one m64n128 accumulator), issues the wgmmas and runs the
-// epilogue (q, ex2 or histogram, masks, class sums) on the accumulator fragment in its registers - no shared-memory
-// round trip of the tile.  Stage = {A_hi, A_lo, B_hi, B_lo} boxes of 128 rows x 64 columns (64 KiB), 3 stages.
 #pragma once
-#include "sm90.cuh"
-#include "conv_gemm.cuh"
+#include "pair_tile.cuh"
 
 namespace fad {
 
-constexpr int kKadThreads = 384;
-constexpr int kKadStages = 3;
-constexpr int kKadConsumerRegs = 232;               // 40 x 128 + 232 x 256 <= 65536
-constexpr uint32_t kKadBox = 128 * 64 * 2;          // one 128-row x 64-column fp16 box (16 KiB)
-constexpr uint32_t kKadStageBytes = 4 * kKadBox;    // A_hi, A_lo, B_hi, B_lo
 constexpr int kKadHistBins = 2048;                  // per target; the largest radix digit has 11 bits
 constexpr uint32_t kKadHistBytes = 2 * kKadHistBins * 4;
-constexpr uint32_t kKadSmemBytes = kKadStages * kKadStageBytes + 1024 /*align slack*/ + 256 /*barriers*/
-                                 + 256 /*unit reduction*/ + kKadHistBytes;
-// q below this fraction of |y_i|^2 + |y_j|^2 is not resolved by the expanded form in fp32 (worst-case accumulator
-// rounding at d = 1024 is ~2e-5 of it) and is taken as 0
-constexpr float kQResolution = 6.103515625e-05f;    // 2^-14
-constexpr int kKadColRows = 4096;                   // rows per partial column sum of the shift prologue
-static_assert(40 * 128 + kKadConsumerRegs * 256 <= 65536, "register file over-subscribed");
+constexpr uint32_t kKadSmemBytes = kPairSmemBytes + 256 /*unit reduction*/ + kKadHistBytes;
 static_assert(kKadSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
 
 struct KadParams {
@@ -82,142 +60,28 @@ struct KadParams {
     // MODE 2 (per-song sums): A = a 128-row tile of Y (rows m + 128 t ...), B = the tiles of X, then the song band
     const int4* work;        // [units] {t, v0, v1}: virtual column tiles [v0, v1) of Y tile t; v < Tx: X tile v,
                              // v >= Tx: Y tile t + v - Tx
-    const int* row_end;      // [Ty * 128] per Y row: the end row (in Z) of its song; 0 past the last row
+    const int* song_of;      // [Ty * 128] the song of each Y row, -1 past the last row (pair_song_of_kernel)
+    const long long* offsets;// [songs + 1] song s = Y rows [offsets[s], offsets[s + 1])
     int Tx;                  // ceil(m / 128)
 };
 
-// --------------------------------------------------------------------------------------------- prologue
-// part[chunk][col] = sum of z[r][col] over the rows of chunk (fp64, fixed order)
-__global__ void kad_colsum_kernel(const __half* __restrict__ z, int m, int d, double* __restrict__ part) {
-    const int r0 = blockIdx.x * kKadColRows;
-    const int r1 = min(m, r0 + kKadColRows);
-    for (int col = threadIdx.x; col < d; col += blockDim.x) {
-        double s = 0.0;
-        for (int r = r0; r < r1; ++r) s += (double)__half2float(z[(size_t)r * d + col]);
-        part[(size_t)blockIdx.x * d + col] = s;
-    }
-}
-// shift = fp16(mean of the first m rows), the partial sums added in chunk order
-__global__ void kad_shift_kernel(const double* __restrict__ part, int chunks, int m, int d, __half* __restrict__ shift) {
-    for (int col = threadIdx.x; col < d; col += blockDim.x) {
-        double s = 0.0;
-        for (int c = 0; c < chunks; ++c) s += part[(size_t)c * d + col];
-        shift[col] = __double2half(s / (double)m);
-    }
-}
-// one warp per row: y = z - shift (exact in fp32), hi = fp16(y), lo = fp16(y - hi); norm = sum hi^2 + 2 hi lo (fp64,
-// fixed lane order, then a fixed shuffle tree), the terms the tile kernel's dot products contain
-__global__ void kad_split_kernel(const __half* __restrict__ z, int N, int rows_pad, int d, const __half* __restrict__ shift,
-                                 __half* __restrict__ hi, __half* __restrict__ lo, float* __restrict__ norm) {
-    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    const int lane = threadIdx.x & 31;
-    if (row >= rows_pad) return;
-    double acc = 0.0;
-    if (row < N) {
-        for (int col = lane; col < d; col += 32) {
-            const size_t e = (size_t)row * d + col;
-            const float y = __half2float(z[e]) - __half2float(shift[col]);
-            const __half h = __float2half_rn(y);
-            const __half l = __float2half_rn(y - __half2float(h));
-            hi[e] = h;
-            lo[e] = l;
-            const double hd = (double)__half2float(h), ld = (double)__half2float(l);
-            acc += hd * hd + 2.0 * hd * ld;
-        }
-    }
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-    if (lane == 0) norm[row] = (float)acc;
-}
-
-// ------------------------------------------------------------------------------------------ tile kernel
-// producer: the ksteps stages of one tile, A = rows [arow, arow + 128), B = rows [brow, brow + 128) of Z (rows past N
-// are zero-filled by the TMA unit; neither coordinate needs to be a multiple of 128)
-__device__ __forceinline__ void kad_load_tile(uint8_t* smem, uint64_t* full, uint64_t* empty, int& s, uint32_t& ph,
-                                              const CUtensorMap* map_hi, const CUtensorMap* map_lo, int ksteps,
-                                              int arow, int brow) {
-    using namespace sm90;
-    for (int ks = 0; ks < ksteps; ++ks) {
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* st = smem + s * kKadStageBytes;
-        mbar_expect_tx(&full[s], kKadStageBytes);
-        tma_load_2d(st, map_hi, &full[s], ks * 64, arow);
-        tma_load_2d(st + kKadBox, map_lo, &full[s], ks * 64, arow);
-        tma_load_2d(st + 2 * kKadBox, map_hi, &full[s], ks * 64, brow);
-        tma_load_2d(st + 3 * kKadBox, map_lo, &full[s], ks * 64, brow);
-        if (++s == kKadStages) { s = 0; ph ^= 1; }
-    }
-}
-
-// consumer c: sum = the fp32 dot products y_i.y_j (hi.hi + hi.lo + lo.hi) of its 64 x 128 block of one tile, in the
-// m64n128 fragment layout
-__device__ __forceinline__ void kad_mma_tile(float (&sum)[64], uint8_t* smem, uint64_t* full, uint64_t* empty, int& s,
-                                             uint32_t& ph, int c, int lane, int d, int ksteps, int chunk_len) {
-    using namespace sm90;
-    float acc[64];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) sum[i] = 0.f;
-    for (int ks0 = 0; ks0 < ksteps; ks0 += chunk_len) {
-        const int ks1 = min(ks0 + chunk_len, ksteps);
-        // three products per real column accumulate into each element (zero-filled columns add exact zeros, which do
-        // not truncate)
-        const int cols = min(d, ks1 * 64) - ks0 * 64;
-        const float unshrink = kAccumShrinkPerElement * (float)(3 * cols);
-        int prev_s = -1;
-        for (int ks = ks0; ks < ks1; ++ks) {
-            mbar_wait(&full[s], ph);
-            const uint32_t base = smem_u32(smem + s * kKadStageBytes);
-            const uint64_t ah = kmajor_sw128_desc(base + c * 64 * 128);
-            const uint64_t al = kmajor_sw128_desc(base + kKadBox + c * 64 * 128);
-            const uint64_t bh = kmajor_sw128_desc(base + 2 * kKadBox);
-            const uint64_t bl = kmajor_sw128_desc(base + 3 * kKadBox);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bh + 2 * k, (ks > ks0) || (k > 0));
-                wgmma_m64n128k16_f16<0, 0>(acc, ah + 2 * k, bl + 2 * k, 1);
-                wgmma_m64n128k16_f16<0, 0>(acc, al + 2 * k, bh + 2 * k, 1);
-            }
-            wgmma_commit();
-            wgmma_wait<1>();
-            if (prev_s >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev_s]); }
-            prev_s = s;
-            if (++s == kKadStages) { s = 0; ph ^= 1; }
-        }
-        wgmma_wait<0>();
-        fence_regs(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[prev_s]);
-#pragma unroll
-        for (int i = 0; i < 64; ++i) sum[i] += fmaf(acc[i], unshrink, acc[i]);
-    }
-}
-
 template <int MODE>
-__global__ void __launch_bounds__(kKadThreads, 1)
+__global__ void __launch_bounds__(kPairThreads, 1)
 kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const KadParams p) {
     using namespace sm90;
     static_assert(MODE == 0 || MODE == 1 || MODE == 2, "0: kernel sums, 1: radix histogram of q, 2: per-row song sums");
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
-    uint64_t* empty = full + kKadStages;
-    double* red = reinterpret_cast<double*>(smem + kKadStages * kKadStageBytes + 256);        // [8 warps][3]
-    uint32_t* hist = reinterpret_cast<uint32_t*>(smem + kKadStages * kKadStageBytes + 512);   // [2][kKadHistBins]
-
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int ksteps = (p.d + 63) / 64;
-    const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
-    const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&map_hi);
-        tma_prefetch_desc(&map_lo);
-        for (int s = 0; s < kKadStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
-        mbar_fence_init();
-    }
+    const PairTile pt = pair_tile_open(smem_raw, &map_hi, &map_lo, p.d, warp, lane);
+    uint8_t* smem = pt.smem;
+    uint64_t* full = pt.full;
+    uint64_t* empty = pt.empty;
+    const int ksteps = pt.ksteps, chunk_len = pt.chunk_len;
+    double* red = reinterpret_cast<double*>(pt.own);                // [8 warps][3]
+    uint32_t* hist = reinterpret_cast<uint32_t*>(pt.own + 256);     // [2][kKadHistBins]
     if (MODE == 1)
-        for (int b = threadIdx.x; b < 2 * kKadHistBins; b += kKadThreads) hist[b] = 0;
+        for (int b = threadIdx.x; b < 2 * kKadHistBins; b += kPairThreads) hist[b] = 0;
     __syncthreads();
 
     if (warp < 4) {
@@ -230,8 +94,8 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                     const int4 wk = p.work[u];
                     const int arow = p.m + wk.x * 128;
                     for (int v = wk.y; v < wk.z; ++v)
-                        kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, arow,
-                                      v < p.Tx ? v * 128 : arow + (v - p.Tx) * 128);
+                        pair_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, arow,
+                                       v < p.Tx ? v * 128 : arow + (v - p.Tx) * 128);
                 }
             } else {
                 for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
@@ -239,14 +103,14 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                         const int r = half == 0 ? u : p.T - 1 - u;
                         if (half == 1 && r == u) break;                // odd T: the middle row once
                         for (int ct = r; ct < p.T; ++ct)
-                            kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, r * 128, ct * 128);
+                            pair_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, r * 128, ct * 128);
                     }
                 }
             }
         }
     } else {
         // ------------------------------------------------------------ consumers: wgmma + epilogue in registers
-        setmaxnreg_inc<kKadConsumerRegs>();
+        setmaxnreg_inc<kPairConsumerRegs>();
         const int c = (warp >> 2) - 1;                    // tile rows [64 c, 64 c + 64)
         const int wq = warp & 3;
         const int ct_id = threadIdx.x - 128;              // 0..255
@@ -259,7 +123,13 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                 const int4 wk = p.work[u];
                 const int row0 = p.m + wk.x * 128 + lr0;                       // rows of Z
                 const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
-                const int end[2] = {__ldg(p.row_end + row0 - p.m), __ldg(p.row_end + row0 + 8 - p.m)};
+                // the end row (in Z) of each row's song; 0 past the last row
+                int end[2];
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    const int sg = __ldg(p.song_of + row0 + 8 * i - p.m);
+                    end[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg + 1);
+                }
                 double axy[2] = {0.0, 0.0}, ayy[2] = {0.0, 0.0};
                 for (int v = wk.y; v < wk.z; ++v) {
                     const bool xt = v < p.Tx;
@@ -273,7 +143,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                         hi[i] = xt ? (end[i] > 0 ? p.m : 0) : end[i];
                     }
                     float sum[64];
-                    kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                    pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
                     float rs[2] = {0.f, 0.f};
 #pragma unroll
                     for (int j = 0; j < 16; ++j) {
@@ -284,9 +154,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int gj = col0 + 8 * j + e;
-                                const float sn = nr[i] + nc[e];
-                                float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
-                                q = q > kQResolution * sn ? q : 0.f;
+                                const float q = pair_q(sum[4 * j + 2 * i + e], nr[i], nc[e]);
                                 float kv;
                                 asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(kv) : "f"(q * neg_coef));
                                 rs[i] += (gj > lo[i] && gj < hi[i]) ? kv : 0.f;
@@ -334,7 +202,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
                 const float nr0 = __ldg(p.norm + row0), nr1 = __ldg(p.norm + row0 + 8);
                 for (int ct = r; ct < p.T; ++ct) {
                     float sum[64];
-                    kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                    pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
 
                     // ---- epilogue on the fragment: element (row0 + 8 i, col0 + 8 j + e) is sum[4 j + 2 i + e]
                     const int col0 = ct * 128 + 2 * (lane & 3);
@@ -347,9 +215,7 @@ kad_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constan
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int gi = row0 + 8 * i, gj = col0 + 8 * j + e;
-                                const float sn = (i ? nr1 : nr0) + (e ? nc.y : nc.x);
-                                float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
-                                q = q > kQResolution * sn ? q : 0.f;           // also clamps q < 0
+                                const float q = pair_q(sum[4 * j + 2 * i + e], i ? nr1 : nr0, e ? nc.y : nc.x);
                                 const bool valid = gj > gi && gj < p.N;        // index masks: j > i, no zero-filled row
                                 if (MODE == 0) {
                                     float kv;
@@ -413,58 +279,6 @@ __global__ void kad_reduce_kernel(const double* __restrict__ partial, int units,
     double s = 0.0;
     for (int u = 0; u < units; ++u) s += partial[(size_t)u * 3 + t];
     out[t] = s;
-}
-
-// sharded passes (pairwise_host.inc, exchange): buf[i] = buf[i] + buf[n + i] + ... over the shards' copies in shard
-// order.  Each value is written by one shard and zero in the others, so the sum is that value exactly.
-template <typename T>
-__global__ void kad_shard_sum_kernel(T* __restrict__ buf, long long n, int shards) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-        T s = buf[i];
-        for (int c = 1; c < shards; ++c) s += buf[(size_t)c * n + i];
-        buf[i] = s;
-    }
-}
-
-// *out += the wrapping sum over the 16-bit elements of z, read as n_vec words W (uint4: 8 elements, uint32_t: 2), of a
-// 64-bit mix of (element index, element bits): an order-independent digest the ranks of a sharded call compare before
-// any tile work.  uint4 for the fp16 rows; uint32_t for fp32 arrays, which are only 4-byte aligned and need not fill
-// a whole number of uint4.
-__host__ __device__ __forceinline__ unsigned long long kad_mix64(unsigned long long x) {   // splitmix64 finaliser
-    x += 0x9E3779B97F4A7C15ull;
-    x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
-    x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
-    return x ^ (x >> 31);
-}
-template <typename W>
-__global__ void kad_digest_kernel(const W* __restrict__ z, long long n_vec, unsigned long long* __restrict__ out) {
-    constexpr int kElems = sizeof(W) / 2;
-    unsigned long long s = 0;
-    for (long long v = (long long)blockIdx.x * blockDim.x + threadIdx.x; v < n_vec; v += (long long)gridDim.x * blockDim.x) {
-        const W q = z[v];
-        const uint32_t* w = reinterpret_cast<const uint32_t*>(&q);
-#pragma unroll
-        for (int k = 0; k < kElems; ++k) {
-            const unsigned long long e = (unsigned long long)(kElems * v + k);
-            s += kad_mix64((e << 16) | ((w[k >> 1] >> (16 * (k & 1))) & 0xFFFFu));
-        }
-    }
-    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-    if ((threadIdx.x & 31) == 0) atomicAdd(out, s);
-}
-
-// per-song sums, MODE 2: row_end[r] for the Y rows r < rows (Ty * 128) = m + the end row (in Y) of r's song; 0 past n_total
-__global__ void kad_row_end_kernel(const long long* __restrict__ offsets, long long n_items, int m, long long n_total,
-                                   int rows, int* __restrict__ row_end) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= rows) return;
-    if (r >= n_total) { row_end[r] = 0; return; }
-    long long lo = 0, hi = n_items;                 // offsets[lo] <= r < offsets[hi]
-    while (hi - lo > 1) {
-        const long long mid = (lo + hi) >> 1;
-        if (offsets[mid] <= r) lo = mid; else hi = mid;
-    }
-    row_end[r] = m + (int)offsets[lo + 1];
 }
 
 // one block per song: out[1 + 2k] = S_yy,k, out[2 + 2k] = S_xy,k.  Each row's partials are summed over the units of its

@@ -1,17 +1,21 @@
 // Precision, recall, density and coverage (PRDC) of two embedding sets on Hopper tensor cores: the k-nearest-neighbour
 // radii of each set and the ball counts between the sets (DESIGN.md section 5.12).
 //
-// Z = [X; Y] (fp16 [m + n, d], X first).  The distances are the KAD ones (kad.cuh): the same prologue (shared fp16
-// shift, hi/lo split, fp64 row norms), the same TMA + wgmma tile loop (kad_load_tile, kad_mma_tile) and the same fp32
-// q = |y_i|^2 + |y_j|^2 - 2 y_i.y_j with q below kQResolution * (|y_i|^2 + |y_j|^2) taken as 0.  Only the epilogue
-// differs, and every output is a selected fp32 value or an integer count, so both passes are bitwise reproducible and
-// independent of the grid without any partial-sum bookkeeping.
+// Z = [X; Y] (fp16 [m + n, d], X first).  The distances are the ones KAD computes: the pair-tile prologue (shared fp16
+// shift, hi/lo split, fp64 row norms), tile loop (pair_load_tile, pair_mma_tile) and q (pair_q) of pair_tile.cuh.
+// Only the epilogue differs, and every output is a selected fp32 value or an integer count, so every pass is bitwise
+// reproducible and independent of the grid without any partial-sum bookkeeping.
 //
-// Radii (PASS 0).  Unit u < Tx: the A operand is X tile u (rows 128 u), the B operands are every X tile; unit Tx + t:
-// the A operand is the 128-row tile of Y at row m + 128 t (as kad_tile_kernel<2>), the B operands are every Y tile.
-// Each consumer thread holds two rows and keeps, per row, the k smallest q of its columns in a sorted register list
-// (an insertion runs only when q is below the current k-th value); the columns j != i, j < the set's size of the same
-// set count (masks by index only: the rows the TMA unit zero-fills never count, duplicate rows are neighbours at 0).
+// Radii (PASS 0; per song PASS 2, the same body).  Unit u < Tx: the A operand is X tile u (rows 128 u), the B operands
+// are every X tile; unit Tx + t: the A operand is the 128-row tile of Y at row m + 128 t (not tile-aligned in Z), the
+// B operands are every Y tile (PASS 2: the song band, 128-row boxes from the first row of the song that owns the
+// tile's first row up to the end of the song that owns its last row; song_of[r] = the song of Y row r, -1 past the
+// last row).  Each consumer thread holds two rows and keeps, per row, the k smallest q of its columns in a sorted
+// register list (an insertion runs only when q is below the current k-th value).  A row counts the columns of its own
+// set other than itself (PASS 2: of its own song, the row's range [offsets[s], offsets[s + 1]) of Y, so s_j is the
+// radius calc_prdc(X, Y_k) computes for y_j: the same operand orientation and chunking, only the tile position
+// differs).  Masks are by index only: the rows the TMA unit zero-fills never count, duplicate rows are neighbours at 0.
+// PASS 0 compares no lower bound, at compile time: at d = 128 the epilogue is part of the pass's cost (DESIGN.md 7).
 // The full square is run, not the triangle: a column-wise top-k would need a second sorted list per column of the
 // fragment, and the unit then owns whole rows.  At the end of the unit the four lanes of a quad (same rows) merge
 // their lists by a fixed xor tree, and one lane writes radii_sq[row of Z] = the k-th smallest of the set's q values.
@@ -22,17 +26,9 @@
 // are.  Every xy pair is evaluated once, so the four metrics see one fp32 q per pair:
 //   row i:    covered |= q < r_i^2,   recalled |= q < s_j^2   (ORed over the quad, then atomicOr of 1 into the
 //                                                               covered and recalled planes of row_flags at row i)
-//   column j: inside[j] += #{i : q < r_i^2}                    (integer shuffle tree over the 8 row groups of a warp,
-//                                                               then integer atomicAdd; order-independent)
+//   column j: inside[j] += #{i : q < r_i^2}                    (prdc_tally: integer shuffle tree over the 8 row
+//                                                               groups of a warp, then integer atomicAdd)
 // No floating-point atomic anywhere.  prdc_flags_kernel packs the two planes into the uint8 flags.
-//
-// Per-song radii (PASS 2).  Z = [X; Y_1; ...; Y_K]; song_of[r] = the song of Y row r (-1 past the last row).  Units
-// u < Tx are PASS 0's X units; unit Tx + t has the A operand at row m + 128 t as in PASS 0, and its B operands are the
-// song band: 128-row boxes from the first row of the song that owns the tile's first row up to the end of the song that
-// owns its last row (boxes need not be tile-aligned).  A row counts the columns of its own
-// song other than itself (song_of[j] == song_of[i], j != i, applied as the row's song range [offsets[s], offsets[s+1])),
-// so s_j is the radius calc_prdc(X, Y_k) computes for y_j: the same operand orientation and chunking, only the tile
-// position differs.
 //
 // Per-song counts (PASS 3).  Unit = (X tile row, span): a span is a run of whole songs cut by the host (spans[]); the B
 // boxes start at the span's first row and count the columns of its songs.  inside[j] as in PASS 1.  Per (baseline row,
@@ -46,32 +42,31 @@
 // shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
 // one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
 //
-// Warp roles and stages are kad_tile_kernel's: warpgroup 0 = TMA producer, warpgroups 1-2 = consumers on rows
+// Warp roles and stages are the pair-tile ones: warpgroup 0 = TMA producer, warpgroups 1-2 = consumers on rows
 // [64 c, 64 c + 64) of the tile.
 #pragma once
-#include "kad.cuh"
+#include "pair_tile.cuh"
 
 namespace fad {
 
 constexpr int kPrdcMaxK = 16;
-constexpr uint32_t kPrdcSmemBytes = kKadStages * kKadStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-static_assert(kPrdcSmemBytes <= kKadSmemBytes, "within the KAD shared-memory budget");
+static_assert(kPairSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
 // PASS 3: at most kPrdcSpanSongs songs per span, a bitmap of [songs][128 / 32 words][2 planes] after the barriers
 constexpr int kPrdcSpanSongs = 512;
 constexpr uint32_t kPrdcBitmapWords = kPrdcSpanSongs * 4 * 2;
-constexpr uint32_t kPrdcSongSmemBytes = kPrdcSmemBytes + kPrdcBitmapWords * 4;
-static_assert(kPrdcSongSmemBytes <= kKadSmemBytes, "the bitmap takes the histogram's share of the KAD budget");
+constexpr uint32_t kPrdcSongSmemBytes = kPairSmemBytes + kPrdcBitmapWords * 4;
+static_assert(kPrdcSongSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
 
 struct PrdcParams {
     int m, n, d;             // rows of X, rows of Y, columns
     int Tx, Ty;              // ceil(m / 128), ceil(n / 128)
-    int unit0, unit1;        // this launch's units [unit0, unit1) of Tx + Ty (PASS 0) or Tx * cuts (PASS 1): all of
-                             // them, or one shard of a sharded call; outputs stay indexed by the global row / column
-    const float* norm;       // [m + Ty * 128] |y_i|^2 of the rows of Z (zero past m + n)
-    // PASS 0
+    int unit0, unit1;        // this launch's units [unit0, unit1) of Tx + Ty (PASS 0, 2) or Tx * cuts (PASS 1, 3): all
+                             // of them, or one shard of a sharded call; outputs stay indexed by the global row / column
+    const float* norm;       // [m + Ty * 128] |y_i|^2 of the rows of Z (zero past m + n; per song: one box more)
+    // PASS 0 and 2
     int k;                   // 1 .. kPrdcMaxK
     float* radii_sq;         // [m + n] out
-    // PASS 1
+    // PASS 1 and 3
     const float* radii;      // [m + n] r_i^2 of X, then s_j^2 of Y
     int cuts;                // column runs per X tile row: run i = Y tiles [i Ty / cuts, (i + 1) Ty / cuts)
     int* inside;             // [n], zeroed by the host
@@ -92,9 +87,6 @@ __device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
     if constexpr (PASS == 0) {
         if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
         return {p.m + (u - p.Tx) * 128, p.m, 0, p.Ty};
-    } else if constexpr (PASS == 1) {
-        const int tx = u / p.cuts, i = u - tx * p.cuts;
-        return {tx * 128, p.m, (int)((long long)i * p.Ty / p.cuts), (int)((long long)(i + 1) * p.Ty / p.cuts)};
     } else if constexpr (PASS == 2) {
         // Y tile t: the band from the first row of the song of row 128 t to the end of the song of its last row
         if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
@@ -102,6 +94,9 @@ __device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
         const int first = (int)__ldg(p.offsets + __ldg(p.song_of + 128 * t));
         const int end = (int)__ldg(p.offsets + __ldg(p.song_of + min(128 * t + 127, p.n - 1)) + 1);
         return {p.m + 128 * t, p.m + first, 0, (end - first + 127) / 128};
+    } else if constexpr (PASS == 1) {
+        const int tx = u / p.cuts, i = u - tx * p.cuts;
+        return {tx * 128, p.m, (int)((long long)i * p.Ty / p.cuts), (int)((long long)(i + 1) * p.Ty / p.cuts)};
     } else {
         const int tx = u / p.cuts;
         const int4 sp = p.spans[u - tx * p.cuts];
@@ -142,37 +137,39 @@ __device__ __forceinline__ void prdc_topk_merge(float (&a)[2][kPrdcMaxK]) {
 // q < s2 (where the row counts).  r2 = 0 for a row past m and s2 = 0 for a column that does not count: q < 0 is never
 // true
 __device__ __forceinline__ uint32_t prdc_pair(float dot, float nr, float nc, float r2, float s2, bool col_ok, bool row_ok) {
-    const float sn = nr + nc;
-    float q = fmaf(-2.f, dot, sn);
-    q = q > kQResolution * sn ? q : 0.f;
+    const float q = pair_q(dot, nr, nc);
     return (uint32_t)(q < r2 && col_ok) | ((uint32_t)(row_ok && q < s2) << 1);
 }
 
+// counts: inside[jj] += the low 16 bits of cj, inside[jj + 1] += the high 16 bits, summed over the warp.  Rarely taken:
+// the 8 row groups of the warp hold the same columns, lanes l, l ^ 4, ..., l ^ 28 (at most 16 rows per column, so the
+// two 16-bit halves do not carry into each other)
+__device__ __forceinline__ void prdc_tally(uint32_t cj, int* inside, int jj, int lane) {
+    if (__any_sync(0xffffffffu, cj != 0)) {
+        for (int o = 4; o < 32; o <<= 1) cj += __shfl_xor_sync(0xffffffffu, cj, o);
+        if (lane < 4) {
+            if (cj & 0xFFFFu) atomicAdd(inside + jj, (int)(cj & 0xFFFFu));
+            if (cj >> 16) atomicAdd(inside + jj + 1, (int)(cj >> 16));
+        }
+    }
+}
+
 template <int PASS>
-__global__ void __launch_bounds__(kKadThreads, 1)
+__global__ void __launch_bounds__(kPairThreads, 1)
 prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
     using namespace sm90;
     static_assert(PASS >= 0 && PASS <= 3, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts");
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + kKadStages * kKadStageBytes);
-    uint64_t* empty = full + kKadStages;
-
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    const int ksteps = (p.d + 63) / 64;
-    const int n_chunks = (ksteps + kChunkSteps - 1) / kChunkSteps;
-    const int chunk_len = (ksteps + n_chunks - 1) / n_chunks;
-
-    if (warp == 0 && lane == 0) {
-        tma_prefetch_desc(&map_hi);
-        tma_prefetch_desc(&map_lo);
-        for (int s = 0; s < kKadStages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }   // 8 consumer warps
-        mbar_fence_init();
-    }
-    uint32_t* bitmap = reinterpret_cast<uint32_t*>(smem + kKadStages * kKadStageBytes + 256);   // PASS 3
+    const PairTile pt = pair_tile_open(smem_raw, &map_hi, &map_lo, p.d, warp, lane);
+    uint8_t* smem = pt.smem;
+    uint64_t* full = pt.full;
+    uint64_t* empty = pt.empty;
+    const int ksteps = pt.ksteps, chunk_len = pt.chunk_len;
+    uint32_t* bitmap = reinterpret_cast<uint32_t*>(pt.own);        // PASS 3
     if constexpr (PASS == 3)
-        for (int b = threadIdx.x; b < (int)kPrdcBitmapWords; b += kKadThreads) bitmap[b] = 0;
+        for (int b = threadIdx.x; b < (int)kPrdcBitmapWords; b += kPairThreads) bitmap[b] = 0;
     __syncthreads();
 
     if (warp < 4) {
@@ -183,13 +180,13 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
                 const PrdcUnit w = prdc_unit<PASS>(p, u);
                 for (int ct = w.c0; ct < w.c1; ++ct)
-                    kad_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, w.arow, w.bbase + ct * 128);
+                    pair_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, w.arow, w.bbase + ct * 128);
             }
         }
         return;
     }
     // ---------------------------------------------------------------- consumers: wgmma + epilogue in registers
-    setmaxnreg_inc<kKadConsumerRegs>();
+    setmaxnreg_inc<kPairConsumerRegs>();
     const int c = (warp >> 2) - 1;                        // tile rows [64 c, 64 c + 64)
     const int lr0 = c * 64 + (warp & 3) * 16 + (lane >> 2);   // tile rows lr0, lr0 + 8
     int s = 0; uint32_t ph = 0;
@@ -197,9 +194,23 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
         const PrdcUnit w = prdc_unit<PASS>(p, u);
         const int row0 = w.arow + lr0;                    // rows of Z
         const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
-        if constexpr (PASS == 0) {
-            const int set_n = w.bbase == 0 ? p.m : p.n;
-            const int ii0 = row0 - w.bbase;               // rows within the set
+        if constexpr (PASS == 0 || PASS == 2) {
+            // each row's set as a range [lo, hi) of the unit's columns jj (rows bbase + jj of Z): the whole set (lo = 0
+            // is not compared); per song, for the Y units, the row's song, empty past the last row (song_of = -1)
+            constexpr bool songs = PASS == 2;
+            const int ii0 = row0 - w.bbase;               // the rows' own columns
+            int lo[2], hi[2];
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                if (!songs || w.bbase == 0) {
+                    lo[i] = 0;
+                    hi[i] = w.bbase == 0 ? p.m : p.n;
+                } else {
+                    const int sg = __ldg(p.song_of + row0 + 8 * i - p.m);
+                    lo[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg) - w.bbase;
+                    hi[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg + 1) - w.bbase;
+                }
+            }
             float a[2][kPrdcMaxK];
 #pragma unroll
             for (int t = 0; t < kPrdcMaxK; ++t) {
@@ -207,8 +218,8 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             }
             for (int ct = w.c0; ct < w.c1; ++ct) {
                 float sum[64];
-                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
-                // element (row0 + 8 i, column jj0 + 8 j + e of the set) is sum[4 j + 2 i + e]
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                // element (row0 + 8 i, column jj0 + 8 j + e) is sum[4 j + 2 i + e]
                 const int jj0 = ct * 128 + 2 * (lane & 3);
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -219,10 +230,9 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
                             const int jj = jj0 + 8 * j + e;
-                            const float sn = nr[i] + nc[e];
-                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
-                            q = q > kQResolution * sn ? q : 0.f;     // also clamps q < 0
-                            if (jj < set_n && jj != ii0 + 8 * i && q < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], q);
+                            const float q = pair_q(sum[4 * j + 2 * i + e], nr[i], nc[e]);
+                            if ((!songs || jj >= lo[i]) && jj < hi[i] && jj != ii0 + 8 * i && q < a[i][kPrdcMaxK - 1])
+                                prdc_insert(a[i], q);
                         }
                     }
                 }
@@ -231,54 +241,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             if ((lane & 3) == 0) {
 #pragma unroll
                 for (int i = 0; i < 2; ++i)
-                    if (ii0 + 8 * i < set_n) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
-            }
-        } else if constexpr (PASS == 2) {
-            // each row's set as a range [lo, hi) of rows of Z: X for the X units; for the Y units the row's song, and
-            // empty past the last row (song_of = -1)
-            int lo[2], hi[2];
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                if (w.bbase == 0) {
-                    lo[i] = 0;
-                    hi[i] = p.m;
-                } else {
-                    const int sg = __ldg(p.song_of + row0 + 8 * i - p.m);
-                    lo[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg);
-                    hi[i] = sg < 0 ? 0 : p.m + (int)__ldg(p.offsets + sg + 1);
-                }
-            }
-            float a[2][kPrdcMaxK];
-#pragma unroll
-            for (int t = 0; t < kPrdcMaxK; ++t) {
-                a[0][t] = a[1][t] = t < kPrdcMaxK - p.k ? -INFINITY : INFINITY;
-            }
-            for (int ct = w.c0; ct < w.c1; ++ct) {
-                float sum[64];
-                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
-                // element (row0 + 8 i, column j0 + 8 j + e of Z) is sum[4 j + 2 i + e]
-                const int j0 = w.bbase + ct * 128 + 2 * (lane & 3);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) {
-                    const float nc[2] = {__ldg(p.norm + j0 + 8 * j), __ldg(p.norm + j0 + 8 * j + 1)};
-#pragma unroll
-                    for (int i = 0; i < 2; ++i) {
-#pragma unroll
-                        for (int e = 0; e < 2; ++e) {
-                            const int jz = j0 + 8 * j + e;
-                            const float sn = nr[i] + nc[e];
-                            float q = fmaf(-2.f, sum[4 * j + 2 * i + e], sn);
-                            q = q > kQResolution * sn ? q : 0.f;
-                            if (jz >= lo[i] && jz < hi[i] && jz != row0 + 8 * i && q < a[i][kPrdcMaxK - 1]) prdc_insert(a[i], q);
-                        }
-                    }
-                }
-            }
-            prdc_topk_merge(a);
-            if ((lane & 3) == 0) {
-#pragma unroll
-                for (int i = 0; i < 2; ++i)
-                    if (row0 + 8 * i >= lo[i] && row0 + 8 * i < hi[i]) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
+                    if ((!songs || ii0 + 8 * i >= lo[i]) && ii0 + 8 * i < hi[i]) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
             }
         } else if constexpr (PASS == 1) {
             // rows of X past m (the first rows of Y, or zero-filled) count nothing
@@ -287,7 +250,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             bool cov[2] = {false, false}, rec[2] = {false, false};
             for (int ct = w.c0; ct < w.c1; ++ct) {
                 float sum[64];
-                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
                 const int jj0 = ct * 128 + 2 * (lane & 3);    // rows of Y
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -306,15 +269,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                             cj += (b & 1u) << (16 * e);
                         }
                     }
-                    // rarely taken: the 8 row groups of the warp hold the same columns, lanes l, l ^ 4, ..., l ^ 28 (at
-                    // most 16 rows per column, so the two 16-bit halves do not carry into each other)
-                    if (__any_sync(0xffffffffu, cj != 0)) {
-                        for (int o = 4; o < 32; o <<= 1) cj += __shfl_xor_sync(0xffffffffu, cj, o);
-                        if (lane < 4) {
-                            if (cj & 0xFFFFu) atomicAdd(p.inside + jj, (int)(cj & 0xFFFFu));
-                            if (cj >> 16) atomicAdd(p.inside + jj + 1, (int)(cj >> 16));
-                        }
-                    }
+                    prdc_tally(cj, p.inside, jj, lane);
                 }
             }
             uint32_t bits[2] = {(uint32_t)cov[0] | ((uint32_t)rec[0] << 1), (uint32_t)cov[1] | ((uint32_t)rec[1] << 1)};
@@ -346,7 +301,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             };
             for (int ct = w.c0; ct < w.c1; ++ct) {
                 float sum[64];
-                kad_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
                 const int jj0 = sp.x + ct * 128 + 2 * (lane & 3);   // rows of Y
 #pragma unroll
                 for (int j = 0; j < 16; ++j) {
@@ -375,13 +330,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                             fl[1] |= b[1];
                         }
                     }
-                    if (__any_sync(0xffffffffu, cj != 0)) {
-                        for (int o = 4; o < 32; o <<= 1) cj += __shfl_xor_sync(0xffffffffu, cj, o);
-                        if (lane < 4) {
-                            if (cj & 0xFFFFu) atomicAdd(p.inside + jj, (int)(cj & 0xFFFFu));
-                            if (cj >> 16) atomicAdd(p.inside + jj + 1, (int)(cj >> 16));
-                        }
-                    }
+                    prdc_tally(cj, p.inside, jj, lane);
                 }
             }
             flush();
@@ -397,20 +346,6 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             named_bar_sync(1, 256);
         }
     }
-}
-
-// per-song passes: song_of[r] for the Y rows r < rows = the song s with offsets[s] <= r < offsets[s + 1]; -1 from n_total
-__global__ void prdc_song_of_kernel(const long long* __restrict__ offsets, long long n_items, long long n_total, int rows,
-                                    int* __restrict__ song_of) {
-    const int r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= rows) return;
-    if (r >= n_total) { song_of[r] = -1; return; }
-    long long lo = 0, hi = n_items;                 // offsets[lo] <= r < offsets[hi]
-    while (hi - lo > 1) {
-        const long long mid = (lo + hi) >> 1;
-        if (offsets[mid] <= r) lo = mid; else hi = mid;
-    }
-    song_of[r] = (int)lo;
 }
 
 // flags[i] = bit 0 covered, bit 1 recalled: a plane entry is the number of shards that set it (1 unsharded), so a
