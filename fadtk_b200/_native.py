@@ -116,6 +116,9 @@ SIGNATURES = {
     "fad_prdc_song_counts_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp,
                                                c_vp]),
     "fad_prdc_song_spans": (C.c_int, [c_vp, c_ll, c_ll, c_vp, c_vp]),
+    "fad_realism": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "fad_realism_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp,
+                                      c_vp, c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -869,6 +872,29 @@ class Engine:
         n = np.zeros(1, dtype=np.int64)
         _check(lib().fad_prdc_song_spans(off.ctypes.data, n_items, int(m), spans.ctypes.data, n.ctypes.data))
         return spans[:int(n[0])]
+
+    # ------------------------------------------- per-sample realism and nearest baseline row
+    def realism(self, z: torch.Tensor, m: int, k: int):
+        """z fp16 [m + n, d] (cuda, X rows first) -> (kept_radii_sq fp32 [m], realism fp32 [n], nearest int32 [n],
+        nearest_sq fp32 [n]) (cuda) and the threshold T (float): the pruned baseline radii, each eval row's realism
+        score, and its nearest baseline row and squared distance (fad_realism)."""
+        return self._realism(lib().fad_realism, (), z, m, k)
+
+    def realism_sharded(self, z: torch.Tensor, m: int, k: int, local_shards: int = 0):
+        """fad_realism_sharded: realism over shards (local_shards as for kad_sums_sharded)"""
+        return self._realism(lib().fad_realism_sharded, (None, int(local_shards)), z, m, k)
+
+    def _realism(self, fn, shard_args, z, m, k):
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        m, n = int(m), z.shape[0] - int(m)
+        kept = torch.empty(max(m, 0), dtype=torch.float32, device=z.device)
+        realism = torch.empty(max(n, 0), dtype=torch.float32, device=z.device)
+        nearest = torch.empty(max(n, 0), dtype=torch.int32, device=z.device)
+        nearest_sq = torch.empty(max(n, 0), dtype=torch.float32, device=z.device)
+        t = C.c_double(0.0)
+        _check(fn(self._h, *shard_args, z.data_ptr(), m, n, z.shape[1], int(k), kept.data_ptr(), realism.data_ptr(),
+                  nearest.data_ptr(), nearest_sq.data_ptr(), C.addressof(t), _stream()))
+        return kept, realism, nearest, nearest_sq, t.value
 
 
 class Baseline:

@@ -38,6 +38,17 @@
 // consumers popcount each song's words into song_counts[song][covered | recalled] (integer atomicAdd) and clear the
 // bitmap.  Each (X tile, song) pair belongs to one unit, so no (row, song) pair is counted twice.
 //
+// Realism (PASS 4, DESIGN.md 5.13).  Unit = (Y tile t, a run of X column tiles [c0, c1)), runs cut by the shape only as
+// in PASS 1.  The A operand is the 128-row box of Y at row m + 128 t, so each thread owns two eval rows and reduces
+// along the fragment's columns in registers over all the unit's tiles: no per-tile shuffle, no atomic.  Per row it
+// keeps the best quotient b = max r~_i^2 / q (r~_i^2, the pruned radius of column i, read through the read-only cache)
+// without a division per pair: fmaf(b, q, -r~^2) < 0 is the exact sign of b q - r~^2, and only then is b set to the
+// correctly rounded r~^2 / q, so b is exactly the max of fl(r~_i^2 / q) (r~^2 = 0 never improves; q = 0 < r~^2 gives
+// +inf; b = +inf, q = 0 gives NaN, which compares false).  And the nearest column (q, i) by a strict < in ascending
+// column order.  Columns j >= m (the last X tile runs into Y) count nothing.  At the end of the unit the quad merges
+// by a fixed xor tree (max; lexicographic min of (q, i)) and one lane writes the row's slot of this run in part; exactly
+// one unit writes each slot.  realism_reduce_kernel takes the max and the lexicographic min over the runs.
+//
 // Shards (pairwise_host.inc, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
 // shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
 // one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
@@ -76,6 +87,9 @@ struct PrdcParams {
     const long long* offsets;// [songs + 1] song s = Y rows [offsets[s], offsets[s + 1])
     const int4* spans;       // PASS 3: [cuts] {first Y row, end Y row, first song, songs}
     int* song_counts;        // PASS 3: [songs][2] covered, recalled baseline rows, zeroed by the host
+    // PASS 4: radii = [m] the pruned radii r~_i^2 of X; cuts = X column runs per Y tile: run i = X tiles
+    // [i Tx / cuts, (i + 1) Tx / cuts)
+    uint32_t* part;          // [3][cuts][n] out: per (run, Y row) the bits of the best quotient, of the nearest q, its index
 };
 
 // the tiles of unit u: A rows from arow, B tiles [c0, c1) at rows bbase + 128 c
@@ -97,10 +111,13 @@ __device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
     } else if constexpr (PASS == 1) {
         const int tx = u / p.cuts, i = u - tx * p.cuts;
         return {tx * 128, p.m, (int)((long long)i * p.Ty / p.cuts), (int)((long long)(i + 1) * p.Ty / p.cuts)};
-    } else {
+    } else if constexpr (PASS == 3) {
         const int tx = u / p.cuts;
         const int4 sp = p.spans[u - tx * p.cuts];
         return {tx * 128, p.m + sp.x, 0, (sp.y - sp.x + 127) / 128};
+    } else {
+        const int t = u / p.cuts, i = u - t * p.cuts;
+        return {p.m + 128 * t, 0, (int)((long long)i * p.Tx / p.cuts), (int)((long long)(i + 1) * p.Tx / p.cuts)};
     }
 }
 
@@ -158,7 +175,7 @@ template <int PASS>
 __global__ void __launch_bounds__(kPairThreads, 1)
 prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
     using namespace sm90;
-    static_assert(PASS >= 0 && PASS <= 3, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts");
+    static_assert(PASS >= 0 && PASS <= 4, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts, 4: realism");
     extern __shared__ uint8_t smem_raw[];
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -281,6 +298,47 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                     if (bits[i] & 2u) atomicOr(p.row_flags + p.m + row0 + 8 * i, 1);
                 }
             }
+        } else if constexpr (PASS == 4) {
+            float best[2] = {0.f, 0.f};                       // max r~^2 / q so far
+            float nq[2] = {INFINITY, INFINITY};               // the nearest column's q and index
+            int ni[2] = {INT_MAX, INT_MAX};
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                const int jj0 = ct * 128 + 2 * (lane & 3);    // rows of X
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int jj = jj0 + 8 * j;
+                    const float nc[2] = {__ldg(p.norm + jj), __ldg(p.norm + jj + 1)};
+                    const float r2[2] = {jj < p.m ? __ldg(p.radii + jj) : 0.f, jj + 1 < p.m ? __ldg(p.radii + jj + 1) : 0.f};
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const float q = pair_q(sum[4 * j + 2 * i + e], nr[i], nc[e]);
+                            if (fmaf(best[i], q, -r2[e]) < 0.f) best[i] = r2[e] / q;
+                            if (q < nq[i] && jj + e < p.m) { nq[i] = q; ni[i] = jj + e; }
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                for (int o = 1; o < 4; o <<= 1) {
+                    const float b = __shfl_xor_sync(0xffffffffu, best[i], o);
+                    const float oq = __shfl_xor_sync(0xffffffffu, nq[i], o);
+                    const int oi = __shfl_xor_sync(0xffffffffu, ni[i], o);
+                    best[i] = fmaxf(best[i], b);
+                    if (oq < nq[i] || (oq == nq[i] && oi < ni[i])) { nq[i] = oq; ni[i] = oi; }
+                }
+                const int r = row0 + 8 * i - p.m;             // row of Y
+                if ((lane & 3) == 0 && r < p.n) {
+                    const size_t slot = (size_t)(u % p.cuts) * p.n + r, plane = (size_t)p.cuts * p.n;
+                    p.part[slot] = __float_as_uint(best[i]);
+                    p.part[plane + slot] = __float_as_uint(nq[i]);
+                    p.part[2 * plane + slot] = (uint32_t)ni[i];
+                }
+            }
         } else {
             const int4 sp = p.spans[u % p.cuts];             // Y rows [sp.x, sp.y), songs [sp.z, sp.z + sp.w)
             const bool rv[2] = {row0 < p.m, row0 + 8 < p.m};
@@ -353,6 +411,31 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
 __global__ void prdc_flags_kernel(const int* __restrict__ row_flags, int m, unsigned char* __restrict__ flags) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < m) flags[i] = (unsigned char)((row_flags[i] != 0) | ((row_flags[m + i] != 0) << 1));
+}
+
+// realism: r~_i^2 = r_i^2 where r_i^2 <= t (the median, fp64), 0 otherwise, in place
+__global__ void realism_prune_kernel(float* __restrict__ radii_sq, int m, double t) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < m && !((double)radii_sq[i] <= t)) radii_sq[i] = 0.f;
+}
+
+// realism: per Y row the max of the runs' quotients and the lexicographic min of their (nearest q bits, index); both
+// exact, so the outputs do not depend on the cut or the grid
+__global__ void realism_reduce_kernel(const uint32_t* __restrict__ part, int cuts, int n, float* __restrict__ realism,
+                                      int* __restrict__ nearest, float* __restrict__ nearest_sq) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const size_t plane = (size_t)cuts * n;
+    float b = 0.f;
+    unsigned long long key = ~0ull;
+    for (int i = 0; i < cuts; ++i) {
+        const size_t s = (size_t)i * n + r;
+        b = fmaxf(b, __uint_as_float(part[s]));
+        key = min(key, ((unsigned long long)part[plane + s] << 32) | part[2 * plane + s]);
+    }
+    realism[r] = sqrtf(b);
+    nearest[r] = (int)(uint32_t)key;
+    nearest_sq[r] = __uint_as_float((uint32_t)(key >> 32));
 }
 
 }  // namespace fad

@@ -7,6 +7,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_kernel_audio_distance_songs                       -> the same, every song against one baseline in one pass
     calc_prdc                   (no reference counterpart) -> k-NN radii and ball-count tile kernels (csrc/prdc.cuh)
     calc_prdc_songs                                        -> the same, every song against one baseline in one pass
+    calc_realism                (no reference counterpart) -> k-NN radii and one max / argmin tile pass (csrc/prdc.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -90,6 +91,16 @@ class PRDCResults(NamedTuple):
     recall: float
     density: float
     coverage: float
+    k: int
+    n_baseline: int
+    n_eval: int
+
+
+class RealismResults(NamedTuple):
+    realism: np.ndarray             # float32 [n]
+    nearest: np.ndarray             # int64 [n], rows of the baseline
+    nearest_distance: np.ndarray    # float32 [n]
+    threshold_sq: float
     k: int
     n_baseline: int
     n_eval: int
@@ -270,10 +281,56 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> 
                        k=k, n_baseline=m, n_eval=n)
 
 
-def _prdc_k(k) -> int:
+def _prdc_k(k, metric: str = "PRDC") -> int:
     if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= 16:
-        raise ValueError(f"PRDC needs an integer k in [1, 16], not {k!r}")
+        raise ValueError(f"{metric} needs an integer k in [1, 16], not {k!r}")
     return int(k)
+
+
+def calc_realism(emb_baseline, emb_eval, k: int = 3, distributed: bool = False) -> RealismResults:
+    """Per-sample realism score (Kynkaanniemi et al., 2019) and nearest baseline row of every row of an eval set
+    Y [n, d] against a baseline X [m, d], both fp16 with the values taken as exact reals, q(a, b) = |a - b|^2:
+
+        r_i^2        = the k-NN radius of x_i within X, as calc_prdc defines it (self excluded by index),
+        T            = numpy.median of the m values r_i^2 in fp64 (for even m the fp64 mean of the two middle values),
+        r~_i^2       = r_i^2 where r_i^2 <= T, 0 otherwise (the half of the balls with the largest radii is dropped),
+        realism_j    = sqrt(max_i r~_i^2 / q(x_i, y_j)) over the rows with r~_i^2 > 0: +inf when such a row has
+                       q = 0 (y_j copies a kept baseline row), 0 when every r~_i^2 is 0; realism >= 1 means y_j lies in
+                       or on the edge of a kept ball,
+        nearest_j    = argmin_i q(x_i, y_j) over all rows of X, ties to the smallest i; nearest_distance_j its
+                       distance.
+
+    k defaults to the paper's 3.  The authors' code is reported to return the squared ratio with 1e-5 added to q; this
+    is the definition above.  realism_j and nearest_j depend on y_j and X alone, so the rows of several eval sets
+    scored in one call get the values separate calls give.  The radii and one pass over all (x, y) pairs run on the GPU
+    (fad_realism) without forming a distance matrix.  A width that is not a multiple of 8 is zero-padded.  Raises
+    ValueError for k outside [1, 16], m <= k, n < 1, non-fp16 or non-2-D input, mismatched widths, and T = 0 (more than
+    half of the baseline rows have k exact duplicates).  distributed: as for calc_prdc (fad_realism_sharded)."""
+    k = _prdc_k(k, "realism")
+    x, y = _kad_rows(emb_baseline, "baseline", "realism"), _kad_rows(emb_eval, "eval", "realism")
+    m, n = int(x.shape[0]), int(y.shape[0])
+    _realism_rows(m, n, k)
+    if x.shape[1] != y.shape[1]:
+        raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
+    return _realism(torch.cat([x, y]), m, k, distributed)
+
+
+def _realism_rows(m: int, n: int, k: int):
+    if m <= k or n < 1:
+        raise ValueError(f"realism with k = {k} needs more than k baseline rows and at least one eval row "
+                         f"(baseline {m}, eval {n})")
+
+
+def _realism(z: torch.Tensor, m: int, k: int, distributed: bool = False) -> RealismResults:
+    """z = [X; Y] fp16 (host or device) -> RealismResults of the rows after X"""
+    eng, collective = _kad_engine(distributed, "realism")
+    z = _kad_device_rows(z, eng)
+    _, realism, nearest, nearest_sq, t = eng.realism_sharded(z, m, k) if collective else eng.realism(z, m, k)
+    if not t > 0.0:
+        raise ValueError("realism threshold is 0: more than half of the baseline rows have k exact duplicates")
+    return RealismResults(realism=realism.cpu().numpy(), nearest=nearest.cpu().numpy().astype(np.int64),
+                          nearest_distance=np.sqrt(nearest_sq.cpu().numpy()), threshold_sq=float(t), k=k,
+                          n_baseline=m, n_eval=int(z.shape[0]) - m)
 
 
 def calc_prdc_songs(emb_baseline, songs, k: int = 5, distributed: bool = False) -> list[PRDCResults]:
@@ -691,8 +748,8 @@ class FrechetAudioDistance:
                 log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
-        x, host, offs, names = self._individual_sets(baseline_dir, eval_dir, "KAD", 2, "at least two embedding rows",
-                                                     collective, writer)
+        x, host, offs, names, _, _ = self._individual_sets(baseline_dir, eval_dir, "KAD", 2,
+                                                           "at least two embedding rows", collective, writer)
         pairs = []
         if names:
             res = _kad_songs(host, x.shape[0], offs, distributed)
@@ -727,8 +784,8 @@ class FrechetAudioDistance:
                 log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
-        x, host, offs, names = self._individual_sets(baseline_dir, eval_dir, "PRDC", k + 1,
-                                                     f"more than k = {k} embedding rows", collective, writer)
+        x, host, offs, names, _, _ = self._individual_sets(baseline_dir, eval_dir, "PRDC", k + 1,
+                                                           f"more than k = {k} embedding rows", collective, writer)
         rows = []
         if names:
             res = _prdc_songs(host, x.shape[0], np.diff(offs).tolist(), k, distributed)
@@ -746,19 +803,67 @@ class FrechetAudioDistance:
         csv.write_text("\n".join(lines) + "\n")
         return csv
 
+    def score_realism_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
+                                 k: int = 3, distributed: bool = False) -> Path:
+        """Realism and nearest baseline clip of every file in eval_dir against the embeddings of baseline_dir: one
+        calc_realism call over the rows of all files (a row's values depend on that row and the baseline alone).  The
+        table has the header ``file,realism_median,realism_min,nearest_baseline,nearest_distance,n_eval`` and one row
+        per file: the median and the least realism of its rows, the baseline embedding cache that holds the nearest
+        baseline row of its nearest row, and that distance.  Rows are sorted by realism_median, least realistic first,
+        ties by path; commas in names are replaced.  A str csv_name goes under data/realism-individual/<model>/, and an
+        existing table is returned untouched.  Files whose cache is missing, unreadable, not an fp16 [rows, d] array of
+        the baseline's width, or empty are logged and dropped.  distributed=True under torchrun: as for
+        score_kad_individual, over the radii and realism tiles."""
+        k = _prdc_k(k, "realism")
+        csv = Path(csv_name)
+        if isinstance(csv_name, str):
+            csv = Path('data') / 'realism-individual' / self.ml.name / csv_name
+        collective = distributed and _kad_engine(True, "realism")[1]
+        from . import dist
+        writer = not collective or dist.rank() == 0
+        if _on_rank0(csv.exists, collective):
+            if writer:
+                log.info(f"CSV file {csv} already exists, exiting...")
+            return csv
+
+        x, host, offs, names, base_files, base_offs = self._individual_sets(
+            baseline_dir, eval_dir, "realism", 1, "at least one embedding row", collective, writer)
+        _realism_rows(x.shape[0], 1, k)
+        rows = []
+        if names:
+            res = _realism(host, x.shape[0], k, distributed)
+            for s, f in enumerate(names):
+                if f is None:
+                    continue
+                a, b = int(offs[s]), int(offs[s + 1])
+                real = res.realism[a:b].astype(np.float64)
+                j = a + int(np.argmin(res.nearest_distance[a:b]))
+                base = base_files[int(np.searchsorted(base_offs, res.nearest[j], side="right")) - 1]
+                rows.append((f, float(np.median(real)), float(real.min()), base, float(res.nearest_distance[j]), b - a))
+
+        if not writer:
+            return csv
+        rows.sort(key=lambda t: (t[1], str(t[0])))
+        csv.parent.mkdir(parents=True, exist_ok=True)
+        lines = ["file,realism_median,realism_min,nearest_baseline,nearest_distance,n_eval"]
+        lines += [",".join(str(v).replace(',', '_') for v in row) for row in rows]
+        csv.write_text("\n".join(lines) + "\n")
+        return csv
+
     def _individual_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, min_rows: int, need: str,
                          collective: bool, writer: bool):
-        """The embeddings score_kad_individual and score_prdc_individual score -> (x, host, offs, names): x the
+        """The embeddings the score_*_individual methods score -> (x, host, offs, names, base_files, base_offs): x the
         baseline's fp16 rows; host = [x; the kept files' rows] fp16 (pinned when there is a GPU), offs their int64
         offsets after x, names[k] the file of kept song k, or None when its cache could not be read (its rows are
-        zeros: score it and drop it).  A file is kept when its cache is an fp16 [rows, d] array of the baseline's width
-        with at least min_rows rows (`need` says so in the log); the others are logged (by the writer) and dropped.
+        zeros: score it and drop it); base_files the baseline's cache files, base_offs their int64 row offsets in x.  A
+        file is kept when its cache is an fp16 [rows, d] array of the baseline's width with at least min_rows rows
+        (`need` says so in the log); the others are logged (by the writer) and dropped.
         Collective: rank 0 lists the directories, every rank reads the caches."""
         from . import _io_native
         files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name, metric)), collective)
         if not files:
             raise ValueError(f"no {self.ml.name} embeddings cached under {baseline_dir}: embed the baseline directory first")
-        x, _ = _io_native.load_embedding_files(files, self.audio_load_worker)
+        x, base_offs = _io_native.load_embedding_files(files, self.audio_load_worker)
         if x.dtype != np.float16:
             raise ValueError(f"{metric} needs fp16 embedding caches; {baseline_dir} holds {x.dtype}")
         kad_embedding_dir(eval_dir, self.ml.name, metric)
@@ -787,7 +892,7 @@ class FrechetAudioDistance:
             else:
                 keep.append(i)
         if not keep:
-            return x, None, None, []
+            return x, None, None, [], files, base_offs
         rows = n_rows[keep]
         offs = np.zeros(len(keep) + 1, dtype=np.int64)
         offs[1:] = np.cumsum(rows)
@@ -798,7 +903,8 @@ class FrechetAudioDistance:
         for k in np.nonzero(st != _io_native.OK)[0]:     # vanished / rewritten since the probe: dropped by the caller
             _report(all_files[keep[k]], f"cannot read {caches[keep[k]]} (status {int(st[k])})")
             host[m + offs[k]:m + offs[k + 1]] = 0.0
-        return x, host, offs, [all_files[i] if st[k] == _io_native.OK else None for k, i in enumerate(keep)]
+        return (x, host, offs, [all_files[i] if st[k] == _io_native.OK else None for k, i in enumerate(keep)], files,
+                base_offs)
 
     def score_inf(self, baseline: PathLike, eval_files: list[Path], steps: int = 25, min_n=500, raw: bool = False):
         """FAD for growing sample counts and the FAD-inf extrapolation (fad.py:304-351).

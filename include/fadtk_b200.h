@@ -410,6 +410,25 @@ int fad_prdc_song_counts_sharded(fad_handle* h, void* nccl_comm_or_null, int loc
                                  long long m, const long long* offsets, long long n_items, int d,
                                  const float* radii_sq, int* inside, int* song_counts, void* stream);
 int fad_prdc_song_spans(const long long* offsets, long long n_items, long long m, long long* spans, long long* n_spans);
+/* Per-sample realism (Kynkaanniemi et al. 2019) and nearest baseline row of each eval row (DESIGN.md section 5.13):
+ * z = [X; Y] (fp16 [m + n, d], X first, 16-byte aligned), d a multiple of 8, q as for PRDC.  Every argument is checked
+ * first (null or misaligned pointers, 1 <= k <= 16, m > k, n >= 1, d, at most 2^30 rows); a rejected call launches
+ * nothing and writes nothing.  The radii are read back to the host, so the call synchronises the stream once.
+ *   kept_radii_sq (device fp32 [m]) = r~_i^2: r_i^2, the radius fad_knn_radii_sq gives row i of X (bitwise), where
+ *                 r_i^2 <= T and 0 otherwise; T = numpy.median of the m values r_i^2 in fp64 (for even m the fp64 mean of
+ *                 the two middle values), also written to *threshold_sq (host fp64)
+ *   realism       (device fp32 [n]) = sqrt(max_i r~_i^2 / q(x_i, y_j)) over the rows with r~_i^2 > 0: +inf where such a
+ *                 row has q = 0, 0 where every r~_i^2 is 0 (fl(sqrt(max_i fl(r~_i^2 / q))), exactly)
+ *   nearest       (device int32 [n]) = argmin_i q(x_i, y_j) over all rows of X, ties to the smallest i;
+ *   nearest_sq    (device fp32 [n]) = that q
+ * All outputs are bitwise reproducible and depend on y_j and X alone.  fad_realism_sharded splits the tile work as
+ * fad_knn_radii_sq_sharded does (local_shards as for fad_kad_*_sharded; collective calls compare m, n, d, k and a digest
+ * of z), bitwise equal to fad_realism, which is its local_shards = 1 case. */
+int fad_realism(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, float* kept_radii_sq,
+                float* realism, int* nearest, float* nearest_sq, double* threshold_sq, void* stream);
+int fad_realism_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                        long long n, int d, int k, float* kept_radii_sq, float* realism, int* nearest, float* nearest_sq,
+                        double* threshold_sq, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
