@@ -119,6 +119,9 @@ SIGNATURES = {
     "fad_realism": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp, c_vp]),
     "fad_realism_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_vp, c_vp, c_vp,
                                       c_vp, c_vp]),
+    "fad_nearest": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_vp, c_vp]),
+    "fad_nearest_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_vp,
+                                      c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -895,6 +898,31 @@ class Engine:
         _check(fn(self._h, *shard_args, z.data_ptr(), m, n, z.shape[1], int(k), kept.data_ptr(), realism.data_ptr(),
                   nearest.data_ptr(), nearest_sq.data_ptr(), C.addressof(t), _stream()))
         return kept, realism, nearest, nearest_sq, t.value
+
+    # ------------------------------------------- k nearest distinct baseline groups
+    def nearest(self, z: torch.Tensor, m: int, k: int, offsets: "torch.Tensor | None" = None):
+        """z fp16 [m + n, d] (cuda, X rows first), offsets int64 [groups + 1] (cuda) or None (every baseline row its own
+        group) -> (nearest int32 [n, k], nearest_sq fp32 [n, k]) (cuda): per eval row the k nearest distinct groups of
+        X, each as the row and q of its nearest row, ascending; -1 / +inf past the last non-empty group (fad_nearest)."""
+        return self._nearest(lib().fad_nearest, (), z, m, k, offsets)
+
+    def nearest_sharded(self, z: torch.Tensor, m: int, k: int, offsets: "torch.Tensor | None" = None,
+                        local_shards: int = 0):
+        """fad_nearest_sharded: nearest over shards (local_shards as for kad_sums_sharded)"""
+        return self._nearest(lib().fad_nearest_sharded, (None, int(local_shards)), z, m, k, offsets)
+
+    def _nearest(self, fn, shard_args, z, m, k, offsets):
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        m, n = int(m), z.shape[0] - int(m)
+        shape = (max(n, 0), max(int(k), 0))
+        nearest = torch.empty(shape, dtype=torch.int32, device=z.device)
+        nearest_sq = torch.empty(shape, dtype=torch.float32, device=z.device)
+        if offsets is not None:
+            assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous()
+        off, groups = (None, 0) if offsets is None else (offsets.data_ptr(), offsets.numel() - 1)
+        _check(fn(self._h, *shard_args, z.data_ptr(), m, n, z.shape[1], int(k), off, groups, nearest.data_ptr(),
+                  nearest_sq.data_ptr(), _stream()))
+        return nearest, nearest_sq
 
 
 class Baseline:

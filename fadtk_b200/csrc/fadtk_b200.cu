@@ -201,7 +201,7 @@ struct fad_handle {
     DeviceBuffer fr_buf;                            // Frechet (FrechetWorkspace)
     DeviceBuffer rs_bank, rs_mono;                  // resampler filter bank and mono mix
     int rs_in = 0, rs_out = 0;                      // the rate pair of rs_bank
-    DeviceBuffer pair_buf;                          // fad_kad_*, fad_knn_radii_sq, fad_prdc_counts, fad_realism (pair_prepare)
+    DeviceBuffer pair_buf;                          // fad_kad_*, fad_knn_radii_sq, fad_prdc_counts, fad_realism, fad_nearest (pair_prepare)
     DeviceBuffer agree_buf;                         // the sharded entries: the ranks' argument descriptor (agree)
     // hi/lo weight tensors whose lo parts are all zero, by address (note_split_weights).  Every hi/lo tensor is noted
     // at its current address before any GEMM reads it: upload_split and fad_vggish_load note each one they upload,
@@ -573,6 +573,7 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::prdc_tile_kernel<2>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<3>, fad::kPrdcSongSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<4>, fad::kPairSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<5>, fad::kPrdcNearestSmemBytes));
     if (setup_gemm<0>(h.get()) || setup_gemm<1>(h.get())) return 1;
     *out = h.release();
     return 0;

@@ -49,6 +49,20 @@
 // by a fixed xor tree (max; lexicographic min of (q, i)) and one lane writes the row's slot of this run in part; exactly
 // one unit writes each slot.  realism_reduce_kernel takes the max and the lexicographic min over the runs.
 //
+// Nearest groups (PASS 5, DESIGN.md 5.14).  The units, the orientation and the masks of PASS 4.  The baseline rows are
+// cut into groups (contiguous row ranges, song_of = the group of each X row, offsets = the group bounds); per eval row
+// the thread keeps the k nearest distinct groups, each by its smallest key (q, row of X), in a sorted list: the q values
+// in registers as prdc_insert keeps them (dead entries -inf, empty ones +inf, the k-th at index 15), the rows in the
+// kernel's own shared memory (a second list of 16 in registers would spill next to the accumulators).  The common path
+// is one compare of q with the k-th q: the thread walks its columns in ascending row order, so a candidate with an equal
+// q has the larger key.  The fragment loop only marks such candidates in a mask per row, drained in ascending order at
+// one insertion site per row (inlined at every fragment position the kernel ran 11 x slower, out of the instruction
+// cache).  Only a candidate that beats the k-th reads its group's bounds (nearest_insert).  At the end of the
+// unit the quad merges by a fixed xor tree with the same insertion on full keys, and one lane writes the row's k entries
+// of this run in part; exactly one unit writes each slot.  nearest_reduce_kernel merges the runs the same way.  The top
+// k groups of a union of column sets are the top k of the merged top-k lists (a group in the union's top k is in the
+// top k of the set that attains its minimum), and keys are distinct, so every result is exact and grid-independent.
+//
 // Shards (pairwise_host.inc, DESIGN.md 5.12).  A launch runs the units [unit0, unit1).  A radii unit owns whole rows, so a
 // shard writes exactly its units' radii; a counts shard adds into its own inside and row_flags.  The flags are kept as
 // one 0/1 plane per bit, not as packed bits, so that the host can add the shards' copies and read "nonzero" as OR.
@@ -67,6 +81,10 @@ constexpr int kPrdcSpanSongs = 512;
 constexpr uint32_t kPrdcBitmapWords = kPrdcSpanSongs * 4 * 2;
 constexpr uint32_t kPrdcSongSmemBytes = kPairSmemBytes + kPrdcBitmapWords * 4;
 static_assert(kPrdcSongSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
+// PASS 5: the rows of each consumer thread's two lists, [entry][list][consumer thread] words after the barriers
+constexpr int kNearestListStride = 2 * 256;
+constexpr uint32_t kPrdcNearestSmemBytes = kPairSmemBytes + kPrdcMaxK * kNearestListStride * 4;
+static_assert(kPrdcNearestSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
 
 struct PrdcParams {
     int m, n, d;             // rows of X, rows of Y, columns
@@ -90,6 +108,8 @@ struct PrdcParams {
     // PASS 4: radii = [m] the pruned radii r~_i^2 of X; cuts = X column runs per Y tile: run i = X tiles
     // [i Tx / cuts, (i + 1) Tx / cuts)
     uint32_t* part;          // [3][cuts][n] out: per (run, Y row) the bits of the best quotient, of the nearest q, its index
+    // PASS 5: cuts as PASS 4; song_of = [Tx * 128] the group of each X row, offsets = [groups + 1] the group bounds in X;
+    // part = [2][cuts][n][k] out: per (run, Y row) the k entries' q bits, then their rows (+inf bits, 0xFFFFFFFF: empty)
 };
 
 // the tiles of unit u: A rows from arow, B tiles [c0, c1) at rows bbase + 128 c
@@ -150,6 +170,60 @@ __device__ __forceinline__ void prdc_topk_merge(float (&a)[2][kPrdcMaxK]) {
     }
 }
 
+// nearest groups: the rows of a list, in the kernel's shared memory (stride kNearestListStride) or in registers; the
+// index is always a compile-time constant
+struct NearestSmemRows {
+    uint32_t* p;
+    __device__ __forceinline__ uint32_t get(int t) const { return p[t * kNearestListStride]; }
+    __device__ __forceinline__ void set(int t, uint32_t v) const { p[t * kNearestListStride] = v; }
+};
+struct NearestRegRows {
+    uint32_t (&r)[kPrdcMaxK];
+    __device__ __forceinline__ uint32_t get(int t) const { return r[t]; }
+    __device__ __forceinline__ void set(int t, uint32_t v) const { r[t] = v; }
+};
+
+// key (q, row) below key (qb, rb): the fp32 order of q >= 0, then the row
+__device__ __forceinline__ bool nearest_less(float q, uint32_t row, float qb, uint32_t rb) {
+    return q < qb || (q == qb && row < rb);
+}
+
+// a[0..15] / r ascending by key, the live entries last as in prdc_insert (dead: -inf, empty: +inf, both row 0xFFFFFFFF,
+// which lies in no group), at most one entry per group.  The candidate (q, row), row < m, has a key below the k-th
+// (a[15], r[15]).  If its group has an entry, the candidate replaces it when its key is smaller and is dropped
+// otherwise; else it replaces the k-th entry.  One compare-exchange sweep then moves it to its place.
+template <typename Rows>
+__device__ __forceinline__ void nearest_insert(float (&a)[kPrdcMaxK], const Rows& r, float q, uint32_t row,
+                                               const int* __restrict__ song_of, const long long* __restrict__ offsets) {
+    const int g = __ldg(song_of + row);
+    const uint32_t lo = (uint32_t)__ldg(offsets + g), span = (uint32_t)__ldg(offsets + g + 1) - lo;
+    int at = kPrdcMaxK - 1;
+    bool drop = false;
+#pragma unroll
+    for (int t = 0; t < kPrdcMaxK; ++t) {
+        const uint32_t rt = r.get(t);
+        if (rt - lo < span) {
+            if (nearest_less(a[t], rt, q, row)) drop = true;
+            else at = t;
+        }
+    }
+    if (drop) return;
+#pragma unroll
+    for (int t = 0; t < kPrdcMaxK; ++t)
+        if (t == at) { a[t] = q; r.set(t, row); }
+#pragma unroll
+    for (int s = kPrdcMaxK - 1; s > 0; --s) {
+        if (s <= at && (a[s - 1] > a[s] || (a[s - 1] == a[s] && r.get(s - 1) > r.get(s)))) {
+            const float t = a[s - 1];
+            a[s - 1] = a[s];
+            a[s] = t;
+            const uint32_t lo_row = r.get(s), hi_row = r.get(s - 1);
+            r.set(s - 1, lo_row);
+            r.set(s, hi_row);
+        }
+    }
+}
+
 // counts: the decisions of one xy pair from its dot product and norms, bit 0 q < r2 (where the column counts), bit 1
 // q < s2 (where the row counts).  r2 = 0 for a row past m and s2 = 0 for a column that does not count: q < 0 is never
 // true
@@ -175,7 +249,8 @@ template <int PASS>
 __global__ void __launch_bounds__(kPairThreads, 1)
 prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
     using namespace sm90;
-    static_assert(PASS >= 0 && PASS <= 4, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts, 4: realism");
+    static_assert(PASS >= 0 && PASS <= 5,
+                  "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts, 4: realism, 5: nearest groups");
     extern __shared__ uint8_t smem_raw[];
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -339,6 +414,86 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
                     p.part[2 * plane + slot] = (uint32_t)ni[i];
                 }
             }
+        } else if constexpr (PASS == 5) {
+            // list i: q values in a[i], rows in shared memory at [t][i][consumer thread]
+            const NearestSmemRows rows[2] = {{reinterpret_cast<uint32_t*>(pt.own) + (threadIdx.x - 128)},
+                                             {reinterpret_cast<uint32_t*>(pt.own) + 256 + (threadIdx.x - 128)}};
+            float a[2][kPrdcMaxK];
+#pragma unroll
+            for (int t = 0; t < kPrdcMaxK; ++t) {
+                a[0][t] = a[1][t] = t < kPrdcMaxK - p.k ? -INFINITY : INFINITY;
+                rows[0].set(t, 0xFFFFFFFFu);
+                rows[1].set(t, 0xFFFFFFFFu);
+            }
+            for (int ct = w.c0; ct < w.c1; ++ct) {
+                float sum[64];
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                const int jj0 = ct * 128 + 2 * (lane & 3);    // rows of X: column 2 j + e of the thread is row jj0 + 8 j + e
+                // q in place of the dot products; hit[i] bit 2 j + e: the pair beats row i's k-th q
+                uint32_t hit[2] = {0u, 0u};
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const int jj = jj0 + 8 * j;
+                    const float nc[2] = {__ldg(p.norm + jj), __ldg(p.norm + jj + 1)};
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+#pragma unroll
+                        for (int i = 0; i < 2; ++i) {
+                            const float q = pair_q(sum[4 * j + 2 * i + e], nr[i], nc[e]);
+                            sum[4 * j + 2 * i + e] = q;
+                            if (q < a[i][kPrdcMaxK - 1] && jj + e < p.m) hit[i] |= 1u << (2 * j + e);
+                        }
+                    }
+                }
+                // the candidates in ascending row order, each against the k-th as it is then: one insertion site per
+                // row, so the unrolled loop above stays small
+#pragma unroll
+                for (int i = 0; i < 2; ++i) {
+                    while (hit[i]) {
+                        const int b = __ffs(hit[i]) - 1;
+                        hit[i] &= hit[i] - 1;
+                        float q = 0.f;
+#pragma unroll
+                        for (int t = 0; t < 32; ++t)
+                            if (t == b) q = sum[4 * (t >> 1) + 2 * i + (t & 1)];
+                        if (q < a[i][kPrdcMaxK - 1])
+                            nearest_insert(a[i], rows[i], q, (uint32_t)(jj0 + 8 * (b >> 1) + (b & 1)), p.song_of, p.offsets);
+                    }
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                for (int o = 1; o < 4; o <<= 1) {
+                    float bq[kPrdcMaxK];
+                    uint32_t br[kPrdcMaxK];
+#pragma unroll
+                    for (int t = 0; t < kPrdcMaxK; ++t) {
+                        bq[t] = __shfl_xor_sync(0xffffffffu, a[i][t], o);
+                        br[t] = __shfl_xor_sync(0xffffffffu, rows[i].get(t), o);
+                    }
+                    // the partner's live entries, ascending: the first that does not beat the k-th ends the merge
+                    for (int t = kPrdcMaxK - p.k; t < kPrdcMaxK; ++t) {
+                        float q = 0.f;
+                        uint32_t row = 0u;
+#pragma unroll
+                        for (int v = 0; v < kPrdcMaxK; ++v)
+                            if (v == t) { q = bq[v]; row = br[v]; }
+                        if (!nearest_less(q, row, a[i][kPrdcMaxK - 1], rows[i].get(kPrdcMaxK - 1))) break;
+                        nearest_insert(a[i], rows[i], q, row, p.song_of, p.offsets);
+                    }
+                }
+                const int r = row0 + 8 * i - p.m;             // row of Y
+                if ((lane & 3) == 0 && r < p.n) {
+                    const size_t slot = ((size_t)(u % p.cuts) * p.n + r) * p.k, plane = (size_t)p.cuts * p.n * p.k;
+#pragma unroll
+                    for (int t = 0; t < kPrdcMaxK; ++t) {
+                        if (t >= kPrdcMaxK - p.k) {
+                            p.part[slot + t - (kPrdcMaxK - p.k)] = __float_as_uint(a[i][t]);
+                            p.part[plane + slot + t - (kPrdcMaxK - p.k)] = rows[i].get(t);
+                        }
+                    }
+                }
+            }
         } else {
             const int4 sp = p.spans[u % p.cuts];             // Y rows [sp.x, sp.y), songs [sp.z, sp.z + sp.w)
             const bool rv[2] = {row0 < p.m, row0 + 8 < p.m};
@@ -436,6 +591,41 @@ __global__ void realism_reduce_kernel(const uint32_t* __restrict__ part, int cut
     realism[r] = sqrtf(b);
     nearest[r] = (int)(uint32_t)key;
     nearest_sq[r] = __uint_as_float((uint32_t)(key >> 32));
+}
+
+// nearest groups: per Y row the runs' lists (part as PASS 5 writes it) merged by nearest_insert in run order, each
+// list's entries ascending, so the first that does not beat the k-th ends it; nearest [n][k] = the rows (-1: empty),
+// nearest_sq [n][k] = their q (+inf: empty)
+__global__ void nearest_reduce_kernel(const uint32_t* __restrict__ part, int cuts, int n, int k,
+                                      const int* __restrict__ song_of, const long long* __restrict__ offsets,
+                                      int* __restrict__ nearest, float* __restrict__ nearest_sq) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    float a[kPrdcMaxK];
+    uint32_t rows[kPrdcMaxK];
+#pragma unroll
+    for (int t = 0; t < kPrdcMaxK; ++t) {
+        a[t] = t < kPrdcMaxK - k ? -INFINITY : INFINITY;
+        rows[t] = 0xFFFFFFFFu;
+    }
+    const NearestRegRows list{rows};
+    const size_t plane = (size_t)cuts * n * k;
+    for (int i = 0; i < cuts; ++i) {
+        const size_t s = ((size_t)i * n + r) * k;
+        for (int t = 0; t < k; ++t) {
+            const float q = __uint_as_float(part[s + t]);
+            const uint32_t row = part[plane + s + t];
+            if (!nearest_less(q, row, a[kPrdcMaxK - 1], rows[kPrdcMaxK - 1])) break;
+            nearest_insert(a, list, q, row, song_of, offsets);
+        }
+    }
+#pragma unroll
+    for (int t = 0; t < kPrdcMaxK; ++t) {
+        if (t >= kPrdcMaxK - k) {
+            nearest[(size_t)r * k + t - (kPrdcMaxK - k)] = (int)rows[t];
+            nearest_sq[(size_t)r * k + t - (kPrdcMaxK - k)] = a[t];
+        }
+    }
 }
 
 }  // namespace fad

@@ -8,6 +8,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_prdc                   (no reference counterpart) -> k-NN radii and ball-count tile kernels (csrc/prdc.cuh)
     calc_prdc_songs                                        -> the same, every song against one baseline in one pass
     calc_realism                (no reference counterpart) -> k-NN radii and one max / argmin tile pass (csrc/prdc.cuh)
+    calc_nearest                (no reference counterpart) -> one distinct-group top-k tile pass (csrc/prdc.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -101,6 +102,15 @@ class RealismResults(NamedTuple):
     nearest: np.ndarray             # int64 [n], rows of the baseline
     nearest_distance: np.ndarray    # float32 [n]
     threshold_sq: float
+    k: int
+    n_baseline: int
+    n_eval: int
+
+
+class NearestResults(NamedTuple):
+    rows: np.ndarray                # int64 [n, k], rows of the baseline, -1 past the last non-empty group
+    groups: np.ndarray              # int64 [n, k], the groups of those rows, -1 likewise
+    distance: np.ndarray            # float32 [n, k], +inf likewise
     k: int
     n_baseline: int
     n_eval: int
@@ -331,6 +341,82 @@ def _realism(z: torch.Tensor, m: int, k: int, distributed: bool = False) -> Real
     return RealismResults(realism=realism.cpu().numpy(), nearest=nearest.cpu().numpy().astype(np.int64),
                           nearest_distance=np.sqrt(nearest_sq.cpu().numpy()), threshold_sq=float(t), k=k,
                           n_baseline=m, n_eval=int(z.shape[0]) - m)
+
+
+def calc_nearest(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> NearestResults:
+    """The k nearest distinct baseline groups of every row of an eval set Y [n, d]: a memorisation audit, "which
+    baseline clips does this generated frame come closest to, and where".  emb_baseline is one fp16 [m, d] array, each
+    row its own group (a plain k-NN), or a list of fp16 [m_g, d] arrays, one group each (e.g. one per baseline file;
+    empty arrays are empty groups).  With the fp16 values taken as exact reals and q(a, b) = |a - b|^2, the baseline
+    rows are ordered for y_j by the key (q(x_i, y_j), i); each group is represented by its smallest key, and the k groups
+    with the smallest representative keys are returned, ascending:
+
+        rows[j, r]     = the baseline row (index into all baseline rows, in order) of the r-th group's smallest key,
+        groups[j, r]   = that group,
+        distance[j, r] = sqrt(q) of that pair,
+
+    with -1, -1, +inf where fewer than k groups are non-empty.  The nearest rows of an eval frame are mostly
+    neighbouring frames of one clip; distinct groups give k different clips instead.  Each row's result depends on that
+    row and the baseline alone, so several eval sets scored in one call get the values separate calls give.  With k = 1
+    and one array, rows[:, 0] and distance[:, 0] are calc_realism's nearest and nearest_distance.  One GPU pass over all
+    (x, y) pairs (fad_nearest) keeps the lists in registers; no distance matrix is formed.  A width that is not a
+    multiple of 8 is zero-padded.  Raises ValueError for k outside [1, 16], no baseline or no eval rows, non-fp16 or
+    non-2-D input and mismatched widths.  distributed: as for calc_prdc (fad_nearest_sharded)."""
+    k = _prdc_k(k, "nearest")
+    parts = list(emb_baseline) if isinstance(emb_baseline, (list, tuple)) else [emb_baseline]
+    if not parts:
+        raise ValueError("nearest needs at least one baseline group")
+    xs = [_kad_rows(p, "baseline", "nearest") for p in parts]
+    y = _kad_rows(emb_eval, "eval", "nearest")
+    for x in xs:
+        if x.shape[1] != y.shape[1]:
+            raise ValueError(f"embedding widths differ (baseline {x.shape[1]}, eval {y.shape[1]})")
+    offsets = None
+    if isinstance(emb_baseline, (list, tuple)):
+        offsets = np.zeros(len(xs) + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([x.shape[0] for x in xs])
+    x = torch.cat(xs) if len(xs) > 1 else xs[0]
+    m, n = int(x.shape[0]), int(y.shape[0])
+    _nearest_rows(m, n)
+    return _nearest(torch.cat([x, y]), m, k, offsets, distributed)[0]
+
+
+def _nearest_rows(m: int, n: int):
+    if m < 1 or n < 1:
+        raise ValueError(f"nearest needs at least one baseline row and one eval row (baseline {m}, eval {n})")
+
+
+def _nearest(z: torch.Tensor, m: int, k: int, offsets, distributed: bool = False):
+    """z = [X; Y] fp16 (host or device), offsets int64 [groups + 1] of X or None -> (NearestResults of the rows after
+    X, the squared distances fp32 [n, k])"""
+    eng, collective = _kad_engine(distributed, "nearest")
+    z = _kad_device_rows(z, eng)
+    off = None if offsets is None else torch.from_numpy(np.asarray(offsets, dtype=np.int64)).to(eng.torch_device)
+    rows, q = eng.nearest_sharded(z, m, k, off) if collective else eng.nearest(z, m, k, off)
+    rows, q = rows.cpu().numpy().astype(np.int64), q.cpu().numpy()
+    if offsets is None:
+        groups = rows.copy()
+    else:
+        groups = np.where(rows >= 0, np.searchsorted(np.asarray(offsets), rows, side="right") - 1, -1)
+    res = NearestResults(rows=rows, groups=groups, distance=np.sqrt(q), k=k, n_baseline=m, n_eval=int(z.shape[0]) - m)
+    return res, q
+
+
+def _file_nearest(groups: np.ndarray, rows: np.ndarray, q: np.ndarray, k: int) -> list:
+    """The k nearest groups of a file of eval rows from the rows' lists (groups, rows, q [rows, k]): per group the
+    smallest (q, eval row, baseline row) over the file, the groups ranked by that triple -> [(eval row, slot)] of the
+    first k.  Merging the rows' lists gives exactly this: a group in the file's top k is in the top k of the row that
+    attains its minimum, since every group ahead of it at that row is ahead of it for the file."""
+    j, r = np.nonzero(rows >= 0)
+    out, seen = [], set()
+    for e in np.lexsort((rows[j, r], j, q[j, r])):
+        g = int(groups[j[e], r[e]])
+        if g not in seen:
+            seen.add(g)
+            out.append((int(j[e]), int(r[e])))
+            if len(out) == k:
+                break
+    return out
 
 
 def calc_prdc_songs(emb_baseline, songs, k: int = 5, distributed: bool = False) -> list[PRDCResults]:
@@ -847,6 +933,55 @@ class FrechetAudioDistance:
         csv.parent.mkdir(parents=True, exist_ok=True)
         lines = ["file,realism_median,realism_min,nearest_baseline,nearest_distance,n_eval"]
         lines += [",".join(str(v).replace(',', '_') for v in row) for row in rows]
+        csv.write_text("\n".join(lines) + "\n")
+        return csv
+
+    def score_nearest_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
+                                 k: int = 5, distributed: bool = False) -> Path:
+        """The k baseline files every file of eval_dir comes closest to: a memorisation audit.  One calc_nearest call
+        over the rows of all eval files, with each baseline embedding cache one group; then per eval file, per baseline
+        file, the smallest (distance, eval row, baseline row) over the file's rows, and the first k baseline files in
+        that order.  The table has the header ``file,rank,nearest_baseline,distance,eval_row,baseline_row,n_eval`` and
+        one line per (file, rank): the baseline cache, the distance and the pair of rows (each within its own file)
+        where the two come closest.  Files are sorted by their rank-1 distance, closest (most copy-like) first, ties by
+        path; commas in names are replaced.  A str csv_name goes under data/nearest-individual/<model>/, and an
+        existing table is returned untouched.  Files whose cache is missing, unreadable, not an fp16 [rows, d] array
+        of the baseline's width, or empty are logged and dropped.  distributed=True under torchrun: as for
+        score_kad_individual, over the nearest tiles."""
+        k = _prdc_k(k, "nearest")
+        csv = Path(csv_name)
+        if isinstance(csv_name, str):
+            csv = Path('data') / 'nearest-individual' / self.ml.name / csv_name
+        collective = distributed and _kad_engine(True, "nearest")[1]
+        from . import dist
+        writer = not collective or dist.rank() == 0
+        if _on_rank0(csv.exists, collective):
+            if writer:
+                log.info(f"CSV file {csv} already exists, exiting...")
+            return csv
+
+        x, host, offs, names, base_files, base_offs = self._individual_sets(
+            baseline_dir, eval_dir, "nearest", 1, "at least one embedding row", collective, writer)
+        _nearest_rows(x.shape[0], 1)
+        tables = []
+        if names:
+            res, q = _nearest(host, x.shape[0], k, base_offs, distributed)
+            for s, f in enumerate(names):
+                if f is None:
+                    continue
+                a, b = int(offs[s]), int(offs[s + 1])
+                lines = []
+                for rank, (j, r) in enumerate(_file_nearest(res.groups[a:b], res.rows[a:b], q[a:b], k)):
+                    g, i = int(res.groups[a + j, r]), int(res.rows[a + j, r])
+                    lines.append((rank + 1, base_files[g], float(res.distance[a + j, r]), j, i - int(base_offs[g]), b - a))
+                tables.append((f, lines))
+
+        if not writer:
+            return csv
+        tables.sort(key=lambda t: (t[1][0][2], str(t[0])))
+        csv.parent.mkdir(parents=True, exist_ok=True)
+        lines = ["file,rank,nearest_baseline,distance,eval_row,baseline_row,n_eval"]
+        lines += [",".join(str(v).replace(',', '_') for v in (f, *row)) for f, rows in tables for row in rows]
         csv.write_text("\n".join(lines) + "\n")
         return csv
 

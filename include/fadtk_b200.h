@@ -429,6 +429,25 @@ int fad_realism(fad_handle* h, const void* z_f16, long long m, long long n, int 
 int fad_realism_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
                         long long n, int d, int k, float* kept_radii_sq, float* realism, int* nearest, float* nearest_sq,
                         double* threshold_sq, void* stream);
+/* The k nearest distinct baseline groups of each eval row (DESIGN.md section 5.14): z = [X; Y] (fp16 [m + n, d], X first,
+ * 16-byte aligned), d a multiple of 8, q as for PRDC.  The baseline is cut into groups by base_offsets (device int64
+ * [n_groups + 1], 8-byte aligned: offsets[0] = 0, non-decreasing, offsets[n_groups] = m; empty groups allowed), group g =
+ * rows [offsets[g], offsets[g + 1]) of X; base_offsets = NULL makes every row its own group (a plain k-NN; n_groups is
+ * then ignored).  Every argument is checked first (null or misaligned pointers, 1 <= k <= 16, m >= 1, n >= 1, d, at most
+ * 2^30 rows, the offsets read back once); a rejected call launches nothing and writes nothing.
+ *   nearest    (device int32 [n][k]): for eval row j, the rows of X ordered by the key (q(x_i, y_j), i); each group is
+ *              represented by its smallest key; the k groups with the smallest representative keys, ascending, each as
+ *              the row i of that key; -1 where fewer than k groups are non-empty
+ *   nearest_sq (device fp32 [n][k]) = those q values (+inf for the empty slots)
+ * With k = 1 and no offsets, the outputs are bitwise fad_realism's nearest and nearest_sq.  All outputs are bitwise
+ * reproducible and depend on y_j and X (and its groups) alone.  fad_nearest_sharded splits the tile work as
+ * fad_realism_sharded does (local_shards as for fad_kad_*_sharded; collective calls compare m, n, d, k, the number of
+ * groups, a digest of the offsets and a digest of z), bitwise equal to fad_nearest, which is its local_shards = 1 case. */
+int fad_nearest(fad_handle* h, const void* z_f16, long long m, long long n, int d, int k, const long long* base_offsets,
+                long long n_groups, int* nearest, float* nearest_sq, void* stream);
+int fad_nearest_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                        long long n, int d, int k, const long long* base_offsets, long long n_groups, int* nearest,
+                        float* nearest_sq, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
