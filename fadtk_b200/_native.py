@@ -7,6 +7,7 @@ the import of a compute entry point raises.
 from __future__ import annotations
 
 import ctypes as C
+import json
 import os
 from pathlib import Path
 
@@ -122,6 +123,17 @@ SIGNATURES = {
     "fad_nearest": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_vp, c_vp]),
     "fad_nearest_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, C.c_int, c_vp, c_ll, c_vp, c_vp,
                                       c_vp]),
+    "fad_pair_digest": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
+    "fad_knn_lists_sq": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_knn_lists_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_kad_eval_sums": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_eval_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_knn_eval_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_knn_eval_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp,
+                                                c_vp]),
+    "fad_realism_prepared": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp, c_vp]),
+    "fad_realism_prepared_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, c_vp, c_vp, c_vp,
+                                               c_vp]),
     "fad_comm_unique_id": (C.c_int, [c_vp]),
     "fad_comm_init": (C.c_int, [c_vp, c_vp, C.c_int, C.c_int]),
     "fad_comm_destroy": (C.c_int, [c_vp]),
@@ -924,6 +936,87 @@ class Engine:
                   nearest_sq.data_ptr(), _stream()))
         return nearest, nearest_sq
 
+    # ------------------------------------------- a prepared baseline (DESIGN.md 5.15)
+    # The _sharded forms take local_shards as kad_sums_sharded does; None runs the unsharded entry.
+    def pair_digest(self, z: torch.Tensor) -> int:
+        """z fp16 [rows, d] (cuda) -> the row digest the sharded entries compare (fad_pair_digest), as an int"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        out = torch.empty(1, dtype=torch.int64, device=z.device)
+        _check(lib().fad_pair_digest(self._h, z.data_ptr(), z.shape[0], z.shape[1], out.data_ptr(), _stream()))
+        return int(out.cpu().numpy().view(np.uint64)[0])
+
+    def knn_lists_sq(self, x: torch.Tensor, k_max: int, local_shards: "int | None" = None) -> torch.Tensor:
+        """x fp16 [m, d] (cuda) -> fp32 [m, k_max] (cuda): per row the k_max smallest q to the other rows, ascending
+        (fad_knn_lists_sq, or fad_knn_lists_sq_sharded)"""
+        assert x.dtype == torch.float16 and x.is_cuda and x.is_contiguous() and x.ndim == 2
+        out = torch.empty((x.shape[0], max(int(k_max), 0)), dtype=torch.float32, device=x.device)
+        fn, sa = _prepared_fn("fad_knn_lists_sq", local_shards)
+        _check(fn(self._h, *sa, x.data_ptr(), x.shape[0], x.shape[1], int(k_max), out.data_ptr(), _stream()))
+        return out
+
+    def kad_eval_sums(self, z: torch.Tensor, m: int, offsets: torch.Tensor, sigma: torch.Tensor,
+                      local_shards: "int | None" = None) -> torch.Tensor:
+        """kad_song_sums without S_xx -> fp64 [n_items, 2] (cuda): S_yy,k, S_xy,k per item (fad_kad_eval_sums)"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        n_items = offsets.shape[0] - 1
+        out = torch.empty((max(n_items, 0), 2), dtype=torch.float64, device=z.device)
+        fn, sa = _prepared_fn("fad_kad_eval_sums", local_shards)
+        _check(fn(self._h, *sa, z.data_ptr(), int(m), offsets.data_ptr(), n_items, z.shape[1], sigma.data_ptr(),
+                  out.data_ptr(), _stream()))
+        return out
+
+    def knn_eval_radii_sq(self, z: torch.Tensor, m: int, k: int, offsets: "torch.Tensor | None" = None,
+                          local_shards: "int | None" = None) -> torch.Tensor:
+        """z fp16 [m + n, d] (cuda, X rows first) -> fp32 [n] (cuda): s_j^2 of each eval row within the eval set, or
+        within its own song when offsets (int64 [n_items + 1], cuda) are given (fad_knn_eval_radii_sq)"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        n = z.shape[0] - int(m)
+        if offsets is None:
+            off, n_items = None, n
+        else:
+            assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+            off, n_items = offsets.data_ptr(), offsets.shape[0] - 1
+        out = torch.empty(max(n, 0), dtype=torch.float32, device=z.device)
+        fn, sa = _prepared_fn("fad_knn_eval_radii_sq", local_shards)
+        _check(fn(self._h, *sa, z.data_ptr(), int(m), off, n_items, z.shape[1], int(k), out.data_ptr(), _stream()))
+        return out
+
+    def realism_prepared(self, z: torch.Tensor, m: int, kept_radii_sq: torch.Tensor,
+                         local_shards: "int | None" = None):
+        """z fp16 [m + n, d] (cuda, X rows first), kept_radii_sq fp32 [m] (cuda) -> (realism fp32 [n], nearest int32
+        [n], nearest_sq fp32 [n]) (cuda): fad_realism's tile pass alone (fad_realism_prepared)"""
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert kept_radii_sq.dtype == torch.float32 and kept_radii_sq.is_cuda and kept_radii_sq.is_contiguous()
+        m, n = int(m), z.shape[0] - int(m)
+        realism = torch.empty(max(n, 0), dtype=torch.float32, device=z.device)
+        nearest = torch.empty(max(n, 0), dtype=torch.int32, device=z.device)
+        nearest_sq = torch.empty(max(n, 0), dtype=torch.float32, device=z.device)
+        fn, sa = _prepared_fn("fad_realism_prepared", local_shards)
+        _check(fn(self._h, *sa, z.data_ptr(), m, n, z.shape[1], kept_radii_sq.data_ptr(), realism.data_ptr(),
+                  nearest.data_ptr(), nearest_sq.data_ptr(), _stream()))
+        return realism, nearest, nearest_sq
+
+
+_build_id = None
+
+
+def build_id() -> str:
+    """sha1 of the loaded library file: a saved preparation is trusted only by the build that wrote it"""
+    global _build_id
+    if _build_id is None:
+        import hashlib
+        _build_id = hashlib.sha1(_LIB_PATH.read_bytes()).hexdigest()
+    return _build_id
+
+
+def _prepared_fn(name: str, local_shards):
+    """the entry `name` and its extra arguments: unsharded (local_shards None), else its _sharded form"""
+    if local_shards is None:
+        return getattr(lib(), name), ()
+    return getattr(lib(), name + "_sharded"), (None, int(local_shards))
+
 
 class Baseline:
     """Device-resident baseline statistics with the matrix square root precomputed."""
@@ -959,6 +1052,100 @@ class Baseline:
         _check(lib().fad_frechet_batched(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
                                          emb.data_ptr(), offsets.data_ptr(), n_items, self.d, 0, out.data_ptr(), _stream()))
         return out
+
+
+class PairwiseBaseline:
+    """A prepared baseline for the pairwise metrics (DESIGN.md 5.15): the baseline rows X on the device and what depends
+    on them alone, computed once - the row digest (fad_pair_digest), the KAD bandwidth (the two middle q of the xx pairs
+    and sigma), S_xx (fad_kad_song_sums with no songs), and per row the k_max smallest q to the other rows
+    (fad_knn_lists_sq).  KAD, PRDC (k <= k_max), realism (k <= k_max) and nearest then pay for the eval rows only.
+    x: fp16 [m, d] (cuda, d a multiple of 8); d_orig: the width before zero-padding; offsets: int64 [files + 1] of the
+    baseline's files, or None; local_shards as for Engine.knn_lists_sq.  sigma is 0 and s_xx NaN when more than half of
+    the baseline pairs are identical rows (KAD refuses such a baseline, PRDC does not need them)."""
+    VERSION = 1
+
+    def __init__(self, eng: "Engine", x: torch.Tensor, k_max: int, d_orig: int, offsets=None,
+                 local_shards: "int | None" = None, _state: "dict | None" = None):
+        assert x.dtype == torch.float16 and x.is_contiguous() and x.ndim == 2
+        self.eng, self.x, self.k_max, self.d = eng, x, int(k_max), int(d_orig)
+        self.m = int(x.shape[0])
+        self.offsets = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.int64)
+        self._kept: dict = {}
+        self.digest = eng.pair_digest(x)
+        if _state is not None:
+            self.median_sq = np.asarray(_state["median_sq"], dtype=np.float64)
+            self.sigma, self.s_xx = float(_state["sigma"]), float(_state["s_xx"])
+            self.lists = torch.from_numpy(np.ascontiguousarray(_state["lists"], dtype=np.float32)).to(x.device)
+            return
+        sh = () if local_shards is None else (int(local_shards),)
+        self.median_sq = (eng.kad_median_sq_sharded(x, *sh) if sh else eng.kad_median_sq(x)).cpu().numpy()
+        self.sigma = 0.5 * (float(np.sqrt(self.median_sq[0])) + float(np.sqrt(self.median_sq[1])))
+        self.s_xx = float("nan")
+        if self.sigma > 0.0:
+            none = torch.zeros(1, dtype=torch.int64, device=x.device)
+            sig = torch.tensor([self.sigma], dtype=torch.float64, device=x.device)
+            sums = eng.kad_song_sums_sharded(x, self.m, none, sig, *sh) if sh else eng.kad_song_sums(x, self.m, none, sig)
+            self.s_xx = float(sums.cpu().numpy()[0])
+        self.lists = eng.knn_lists_sq(x, self.k_max, local_shards)
+
+    def kept_radii(self, k: int):
+        """-> (kept radii fp32 [m] (cuda), T) of realism at k <= k_max, by fad_realism's rule: r_i^2 = list column
+        k - 1, T = their numpy.median in fp64, r~_i^2 = r_i^2 where r_i^2 <= T, else 0"""
+        if k not in self._kept:
+            r = self.lists[:, k - 1].contiguous()
+            h = np.sort(r.cpu().numpy().astype(np.float64))
+            mid = self.m // 2
+            t = float(h[mid]) if self.m % 2 else float((h[mid - 1] + h[mid]) / 2.0)
+            self._kept[k] = (torch.where(r.double() <= t, r, torch.zeros_like(r)), t)
+        return self._kept[k]
+
+    def save(self, path, fingerprint: dict) -> None:
+        """Write the preparation to path (.npz) atomically: a temporary file in the same directory, then os.replace."""
+        path = Path(path)
+        path.parent.mkdir(parents=True, exist_ok=True)
+        tmp = path.with_name(path.name + f".tmp{os.getpid()}")
+        with open(tmp, "wb") as fh:
+            np.savez(fh, version=np.int64(self.VERSION), build=np.array(build_id()), m=np.int64(self.m),
+                     d=np.int64(self.d), k_max=np.int64(self.k_max), digest=np.uint64(self.digest),
+                     median_sq=self.median_sq, sigma=np.float64(self.sigma), s_xx=np.float64(self.s_xx),
+                     lists=self.lists.cpu().numpy(),
+                     offsets=self.offsets if self.offsets is not None else np.zeros(0, dtype=np.int64),
+                     fingerprint=np.array(json.dumps(fingerprint, sort_keys=True)))
+        os.replace(tmp, path)
+
+    @classmethod
+    def load(cls, path, eng: "Engine", x: torch.Tensor, k_max: int, d_orig: int, fingerprint: dict, offsets=None):
+        """-> (PairwiseBaseline, "") when the file at path was written for these rows by this build: the same format
+        version and library (build_id), m, d, k_max >= the one asked for, the fingerprint of the embedding files and the digest of x;
+        else (None, why it is not used).  x, d_orig, offsets as for the constructor."""
+        path = Path(path)
+        if not path.exists():
+            return None, "no saved preparation"
+        try:
+            with np.load(path, allow_pickle=False) as f:
+                st = {k: f[k] for k in f.files}
+            if int(st["version"]) != cls.VERSION:
+                return None, f"its format version is {int(st['version'])}, not {cls.VERSION}"
+            if str(st["build"]) != build_id():
+                return None, "another build of the library wrote it"
+            if json.loads(str(st["fingerprint"])) != fingerprint:
+                return None, "the embedding files changed"
+            for key, v in (("m", int(x.shape[0])), ("d", int(d_orig))):
+                if int(st[key]) != v:
+                    return None, f"its {key} is {int(st[key])}, not {v}"
+            if int(st["k_max"]) < int(k_max):
+                return None, f"its k_max is {int(st['k_max'])}, below {int(k_max)}"
+            if st["lists"].shape != (int(x.shape[0]), int(st["k_max"])) or st["lists"].dtype != np.float32:
+                return None, "its radius lists have the wrong shape"
+            off = None if offsets is None else np.asarray(offsets, dtype=np.int64)
+            if (off is None and st["offsets"].size) or (off is not None and not np.array_equal(off, st["offsets"])):
+                return None, "the file offsets differ"
+        except (OSError, ValueError, KeyError) as e:
+            return None, f"it cannot be read ({e})"
+        pb = cls(eng, x, int(st["k_max"]), d_orig, offsets, _state=st)
+        if pb.digest != int(st["digest"]):
+            return None, "the rows on the device differ from the ones it was computed from"
+        return pb, ""
 
 
 _engines: dict = {}

@@ -574,6 +574,7 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::prdc_tile_kernel<3>, fad::kPrdcSongSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<4>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<5>, fad::kPrdcNearestSmemBytes));
+    CK(smem((const void*)fad::prdc_tile_kernel<6>, fad::kPairSmemBytes));
     if (setup_gemm<0>(h.get()) || setup_gemm<1>(h.get())) return 1;
     *out = h.release();
     return 0;

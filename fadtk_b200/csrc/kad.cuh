@@ -281,7 +281,7 @@ __global__ void kad_reduce_kernel(const double* __restrict__ partial, int units,
     out[t] = s;
 }
 
-// one block per song: out[1 + 2k] = S_yy,k, out[2 + 2k] = S_xy,k.  Each row's partials are summed over the units of its
+// one block per song: out[2k] = S_yy,k, out[2k + 1] = S_xy,k.  Each row's partials are summed over the units of its
 // tile in unit order, a thread's rows in row order, then the block in a fixed tree - a fixed order for a given shape.
 constexpr int kKadSongReduceThreads = 128;
 __global__ void __launch_bounds__(kKadSongReduceThreads)
@@ -310,8 +310,8 @@ kad_song_reduce_kernel(const double* __restrict__ partial, const int* __restrict
     if (threadIdx.x == 0) {
         double sxy = 0.0, syy = 0.0;
         for (int i = 0; i < kKadSongReduceThreads / 32; ++i) { sxy += red[0][i]; syy += red[1][i]; }
-        out[1 + 2 * (size_t)k] = syy;
-        out[2 + 2 * (size_t)k] = sxy;
+        out[2 * (size_t)k] = syy;
+        out[2 * (size_t)k + 1] = sxy;
     }
 }
 

@@ -21,6 +21,10 @@
 // their lists by a fixed xor tree, and one lane writes radii_sq[row of Z] = the k-th smallest of the set's q values.
 // Selection does not depend on order, so the value is exact and grid-independent.
 //
+// Radius lists (PASS 6): PASS 0 on X alone (n = 0), but one lane writes the row's whole list, the k smallest q
+// ascending, to radii_sq[row][k]: entry k' - 1 is bitwise the PASS 0 radius at k' <= k, both being exact selections
+// of the same fp32 values (DESIGN.md 5.15).
+//
 // Counts (PASS 1).  Unit = (X tile tx, a run of Y column tiles [c0, c1)), runs cut by the shape only.  r_i^2 of the
 // two rows of a thread sit in registers; s_j^2 is read per column through the read-only cache, as the column norms
 // are.  Every xy pair is evaluated once, so the four metrics see one fp32 q per pair:
@@ -92,9 +96,9 @@ struct PrdcParams {
     int unit0, unit1;        // this launch's units [unit0, unit1) of Tx + Ty (PASS 0, 2) or Tx * cuts (PASS 1, 3): all
                              // of them, or one shard of a sharded call; outputs stay indexed by the global row / column
     const float* norm;       // [m + Ty * 128] |y_i|^2 of the rows of Z (zero past m + n; per song: one box more)
-    // PASS 0 and 2
+    // PASS 0, 2 and 6
     int k;                   // 1 .. kPrdcMaxK
-    float* radii_sq;         // [m + n] out
+    float* radii_sq;         // [m + n] out (PASS 6: [m][k])
     // PASS 1 and 3
     const float* radii;      // [m + n] r_i^2 of X, then s_j^2 of Y
     int cuts;                // column runs per X tile row: run i = Y tiles [i Ty / cuts, (i + 1) Ty / cuts)
@@ -118,7 +122,7 @@ struct PrdcUnit {
 };
 template <int PASS>
 __device__ __forceinline__ PrdcUnit prdc_unit(const PrdcParams& p, int u) {
-    if constexpr (PASS == 0) {
+    if constexpr (PASS == 0 || PASS == 6) {
         if (u < p.Tx) return {u * 128, 0, 0, p.Tx};
         return {p.m + (u - p.Tx) * 128, p.m, 0, p.Ty};
     } else if constexpr (PASS == 2) {
@@ -249,8 +253,8 @@ template <int PASS>
 __global__ void __launch_bounds__(kPairThreads, 1)
 prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const PrdcParams p) {
     using namespace sm90;
-    static_assert(PASS >= 0 && PASS <= 5,
-                  "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts, 4: realism, 5: nearest groups");
+    static_assert(PASS >= 0 && PASS <= 6, "0: k-NN radii, 1: ball counts, 2: per-song radii, 3: per-song counts, "
+                  "4: realism, 5: nearest groups, 6: k-NN radius lists");
     extern __shared__ uint8_t smem_raw[];
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -286,7 +290,7 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
         const PrdcUnit w = prdc_unit<PASS>(p, u);
         const int row0 = w.arow + lr0;                    // rows of Z
         const float nr[2] = {__ldg(p.norm + row0), __ldg(p.norm + row0 + 8)};
-        if constexpr (PASS == 0 || PASS == 2) {
+        if constexpr (PASS == 0 || PASS == 2 || PASS == 6) {
             // each row's set as a range [lo, hi) of the unit's columns jj (rows bbase + jj of Z): the whole set (lo = 0
             // is not compared); per song, for the Y units, the row's song, empty past the last row (song_of = -1)
             constexpr bool songs = PASS == 2;
@@ -332,8 +336,18 @@ prdc_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_consta
             prdc_topk_merge(a);
             if ((lane & 3) == 0) {
 #pragma unroll
-                for (int i = 0; i < 2; ++i)
-                    if ((!songs || ii0 + 8 * i >= lo[i]) && ii0 + 8 * i < hi[i]) p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
+                for (int i = 0; i < 2; ++i) {
+                    if ((!songs || ii0 + 8 * i >= lo[i]) && ii0 + 8 * i < hi[i]) {
+                        if constexpr (PASS == 6) {
+#pragma unroll
+                            for (int t = 0; t < kPrdcMaxK; ++t)
+                                if (t >= kPrdcMaxK - p.k)
+                                    p.radii_sq[(size_t)(row0 + 8 * i) * p.k + t - (kPrdcMaxK - p.k)] = a[i][t];
+                        } else {
+                            p.radii_sq[row0 + 8 * i] = a[i][kPrdcMaxK - 1];
+                        }
+                    }
+                }
             }
         } else if constexpr (PASS == 1) {
             // rows of X past m (the first rows of Y, or zero-filled) count nothing

@@ -9,6 +9,7 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_prdc_songs                                        -> the same, every song against one baseline in one pass
     calc_realism                (no reference counterpart) -> k-NN radii and one max / argmin tile pass (csrc/prdc.cuh)
     calc_nearest                (no reference counterpart) -> one distinct-group top-k tile pass (csrc/prdc.cuh)
+    prepare_pairwise_baseline                              -> the baseline-only work of the four above, done once
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -145,7 +146,18 @@ def calc_kernel_audio_distance(emb_baseline, emb_eval, distributed: bool = False
     distributed=True under torchrun (world size > 1): a collective call that every rank makes with the same sets.  The
     pair tiles are split over the ranks (fad_kad_*_sharded over the library's NCCL communicator), and every rank gets
     the result, bitwise equal to one GPU's.  The ranks' arguments are compared first; a difference raises NativeError
-    on every rank.  RuntimeError when that communicator cannot be set up (gloo backend, FADTK_NATIVE_ALLREDUCE=0)."""
+    on every rank.  RuntimeError when that communicator cannot be set up (gloo backend, FADTK_NATIVE_ALLREDUCE=0).
+
+    emb_baseline may be a PairwiseBaseline (prepare_pairwise_baseline): sigma and S_xx are then the prepared ones, and
+    the score is bitwise the one calc_kernel_audio_distance_songs gives for emb_eval as one song (S_xy sums in another
+    order than the whole-set pass; DESIGN.md 5.15)."""
+    if _is_prepared(emb_baseline):
+        y = _kad_rows(emb_eval, "eval")
+        if y.shape[0] < 2:
+            raise ValueError(f"KAD needs at least two embedding rows in each set (baseline {emb_baseline.m}, "
+                             f"eval {y.shape[0]})")
+        _prepared_width(emb_baseline, y, "eval")
+        return _kad_prepared(emb_baseline, y, np.array([0, y.shape[0]], dtype=np.int64), distributed)[0]
     x, y = _kad_rows(emb_baseline, "baseline"), _kad_rows(emb_eval, "eval")
     m, n = int(x.shape[0]), int(y.shape[0])
     if m < 2 or n < 2:
@@ -221,7 +233,13 @@ def calc_kernel_audio_distance_songs(emb_baseline, songs, distributed: bool = Fa
     with sigma and the baseline's own pair sum computed once for all songs and every song's sums in one GPU pass
     (fad_kad_song_sums).  A song with fewer than two rows gets score NaN (n_eval still says how many rows it had).
     Raises ValueError like calc_kernel_audio_distance: non-fp16 or non-2-D input, widths that differ from the
-    baseline's, fewer than two baseline rows, sigma = 0.  distributed: as for calc_kernel_audio_distance."""
+    baseline's, fewer than two baseline rows, sigma = 0.  distributed: as for calc_kernel_audio_distance.  emb_baseline
+    may be a PairwiseBaseline: the same values, bitwise, without the baseline's own passes."""
+    if _is_prepared(emb_baseline):
+        ys = [_prepared_width(emb_baseline, _kad_rows(y, f"song {k}"), f"song {k}") for k, y in enumerate(songs)]
+        offsets = np.zeros(len(ys) + 1, dtype=np.int64)
+        offsets[1:] = np.cumsum([int(y.shape[0]) for y in ys])
+        return _kad_prepared(emb_baseline, torch.cat(ys) if ys else None, offsets, distributed)
     x = _kad_rows(emb_baseline, "baseline")
     ys = [_kad_rows(y, f"song {k}") for k, y in enumerate(songs)]
     for k, y in enumerate(ys):
@@ -271,8 +289,22 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> 
     The radii and ball-count tiles are split over the ranks (fad_knn_radii_sq_sharded, fad_prdc_counts_sharded over the
     library's NCCL communicator), and every rank gets the result, bitwise equal to one GPU's.  The ranks' arguments are
     compared first; a difference raises NativeError on every rank.  RuntimeError when that communicator cannot be set
-    up, as for calc_kernel_audio_distance."""
+    up, as for calc_kernel_audio_distance.
+
+    emb_baseline may be a PairwiseBaseline with k_max >= k: r_i^2 is then column k - 1 of its radius lists, and the
+    results are bitwise the ones the baseline rows give."""
     k = _prdc_k(k)
+    if _is_prepared(emb_baseline):
+        pb, y = emb_baseline, _kad_rows(emb_eval, "eval", "PRDC")
+        _prepared_k(pb, k, "PRDC")
+        if y.shape[0] <= k:
+            raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {pb.m}, "
+                             f"eval {y.shape[0]})")
+        _prepared_width(pb, y, "eval")
+        eng, collective = _kad_engine(distributed, "PRDC")
+        z = torch.cat([pb.x, _kad_device_rows(y, eng)])
+        radii_sq = torch.cat([pb.lists[:, k - 1], eng.knn_eval_radii_sq(z, pb.m, k, None, 0 if collective else None)])
+        return _prdc_results(eng, z, pb.m, k, radii_sq, collective)
     x, y = _kad_rows(emb_baseline, "baseline", "PRDC"), _kad_rows(emb_eval, "eval", "PRDC")
     m, n = int(x.shape[0]), int(y.shape[0])
     if m <= k or n <= k:
@@ -282,6 +314,12 @@ def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> 
     eng, collective = _kad_engine(distributed, "PRDC")
     z = _kad_device_rows(torch.cat([x, y]), eng)
     radii_sq = eng.knn_radii_sq_sharded(z, m, k) if collective else eng.knn_radii_sq(z, m, k)
+    return _prdc_results(eng, z, m, k, radii_sq, collective)
+
+
+def _prdc_results(eng, z: torch.Tensor, m: int, k: int, radii_sq: torch.Tensor, collective: bool) -> PRDCResults:
+    """the ball counts of z = [X; Y] (device) under radii_sq [m + n] -> PRDCResults"""
+    n = int(z.shape[0]) - m
     counts = eng.prdc_counts_sharded(z, m, radii_sq) if collective else eng.prdc_counts(z, m, radii_sq)
     inside, flags = (t.cpu().numpy() for t in counts)
     return PRDCResults(precision=float(np.count_nonzero(inside)) / n,
@@ -315,8 +353,15 @@ def calc_realism(emb_baseline, emb_eval, k: int = 3, distributed: bool = False) 
     scored in one call get the values separate calls give.  The radii and one pass over all (x, y) pairs run on the GPU
     (fad_realism) without forming a distance matrix.  A width that is not a multiple of 8 is zero-padded.  Raises
     ValueError for k outside [1, 16], m <= k, n < 1, non-fp16 or non-2-D input, mismatched widths, and T = 0 (more than
-    half of the baseline rows have k exact duplicates).  distributed: as for calc_prdc (fad_realism_sharded)."""
+    half of the baseline rows have k exact duplicates).  distributed: as for calc_prdc (fad_realism_sharded).
+
+    emb_baseline may be a PairwiseBaseline with k_max >= k: r_i^2 is then column k - 1 of its radius lists, pruned by
+    the same rule, and the results are bitwise the ones the baseline rows give (fad_realism_prepared)."""
     k = _prdc_k(k, "realism")
+    if _is_prepared(emb_baseline):
+        y = _prepared_width(emb_baseline, _kad_rows(emb_eval, "eval", "realism"), "eval")
+        _realism_rows(emb_baseline.m, int(y.shape[0]), k)
+        return _realism(y, emb_baseline.m, k, distributed, emb_baseline)
     x, y = _kad_rows(emb_baseline, "baseline", "realism"), _kad_rows(emb_eval, "eval", "realism")
     m, n = int(x.shape[0]), int(y.shape[0])
     _realism_rows(m, n, k)
@@ -331,11 +376,18 @@ def _realism_rows(m: int, n: int, k: int):
                          f"(baseline {m}, eval {n})")
 
 
-def _realism(z: torch.Tensor, m: int, k: int, distributed: bool = False) -> RealismResults:
-    """z = [X; Y] fp16 (host or device) -> RealismResults of the rows after X"""
+def _realism(z: torch.Tensor, m: int, k: int, distributed: bool = False, prepared=None) -> RealismResults:
+    """z = [X; Y] fp16 (host or device) -> RealismResults of the rows after X.  prepared: a PairwiseBaseline of X
+    (k_max >= k), and z = Y alone"""
     eng, collective = _kad_engine(distributed, "realism")
     z = _kad_device_rows(z, eng)
-    _, realism, nearest, nearest_sq, t = eng.realism_sharded(z, m, k) if collective else eng.realism(z, m, k)
+    if prepared is not None:
+        _prepared_k(prepared, k, "realism")
+        z = torch.cat([prepared.x, z])
+        kept, t = prepared.kept_radii(k)
+        realism, nearest, nearest_sq = eng.realism_prepared(z, m, kept, 0 if collective else None)
+    else:
+        _, realism, nearest, nearest_sq, t = eng.realism_sharded(z, m, k) if collective else eng.realism(z, m, k)
     if not t > 0.0:
         raise ValueError("realism threshold is 0: more than half of the baseline rows have k exact duplicates")
     return RealismResults(realism=realism.cpu().numpy(), nearest=nearest.cpu().numpy().astype(np.int64),
@@ -361,8 +413,13 @@ def calc_nearest(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) 
     and one array, rows[:, 0] and distance[:, 0] are calc_realism's nearest and nearest_distance.  One GPU pass over all
     (x, y) pairs (fad_nearest) keeps the lists in registers; no distance matrix is formed.  A width that is not a
     multiple of 8 is zero-padded.  Raises ValueError for k outside [1, 16], no baseline or no eval rows, non-fp16 or
-    non-2-D input and mismatched widths.  distributed: as for calc_prdc (fad_nearest_sharded)."""
+    non-2-D input and mismatched widths.  distributed: as for calc_prdc (fad_nearest_sharded).  emb_baseline may be a
+    PairwiseBaseline: its resident rows, grouped by its file offsets (each row its own group without them)."""
     k = _prdc_k(k, "nearest")
+    if _is_prepared(emb_baseline):
+        y = _prepared_width(emb_baseline, _kad_rows(emb_eval, "eval", "nearest"), "eval")
+        _nearest_rows(emb_baseline.m, int(y.shape[0]))
+        return _nearest(y, emb_baseline.m, k, emb_baseline.offsets, distributed, emb_baseline)[0]
     parts = list(emb_baseline) if isinstance(emb_baseline, (list, tuple)) else [emb_baseline]
     if not parts:
         raise ValueError("nearest needs at least one baseline group")
@@ -386,11 +443,13 @@ def _nearest_rows(m: int, n: int):
         raise ValueError(f"nearest needs at least one baseline row and one eval row (baseline {m}, eval {n})")
 
 
-def _nearest(z: torch.Tensor, m: int, k: int, offsets, distributed: bool = False):
+def _nearest(z: torch.Tensor, m: int, k: int, offsets, distributed: bool = False, prepared=None):
     """z = [X; Y] fp16 (host or device), offsets int64 [groups + 1] of X or None -> (NearestResults of the rows after
-    X, the squared distances fp32 [n, k])"""
+    X, the squared distances fp32 [n, k]).  prepared: a PairwiseBaseline of X, and z = Y alone"""
     eng, collective = _kad_engine(distributed, "nearest")
     z = _kad_device_rows(z, eng)
+    if prepared is not None:
+        z = torch.cat([prepared.x, z])
     off = None if offsets is None else torch.from_numpy(np.asarray(offsets, dtype=np.int64)).to(eng.torch_device)
     rows, q = eng.nearest_sharded(z, m, k, off) if collective else eng.nearest(z, m, k, off)
     rows, q = rows.cpu().numpy().astype(np.int64), q.cpu().numpy()
@@ -427,8 +486,14 @@ def calc_prdc_songs(emb_baseline, songs, k: int = 5, distributed: bool = False) 
     (fad_knn_song_radii_sq, fad_prdc_song_counts).  A song with at most k rows (empty ones included) gets NaN for all
     four values, n_eval still saying how many rows it had, and is never sent to the GPU.  Coverage and recall of a short
     song against a large baseline are small by definition.  Raises ValueError like calc_prdc: k outside [1, 16],
-    m <= k, non-fp16 or non-2-D input, widths that differ from the baseline's.  distributed: as for calc_prdc."""
+    m <= k, non-fp16 or non-2-D input, widths that differ from the baseline's.  distributed: as for calc_prdc.
+    emb_baseline may be a PairwiseBaseline with k_max >= k: the same values, bitwise."""
     k = _prdc_k(k)
+    if _is_prepared(emb_baseline):
+        ys = [_prepared_width(emb_baseline, _kad_rows(y, f"song {i}", "PRDC"), f"song {i}") for i, y in enumerate(songs)]
+        kept = [y for y in ys if y.shape[0] > k]
+        return _prdc_songs(torch.cat(kept) if kept else None, emb_baseline.m, [int(y.shape[0]) for y in ys], k,
+                           distributed, emb_baseline)
     x = _kad_rows(emb_baseline, "baseline", "PRDC")
     ys = [_kad_rows(y, f"song {i}", "PRDC") for i, y in enumerate(songs)]
     for i, y in enumerate(ys):
@@ -438,9 +503,13 @@ def calc_prdc_songs(emb_baseline, songs, k: int = 5, distributed: bool = False) 
     return _prdc_songs(torch.cat([x, *kept]), int(x.shape[0]), [int(y.shape[0]) for y in ys], k, distributed)
 
 
-def _prdc_songs(z: torch.Tensor, m: int, rows: list, k: int, distributed: bool = False) -> list[PRDCResults]:
+def _prdc_songs(z: torch.Tensor, m: int, rows: list, k: int, distributed: bool = False,
+                prepared=None) -> list[PRDCResults]:
     """z = [X; the songs of more than k rows, in order] fp16 (host or device), rows = the row counts of all songs ->
-    one PRDCResults per song (NaN for the songs not in z)"""
+    one PRDCResults per song (NaN for the songs not in z).  prepared: a PairwiseBaseline of X (k_max >= k), and z the
+    songs' rows alone"""
+    if prepared is not None:
+        _prepared_k(prepared, k, "PRDC")
     if m <= k:
         raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {m})")
     nan = float("nan")
@@ -453,7 +522,11 @@ def _prdc_songs(z: torch.Tensor, m: int, rows: list, k: int, distributed: bool =
     eng, collective = _kad_engine(distributed, "PRDC")
     z = _kad_device_rows(z, eng)
     off = torch.from_numpy(offsets).to(eng.torch_device)
-    radii_sq = (eng.knn_song_radii_sq_sharded(z, m, off, k) if collective else eng.knn_song_radii_sq(z, m, off, k))
+    if prepared is not None:
+        z = torch.cat([prepared.x, z])
+        radii_sq = torch.cat([prepared.lists[:, k - 1], eng.knn_eval_radii_sq(z, m, k, off, 0 if collective else None)])
+    else:
+        radii_sq = (eng.knn_song_radii_sq_sharded(z, m, off, k) if collective else eng.knn_song_radii_sq(z, m, off, k))
     counts = (eng.prdc_song_counts_sharded(z, m, off, radii_sq) if collective
               else eng.prdc_song_counts(z, m, off, radii_sq))
     inside, per_song = (t.cpu().numpy() for t in counts)
@@ -464,6 +537,68 @@ def _prdc_songs(z: torch.Tensor, m: int, rows: list, k: int, distributed: bool =
                              density=float(ins.sum(dtype=np.int64)) / (k * n),
                              coverage=float(per_song[s, 0]) / m,
                              k=k, n_baseline=m, n_eval=n)
+    return out
+
+
+def prepare_pairwise_baseline(emb_baseline, k_max: int = 16, offsets=None, distributed: bool = False):
+    """The baseline-only work of KAD, PRDC, realism and nearest, done once (DESIGN.md 5.15): the fp16 rows X [m, d]
+    are moved to the GPU and kept there with their digest, the KAD bandwidth sigma, S_xx, and per row the k_max smallest
+    squared distances to the other rows.  The result can be passed wherever these metrics take the baseline rows
+    (calc_kernel_audio_distance[_songs], calc_prdc[_songs] and calc_realism for k <= k_max, calc_nearest), which then pay
+    for the eval rows only and give the values the rows give (bitwise; KAD: bitwise the per-song value).  offsets: int64
+    [files + 1] row offsets of the baseline's files (calc_nearest's groups), or None.  Raises ValueError for k_max
+    outside [1, 16], m <= k_max, non-fp16 or non-2-D rows and bad offsets.  distributed: as for calc_prdc, over the
+    sharded entries.  FrechetAudioDistance.prepare_pairwise saves it and loads it back."""
+    from ._native import PairwiseBaseline
+    k_max = _prdc_k(k_max, "a prepared baseline")
+    x = _kad_rows(emb_baseline, "baseline", "a prepared baseline")
+    m = int(x.shape[0])
+    if m <= k_max:
+        raise ValueError(f"a prepared baseline with k_max = {k_max} needs more than k_max rows (baseline {m})")
+    offsets = _baseline_offsets(offsets, m)
+    eng, collective = _kad_engine(distributed, "a prepared baseline")
+    return PairwiseBaseline(eng, _kad_device_rows(x, eng), k_max, int(x.shape[1]), offsets, 0 if collective else None)
+
+
+def _baseline_offsets(offsets, m: int):
+    if offsets is None:
+        return None
+    offsets = np.asarray(offsets, dtype=np.int64)
+    if offsets.ndim != 1 or offsets.size < 2 or offsets[0] != 0 or offsets[-1] != m or np.any(np.diff(offsets) < 0):
+        raise ValueError(f"baseline offsets must rise from 0 to m = {m}")
+    return offsets
+
+
+def _is_prepared(b) -> bool:
+    from ._native import PairwiseBaseline
+    return isinstance(b, PairwiseBaseline)
+
+
+def _prepared_width(pb, y: torch.Tensor, what: str) -> torch.Tensor:
+    if y.shape[1] != pb.d:
+        raise ValueError(f"embedding widths differ (baseline {pb.d}, {what} {y.shape[1]})")
+    return y
+
+
+def _prepared_k(pb, k: int, metric: str):
+    if k > pb.k_max:
+        raise ValueError(f"{metric} with k = {k} needs a baseline prepared with k_max >= k (it has {pb.k_max})")
+
+
+def _kad_prepared(pb, y, offsets: np.ndarray, distributed: bool = False) -> list[KADResults]:
+    """KAD of the items of y (fp16 [n_total, d], host or device, or None when n_total = 0; items at offsets [K + 1])
+    against a prepared baseline: its sigma and S_xx, then the eval sums alone (fad_kad_eval_sums)"""
+    if not pb.sigma > 0.0:
+        raise ValueError("KAD bandwidth is 0: more than half of the baseline pairs are identical rows")
+    eng, collective = _kad_engine(distributed)
+    dev = eng.torch_device
+    z = pb.x if y is None or not y.shape[0] else torch.cat([pb.x, _kad_device_rows(y, eng)])
+    sig = torch.tensor([pb.sigma], dtype=torch.float64, device=dev)
+    sums = eng.kad_eval_sums(z, pb.m, torch.from_numpy(offsets).to(dev), sig, 0 if collective else None).cpu().numpy()
+    out = []
+    for k, n in enumerate(np.diff(offsets).tolist()):
+        score = _kad_score(pb.s_xx, float(sums[k, 0]), float(sums[k, 1]), pb.m, n) if n >= 2 else float("nan")
+        out.append(KADResults(score=score, bandwidth=pb.sigma, n_baseline=pb.m, n_eval=n))
     return out
 
 
@@ -781,21 +916,89 @@ class FrechetAudioDistance:
         mu_eval, cov_eval = self.load_stats(eval)
         return calc_frechet_distance(mu_bg, cov_bg, mu_eval, cov_eval)
 
-    def score_kad(self, baseline_dir: PathLike, eval_dir: PathLike, distributed: bool = False) -> KADResults:
+    def prepare_pairwise(self, baseline_dir: PathLike, k_max: int = 16, distributed: bool = False):
+        """The PairwiseBaseline (prepare_pairwise_baseline) of the cached embeddings of baseline_dir, grouped by file:
+        loaded from <baseline_dir>/stats/<model>/pairwise.npz when that file was written by this build for these
+        embedding files (the fingerprint statistics caches keep in source.json) and these rows (their digest) with
+        k_max at least the one asked for; otherwise computed and saved there atomically, with one log line that says
+        why.  distributed=True under torchrun: a collective call; rank 0 decides and writes, every rank computes its
+        share."""
+        k_max = _prdc_k(k_max, "a prepared baseline")
+        collective = distributed and _kad_engine(True, "a prepared baseline")[1]
+        x, _, base_offs = self._baseline_rows(baseline_dir, "a prepared baseline", collective)
+        return self._prepared(baseline_dir, x, base_offs, k_max, distributed, k_max)
+
+    def _baseline_rows(self, baseline_dir: PathLike, metric: str, collective: bool):
+        """-> (x, files, offsets): the baseline's fp16 rows, its cache files and their int64 row offsets in x"""
+        from . import _io_native
+        files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name, metric)), collective)
+        if not files:
+            raise ValueError(f"no {self.ml.name} embeddings cached under {baseline_dir}: embed the baseline directory first")
+        x, offs = _io_native.load_embedding_files(files, self.audio_load_worker)
+        if x.dtype != np.float16:
+            raise ValueError(f"{metric} needs fp16 embedding caches; {baseline_dir} holds {x.dtype}")
+        return x, files, offs
+
+    def _prepared(self, baseline_dir: PathLike, x: np.ndarray, base_offs: np.ndarray, k: int, distributed: bool,
+                  k_max: "int | None" = None):
+        """prepare_pairwise over rows already read (x, base_offs), good for k: a saved preparation with k_max >= k, else
+        a new one with k_max (default max(k, min(16, m - 1)), so that one preparation serves every k a metric allows)"""
+        from . import dist
+        from ._native import PairwiseBaseline
+        eng, collective = _kad_engine(distributed, "a prepared baseline")
+        path = Path(baseline_dir) / "stats" / self.ml.name / "pairwise.npz"
+        emb_dir = Path(baseline_dir) / "embeddings" / self.ml.name
+        fingerprint = self._embedding_fingerprint(emb_dir)
+        xd = _kad_device_rows(torch.from_numpy(x), eng)
+        pb, why = PairwiseBaseline.load(path, eng, xd, k, int(x.shape[1]), fingerprint, base_offs)
+        # every rank takes rank 0's branch: a collective preparation needs all of them
+        if _on_rank0(lambda: pb is not None, collective):
+            if pb is None:
+                raise ValueError(f"the saved preparation {path} cannot be read on every rank ({why})")
+            log.info(f"Pairwise baseline preparation loaded from {path}")
+            return pb
+        if not collective or dist.rank() == 0:
+            log.info(f"Pairwise baseline preparation of {baseline_dir}: {why}, computing...")
+        k_max = k_max or max(k, min(16, int(x.shape[0]) - 1))
+        pb = prepare_pairwise_baseline(x, k_max, base_offs, distributed)
+        if not collective or dist.rank() == 0:
+            pb.save(path, fingerprint)
+        return pb
+
+    def score_kad(self, baseline_dir: PathLike, eval_dir: PathLike, distributed: bool = False,
+                  prepared: bool = False) -> KADResults:
         """Kernel Audio Distance between the cached embeddings of two directories (calc_kernel_audio_distance): all rows
         of all <dir>/embeddings/<model>/*.npy in sorted file order, the files the directory statistics read.
         distributed=True under torchrun: a collective call; rank 0 lists the files, every rank reads them and takes its
-        share of the pair tiles, and every rank gets the result."""
-        return calc_kernel_audio_distance(*self._cached_sets(baseline_dir, eval_dir, "KAD", distributed),
-                                          distributed=distributed)
+        share of the pair tiles, and every rank gets the result.  prepared=True: against prepare_pairwise(baseline_dir),
+        loaded or built and saved (bitwise the per-song value of the eval set as one song)."""
+        x, y = self._cached_sets(baseline_dir, eval_dir, "KAD", distributed)
+        if prepared:
+            x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", distributed), 1, distributed)
+        return calc_kernel_audio_distance(x, y, distributed=distributed)
 
-    def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5, distributed: bool = False) -> PRDCResults:
+    def _cached_offsets(self, baseline_dir: PathLike, metric: str, distributed: bool) -> np.ndarray:
+        """the int64 row offsets of the baseline's cache files, from their headers"""
+        from . import _io_native
+        collective = distributed and _kad_engine(True, metric)[1]
+        files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(baseline_dir, self.ml.name, metric)), collective)
+        rows = _io_native.npy_probe(files, self.audio_load_worker)[0]
+        offs = np.zeros(len(files) + 1, dtype=np.int64)
+        offs[1:] = np.cumsum(rows)
+        return offs
+
+    def score_prdc(self, baseline_dir: PathLike, eval_dir: PathLike, k: int = 5, distributed: bool = False,
+                   prepared: bool = False) -> PRDCResults:
         """Precision, recall, density and coverage (calc_prdc) of the cached embeddings of eval_dir against those of
         baseline_dir, read as score_kad reads them: all rows of all <dir>/embeddings/<model>/*.npy in sorted file
         order.  Statistics files and names are refused.  distributed=True under torchrun: a collective call; rank 0
         lists the files, every rank reads them and takes its share of the radii and ball-count tiles, and every rank
-        gets the result."""
-        return calc_prdc(*self._cached_sets(baseline_dir, eval_dir, "PRDC", distributed), k=k, distributed=distributed)
+        gets the result.  prepared=True: against prepare_pairwise(baseline_dir) (bitwise the same values)."""
+        x, y = self._cached_sets(baseline_dir, eval_dir, "PRDC", distributed)
+        if prepared:
+            x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "PRDC", distributed), _prdc_k(k),
+                               distributed)
+        return calc_prdc(x, y, k=k, distributed=distributed)
 
     def _cached_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, distributed: bool) -> list:
         """The fp16 embeddings of the two directories that score_kad and score_prdc score, for `metric` (named in the
@@ -814,7 +1017,7 @@ class FrechetAudioDistance:
         return sets
 
     def score_kad_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
-                             distributed: bool = False) -> Path:
+                             distributed: bool = False, prepared: bool = False) -> Path:
         """KAD of every file in eval_dir against the embeddings of baseline_dir (calc_kernel_audio_distance_songs: the
         bandwidth and the baseline's pair sum once, every song's sums in one GPU pass), written as score_individual
         writes FAD: rows ``file,score`` sorted by |score|, commas in names replaced, no header; a str csv_name goes
@@ -822,7 +1025,8 @@ class FrechetAudioDistance:
         missing, unreadable or not an fp16 [rows, d] array of the baseline's width, and files with fewer than two
         embedding rows, are logged and dropped.  distributed=True under torchrun: a collective call; rank 0 lists the
         directories and decides whether the table exists, every rank reads the caches and takes its share of the pair
-        tiles, and rank 0 alone logs the dropped files and writes the table."""
+        tiles, and rank 0 alone logs the dropped files and writes the table.  prepared=True: against
+        prepare_pairwise(baseline_dir), loaded or built and saved; the same table."""
         csv = Path(csv_name)
         if isinstance(csv_name, str):
             csv = Path('data') / 'kad-individual' / self.ml.name / csv_name
@@ -834,10 +1038,14 @@ class FrechetAudioDistance:
                 log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
-        x, host, offs, names, _, _ = self._individual_sets(baseline_dir, eval_dir, "KAD", 2,
-                                                           "at least two embedding rows", collective, writer)
+        x, host, offs, names, _, base_offs = self._individual_sets(baseline_dir, eval_dir, "KAD", 2,
+                                                                   "at least two embedding rows", collective, writer)
         pairs = []
-        if names:
+        if names and prepared:
+            pb = self._prepared(baseline_dir, x, base_offs, 1, distributed)
+            res = _kad_prepared(pb, host[x.shape[0]:], offs, distributed)
+            pairs = [(f, r.score) for f, r in zip(names, res) if f is not None]
+        elif names:
             res = _kad_songs(host, x.shape[0], offs, distributed)
             pairs = [(f, r.score) for f, r in zip(names, res) if f is not None]
 
@@ -849,7 +1057,7 @@ class FrechetAudioDistance:
         return csv
 
     def score_prdc_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
-                              k: int = 5, distributed: bool = False) -> Path:
+                              k: int = 5, distributed: bool = False, prepared: bool = False) -> Path:
         """Precision, recall, density and coverage of every file in eval_dir against the embeddings of baseline_dir
         (calc_prdc_songs: the baseline radii once, every file's radii and counts in one GPU pass each).  The table has
         the header ``file,precision,recall,density,coverage,n_eval`` and one row per file, sorted by density, highest
@@ -857,7 +1065,7 @@ class FrechetAudioDistance:
         data/prdc-individual/<model>/, and an existing table is returned untouched.  Files whose cache is missing,
         unreadable or not an fp16 [rows, d] array of the baseline's width, and files with at most k embedding rows,
         are logged and dropped.  distributed=True under torchrun: as for score_kad_individual, over the radii and
-        ball-count tiles."""
+        ball-count tiles.  prepared=True: as for score_kad_individual; the same table."""
         k = _prdc_k(k)
         csv = Path(csv_name)
         if isinstance(csv_name, str):
@@ -870,11 +1078,13 @@ class FrechetAudioDistance:
                 log.info(f"CSV file {csv} already exists, exiting...")
             return csv
 
-        x, host, offs, names, _, _ = self._individual_sets(baseline_dir, eval_dir, "PRDC", k + 1,
-                                                           f"more than k = {k} embedding rows", collective, writer)
+        x, host, offs, names, _, base_offs = self._individual_sets(baseline_dir, eval_dir, "PRDC", k + 1,
+                                                                   f"more than k = {k} embedding rows", collective, writer)
         rows = []
         if names:
-            res = _prdc_songs(host, x.shape[0], np.diff(offs).tolist(), k, distributed)
+            pb = self._prepared(baseline_dir, x, base_offs, k, distributed) if prepared and x.shape[0] > k else None
+            res = _prdc_songs(host if pb is None else host[x.shape[0]:], x.shape[0], np.diff(offs).tolist(), k,
+                              distributed, pb)
             rows = [(f, r) for f, r in zip(names, res) if f is not None]
         elif x.shape[0] <= k:
             raise ValueError(f"PRDC with k = {k} needs more than k embedding rows in each set (baseline {x.shape[0]})")
@@ -890,7 +1100,7 @@ class FrechetAudioDistance:
         return csv
 
     def score_realism_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
-                                 k: int = 3, distributed: bool = False) -> Path:
+                                 k: int = 3, distributed: bool = False, prepared: bool = False) -> Path:
         """Realism and nearest baseline clip of every file in eval_dir against the embeddings of baseline_dir: one
         calc_realism call over the rows of all files (a row's values depend on that row and the baseline alone).  The
         table has the header ``file,realism_median,realism_min,nearest_baseline,nearest_distance,n_eval`` and one row
@@ -899,7 +1109,8 @@ class FrechetAudioDistance:
         ties by path; commas in names are replaced.  A str csv_name goes under data/realism-individual/<model>/, and an
         existing table is returned untouched.  Files whose cache is missing, unreadable, not an fp16 [rows, d] array of
         the baseline's width, or empty are logged and dropped.  distributed=True under torchrun: as for
-        score_kad_individual, over the radii and realism tiles."""
+        score_kad_individual, over the radii and realism tiles.  prepared=True: as for score_kad_individual; the same
+        table."""
         k = _prdc_k(k, "realism")
         csv = Path(csv_name)
         if isinstance(csv_name, str):
@@ -917,7 +1128,8 @@ class FrechetAudioDistance:
         _realism_rows(x.shape[0], 1, k)
         rows = []
         if names:
-            res = _realism(host, x.shape[0], k, distributed)
+            pb = self._prepared(baseline_dir, x, base_offs, k, distributed) if prepared else None
+            res = _realism(host if pb is None else host[x.shape[0]:], x.shape[0], k, distributed, pb)
             for s, f in enumerate(names):
                 if f is None:
                     continue
@@ -937,7 +1149,7 @@ class FrechetAudioDistance:
         return csv
 
     def score_nearest_individual(self, baseline_dir: PathLike, eval_dir: PathLike, csv_name: Union[Path, str],
-                                 k: int = 5, distributed: bool = False) -> Path:
+                                 k: int = 5, distributed: bool = False, prepared: bool = False) -> Path:
         """The k baseline files every file of eval_dir comes closest to: a memorisation audit.  One calc_nearest call
         over the rows of all eval files, with each baseline embedding cache one group; then per eval file, per baseline
         file, the smallest (distance, eval row, baseline row) over the file's rows, and the first k baseline files in
@@ -947,7 +1159,8 @@ class FrechetAudioDistance:
         path; commas in names are replaced.  A str csv_name goes under data/nearest-individual/<model>/, and an
         existing table is returned untouched.  Files whose cache is missing, unreadable, not an fp16 [rows, d] array
         of the baseline's width, or empty are logged and dropped.  distributed=True under torchrun: as for
-        score_kad_individual, over the nearest tiles."""
+        score_kad_individual, over the nearest tiles.  prepared=True: as for score_kad_individual (nearest reuses the
+        resident rows alone); the same table."""
         k = _prdc_k(k, "nearest")
         csv = Path(csv_name)
         if isinstance(csv_name, str):
@@ -965,7 +1178,8 @@ class FrechetAudioDistance:
         _nearest_rows(x.shape[0], 1)
         tables = []
         if names:
-            res, q = _nearest(host, x.shape[0], k, base_offs, distributed)
+            pb = self._prepared(baseline_dir, x, base_offs, 1, distributed) if prepared else None
+            res, q = _nearest(host if pb is None else host[x.shape[0]:], x.shape[0], k, base_offs, distributed, pb)
             for s, f in enumerate(names):
                 if f is None:
                     continue

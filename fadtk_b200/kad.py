@@ -1,12 +1,12 @@
-"""``python -m fadtk_b200.kad <model> <baseline> <eval> [csv] [--indiv] [-w N] [-s sox]`` - Kernel Audio Distance
-between two audio directories (fad.calc_kernel_audio_distance).  Directories without embedding caches are embedded
-first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``).  Under ``torchrun`` every rank
-then takes its share of the pair tiles (``distributed=True``) when the library's NCCL communicator can be set up, and
-rank 0 scores alone otherwise; either way rank 0 alone reports and writes.  With
-``csv``, one row ``model,baseline,eval,kad,bandwidth,n_baseline,n_eval,time`` is appended; a new file gets the header
-first, and an existing file with another header is refused rather than mixed.  With ``--indiv``, every file of the eval
-directory is scored on its own against the baseline (FrechetAudioDistance.score_kad_individual) and ``csv`` is that
-table (default kad-individual-results.csv).  The ``fadtk`` command line itself is unchanged.
+"""``python -m fadtk_b200.kad <model> <baseline> <eval> [csv] [--indiv] [--prepared] [-w N] [-s sox]`` - Kernel Audio
+Distance between two audio directories (fad.calc_kernel_audio_distance). Directories without embedding caches are
+embedded first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``). Under ``torchrun`` every
+rank then takes its share of the pair tiles (``distributed=True``) when the library's NCCL communicator can be set up,
+and rank 0 scores alone otherwise; either way rank 0 alone reports and writes. With ``csv``, one row
+``model,baseline,eval,kad,bandwidth,n_baseline,n_eval,time`` is appended; a new file gets the header first, and an
+existing file with another header is refused rather than mixed. With ``--indiv``, every file of the eval directory is
+scored on its own against the baseline (FrechetAudioDistance.score_kad_individual) and ``csv`` is that table (default
+kad-individual-results.csv). The ``fadtk`` command line itself is unchanged.
 """
 from __future__ import annotations
 
@@ -25,6 +25,9 @@ _KAD_ARGS = (
     (("csv",), dict(type=str, nargs="?", help="append the result row here; with --indiv: where the per-file table "
                                               "goes (default kad-individual-results.csv)")),
     (("--indiv",), dict(action="store_true", help="score every evaluation file on its own against the baseline")),
+    (("--prepared",), dict(action="store_true", help="score against the baseline's saved pairwise preparation "
+                                                     "(python -m fadtk_b200.prepare), built and saved first when it is "
+                                                     "missing or stale")),
 )
 
 
@@ -68,12 +71,12 @@ def main(argv=None) -> int:
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
     if args.indiv:
         table = Path(args.csv or "kad-individual-results.csv")
-        fad.score_kad_individual(args.baseline, args.eval, table, distributed=sharded)
+        fad.score_kad_individual(args.baseline, args.eval, table, distributed=sharded, prepared=args.prepared)
         if dist.rank() == 0:
             log.info(f"Individual KAD scores saved to {table}")
         dist.shutdown()
         return 0
-    res = fad.score_kad(args.baseline, args.eval, distributed=sharded)
+    res = fad.score_kad(args.baseline, args.eval, distributed=sharded, prepared=args.prepared)
     if dist.rank() != 0:
         dist.shutdown()
         return 0

@@ -1,10 +1,10 @@
-"""``python -m fadtk_b200.nearest <model> <baseline> <eval> [csv] [-k K] [-w N] [-s sox]`` - the k baseline files every
-file of an eval directory comes closest to, with the distance and the pair of rows where it does: a memorisation audit
-(FrechetAudioDistance.score_nearest_individual on the cached embeddings).  Directories without embedding caches are
-embedded first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``).  Under ``torchrun`` every
-rank then takes its share of the nearest tiles (``distributed=True``) when the library's NCCL communicator can be set
-up, and rank 0 scores alone otherwise; either way rank 0 alone writes.  ``csv`` is the per-file table (default
-nearest-individual-results.csv).
+"""``python -m fadtk_b200.nearest <model> <baseline> <eval> [csv] [-k K] [--prepared] [-w N] [-s sox]`` - the k baseline
+files every file of an eval directory comes closest to, with the distance and the pair of rows where it does: a
+memorisation audit (FrechetAudioDistance.score_nearest_individual on the cached embeddings). Directories without
+embedding caches are embedded first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``). Under
+``torchrun`` every rank then takes its share of the nearest tiles (``distributed=True``) when the library's NCCL
+communicator can be set up, and rank 0 scores alone otherwise; either way rank 0 alone writes. ``csv`` is the per-file
+table (default nearest-individual-results.csv).
 """
 from __future__ import annotations
 
@@ -20,6 +20,9 @@ _NEAREST_ARGS = (
     (("eval",), dict(type=str, help="evaluation audio directory")),
     (("csv",), dict(type=str, nargs="?", help="where the per-file table goes (default nearest-individual-results.csv)")),
     (("-k",), dict(type=int, default=5, help="nearest baseline files per eval file, 1 to 16 (default 5)")),
+    (("--prepared",), dict(action="store_true", help="score against the baseline's saved pairwise preparation "
+                                                     "(python -m fadtk_b200.prepare), built and saved first when it is "
+                                                     "missing or stale")),
 )
 
 
@@ -42,7 +45,8 @@ def main(argv=None) -> int:
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
     table = Path(args.csv or "nearest-individual-results.csv")
-    fad.score_nearest_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded)
+    fad.score_nearest_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded,
+                                 prepared=args.prepared)
     if dist.rank() == 0:
         log.info(f"Per-file nearest baseline clips saved to {table}")
     dist.shutdown()

@@ -1,13 +1,13 @@
-"""``python -m fadtk_b200.prdc <model> <baseline> <eval> [csv] [-k K] [--indiv] [-w N] [-s sox]`` - precision, recall,
-density and coverage of an eval directory against a baseline directory (fad.calc_prdc on the cached embeddings).
+"""``python -m fadtk_b200.prdc <model> <baseline> <eval> [csv] [-k K] [--indiv] [--prepared] [-w N] [-s sox]`` - precision,
+recall, density and coverage of an eval directory against a baseline directory (fad.calc_prdc on the cached embeddings).
 Directories without embedding caches are embedded first (under ``torchrun`` the embedding is sharded over the ranks as
-for ``fadtk``).  Under ``torchrun`` every rank then takes its share of the radii and ball-count tiles
-(``distributed=True``) when the library's NCCL communicator can be set up, and rank 0 scores alone otherwise; either
-way rank 0 alone reports and writes.  With ``csv``, one row
+for ``fadtk``). Under ``torchrun`` every rank then takes its share of the radii and ball-count tiles
+(``distributed=True``) when the library's NCCL communicator can be set up, and rank 0 scores alone otherwise; either way
+rank 0 alone reports and writes. With ``csv``, one row
 ``model,baseline,eval,k,precision,recall,density,coverage,n_baseline,n_eval,time`` is appended; a new file gets the
-header first, and an existing file with another header is refused rather than mixed.  With ``--indiv``, every file of
-the eval directory is scored on its own against the baseline (FrechetAudioDistance.score_prdc_individual) and ``csv``
-is that table (default prdc-individual-results.csv).
+header first, and an existing file with another header is refused rather than mixed. With ``--indiv``, every file of the
+eval directory is scored on its own against the baseline (FrechetAudioDistance.score_prdc_individual) and ``csv`` is
+that table (default prdc-individual-results.csv).
 """
 from __future__ import annotations
 
@@ -28,6 +28,9 @@ _PRDC_ARGS = (
                                               "goes (default prdc-individual-results.csv)")),
     (("-k",), dict(type=int, default=5, help="nearest neighbour that sets each ball's radius, 1 to 16 (default 5)")),
     (("--indiv",), dict(action="store_true", help="score every evaluation file on its own against the baseline")),
+    (("--prepared",), dict(action="store_true", help="score against the baseline's saved pairwise preparation "
+                                                     "(python -m fadtk_b200.prepare), built and saved first when it is "
+                                                     "missing or stale")),
 )
 
 
@@ -53,12 +56,13 @@ def main(argv=None) -> int:
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
     if args.indiv:
         table = Path(args.csv or "prdc-individual-results.csv")
-        fad.score_prdc_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded)
+        fad.score_prdc_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded,
+                                  prepared=args.prepared)
         if dist.rank() == 0:
             log.info(f"Individual PRDC values saved to {table}")
         dist.shutdown()
         return 0
-    res = fad.score_prdc(args.baseline, args.eval, k=args.k, distributed=sharded)
+    res = fad.score_prdc(args.baseline, args.eval, k=args.k, distributed=sharded, prepared=args.prepared)
     if dist.rank() != 0:
         dist.shutdown()
         return 0

@@ -1,9 +1,9 @@
-"""``python -m fadtk_b200.realism <model> <baseline> <eval> [csv] [-k K] [-w N] [-s sox]`` - the realism score and the
-nearest baseline clip of every file of an eval directory against a baseline directory
-(FrechetAudioDistance.score_realism_individual on the cached embeddings).  Directories without embedding caches are
-embedded first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``).  Under ``torchrun`` every
+"""``python -m fadtk_b200.realism <model> <baseline> <eval> [csv] [-k K] [--prepared] [-w N] [-s sox]`` - the realism score
+and the nearest baseline clip of every file of an eval directory against a baseline directory
+(FrechetAudioDistance.score_realism_individual on the cached embeddings). Directories without embedding caches are
+embedded first (under ``torchrun`` the embedding is sharded over the ranks as for ``fadtk``). Under ``torchrun`` every
 rank then takes its share of the radii and realism tiles (``distributed=True``) when the library's NCCL communicator can
-be set up, and rank 0 scores alone otherwise; either way rank 0 alone writes.  ``csv`` is the per-file table (default
+be set up, and rank 0 scores alone otherwise; either way rank 0 alone writes. ``csv`` is the per-file table (default
 realism-individual-results.csv).
 """
 from __future__ import annotations
@@ -20,6 +20,9 @@ _REALISM_ARGS = (
     (("eval",), dict(type=str, help="evaluation audio directory")),
     (("csv",), dict(type=str, nargs="?", help="where the per-file table goes (default realism-individual-results.csv)")),
     (("-k",), dict(type=int, default=3, help="nearest neighbour that sets each ball's radius, 1 to 16 (default 3)")),
+    (("--prepared",), dict(action="store_true", help="score against the baseline's saved pairwise preparation "
+                                                     "(python -m fadtk_b200.prepare), built and saved first when it is "
+                                                     "missing or stale")),
 )
 
 
@@ -42,7 +45,8 @@ def main(argv=None) -> int:
 
     fad = FrechetAudioDistance(model, audio_load_worker=args.workers, load_model=False)
     table = Path(args.csv or "realism-individual-results.csv")
-    fad.score_realism_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded)
+    fad.score_realism_individual(args.baseline, args.eval, table, k=args.k, distributed=sharded,
+                                 prepared=args.prepared)
     if dist.rank() == 0:
         log.info(f"Per-file realism saved to {table}")
     dist.shutdown()

@@ -448,6 +448,48 @@ int fad_nearest(fad_handle* h, const void* z_f16, long long m, long long n, int 
 int fad_nearest_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
                         long long n, int d, int k, const long long* base_offsets, long long n_groups, int* nearest,
                         float* nearest_sq, void* stream);
+/* A prepared baseline (DESIGN.md section 5.15): the baseline-only work of KAD, PRDC and realism done once, then eval
+ * passes that take its results as device inputs and run no tile of X against X.  z = [X; Y] as above (fp16, X first,
+ * 16-byte aligned), d a multiple of 8, q as for PRDC.  Every argument is checked first (null or misaligned pointers, d,
+ * k, the row limits of the unprepared entry each one stands in for); a rejected call launches nothing and writes nothing.
+ *   fad_pair_digest        out (device uint64, 8-byte aligned) = the order-dependent digest of the rows fp16 [rows, d]
+ *                          that the _sharded entries compare across ranks; a saved preparation records it for its rows
+ *   fad_knn_lists_sq       x = X alone (fp16 [m, d]), 1 <= k_max <= 16, m > k_max; lists (device fp32 [m][k_max]) = per
+ *                          row of X the k_max smallest q to the other rows of X, ascending.  Column k - 1 is bitwise the
+ *                          r_i^2 fad_knn_radii_sq gives at k, for every k <= k_max (both exact selections of one set of
+ *                          fp32 values)
+ *   fad_kad_eval_sums      fad_kad_song_sums without the S_xx pass (offsets, sigma and their checks as there; a whole eval
+ *                          set is one item); out (device fp64 [n_items][2]) = S_yy,k, S_xy,k, bitwise the values
+ *                          fad_kad_song_sums gives from the same work list
+ *   fad_knn_eval_radii_sq  the Y part of fad_knn_radii_sq (offsets NULL: Y = n_items rows, one set; checks as there) or
+ *                          of fad_knn_song_radii_sq (offsets as there); radii_sq (device fp32 [n]) = s_j^2, bitwise those
+ *                          calls' Y values.  With r_i^2 from a list, [r_i^2 | s_j^2] is the radii_sq input of
+ *                          fad_prdc_counts / fad_prdc_song_counts
+ *   fad_realism_prepared   the realism tile pass of fad_realism alone (m >= 2, n >= 1) on the caller's kept radii
+ *                          (device fp32 [m]); realism, nearest, nearest_sq as fad_realism writes them, bitwise equal when
+ *                          given the kept_radii_sq fad_realism writes
+ * The _sharded forms split the tile work as their unprepared counterparts do (local_shards as for fad_kad_*_sharded),
+ * bitwise equal for any number of shards.  Collective calls also compare k_max or k, the bits of sigma, the number of
+ * items and a digest of the offsets, and a digest of the kept radii, as each entry takes them. */
+int fad_pair_digest(fad_handle* h, const void* z_f16, long long rows, int d, unsigned long long* out, void* stream);
+int fad_knn_lists_sq(fad_handle* h, const void* x_f16, long long m, int d, int k_max, float* lists, void* stream);
+int fad_knn_lists_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* x_f16, long long m,
+                             int d, int k_max, float* lists, void* stream);
+int fad_kad_eval_sums(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items, int d,
+                      const double* sigma, double* out, void* stream);
+int fad_kad_eval_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                              const long long* offsets, long long n_items, int d, const double* sigma, double* out,
+                              void* stream);
+int fad_knn_eval_radii_sq(fad_handle* h, const void* z_f16, long long m, const long long* offsets, long long n_items,
+                          int d, int k, float* radii_sq, void* stream);
+int fad_knn_eval_radii_sq_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16,
+                                  long long m, const long long* offsets, long long n_items, int d, int k, float* radii_sq,
+                                  void* stream);
+int fad_realism_prepared(fad_handle* h, const void* z_f16, long long m, long long n, int d, const float* kept_radii_sq,
+                         float* realism, int* nearest, float* nearest_sq, void* stream);
+int fad_realism_prepared_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
+                                 long long n, int d, const float* kept_radii_sq, float* realism, int* nearest,
+                                 float* nearest_sq, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
