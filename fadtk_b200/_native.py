@@ -128,6 +128,11 @@ SIGNATURES = {
     "fad_knn_lists_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_kad_eval_sums": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
     "fad_kad_eval_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_perm_labels": (C.c_int, [c_vp, c_ll, c_ll, C.c_int, C.c_ulonglong, c_vp, c_vp]),
+    "fad_perm_dot": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_kad_perm_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, C.c_int, C.c_ulonglong, c_vp, c_vp]),
+    "fad_kad_perm_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, C.c_int, C.c_ulonglong,
+                                            c_vp, c_vp]),
     "fad_knn_eval_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_knn_eval_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp,
                                                 c_vp]),
@@ -935,6 +940,46 @@ class Engine:
         _check(fn(self._h, *shard_args, z.data_ptr(), m, n, z.shape[1], int(k), off, groups, nearest.data_ptr(),
                   nearest_sq.data_ptr(), _stream()))
         return nearest, nearest_sq
+
+    # ------------------------------------------- permutation tests of KAD (DESIGN.md 5.16)
+    # A pool of n rows, `a` of them labelled; labelling 0 marks rows 0 .. a - 1, labellings 1 .. B come from the seed
+    # (include/fadtk_b200.h).  seed: an int in [0, 2**64).
+    def perm_labels(self, n: int, a: int, labellings: int, seed: int) -> torch.Tensor:
+        """-> int32 [B + 1, 4 ceil(n / 128)] (cuda; the uint32 words' bits): bit i & 31 of word i >> 5 of row b is row i's
+        label in labelling b (fad_perm_labels)"""
+        words = 4 * ((max(int(n), 0) + 127) // 128)
+        out = torch.empty((max(int(labellings), 0) + 1, max(words, 4)), dtype=torch.int32, device=self.torch_device)
+        _check(lib().fad_perm_labels(self._h, int(n), int(a), int(labellings), int(seed), out.data_ptr(), _stream()))
+        return out
+
+    def perm_dot(self, bits: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+        """bits as perm_labels gives them, v fp64 [n] (cuda) -> fp64 [B + 1] (cuda): per labelling the sum of v over the
+        rows it marks, in a fixed order (fad_perm_dot)"""
+        assert bits.dtype == torch.int32 and bits.is_cuda and bits.is_contiguous() and bits.ndim == 2
+        assert v.dtype == torch.float64 and v.is_cuda and v.is_contiguous() and v.ndim == 1
+        assert bits.shape[1] == 4 * ((v.shape[0] + 127) // 128)
+        out = torch.empty(bits.shape[0], dtype=torch.float64, device=v.device)
+        _check(lib().fad_perm_dot(self._h, bits.data_ptr(), v.shape[0], bits.shape[0] - 1, v.data_ptr(), out.data_ptr(),
+                                  _stream()))
+        return out
+
+    def kad_perm_sums(self, z: torch.Tensor, a: int, sigma: torch.Tensor, labellings: int, seed: int) -> torch.Tensor:
+        """z fp16 [n, d] (cuda, the pool), sigma fp64 scalar (cuda) -> fp64 [B + 1, 3] (cuda): (S_aa, S_bb, S_ab) of
+        every labelling, each kernel value rounded to fp16 once (fad_kad_perm_sums)"""
+        return self._perm_sums(lib().fad_kad_perm_sums, (), z, a, sigma, labellings, seed)
+
+    def kad_perm_sums_sharded(self, z: torch.Tensor, a: int, sigma: torch.Tensor, labellings: int, seed: int,
+                              local_shards: int = 0) -> torch.Tensor:
+        """fad_kad_perm_sums_sharded: kad_perm_sums over shards (local_shards as for kad_sums_sharded)"""
+        return self._perm_sums(lib().fad_kad_perm_sums_sharded, (None, int(local_shards)), z, a, sigma, labellings, seed)
+
+    def _perm_sums(self, fn, shard_args, z, a, sigma, labellings, seed):
+        assert z.dtype == torch.float16 and z.is_cuda and z.is_contiguous() and z.ndim == 2
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        out = torch.empty((max(int(labellings), 0) + 1, 3), dtype=torch.float64, device=z.device)
+        _check(fn(self._h, *shard_args, z.data_ptr(), z.shape[0], int(a), z.shape[1], sigma.data_ptr(), int(labellings),
+                  int(seed), out.data_ptr(), _stream()))
+        return out
 
     # ------------------------------------------- a prepared baseline (DESIGN.md 5.15)
     # The _sharded forms take local_shards as kad_sums_sharded does; None runs the unsharded entry.

@@ -568,6 +568,7 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
+    CK(smem((const void*)fad::kad_perm_tile_kernel, fad::kPermSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<0>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<1>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<2>, fad::kPairSmemBytes));

@@ -348,4 +348,338 @@ __global__ void kad_select_kernel(KadSelectState* st, const unsigned long long* 
     }
 }
 
+// ------------------------------------------------------------------------------- permutation tests (DESIGN.md 5.16)
+// Z = a pool of N rows; a labelling marks `a` of them.  Over the pairs i < j, with K_ij the kernel value rounded to fp16
+// once: R_i = sum_{j>i} K_ij, P(l) = sum l_i l_j K_ij, C(l) = sum l_j K_ij.  The tile pass runs MODE 0's units and tiles;
+// each consumer stores its 64 x 128 block of fp16 kernel values to shared memory (K-major, 128-B swizzle) and runs, per
+// block of 64 labellings, U = W_J K_IJ^T as 8 m64n64k16 wgmmas with the labels of the column tile J expanded from bits
+// to fp16 0 / 1 in registers (the A operand).  The accumulator holds (labelling, row i); each thread sums its elements
+// over i in fp32 (C) and over the rows of I the labelling marks (P), a fixed quad tree adds the 4 lanes of a labelling,
+// and each lane keeps one fp64 running sum per block over the unit's tiles.  R_i is summed per thread over the unit's
+// tiles in fp64 and written once (a tile row belongs to one unit).  No atomics: every sum has a fixed order.
+//
+// Label bits: labelling b is words [b * words, (b + 1) * words), words = 4 ceil(N / 128); bit i & 31 of word i >> 5 is
+// row i's label, 0 past N.  Labelling 0 marks rows 0 .. a - 1; labelling b >= 1 marks the a rows with the smallest
+// (pair_mix64(pair_mix64(seed + b) ^ i), i); labellings past the last are all zero.
+constexpr int kPermBlock = 64;                     // labellings per wgmma (its M)
+constexpr int kPermPass = 1024;                    // labellings per tile pass
+constexpr int kPermLabelThreads = 1024;
+constexpr int kPermSumThreads = 256;
+constexpr uint32_t kPermKBytes = 64 * 128 * 2;     // one consumer's fp16 kernel block: two 64-row x 64-column halves
+// the pair tiles, then (1024-aligned: 768 bytes past the barriers) the two consumers' kernel blocks
+constexpr uint32_t kPermSmemBytes = kPairSmemBytes + 768 + 2 * kPermKBytes;
+static_assert(kPermSmemBytes <= 227 * 1024, "over the per-CTA shared-memory limit");
+
+struct KadPermParams {
+    int N, d, T;
+    int units, unit0, unit1;  // MODE 0's units; this launch's [unit0, unit1)
+    const float* norm;        // [T * 128]
+    const double* sigma;      // device scalar
+    const uint32_t* bits;     // this pass's first labelling (layout above)
+    int words;                // words per labelling
+    int blocks;               // blocks of 64 labellings in this pass (1 .. 16)
+    double* partial;          // [units][2 consumers][64 blocks][2]: P, C of each labelling
+    double* rowsum;           // [T * 128] R_i
+};
+
+// bits b0, b1 (bits 0, 1 of x) -> the fp16 pair (b0, b1) as 0 / 1
+__device__ __forceinline__ uint32_t perm_half2(uint32_t x) {
+    return ((x & 1u) | ((x & 2u) << 15)) * 0x3C00u;
+}
+
+__global__ void __launch_bounds__(kPairThreads, 1)
+kad_perm_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
+                     const KadPermParams p) {
+    using namespace sm90;
+    extern __shared__ uint8_t smem_raw[];
+    const int warp = threadIdx.x >> 5;
+    const int lane = threadIdx.x & 31;
+    const PairTile pt = pair_tile_open(smem_raw, &map_hi, &map_lo, p.d, warp, lane);
+    uint8_t* smem = pt.smem;
+    uint64_t* full = pt.full;
+    uint64_t* empty = pt.empty;
+    const int ksteps = pt.ksteps, chunk_len = pt.chunk_len;
+    __syncthreads();
+
+    if (warp < 4) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && elect_one()) {
+            int s = 0; uint32_t ph = 0;
+            for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
+                for (int half = 0; half < 2; ++half) {
+                    const int r = half == 0 ? u : p.T - 1 - u;
+                    if (half == 1 && r == u) break;
+                    for (int ct = r; ct < p.T; ++ct)
+                        pair_load_tile(smem, full, empty, s, ph, &map_hi, &map_lo, ksteps, r * 128, ct * 128);
+                }
+            }
+        }
+        return;
+    }
+    setmaxnreg_inc<kPairConsumerRegs>();
+    const int c = (warp >> 2) - 1;
+    const int wq = warp & 3;
+    const int q = lane & 3;
+    const int lr0 = wq * 16 + (lane >> 2);        // rows lr0, lr0 + 8 of the consumer's 64; also labelling rows of a block
+    const uint32_t kbase = smem_u32(pt.own + 768) + c * kPermKBytes;
+    const double sg = *p.sigma;
+    const float neg_coef = (float)(-1.4426950408889634 / (2.0 * sg * sg));
+    int s = 0; uint32_t ph = 0;
+
+    for (int u = p.unit0 + blockIdx.x; u < p.unit1; u += gridDim.x) {
+        double acc[kPermPass / kPermBlock];
+#pragma unroll
+        for (int lb = 0; lb < kPermPass / kPermBlock; ++lb) acc[lb] = 0.0;
+        for (int half = 0; half < 2; ++half) {
+            const int r = half == 0 ? u : p.T - 1 - u;
+            if (half == 1 && r == u) break;
+            const int row0 = r * 128 + c * 64 + lr0;
+            const float nr0 = __ldg(p.norm + row0), nr1 = __ldg(p.norm + row0 + 8);
+            double rs[2] = {0.0, 0.0};
+            for (int ct = r; ct < p.T; ++ct) {
+                float sum[64];
+                pair_mma_tile(sum, smem, full, empty, s, ph, c, lane, p.d, ksteps, chunk_len);
+                // ---- kernel values, rounded to fp16 once, into R and into this consumer's block (row lr, column j at
+                // half j / 64, 16-B chunk ((j % 64) / 8) ^ (lr % 8): the 128-B swizzle)
+                const int col0 = ct * 128 + 2 * q;
+                float rt[2] = {0.f, 0.f};
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    const float2 nc = __ldg(reinterpret_cast<const float2*>(p.norm + col0 + 8 * j));
+#pragma unroll
+                    for (int i = 0; i < 2; ++i) {
+                        __half kh[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int gi = row0 + 8 * i, gj = col0 + 8 * j + e;
+                            const float qd = pair_q(sum[4 * j + 2 * i + e], i ? nr1 : nr0, e ? nc.y : nc.x);
+                            float kv;
+                            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(kv) : "f"(qd * neg_coef));
+                            kh[e] = __float2half_rn(gj > gi && gj < p.N ? kv : 0.f);
+                            rt[i] += __half2float(kh[e]);
+                        }
+                        const int lr = lr0 + 8 * i;
+                        const uint32_t addr = kbase + (j >> 3) * (kPermKBytes / 2) + lr * 128 + (((j & 7) ^ (lr & 7)) << 4) + 4 * q;
+                        const uint32_t v = (uint32_t)__half_as_ushort(kh[0]) | ((uint32_t)__half_as_ushort(kh[1]) << 16);
+                        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+                    }
+                }
+                rs[0] += (double)rt[0];
+                rs[1] += (double)rt[1];
+                fence_proxy_async_smem();
+                named_bar_sync(2 + c, 128);
+
+                // ---- per block of 64 labellings: U = W_J K^T, then P and C over the rows of I.  bl = labelling row lr0
+                // of the block, advanced through an empty asm so that the compiler keeps one pointer live instead of
+                // hoisting (and spilling) one per block
+                const uint32_t* bl = p.bits + (size_t)lr0 * p.words;
+                const size_t row8 = 8 * (size_t)p.words, block = (size_t)kPermBlock * p.words;
+#pragma unroll
+                for (int lb = 0; lb < kPermPass / kPermBlock; ++lb) {
+                    if (lb < p.blocks) {
+                        const uint4 wj0 = __ldg(reinterpret_cast<const uint4*>(bl + ct * 4));
+                        const uint4 wj1 = __ldg(reinterpret_cast<const uint4*>(bl + row8 + ct * 4));
+                        const uint32_t j0[4] = {wj0.x, wj0.y, wj0.z, wj0.w}, j1[4] = {wj1.x, wj1.y, wj1.z, wj1.w};
+                        // A fragment of k-step kk (columns 16 kk ..): a[0] = labelling row lr0, columns 2 q + {0, 1};
+                        // a[1] = row lr0 + 8; a[2], a[3] = columns + 8
+                        uint32_t a[8][4];
+#pragma unroll
+                        for (int kk = 0; kk < 8; ++kk) {
+                            const int sh = 16 * (kk & 1) + 2 * q;
+                            const uint32_t x0 = j0[kk >> 1] >> sh, x1 = j1[kk >> 1] >> sh;
+                            a[kk][0] = perm_half2(x0);
+                            a[kk][1] = perm_half2(x1);
+                            a[kk][2] = perm_half2(x0 >> 8);
+                            a[kk][3] = perm_half2(x1 >> 8);
+                        }
+                        float dl[32];
+                        wgmma_fence();
+#pragma unroll
+                        for (int kk = 0; kk < 8; ++kk)
+                            wgmma_m64n64k16_f16_rs_kmajor(dl, a[kk], kmajor_sw128_desc(kbase + (kk >> 2) * (kPermKBytes / 2)) + 2 * (kk & 3),
+                                                          kk > 0);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        fence_regs(dl);
+                        // element (labelling row lr0 + 8 rr, row 64 c + 8 jj + 2 q + e of I) is dl[4 jj + 2 rr + e]
+                        const uint2 wi0 = __ldg(reinterpret_cast<const uint2*>(bl + r * 4 + 2 * c));
+                        const uint2 wi1 = __ldg(reinterpret_cast<const uint2*>(bl + row8 + r * 4 + 2 * c));
+                        const uint32_t i0[2] = {wi0.x >> (2 * q), wi0.y >> (2 * q)}, i1[2] = {wi1.x >> (2 * q), wi1.y >> (2 * q)};
+                        float pp[2] = {0.f, 0.f}, cc[2] = {0.f, 0.f};
+#pragma unroll
+                        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+                            for (int rr = 0; rr < 2; ++rr) {
+                                const uint32_t w = (rr ? i1 : i0)[jj >> 2] >> (8 * (jj & 3));
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const float v = dl[4 * jj + 2 * rr + e];
+                                    cc[rr] += v;
+                                    pp[rr] += ((w >> e) & 1u) ? v : 0.f;
+                                }
+                            }
+                        }
+#pragma unroll
+                        for (int o = 1; o < 4; o <<= 1) {
+#pragma unroll
+                            for (int rr = 0; rr < 2; ++rr) {
+                                pp[rr] += __shfl_xor_sync(0xffffffffu, pp[rr], o);
+                                cc[rr] += __shfl_xor_sync(0xffffffffu, cc[rr], o);
+                            }
+                        }
+                        // lane q keeps P (q even) or C (q odd) of labelling row lr0 + 8 (q >> 1)
+                        const float mine = q == 0 ? pp[0] : q == 1 ? cc[0] : q == 2 ? pp[1] : cc[1];
+                        // undo the accumulator's truncation shrink (conv_gemm.cuh): an element of U adds one product
+                        // per column the labelling marks (zero products do not truncate); counting every marked
+                        // column also counts the masked j <= i ones of a diagonal tile, a shrink of at most
+                        // 64 kAccumShrinkPerElement ~ 7e-8 over-corrected there
+                        const uint4 jw = q < 2 ? wj0 : wj1;
+                        const int marked = __popc(jw.x) + __popc(jw.y) + __popc(jw.z) + __popc(jw.w);
+                        acc[lb] += (double)fmaf(mine, kAccumShrinkPerElement * (float)marked, mine);
+                        bl += block;
+                        asm volatile("" : "+l"(bl));
+                    }
+                }
+                // every warp of this consumer has read the block (wgmma_wait) before the next tile overwrites it
+                named_bar_sync(2 + c, 128);
+            }
+            // R of rows row0, row0 + 8: the quad's 4 lanes by a fixed xor tree
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                for (int o = 1; o < 4; o <<= 1) rs[i] += __shfl_xor_sync(0xffffffffu, rs[i], o);
+                if (q == 0) p.rowsum[row0 + 8 * i] = rs[i];
+            }
+        }
+        double* part = p.partial + ((size_t)u * 2 + c) * p.blocks * kPermBlock * 2;
+#pragma unroll
+        for (int lb = 0; lb < kPermPass / kPermBlock; ++lb)
+            if (lb < p.blocks) part[(lb * kPermBlock + lr0 + 8 * (q >> 1)) * 2 + (q & 1)] = acc[lb];
+    }
+}
+
+// one block per labelling (grid = all labellings of the call, padding included); layout and rule above.  Labellings
+// b >= 1: an exact radix select (8 passes of 8 bits) of the a-th smallest key K, recomputing the keys each pass; rows
+// with key < K are marked, and of the rows with key K the lowest indices until a rows are marked.
+__global__ void __launch_bounds__(kPermLabelThreads)
+kad_perm_label_kernel(int N, int a, int labellings, unsigned long long seed, int words, uint32_t* __restrict__ bits) {
+    __shared__ uint32_t hist[256];
+    __shared__ unsigned long long s_prefix;
+    __shared__ int s_rank;
+    __shared__ int s_ties[kPermLabelThreads / 32];
+    const int b = blockIdx.x;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint32_t* out = bits + (size_t)b * words;
+    if (b == 0 || b >= labellings) {
+        for (int w = threadIdx.x; w < words; w += blockDim.x) {
+            const int lo = 32 * w;
+            out[w] = b != 0 || lo >= a ? 0u : lo + 32 <= a ? ~0u : (1u << (a - lo)) - 1u;
+        }
+        return;
+    }
+    const unsigned long long base = pair_mix64(seed + (unsigned long long)b);
+    unsigned long long prefix = 0, mask = 0;
+    int rank = a - 1;
+    for (int shift = 56; shift >= 0; shift -= 8) {
+        for (int t = threadIdx.x; t < 256; t += blockDim.x) hist[t] = 0;
+        __syncthreads();
+        for (int i = threadIdx.x; i < N; i += blockDim.x) {
+            const unsigned long long k = pair_mix64(base ^ (unsigned long long)i);
+            if ((k & mask) == prefix) atomicAdd(&hist[(k >> shift) & 255], 1u);
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            int below = 0, bin = 0;
+            for (; bin < 255; ++bin) {
+                if (below + (int)hist[bin] > rank) break;
+                below += (int)hist[bin];
+            }
+            s_prefix = prefix | ((unsigned long long)bin << shift);
+            s_rank = rank - below;
+        }
+        __syncthreads();
+        prefix = s_prefix;
+        rank = s_rank;
+        mask |= 255ull << shift;
+    }
+    const int take = rank + 1;                      // rows with key == prefix to mark
+    int taken = 0;
+    for (int i0 = 0; i0 < 32 * words; i0 += blockDim.x) {
+        const int i = i0 + threadIdx.x;
+        const unsigned long long k = i < N ? pair_mix64(base ^ (unsigned long long)i) : ~0ull;
+        const bool tie = i < N && k == prefix;
+        const uint32_t tb = __ballot_sync(0xffffffffu, tie);
+        if (lane == 0) s_ties[warp] = __popc(tb);
+        __syncthreads();
+        int before = taken, total = 0;
+        for (int w = 0; w < kPermLabelThreads / 32; ++w) {
+            if (w < warp) before += s_ties[w];
+            total += s_ties[w];
+        }
+        const bool in = i < N && (k < prefix || (tie && before + __popc(tb & ((1u << lane) - 1u)) < take));
+        const uint32_t word = __ballot_sync(0xffffffffu, in);
+        if (lane == 0 && (i0 >> 5) + warp < words) out[(i0 >> 5) + warp] = word;
+        taken += total;
+        __syncthreads();
+    }
+}
+
+// a fixed-order sum over a block of kPermSumThreads threads (lanes by a shuffle tree, then the warps in order); the
+// result in thread 0
+__device__ __forceinline__ double perm_block_sum(double s) {
+    __shared__ double red[kPermSumThreads / 32];
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    double t = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < kPermSumThreads / 32; ++w) t += red[w];
+    return t;
+}
+
+// one block per labelling: out[b] = the sum of v[i] over the rows labelling b marks; each thread its words in order
+// (rows in order within a word), then perm_block_sum
+__global__ void __launch_bounds__(kPermSumThreads)
+kad_perm_dot_kernel(const uint32_t* __restrict__ bits, int words, const double* __restrict__ v, double* __restrict__ out) {
+    const uint32_t* w = bits + (size_t)blockIdx.x * words;
+    double s = 0.0;
+    for (int k = threadIdx.x; k < words; k += kPermSumThreads) {
+        uint32_t x = w[k];
+        while (x) {
+            s += v[32 * k + __ffs(x) - 1];
+            x &= x - 1;
+        }
+    }
+    const double t = perm_block_sum(s);
+    if (threadIdx.x == 0) out[blockIdx.x] = t;
+}
+
+// *out = sum of v[0 .. n) (one block): each thread its strided values in order, then perm_block_sum
+__global__ void __launch_bounds__(kPermSumThreads)
+kad_perm_total_kernel(const double* __restrict__ v, int n, double* __restrict__ out) {
+    double s = 0.0;
+    for (int i = threadIdx.x; i < n; i += kPermSumThreads) s += v[i];
+    const double t = perm_block_sum(s);
+    if (threadIdx.x == 0) *out = t;
+}
+
+// this pass's P and C: pc[2 l + k] = the sum over units in order, consumer 0 then 1, of partial[u][c][l][k]
+__global__ void kad_perm_reduce_kernel(const double* __restrict__ partial, int units, int n, double* __restrict__ pc) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= 2 * n) return;
+    double s = 0.0;
+    for (int u = 0; u < 2 * units; ++u) s += partial[(size_t)u * 2 * n + t];
+    pc[t] = s;
+}
+
+// out[b] = (S_aa, S_bb, S_ab) = (P, ((T - L) - C) + P, (L + C) - 2 P) for the first `labellings` labellings
+__global__ void kad_perm_finish_kernel(const double* __restrict__ pc, const double* __restrict__ l,
+                                       const double* __restrict__ total, int labellings, double* __restrict__ out) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= labellings) return;
+    const double P = pc[2 * b], C = pc[2 * b + 1], L = l[b], T = *total;
+    out[3 * (size_t)b] = P;
+    out[3 * (size_t)b + 1] = ((T - L) - C) + P;
+    out[3 * (size_t)b + 2] = (L + C) - 2.0 * P;
+}
+
 }  // namespace fad

@@ -10,6 +10,8 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     calc_realism                (no reference counterpart) -> k-NN radii and one max / argmin tile pass (csrc/prdc.cuh)
     calc_nearest                (no reference counterpart) -> one distinct-group top-k tile pass (csrc/prdc.cuh)
     prepare_pairwise_baseline                              -> the baseline-only work of the four above, done once
+    calc_kad_test, calc_kad_comparison                     -> permutation p-values of KAD: every labelling in one
+                                                              label-product tile pass (csrc/kad.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -86,6 +88,32 @@ class KADResults(NamedTuple):
     bandwidth: float
     n_baseline: int
     n_eval: int
+
+
+class KADTestResults(NamedTuple):
+    score: float                    # calc_kernel_audio_distance(emb_baseline, emb_eval).score, bitwise
+    bandwidth: float
+    p_value: float
+    null_scores: np.ndarray         # float64 [permutations], KAD of each random labelling
+    observed: float                 # KAD of the observed labelling on the permutation path (fp16 kernel values)
+    permutations: int
+    seed: int
+    n_baseline: int
+    n_eval: int
+
+
+class KADComparisonResults(NamedTuple):
+    score_a: float                  # calc_kernel_audio_distance_songs(emb_baseline, [emb_a, emb_b]), bitwise
+    score_b: float
+    difference: float               # score_a - score_b
+    p_value: float
+    null_differences: np.ndarray    # float64 [permutations]
+    bandwidth: float
+    permutations: int
+    seed: int
+    n_baseline: int
+    n_a: int
+    n_b: int
 
 
 class PRDCResults(NamedTuple):
@@ -266,6 +294,137 @@ def _kad_songs(z: torch.Tensor, m: int, offsets: np.ndarray, distributed: bool =
         score = _kad_score(s_xx, float(sums[1 + 2 * k]), float(sums[2 + 2 * k]), m, n) if n >= 2 else float("nan")
         out.append(KADResults(score=score, bandwidth=sigma, n_baseline=m, n_eval=n))
     return out
+
+
+def _perm_args(permutations, seed, metric: str):
+    if isinstance(permutations, bool) or not isinstance(permutations, (int, np.integer)) or not 1 <= permutations <= 9999:
+        raise ValueError(f"{metric} needs permutations in [1, 9999] (got {permutations!r})")
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
+        raise ValueError(f"{metric} needs an integer seed in [0, 2**64) (got {seed!r})")
+    return int(permutations), int(seed)
+
+
+def _perm_p(null: np.ndarray, observed: float) -> float:
+    """(1 + #{null >= observed}) / (B + 1): never 0 (Phipson and Smyth, 2010)"""
+    return (1.0 + float(np.count_nonzero(null >= observed))) / (null.shape[0] + 1.0)
+
+
+def _perm_pool(emb_baseline, pool_parts: list, what: list, metric: str):
+    """-> (the pooled sets' fp16 rows, the baseline rows or None when prepared, m, the pooled sets' sizes, the
+    PairwiseBaseline or None), with calc_kernel_audio_distance's checks"""
+    prepared = emb_baseline if _is_prepared(emb_baseline) else None
+    if prepared is not None:
+        parts = [_prepared_width(prepared, _kad_rows(y, w, metric), w) for y, w in zip(pool_parts, what)]
+        x_rows, m = None, prepared.m
+    else:
+        x_rows = _kad_rows(emb_baseline, "baseline", metric)
+        m = int(x_rows.shape[0])
+        parts = [_kad_rows(y, w, metric) for y, w in zip(pool_parts, what)]
+        for y, w in zip(parts, what):
+            if y.shape[1] != x_rows.shape[1]:
+                raise ValueError(f"embedding widths differ (baseline {x_rows.shape[1]}, {w} {y.shape[1]})")
+    sizes = [int(y.shape[0]) for y in parts]
+    if m < 2 or min(sizes) < 2:
+        raise ValueError(f"{metric} needs at least two embedding rows in each set (baseline {m}, "
+                         + ", ".join(f"{w} {n}" for w, n in zip(what, sizes)) + ")")
+    return parts, x_rows, m, sizes, prepared
+
+
+def _perm_sums(eng, collective: bool, pool: torch.Tensor, a: int, sigma: float, permutations: int, seed: int):
+    sig = torch.tensor([sigma], dtype=torch.float64, device=eng.torch_device)
+    if collective:
+        return eng.kad_perm_sums_sharded(pool, a, sig, permutations, seed).cpu().numpy()
+    return eng.kad_perm_sums(pool, a, sig, permutations, seed).cpu().numpy()
+
+
+def calc_kad_test(emb_baseline, emb_eval, permutations: int = 999, seed: int = 0,
+                  distributed: bool = False) -> KADTestResults:
+    """Permutation test of KAD (Gretton et al., 2012): can the eval set be told apart from the baseline at this sample
+    size?  The pool [X; Y] (m + n rows) is relabelled `permutations` times (B); labelling b marks the m rows with the
+    smallest (pair_mix64(pair_mix64(seed + b) ^ i), i) as the baseline (DESIGN.md 5.16), and KAD is recomputed for each:
+
+        KAD(l) = 1000 * (2 S_aa / (m (m - 1)) + 2 S_bb / (n (n - 1)) - 2 S_ab / (m n)),
+        p      = (1 + #{b >= 1 : KAD_b >= KAD_0}) / (B + 1),
+
+    KAD_0 the observed labelling.  sigma is the bandwidth of the observed baseline (as calc_kernel_audio_distance uses
+    it), held fixed across labellings: the test is conditional on sigma.  `score` is bitwise calc_kernel_audio_distance's
+    value; the rows go to the GPU once and serve both the score and the labellings.
+
+    Precision: every labelling's sums come from one pass over the pair tiles per 1024 labellings (fad_kad_perm_sums),
+    with each kernel value rounded to fp16 once.  That moves each labelling's statistic by an amount of the order of
+    2^-11 sqrt(sum coef^2 K^2) (oracle/kad_test_oracle.py, error_scale), measured at up to about 0.17 of the null
+    distribution's standard deviation on 4 000-row pools.  Null values that close to the observed one can fall either
+    side of it, so a p-value near a threshold can move by a few hundredths against an exact fp64 computation; `observed`
+    (KAD_0 on the same fp16 path) is what the nulls are compared with.
+
+    emb_baseline may be a PairwiseBaseline: its sigma and rows are used, the p-value and nulls are bitwise the
+    unprepared call's, and score is the prepared calc_kernel_audio_distance value.  Raises ValueError as
+    calc_kernel_audio_distance does, and for permutations outside [1, 9999] or a seed outside [0, 2**64).
+    distributed: as for calc_kernel_audio_distance (the permutation pass is sharded too)."""
+    permutations, seed = _perm_args(permutations, seed, "a KAD permutation test")
+    parts, x_rows, m, (n,), prepared = _perm_pool(emb_baseline, [emb_eval], ["eval"], "KAD")
+    eng, collective = _kad_engine(distributed)
+    if prepared is not None:
+        yd = _kad_device_rows(parts[0], eng)
+        score = _kad_prepared(prepared, yd, np.array([0, n], dtype=np.int64), distributed)[0]
+        pool = torch.cat([prepared.x, yd])
+    else:
+        pool = _kad_device_rows(torch.cat([x_rows, parts[0]]), eng)
+        sigma = _kad_bandwidth(eng, pool, m, collective)
+        sig = torch.tensor([sigma], dtype=torch.float64, device=eng.torch_device)
+        sums = eng.kad_sums_sharded(pool, m, sig) if collective else eng.kad_sums(pool, m, sig)
+        s_xx, s_yy, s_xy = (float(v) for v in sums.cpu().numpy())
+        score = KADResults(score=_kad_score(s_xx, s_yy, s_xy, m, n), bandwidth=sigma, n_baseline=m, n_eval=n)
+    s = _perm_sums(eng, collective, pool, m, score.bandwidth, permutations, seed)
+    stats = 1000.0 * (2.0 * s[:, 0] / (m * (m - 1.0)) + 2.0 * s[:, 1] / (n * (n - 1.0)) - 2.0 * s[:, 2] / (float(m) * n))
+    return KADTestResults(score=score.score, bandwidth=score.bandwidth, p_value=_perm_p(stats[1:], stats[0]),
+                          null_scores=stats[1:].copy(), observed=float(stats[0]), permutations=permutations, seed=seed,
+                          n_baseline=m, n_eval=n)
+
+
+def calc_kad_comparison(emb_baseline, emb_a, emb_b, permutations: int = 999, seed: int = 0,
+                        distributed: bool = False) -> KADComparisonResults:
+    """Permutation test of the difference of two systems' KAD against one baseline X: is score_a - score_b real or
+    noise?  The pool [A; B] (n_a + n_b rows) is relabelled as calc_kad_test relabels [X; Y] (labelling b marks n_a rows
+    as system A), X stays put, and
+
+        D(l) = KAD(X, A_l) - KAD(X, B_l)
+             = 1000 * (2 S_aa / (n_a (n_a - 1)) - 2 S_bb / (n_b (n_b - 1)) - 2 S_XA / (m n_a) + 2 S_XB / (m n_b)),
+        p    = (1 + #{b >= 1 : |D_b| >= |D_0|}) / (B + 1)   (two-sided).
+
+    S_xx cancels, and sigma (from X alone, which is not permuted) is the same for every labelling, so the test is exact.
+    S_XA(l) = sum of g_i over the rows l marks, with g_i = sum_x k(x, z_i) taken once per pool row
+    (fad_kad_eval_sums with one item per row); S_aa and S_bb come from fad_kad_perm_sums, with each kernel value
+    rounded to fp16 once (the precision note of calc_kad_test applies to D_b likewise).  score_a and score_b are
+    bitwise calc_kernel_audio_distance_songs(emb_baseline, [emb_a, emb_b]); the rows go to the GPU once.  emb_baseline
+    may be a PairwiseBaseline (the p-value and nulls are then bitwise the unprepared call's).  Raises ValueError as
+    calc_kad_test does."""
+    permutations, seed = _perm_args(permutations, seed, "a KAD comparison")
+    parts, x_rows, m, (na, nb), prepared = _perm_pool(emb_baseline, [emb_a, emb_b], ["eval A", "eval B"], "KAD")
+    eng, collective = _kad_engine(distributed)
+    dev = eng.torch_device
+    offsets = np.array([0, na, na + nb], dtype=np.int64)
+    if prepared is not None:
+        pool = _kad_device_rows(torch.cat(parts), eng)
+        ra, rb = _kad_prepared(prepared, pool, offsets, distributed)
+        z = torch.cat([prepared.x, pool])
+    else:
+        z = _kad_device_rows(torch.cat([x_rows, *parts]), eng)
+        ra, rb = _kad_songs(z, m, offsets, distributed)
+        pool = z[m:]
+    n = na + nb
+    sig = torch.tensor([ra.bandwidth], dtype=torch.float64, device=dev)
+    one_each = torch.arange(n + 1, dtype=torch.int64, device=dev)
+    g = eng.kad_eval_sums(z, m, one_each, sig, 0 if collective else None)[:, 1].contiguous()
+    s = _perm_sums(eng, collective, pool, na, ra.bandwidth, permutations, seed)
+    s_xa = eng.perm_dot(eng.perm_labels(n, na, permutations, seed), g).cpu().numpy()
+    s_xb = float(np.sum(g.cpu().numpy())) - s_xa
+    diff = 1000.0 * (2.0 * s[:, 0] / (na * (na - 1.0)) - 2.0 * s[:, 1] / (nb * (nb - 1.0))
+                     - 2.0 * s_xa / (float(m) * na) + 2.0 * s_xb / (float(m) * nb))
+    return KADComparisonResults(score_a=ra.score, score_b=rb.score, difference=ra.score - rb.score,
+                                p_value=_perm_p(np.abs(diff[1:]), abs(float(diff[0]))),
+                                null_differences=diff[1:].copy(), bandwidth=ra.bandwidth, permutations=permutations,
+                                seed=seed, n_baseline=m, n_a=na, n_b=nb)
 
 
 def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> PRDCResults:
@@ -977,6 +1136,28 @@ class FrechetAudioDistance:
             x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", distributed), 1, distributed)
         return calc_kernel_audio_distance(x, y, distributed=distributed)
 
+    def score_kad_test(self, baseline_dir: PathLike, eval_dir: PathLike, permutations: int = 999, seed: int = 0,
+                       distributed: bool = False, prepared: bool = False) -> KADTestResults:
+        """Permutation test of KAD (calc_kad_test) between the cached embeddings of two directories, read as score_kad
+        reads them; distributed and prepared as there (prepared: the p-value and nulls are bitwise the unprepared
+        ones, score is score_kad's prepared value)."""
+        permutations, seed = _perm_args(permutations, seed, "a KAD permutation test")
+        x, y = self._cached_sets(baseline_dir, eval_dir, "KAD", distributed)
+        if prepared:
+            x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", distributed), 1, distributed)
+        return calc_kad_test(x, y, permutations, seed, distributed=distributed)
+
+    def score_kad_comparison(self, baseline_dir: PathLike, eval_dir: PathLike, versus_dir: PathLike,
+                             permutations: int = 999, seed: int = 0, distributed: bool = False,
+                             prepared: bool = False) -> KADComparisonResults:
+        """Permutation test of KAD(baseline, eval) - KAD(baseline, versus) (calc_kad_comparison) over the cached
+        embeddings of three directories, read as score_kad reads them; distributed and prepared as for score_kad."""
+        permutations, seed = _perm_args(permutations, seed, "a KAD comparison")
+        x, a, b = self._cached_sets(baseline_dir, eval_dir, "KAD", distributed, versus_dir)
+        if prepared:
+            x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", distributed), 1, distributed)
+        return calc_kad_comparison(x, a, b, permutations, seed, distributed=distributed)
+
     def _cached_offsets(self, baseline_dir: PathLike, metric: str, distributed: bool) -> np.ndarray:
         """the int64 row offsets of the baseline's cache files, from their headers"""
         from . import _io_native
@@ -1000,13 +1181,16 @@ class FrechetAudioDistance:
                                distributed)
         return calc_prdc(x, y, k=k, distributed=distributed)
 
-    def _cached_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, distributed: bool) -> list:
-        """The fp16 embeddings of the two directories that score_kad and score_prdc score, for `metric` (named in the
-        errors).  Collective under distributed=True: rank 0 lists the files, every rank reads them."""
+    def _cached_sets(self, baseline_dir: PathLike, eval_dir: PathLike, metric: str, distributed: bool,
+                     versus_dir: "PathLike | None" = None) -> list:
+        """The fp16 embeddings of the two directories that score_kad and score_prdc score (and of versus_dir, when given,
+        third), for `metric` (named in the errors).  Collective under distributed=True: rank 0 lists the files, every
+        rank reads them."""
         from . import _io_native
         collective = distributed and _kad_engine(True, metric)[1]
         sets = []
-        for what, p in (("baseline", baseline_dir), ("eval", eval_dir)):
+        dirs = (("baseline", baseline_dir), ("eval", eval_dir)) + ((("versus", versus_dir),) if versus_dir is not None else ())
+        for what, p in dirs:
             files = _on_rank0(lambda: _sorted_npy_files(kad_embedding_dir(p, self.ml.name, metric)), collective)
             if not files:
                 raise ValueError(f"no {self.ml.name} embeddings cached under {p}: embed the {what} directory first")

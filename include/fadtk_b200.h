@@ -490,6 +490,29 @@ int fad_realism_prepared(fad_handle* h, const void* z_f16, long long m, long lon
 int fad_realism_prepared_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long m,
                                  long long n, int d, const float* kept_radii_sq, float* realism, int* nearest,
                                  float* nearest_sq, void* stream);
+/* Permutation tests of KAD (DESIGN.md section 5.16).  A pool z of N fp16 rows [N, d] (16-byte aligned, d a multiple of
+ * 8); a labelling marks `a` of them (2 <= a <= N - 2), B = labellings in [1, 9999].  Labelling 0 marks rows 0 .. a - 1;
+ * labelling b >= 1 marks the a rows with the smallest (pair_mix64(pair_mix64(seed + b) ^ i), i) in wrapping uint64
+ * (pair_mix64 = the splitmix64 finaliser, kad.cuh).  Every argument is checked first; a rejected call launches nothing
+ * and writes nothing.
+ *   fad_perm_labels    bits (device uint32 [B + 1][4 ceil(N / 128)], 16-byte aligned): bit i & 31 of word i >> 5 of
+ *                      labelling b is row i's label; 0 past N
+ *   fad_perm_dot       out (device fp64 [B + 1]) = per labelling the sum of v (device fp64 [N]) over the rows it marks,
+ *                      from bits as fad_perm_labels writes them; a fixed order, bitwise reproducible
+ *   fad_kad_perm_sums  out (device fp64 [B + 1][3]) = (S_aa, S_bb, S_ab) of every labelling: the sums of
+ *                      exp(-q / (2 sigma^2)) (sigma: device fp64) over the pairs i < j with both rows marked, neither,
+ *                      and one, each kernel value rounded to fp16 once.  Bitwise reproducible and independent of the grid
+ * fad_kad_perm_sums_sharded splits the tile passes as fad_kad_sums_sharded does, bitwise equal for any number of shards;
+ * collective calls also compare a, B, the seed and the bits of sigma. */
+int fad_perm_labels(fad_handle* h, long long N, long long a, int labellings, unsigned long long seed, uint32_t* bits,
+                    void* stream);
+int fad_perm_dot(fad_handle* h, const uint32_t* bits, long long N, int labellings, const double* v, double* out,
+                 void* stream);
+int fad_kad_perm_sums(fad_handle* h, const void* z_f16, long long N, long long a, int d, const double* sigma,
+                      int labellings, unsigned long long seed, double* out, void* stream);
+int fad_kad_perm_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_shards, const void* z_f16, long long N,
+                              long long a, int d, const double* sigma, int labellings, unsigned long long seed,
+                              double* out, void* stream);
 
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
