@@ -133,6 +133,12 @@ SIGNATURES = {
     "fad_kad_perm_sums": (C.c_int, [c_vp, c_vp, c_ll, c_ll, C.c_int, c_vp, C.c_int, C.c_ulonglong, c_vp, c_vp]),
     "fad_kad_perm_sums_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_ll, C.c_int, c_vp, C.c_int, C.c_ulonglong,
                                             c_vp, c_vp]),
+    "fad_record_len": (c_ll, [C.c_int]),
+    "fad_unit_records": (C.c_int, [c_vp, c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp, c_vp]),
+    "fad_perm_record_sums": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, C.c_int, c_vp, c_vp]),
+    "fad_frechet_records": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, c_vp, C.c_int, c_vp, c_vp]),
+    "fad_frechet_perm": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, C.c_ulonglong,
+                                   C.c_int, c_vp, c_vp, c_vp]),
     "fad_knn_eval_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_knn_eval_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp,
                                                 c_vp]),
@@ -981,6 +987,34 @@ class Engine:
                   int(seed), out.data_ptr(), _stream()))
         return out
 
+    # ------------------------------------- permutation test of the FAD difference (DESIGN.md 5.17)
+    @staticmethod
+    def record_len(d: int) -> int:
+        """R(d) = 1 + d + d (d + 1) / 2: the fp64 values of one unit record (fad_record_len)"""
+        return int(lib().fad_record_len(int(d)))
+
+    def unit_records(self, emb: torch.Tensor, offsets: torch.Tensor, shift: torch.Tensor) -> torch.Tensor:
+        """emb fp16 [N, d], offsets int64 [n_units + 1], shift fp16 [d] (all cuda) -> fp64 [n_units, R(d)] (cuda):
+        per unit [n | sum y | upper triangle of sum y y^T], y = x - shift (fad_unit_records)"""
+        assert emb.dtype == torch.float16 and emb.is_cuda and emb.is_contiguous() and emb.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert shift.dtype == torch.float16 and shift.is_cuda and shift.is_contiguous()
+        n_units, d = offsets.shape[0] - 1, emb.shape[1]
+        out = torch.empty((max(n_units, 0), self.record_len(d)), dtype=torch.float64, device=emb.device)
+        _check(lib().fad_unit_records(self._h, emb.data_ptr(), offsets.data_ptr(), n_units, d, shift.data_ptr(),
+                                      out.data_ptr(), _stream()))
+        return out
+
+    def perm_record_sums(self, records: torch.Tensor, bits: torch.Tensor, d: int) -> torch.Tensor:
+        """records fp64 [n_units, R(d)], bits as perm_labels(n_units, ...) gives them -> fp64 [B + 1, 2, R(d)] (cuda):
+        per labelling the sums of the records of the units it marks and of the others (fad_perm_record_sums)"""
+        assert records.dtype == torch.float64 and records.is_cuda and records.is_contiguous() and records.ndim == 2
+        assert bits.dtype == torch.int32 and bits.is_cuda and bits.is_contiguous() and bits.ndim == 2
+        out = torch.empty((bits.shape[0], 2, records.shape[1]), dtype=torch.float64, device=records.device)
+        _check(lib().fad_perm_record_sums(self._h, records.data_ptr(), records.shape[0], int(d), bits.data_ptr(),
+                                          bits.shape[0] - 1, out.data_ptr(), _stream()))
+        return out
+
     # ------------------------------------------- a prepared baseline (DESIGN.md 5.15)
     # The _sharded forms take local_shards as kad_sums_sharded does; None runs the unsharded entry.
     def pair_digest(self, z: torch.Tensor) -> int:
@@ -1097,6 +1131,30 @@ class Baseline:
         _check(lib().fad_frechet_batched(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
                                          emb.data_ptr(), offsets.data_ptr(), n_items, self.d, 0, out.data_ptr(), _stream()))
         return out
+
+
+    def frechet_records(self, sums: torch.Tensor, shift: torch.Tensor) -> torch.Tensor:
+        """sums fp64 [..., R(d)] (cuda, e.g. perm_record_sums' output), shift fp16 [d] -> fp64 [..., 8]: the FAD of
+        each sum's mean and covariance against this baseline, [7] = its row count (fad_frechet_records)"""
+        assert sums.dtype == torch.float64 and sums.is_cuda and sums.is_contiguous()
+        assert shift.dtype == torch.float16 and shift.is_cuda and shift.is_contiguous()
+        items = sums.numel() // sums.shape[-1]
+        out = torch.empty((*sums.shape[:-1], 8), dtype=torch.float64, device=sums.device)
+        _check(lib().fad_frechet_records(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
+                                         sums.data_ptr(), items, self.d, shift.data_ptr(), 0, out.data_ptr(), _stream()))
+        return out
+
+    def frechet_perm(self, emb: torch.Tensor, offsets: torch.Tensor, a: int, labellings: int, seed: int):
+        """emb fp16 [N, d], offsets int64 [n_units + 1] (cuda; units 0 .. a - 1 are system A's) -> (fp64
+        [B + 1, 2, 8], the fp16 shift [d] used) (cuda): the FAD of both sides of every labelling (fad_frechet_perm)"""
+        assert emb.dtype == torch.float16 and emb.is_cuda and emb.is_contiguous() and emb.shape[1] == self.d
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        out = torch.empty((max(int(labellings), 0) + 1, 2, 8), dtype=torch.float64, device=emb.device)
+        shift = torch.empty(self.d, dtype=torch.float16, device=emb.device)
+        _check(lib().fad_frechet_perm(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
+                                      emb.data_ptr(), offsets.data_ptr(), offsets.shape[0] - 1, int(a), self.d,
+                                      int(labellings), int(seed), 0, shift.data_ptr(), out.data_ptr(), _stream()))
+        return out, shift
 
 
 class PairwiseBaseline:

@@ -11,6 +11,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <memory>
 #include <set>
 #include <string>
@@ -1133,6 +1134,7 @@ extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_
 }  // extern "C"
 
 #include "pairwise_host.inc"
+#include "fad_test_host.inc"
 
 #include "resample_host.inc"
 #include "clap_host.inc"

@@ -525,4 +525,184 @@ __global__ void gather_rows_kernel(const __half* __restrict__ src, const long lo
     }
 }
 
+// --------------------------------------------------------------------------------------
+// Permutation test of the FAD difference between two systems (DESIGN.md 5.17).  A unit is one file: rows
+// [offsets[u], offsets[u + 1]) of one fp16 [N, d] pool, d a multiple of 64.  Its record is
+//   R_u = [n_u | sum y (d) | upper triangle of sum y y^T, row by row (d (d + 1) / 2)],   y = x - s,
+// s the fp16 shift of the pool.  Every product of two fp16 differences is exact in fp64, so a record carries only the
+// fp64 summation rounding of gram_tile.  Records add: the statistics of a union of units are the sum of their records.
+__host__ __device__ constexpr long long record_len(int d) { return 1 + (long long)d + (long long)d * (d + 1) / 2; }
+// packed position of (I, J), I <= J, in the upper triangle
+__device__ __forceinline__ long long record_upper(int d, int I, int J) {
+    return (long long)I * d - (long long)I * (I - 1) / 2 + (J - I);
+}
+
+// records[u] of the units u of this launch (offsets: absolute rows of its first unit onwards).  One CTA = (tile pair
+// ti <= tj, unit) as song_stats_dmma_kernel; the diagonal tiles also write sum y, tile pair 0 writes n.
+// grid (n_pairs, units).
+__global__ void __launch_bounds__(256, 2)
+unit_records_kernel(const __half* __restrict__ emb, const long long* __restrict__ offsets, int d,
+                    const __half* __restrict__ shift, double* __restrict__ records)
+{
+    constexpr int T = kSdTile;
+    __shared__ __align__(16) GramStage Ys;
+    const long long r0 = offsets[blockIdx.y], r1 = offsets[blockIdx.y + 1];
+    int ti, tj;
+    pair_to_tiles(blockIdx.x, d / T, ti, tj);
+    double* rec = records + (size_t)blockIdx.y * record_len(d);
+    double c[4][2][2] = {}, cs_i[4] = {0.0, 0.0, 0.0, 0.0}, cs_j[4] = {0.0, 0.0, 0.0, 0.0};
+    gram_tile(Ys, emb, d, r0, r1, ti, tj, shift, c, cs_i, cs_j);
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+    const int fr = lane >> 2, fk = lane & 3;
+    double* upper = rec + 1 + d;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int I = ti * T + wm + i * 8 + fr, J = tj * T + wn + j * 8 + 2 * fk + e;
+                if (I <= J) upper[record_upper(d, I, J)] = c[i][j][e];
+            }
+    if (ti == tj) {
+        const double v = gram_colsums(Ys, cs_i, cs_j, 1);
+        if (t < T) rec[1 + ti * T + t] = v;
+    }
+    if (blockIdx.x == 0 && t == 0) rec[0] = (double)(r1 - r0);
+}
+
+// Labelled record sums: for every labelling b of the launch and both sides,
+//   sums[b][0] += sum_u l_b(u) R_u,   sums[b][1] += sum_u (1 - l_b(u)) R_u
+// as a GEMM on the FP64 tensor pipe (mma.sync m8n8k4 f64): M = labellings, N = record columns, K = units.  The labels
+// of a k-step are expanded from the bits (fad_perm_labels' layout) to fp64 0 / 1 in registers, the A operand of both
+// sides; the B operand (16 units x 64 columns of records) is staged in shared memory as in dgemm_tile.  Each
+// accumulator element runs the units in order, four per DMMA, from zero or from the value a previous launch stored:
+// when every launch but the last covers a multiple of 4 units (the host uses multiples of 64), the result is bitwise
+// the same however the units are cut into launches and the labellings into passes.  No atomics.
+constexpr int kRsTile = 64, kRsUnits = 16, kRsPitch = kRsTile + 4;
+constexpr int kRsUnitAlign = 64;                  // unit0 of every launch is a multiple of this
+
+struct RecordSumsParams {
+    const double* records;       // [units][R]: the launch's units
+    long long R;
+    int units, unit0;            // units of this launch; the first one's index in the pool (label bit position)
+    const uint32_t* bits;        // labelling 0 of this launch
+    int words;                   // words per labelling
+    int rows;                    // labellings of this launch: rows past it are not read nor written
+    int accumulate;              // 0: start from zero, 1: add to sums
+    double* sums;                // [rows][2][R]
+};
+
+__global__ void __launch_bounds__(256, 1)
+record_sums_kernel(const RecordSumsParams p)
+{
+    __shared__ __align__(16) double Rs[2][kRsUnits][kRsPitch];
+    const int m0 = blockIdx.x * kRsTile;
+    const long long n0 = (long long)blockIdx.y * kRsTile;
+    const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+    const int wm = (warp >> 2) * 32, wn = (warp & 3) * 16;
+    const int fr = lane >> 2, fk = lane & 3;
+    const int lu = t >> 4, lc = (t & 15) * 4;                   // loader: unit of the stage, first of 4 columns
+    const long long R = p.R;
+
+    double ca[4][2][2], cb[4][2][2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int m = m0 + wm + i * 8 + fr;
+                const long long n = n0 + wn + j * 8 + 2 * fk + e;
+                const bool in = p.accumulate && m < p.rows && n < R;
+                ca[i][j][e] = in ? p.sums[((size_t)m * 2) * R + n] : 0.0;
+                cb[i][j][e] = in ? p.sums[((size_t)m * 2 + 1) * R + n] : 0.0;
+            }
+    const int mrow = m0 + wm + fr;                               // this thread's labelling rows: mrow + 8 i
+    const uint32_t* lb = p.bits + (size_t)mrow * p.words;
+
+    double rv[4];
+    auto fetch = [&](int st) {
+        const int u = st * kRsUnits + lu;
+        const double* src = p.records + (size_t)u * R + n0 + lc;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) rv[e] = (u < p.units && n0 + lc + e < R) ? __ldg(src + e) : 0.0;
+    };
+    auto stage = [&](int buf) {
+        *reinterpret_cast<double2*>(&Rs[buf][lu][lc]) = make_double2(rv[0], rv[1]);
+        *reinterpret_cast<double2*>(&Rs[buf][lu][lc + 2]) = make_double2(rv[2], rv[3]);
+    };
+    const int stages = (p.units + kRsUnits - 1) / kRsUnits;
+    fetch(0);
+    stage(0);
+    __syncthreads();
+    for (int st = 0; st < stages; ++st) {
+        const int buf = st & 1;
+        if (st + 1 < stages) fetch(st + 1);
+        const int ug = p.unit0 + st * kRsUnits;                  // a multiple of 16: the stage sits in one word
+        uint32_t w[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            w[i] = mrow + 8 * i < p.rows ? __ldg(lb + (size_t)8 * i * p.words + (ug >> 5)) >> (ug & 31) : 0u;
+#pragma unroll
+        for (int kk = 0; kk < kRsUnits; kk += 4) {
+            const bool valid = st * kRsUnits + kk + fk < p.units;
+            double b[2];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) b[j] = Rs[buf][kk + fk][wn + j * 8 + fr];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const uint32_t bit = (w[i] >> (kk + fk)) & 1u;
+                const double a = valid && bit ? 1.0 : 0.0, ac = valid && !bit ? 1.0 : 0.0;
+#pragma unroll
+                for (int j = 0; j < 2; ++j) {
+                    sm90::dmma_884(ca[i][j][0], ca[i][j][1], a, b[j]);
+                    sm90::dmma_884(cb[i][j][0], cb[i][j][1], ac, b[j]);
+                }
+            }
+        }
+        if (st + 1 < stages) stage(buf ^ 1);
+        __syncthreads();
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int m = m0 + wm + i * 8 + fr;
+                const long long n = n0 + wn + j * 8 + 2 * fk + e;
+                if (m < p.rows && n < R) {
+                    p.sums[((size_t)m * 2) * R + n] = ca[i][j][e];
+                    p.sums[((size_t)m * 2 + 1) * R + n] = cb[i][j][e];
+                }
+            }
+}
+
+// Item z of a Frechet group from its labelled sum S = sums + z R: mu = s + sum y / n (fp64), the symmetric
+// C = (sum y y^T - sum y sum y^T / n) / (n - 1), ok[z], and n into out[z][7].  An item with n < 2 gets the identity
+// and ok = 0 as in song_stats_kernel (the assembly writes NaN).  grid (blocks, items).
+__global__ void __launch_bounds__(256)
+record_finalize_kernel(const double* __restrict__ sums, int d, const __half* __restrict__ shift,
+                       double* __restrict__ mu, double* __restrict__ cov, int* __restrict__ ok, double* __restrict__ out)
+{
+    const int z = blockIdx.y;
+    const double* S = sums + (size_t)z * record_len(d);
+    const double n = S[0];
+    const double* sy = S + 1;
+    const double* upper = S + 1 + d;
+    const bool good = n >= 2.0;
+    double* C = cov + (size_t)z * d * d;
+    for (size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x; e < (size_t)d * d; e += (size_t)gridDim.x * blockDim.x) {
+        const int i = (int)(e / d), j = (int)(e % d);
+        C[e] = good ? (upper[record_upper(d, min(i, j), max(i, j))] - sy[i] * sy[j] / n) / (n - 1.0) : (i == j ? 1.0 : 0.0);
+        if (j == 0) mu[(size_t)z * d + i] = good ? (double)__half2float(shift[i]) + sy[i] / n : 0.0;
+    }
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        ok[z] = good ? 1 : 0;
+        out[(size_t)z * 8 + 7] = n;
+    }
+}
+
 }  // namespace fad

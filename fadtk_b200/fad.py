@@ -12,6 +12,8 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
     prepare_pairwise_baseline                              -> the baseline-only work of the four above, done once
     calc_kad_test, calc_kad_comparison                     -> permutation p-values of KAD: every labelling in one
                                                               label-product tile pass (csrc/kad.cuh)
+    calc_fad_comparison                                    -> permutation p-value of a FAD difference: file records,
+                                                              labelled fp64 sums and batched Frechet chains (stats.cuh)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -114,6 +116,21 @@ class KADComparisonResults(NamedTuple):
     n_baseline: int
     n_a: int
     n_b: int
+
+
+class FADComparisonResults(NamedTuple):
+    score_a: float                  # calc_frechet_distance(mu, cov, *calc_embd_statistics(all rows of A)), bitwise
+    score_b: float
+    difference: float               # score_a - score_b
+    observed: float                 # the difference of the observed labelling on the labelled path
+    p_value: float
+    null_differences: np.ndarray    # float64 [permutations]
+    permutations: int
+    seed: int
+    n_units_a: int
+    n_units_b: int
+    n_rows_a: int
+    n_rows_b: int
 
 
 class PRDCResults(NamedTuple):
@@ -425,6 +442,89 @@ def calc_kad_comparison(emb_baseline, emb_a, emb_b, permutations: int = 999, see
                                 p_value=_perm_p(np.abs(diff[1:]), abs(float(diff[0]))),
                                 null_differences=diff[1:].copy(), bandwidth=ra.bandwidth, permutations=permutations,
                                 seed=seed, n_baseline=m, n_a=na, n_b=nb)
+
+
+def _fad_units(emb, what: str, d: int) -> list:
+    """a list of fp16 [rows, d] arrays (files) or one 2-D fp16 array (one unit per row) -> the list of units"""
+    if isinstance(emb, (list, tuple)):
+        units = [np.asarray(u) for u in emb]
+    else:
+        arr = np.asarray(emb)
+        if arr.ndim != 2:
+            raise ValueError(f"{what} must be a list of 2-D arrays (files) or one 2-D array (rows); got shape {arr.shape}")
+        units = [arr[i:i + 1] for i in range(arr.shape[0])]
+    for u in units:
+        if u.ndim != 2 or u.shape[1] != d:
+            raise ValueError(f"every {what} array must be [rows, {d}] (the baseline's width); got shape {u.shape}")
+        if u.dtype != np.float16:
+            raise ValueError(f"the FAD comparison needs fp16 embeddings; {what} holds {u.dtype}")
+        if u.shape[0] == 0:
+            raise ValueError(f"every {what} file needs at least one row")
+    if len(units) < 2:
+        raise ValueError(f"the FAD comparison needs at least two units (files) in {what}; got {len(units)}")
+    return units
+
+
+def calc_fad_comparison(baseline, eval_a, eval_b, permutations: int = 999, seed: int = 0) -> FADComparisonResults:
+    """Permutation test of the difference of two systems' FAD against one baseline: is score_a - score_b real or
+    noise?  baseline = (mu, cov) (the statistics load_stats returns, fp64 or fp16 mu).  eval_a, eval_b: a list of fp16
+    [rows, d] arrays, one per file, or one 2-D fp16 array.  The unit of the test is a file: the pool is the files of A
+    followed by those of B, and labelling b marks n_units_a of them (labelling 0: A's own files; b >= 1: the units with
+    the smallest (pair_mix64(pair_mix64(seed + b) ^ i), i), DESIGN.md 5.17).  Rows of one file are correlated, so
+    files and not rows are exchanged; a single 2-D array is one unit per row, which assumes independent rows.
+
+        D(l) = FAD(X, A_l) - FAD(X, B_l),      p = (1 + #{b >= 1 : |D_b| >= |D_0|}) / (B + 1)   (two-sided),
+
+    A_l (B_l) the union of the rows of the units l marks (does not mark), each with its exact fp64 mean and ddof = 1
+    covariance.  The baseline is never permuted, so the test is exact when A's and B's files are exchangeable.
+
+    score_a and score_b are calc_frechet_distance(mu, cov, *calc_embd_statistics(rows)) of all rows of each system,
+    the values FAD users see.  `observed` is D_0 on the labelled path, which the nulls are compared with; it can differ
+    from score_a - score_b by about 1e-4 relative, because calc_embd_statistics rounds the mean to fp16 (as the
+    reference does) and the labelled statistics keep the exact mean.
+
+    Raises ValueError for a baseline that is not (mu [d], cov [d, d]) with d a multiple of 64, arrays that are not fp16
+    [rows, d], an empty file, fewer than two units on a side, permutations outside [1, 9999] or a seed outside
+    [0, 2**64), before any GPU work."""
+    permutations, seed = _perm_args(permutations, seed, "a FAD comparison")
+    try:
+        mu, cov = baseline
+    except (TypeError, ValueError):
+        raise ValueError("the FAD comparison needs the baseline as (mu, cov)") from None
+    mu, cov = np.asarray(mu), np.asarray(cov)
+    d = int(mu.shape[0]) if mu.ndim == 1 else -1
+    if d <= 0 or cov.shape != (d, d):
+        raise ValueError(f"the baseline must be (mu [d], cov [d, d]); got shapes {mu.shape} and {cov.shape}")
+    if d % 64 != 0 or d > 2048:
+        raise ValueError(f"the FAD comparison needs an embedding width that is a multiple of 64 up to 2048; got {d}")
+    units_a, units_b = _fad_units(eval_a, "eval A", d), _fad_units(eval_b, "eval B", d)
+    return _fad_comparison(mu, cov, units_a, units_b, None, None, permutations, seed)
+
+
+def _fad_comparison(mu, cov, units_a: list, units_b: list, score_a, score_b, permutations: int,
+                    seed: int) -> FADComparisonResults:
+    """calc_fad_comparison on checked units; score_a / score_b None: the array scores"""
+    from . import _native
+    rows_a, rows_b = np.concatenate(units_a), np.concatenate(units_b)
+    if score_a is None:
+        score_a = float(calc_frechet_distance(mu, cov, *calc_embd_statistics(rows_a)))
+        score_b = float(calc_frechet_distance(mu, cov, *calc_embd_statistics(rows_b)))
+    eng = _native.engine()
+    dev = eng.torch_device
+    base = _native.Baseline(eng, mu, cov)
+    sizes = [u.shape[0] for u in units_a + units_b]
+    offsets = torch.from_numpy(np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)).to(dev)
+    pool = torch.from_numpy(np.concatenate([rows_a, rows_b])).to(dev)
+    out, _ = base.frechet_perm(pool, offsets, len(units_a), permutations, seed)
+    fad = out[:, :, 0].cpu().numpy()
+    if not np.isfinite(fad).all():
+        raise ValueError("non-finite covariance statistics (NaN/Inf input)")
+    diff = fad[:, 0] - fad[:, 1]
+    return FADComparisonResults(score_a=score_a, score_b=score_b, difference=score_a - score_b,
+                                observed=float(diff[0]), p_value=_perm_p(np.abs(diff[1:]), abs(float(diff[0]))),
+                                null_differences=diff[1:].copy(), permutations=permutations, seed=seed,
+                                n_units_a=len(units_a), n_units_b=len(units_b), n_rows_a=int(rows_a.shape[0]),
+                                n_rows_b=int(rows_b.shape[0]))
 
 
 def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> PRDCResults:
@@ -1157,6 +1257,23 @@ class FrechetAudioDistance:
         if prepared:
             x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", distributed), 1, distributed)
         return calc_kad_comparison(x, a, b, permutations, seed, distributed=distributed)
+
+    def score_fad_comparison(self, baseline: PathLike, eval_dir: PathLike, versus_dir: PathLike,
+                             permutations: int = 999, seed: int = 0) -> FADComparisonResults:
+        """Permutation test of score(baseline, eval_dir) - score(baseline, versus_dir) (calc_fad_comparison).  baseline
+        is anything load_stats takes (a directory, an .npz file or a named set); the units are the sorted cache files
+        <dir>/embeddings/<model>/*.npy that each eval directory's statistics read, empty files dropped.  score_a and
+        score_b are self.score's values, so a directory score refuses fails here the same way."""
+        permutations, seed = _perm_args(permutations, seed, "a FAD comparison")
+        score_a = float(self.score(baseline, eval_dir))
+        score_b = float(self.score(baseline, versus_dir))
+        mu, cov = self.load_stats(baseline)
+        d = int(np.asarray(mu).shape[0])
+        units = []
+        for p, what in ((eval_dir, "eval A"), (versus_dir, "eval B")):
+            arrs = [np.load(f) for f in _sorted_npy_files(Path(p) / "embeddings" / self.ml.name)]
+            units.append(_fad_units([a for a in arrs if a.shape[0] > 0], what, d))
+        return _fad_comparison(mu, cov, units[0], units[1], score_a, score_b, permutations, seed)
 
     def _cached_offsets(self, baseline_dir: PathLike, metric: str, distributed: bool) -> np.ndarray:
         """the int64 row offsets of the baseline's cache files, from their headers"""

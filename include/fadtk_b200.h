@@ -514,6 +514,35 @@ int fad_kad_perm_sums_sharded(fad_handle* h, void* nccl_comm_or_null, int local_
                               long long a, int d, const double* sigma, int labellings, unsigned long long seed,
                               double* out, void* stream);
 
+/* ---- Permutation test of the FAD difference between two systems (DESIGN.md section 5.17).  A pool of n_units units
+ * (files: rows [offsets[u], offsets[u + 1]) of emb_f16 [N, d], no empty unit), the first a of them system A's.  d a
+ * positive multiple of 64 (at most 2048), 16-byte-aligned device pointers.  Labelling 0 marks units 0 .. a - 1;
+ * labelling b >= 1 marks the a units fad_perm_labels marks (its rule over units).  Every argument is checked first
+ * (offsets are read back, one stream synchronisation); a rejected call launches nothing and writes nothing.
+ *   fad_record_len       R(d) = 1 + d + d (d + 1) / 2 (host only)
+ *   fad_unit_records     records (device fp64 [n_units][R(d)]) = per unit [n_u | sum y | upper triangle of sum y y^T,
+ *                        row by row], y = x - shift (shift_f16: device fp16 [d]); exact products, fp64 sums
+ *   fad_perm_record_sums sums (device fp64 [B + 1][2][R(d)]) = per labelling the sum of the records of the units it
+ *                        marks ([b][0]) and of those it does not ([b][1]); bits as fad_perm_labels writes them for
+ *                        n_units rows.  Fixed order, bitwise reproducible
+ *   fad_frechet_records  out (device fp64 [items][8], fad_frechet's layout, [7] = n) = the FAD against the baseline
+ *                        (mu1, sqrt1 = C1^(1/2), scal1 = {|C1|_F, tr C1}) of the statistics of each of `items` sums:
+ *                        mu = shift + sum y / n, C = (sum y y^T - sum y sum y^T / n) / (n - 1); NaN below 2 rows
+ *   fad_frechet_perm     out (device fp64 [B + 1][2][8]) = the two FADs of every labelling: the whole pass above with
+ *                        the fp16 mean of the pool as shift (written to shift_out, device fp16 [d]), B = labellings in
+ *                        [1, 9999], 2 <= a <= n_units - 2.  Bitwise equal to replaying the three stage entries over
+ *                        all units with shift_out */
+long long fad_record_len(int d);
+int fad_unit_records(fad_handle* h, const void* emb_f16, const long long* offsets, long long n_units, int d,
+                     const void* shift_f16, double* records, void* stream);
+int fad_perm_record_sums(fad_handle* h, const double* records, long long n_units, int d, const uint32_t* bits,
+                         int labellings, double* sums, void* stream);
+int fad_frechet_records(fad_handle* h, const double* mu1, const double* sqrt1, const double* scal1, const double* sums,
+                        long long items, int d, const void* shift_f16, int iters, double* out, void* stream);
+int fad_frechet_perm(fad_handle* h, const double* mu1, const double* sqrt1, const double* scal1, const void* emb_f16,
+                     const long long* offsets, long long n_units, long long a, int d, int labellings,
+                     unsigned long long seed, int iters, void* shift_out, double* out, void* stream);
+
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
  * sinc_interp_kaiser, beta=14.769656459379492) (:151-158), PCM16 quantisation (:160).
