@@ -9,6 +9,7 @@ from .fad import FADInfResults, FrechetAudioDistance, calc_embd_statistics, calc
 from .fad import KADResults, calc_kernel_audio_distance, calc_kernel_audio_distance_songs  # noqa: F401
 from .fad import KADComparisonResults, KADTestResults, calc_kad_comparison, calc_kad_test  # noqa: F401
 from .fad import FADComparisonResults, calc_fad_comparison  # noqa: F401
+from .fad import FADBootstrapResults, KADBootstrapResults, calc_fad_bootstrap, calc_kad_bootstrap  # noqa: F401
 from .fad import PRDCResults, calc_prdc, calc_prdc_songs  # noqa: F401
 from .fad import RealismResults, calc_realism  # noqa: F401
 from .fad import NearestResults, calc_nearest  # noqa: F401

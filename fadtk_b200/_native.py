@@ -139,6 +139,11 @@ SIGNATURES = {
     "fad_frechet_records": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, c_vp, C.c_int, c_vp, c_vp]),
     "fad_frechet_perm": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, c_ll, C.c_int, C.c_int, C.c_ulonglong,
                                    C.c_int, c_vp, c_vp, c_vp]),
+    "fad_boot_counts": (C.c_int, [c_vp, c_ll, C.c_int, C.c_ulonglong, c_vp, c_vp]),
+    "fad_boot_record_sums": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, C.c_int, c_vp, c_vp]),
+    "fad_frechet_boot": (C.c_int, [c_vp, c_vp, c_vp, c_vp, c_vp, c_vp, c_ll, C.c_int, C.c_int, C.c_ulonglong, C.c_int,
+                                   c_vp, c_vp, c_vp]),
+    "fad_kad_boot_sums": (C.c_int, [c_vp, c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp, C.c_int, C.c_ulonglong, c_vp, c_vp]),
     "fad_knn_eval_radii_sq": (C.c_int, [c_vp, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
     "fad_knn_eval_radii_sq_sharded": (C.c_int, [c_vp, c_vp, C.c_int, c_vp, c_ll, c_vp, c_ll, C.c_int, C.c_int, c_vp,
                                                 c_vp]),
@@ -1015,6 +1020,41 @@ class Engine:
                                           bits.shape[0] - 1, out.data_ptr(), _stream()))
         return out
 
+    # ------------------------------------------- bootstrap confidence intervals (DESIGN.md 5.18)
+    # n_units units resampled B = resamples times; resample 0 is the observed set (include/fadtk_b200.h).
+    def boot_counts(self, n_units: int, resamples: int, seed: int) -> torch.Tensor:
+        """-> int32 [B + 1, n_units] (cuda; the uint32 multiplicities): how often resample b draws unit u
+        (fad_boot_counts)"""
+        out = torch.empty((max(int(resamples), 0) + 1, max(int(n_units), 1)), dtype=torch.int32, device=self.torch_device)
+        _check(lib().fad_boot_counts(self._h, int(n_units), int(resamples), int(seed), out.data_ptr(), _stream()))
+        return out
+
+    def boot_record_sums(self, records: torch.Tensor, counts: torch.Tensor, d: int) -> torch.Tensor:
+        """records fp64 [n_units, R(d)], counts as boot_counts(n_units, ...) gives them -> fp64 [B + 1, R(d)] (cuda): per
+        resample the multiplicity-weighted sum of the records (fad_boot_record_sums)"""
+        assert records.dtype == torch.float64 and records.is_cuda and records.is_contiguous() and records.ndim == 2
+        assert counts.dtype == torch.int32 and counts.is_cuda and counts.is_contiguous() and counts.ndim == 2
+        assert counts.shape[1] == records.shape[0]
+        out = torch.empty((counts.shape[0], records.shape[1]), dtype=torch.float64, device=records.device)
+        _check(lib().fad_boot_record_sums(self._h, records.data_ptr(), records.shape[0], int(d), counts.data_ptr(),
+                                          counts.shape[0] - 1, out.data_ptr(), _stream()))
+        return out
+
+    def kad_boot_sums(self, y: torch.Tensor, offsets: torch.Tensor, sigma: torch.Tensor, g_units: torch.Tensor,
+                      resamples: int, seed: int) -> torch.Tensor:
+        """y fp16 [n, d] (cuda, the eval rows, d a multiple of 8), offsets int64 [n_units + 1], sigma fp64 scalar,
+        g_units fp64 [n_units] (cuda) -> fp64 [B + 1, 3] (cuda): (n_b, S_yy(b), S_xy(b)) of every resample
+        (fad_kad_boot_sums)"""
+        assert y.dtype == torch.float16 and y.is_cuda and y.is_contiguous() and y.ndim == 2
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        assert sigma.dtype == torch.float64 and sigma.is_cuda and sigma.numel() == 1
+        assert g_units.dtype == torch.float64 and g_units.is_cuda and g_units.is_contiguous()
+        out = torch.empty((max(int(resamples), 0) + 1, 3), dtype=torch.float64, device=y.device)
+        _check(lib().fad_kad_boot_sums(self._h, y.data_ptr(), offsets.data_ptr(), offsets.shape[0] - 1, y.shape[1],
+                                       sigma.data_ptr(), g_units.data_ptr(), int(resamples), int(seed), out.data_ptr(),
+                                       _stream()))
+        return out
+
     # ------------------------------------------- a prepared baseline (DESIGN.md 5.15)
     # The _sharded forms take local_shards as kad_sums_sharded does; None runs the unsharded entry.
     def pair_digest(self, z: torch.Tensor) -> int:
@@ -1154,6 +1194,18 @@ class Baseline:
         _check(lib().fad_frechet_perm(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
                                       emb.data_ptr(), offsets.data_ptr(), offsets.shape[0] - 1, int(a), self.d,
                                       int(labellings), int(seed), 0, shift.data_ptr(), out.data_ptr(), _stream()))
+        return out, shift
+
+    def frechet_boot(self, emb: torch.Tensor, offsets: torch.Tensor, resamples: int, seed: int):
+        """emb fp16 [N, d], offsets int64 [n_units + 1] (cuda) -> (fp64 [B + 1, 8], the fp16 shift [d] used) (cuda): the
+        FAD of every bootstrap resample of the units, resample 0 the observed set (fad_frechet_boot)"""
+        assert emb.dtype == torch.float16 and emb.is_cuda and emb.is_contiguous() and emb.shape[1] == self.d
+        assert offsets.dtype == torch.int64 and offsets.is_cuda and offsets.is_contiguous() and offsets.ndim == 1
+        out = torch.empty((max(int(resamples), 0) + 1, 8), dtype=torch.float64, device=emb.device)
+        shift = torch.empty(self.d, dtype=torch.float16, device=emb.device)
+        _check(lib().fad_frechet_boot(self.eng._h, self.mu.data_ptr(), self.sqrt.data_ptr(), self.scal.data_ptr(),
+                                      emb.data_ptr(), offsets.data_ptr(), offsets.shape[0] - 1, self.d, int(resamples),
+                                      int(seed), 0, shift.data_ptr(), out.data_ptr(), _stream()))
         return out, shift
 
 

@@ -569,7 +569,8 @@ int fad_create(int device, int max_examples, fad_handle** out) {
     CK(smem((const void*)fad::kad_tile_kernel<0>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<1>, fad::kKadSmemBytes));
     CK(smem((const void*)fad::kad_tile_kernel<2>, fad::kKadSmemBytes));
-    CK(smem((const void*)fad::kad_perm_tile_kernel, fad::kPermSmemBytes));
+    CK(smem((const void*)fad::kad_perm_tile_kernel<false>, fad::kPermSmemBytes));
+    CK(smem((const void*)fad::kad_perm_tile_kernel<true>, fad::kPermSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<0>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<1>, fad::kPairSmemBytes));
     CK(smem((const void*)fad::prdc_tile_kernel<2>, fad::kPairSmemBytes));
@@ -1135,6 +1136,7 @@ extern "C" int fad_bench_dmma_peak(fad_handle* h, int iters, double* tflops_out_
 
 #include "pairwise_host.inc"
 #include "fad_test_host.inc"
+#include "bootstrap_host.inc"
 
 #include "resample_host.inc"
 #include "clap_host.inc"

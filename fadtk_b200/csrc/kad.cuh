@@ -361,6 +361,11 @@ __global__ void kad_select_kernel(KadSelectState* st, const unsigned long long* 
 // Label bits: labelling b is words [b * words, (b + 1) * words), words = 4 ceil(N / 128); bit i & 31 of word i >> 5 is
 // row i's label, 0 past N.  Labelling 0 marks rows 0 .. a - 1; labelling b >= 1 marks the a rows with the smallest
 // (pair_mix64(pair_mix64(seed + b) ^ i), i); labellings past the last are all zero.
+//
+// kBoot (the bootstrap, DESIGN.md 5.18): Q(v) = sum_{i<j} v_i v_j K_ij for row weights v (resamples in place of
+// labellings, the fp16 integer weights [rows][T * 128] in place of the bits; exact up to 2048).  The A operand is the
+// column tile's weights, the reduction over i multiplies by v_i, the shrink is undone counting the nonzero-weight
+// columns, and C and R are not formed (C's partial slots are written as 0).
 constexpr int kPermBlock = 64;                     // labellings per wgmma (its M)
 constexpr int kPermPass = 1024;                    // labellings per tile pass
 constexpr int kPermLabelThreads = 1024;
@@ -380,6 +385,7 @@ struct KadPermParams {
     int blocks;               // blocks of 64 labellings in this pass (1 .. 16)
     double* partial;          // [units][2 consumers][64 blocks][2]: P, C of each labelling
     double* rowsum;           // [T * 128] R_i
+    const __half* weights;    // kBoot: this pass's first resample's row weights [rows][T * 128] (bits, rowsum unused)
 };
 
 // bits b0, b1 (bits 0, 1 of x) -> the fp16 pair (b0, b1) as 0 / 1
@@ -387,6 +393,76 @@ __device__ __forceinline__ uint32_t perm_half2(uint32_t x) {
     return ((x & 1u) | ((x & 2u) << 15)) * 0x3C00u;
 }
 
+// kBoot's label product of one column tile ct of tile row r: per block of 64 resamples, U = V_J K_IJ^T as the 8
+// wgmmas of the labellings with the weights of J as the A operand, then P = sum_i v_i U_i over the rows of I, added to
+// acc[block] with the shrink of the columns of J whose weight is nonzero undone.  The weight rows are advanced through
+// an empty asm as the bits are.
+__device__ __forceinline__ void boot_label_product(double (&acc)[kPermPass / kPermBlock], const KadPermParams& p,
+                                                   uint32_t kbase, int lr0, int q, int c, int r, int ct) {
+    using namespace sm90;
+    const size_t stride = (size_t)p.T * 64;                     // words (fp16 pairs) per resample row
+    const uint32_t* wl = reinterpret_cast<const uint32_t*>(p.weights) + (size_t)lr0 * stride;
+    const size_t row8 = 8 * stride, block = (size_t)kPermBlock * stride;
+#pragma unroll
+    for (int lb = 0; lb < kPermPass / kPermBlock; ++lb) {
+        if (lb < p.blocks) {
+            // A fragment of k-step kk: a[0] = resample row lr0, columns 16 kk + 2 q + {0, 1}; a[1] = row lr0 + 8;
+            // a[2], a[3] = columns + 8
+            const uint32_t* wj = wl + ct * 64 + q;
+            uint32_t a[8][4];
+            int nz[2] = {0, 0};
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk) {
+                a[kk][0] = __ldg(wj + 8 * kk);
+                a[kk][1] = __ldg(wj + row8 + 8 * kk);
+                a[kk][2] = __ldg(wj + 8 * kk + 4);
+                a[kk][3] = __ldg(wj + row8 + 8 * kk + 4);
+#pragma unroll
+                for (int e = 0; e < 4; ++e)
+                    nz[e & 1] += ((a[kk][e] & 0xFFFFu) != 0u) + ((a[kk][e] >> 16) != 0u);
+            }
+            float dl[32];
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < 8; ++kk)
+                wgmma_m64n64k16_f16_rs_kmajor(dl, a[kk], kmajor_sw128_desc(kbase + (kk >> 2) * (kPermKBytes / 2)) + 2 * (kk & 3),
+                                              kk > 0);
+            wgmma_commit();
+            wgmma_wait<0>();
+            fence_regs(dl);
+            // element (resample row lr0 + 8 rr, row 64 c + 8 jj + 2 q + e of I) is dl[4 jj + 2 rr + e]; its weight is
+            // half e of word r * 64 + 32 c + 4 jj + q of the resample row
+            const uint32_t* wi = wl + r * 64 + 32 * c + q;
+            float pp[2] = {0.f, 0.f};
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    const uint32_t w = __ldg(wi + (rr ? row8 : 0) + 4 * jj);
+                    pp[rr] = fmaf(dl[4 * jj + 2 * rr], __half2float(__ushort_as_half((unsigned short)(w & 0xFFFFu))), pp[rr]);
+                    pp[rr] = fmaf(dl[4 * jj + 2 * rr + 1], __half2float(__ushort_as_half((unsigned short)(w >> 16))), pp[rr]);
+                }
+            }
+#pragma unroll
+            for (int o = 1; o < 4; o <<= 1) {
+#pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+                    pp[rr] += __shfl_xor_sync(0xffffffffu, pp[rr], o);
+                    nz[rr] += __shfl_xor_sync(0xffffffffu, nz[rr], o);
+                }
+            }
+            // lane q keeps P of resample row lr0 + 8 (q >> 1) (q even; odd lanes add 0 to C's slot); the shrink is undone
+            // as in the labelled pass, counting the columns of J with a nonzero weight
+            const float mine = q == 0 ? pp[0] : q == 2 ? pp[1] : 0.f;
+            const int marked = q < 2 ? nz[0] : nz[1];
+            acc[lb] += (double)fmaf(mine, kAccumShrinkPerElement * (float)marked, mine);
+            wl += block;
+            asm volatile("" : "+l"(wl));
+        }
+    }
+}
+
+template <bool kBoot>
 __global__ void __launch_bounds__(kPairThreads, 1)
 kad_perm_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
                      const KadPermParams p) {
@@ -456,7 +532,7 @@ kad_perm_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_co
                             float kv;
                             asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(kv) : "f"(qd * neg_coef));
                             kh[e] = __float2half_rn(gj > gi && gj < p.N ? kv : 0.f);
-                            rt[i] += __half2float(kh[e]);
+                            if constexpr (!kBoot) rt[i] += __half2float(kh[e]);
                         }
                         const int lr = lr0 + 8 * i;
                         const uint32_t addr = kbase + (j >> 3) * (kPermKBytes / 2) + lr * 128 + (((j & 7) ^ (lr & 7)) << 4) + 4 * q;
@@ -464,14 +540,21 @@ kad_perm_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_co
                         asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
                     }
                 }
-                rs[0] += (double)rt[0];
-                rs[1] += (double)rt[1];
+                if constexpr (!kBoot) {
+                    rs[0] += (double)rt[0];
+                    rs[1] += (double)rt[1];
+                }
                 fence_proxy_async_smem();
                 named_bar_sync(2 + c, 128);
 
                 // ---- per block of 64 labellings: U = W_J K^T, then P and C over the rows of I.  bl = labelling row lr0
                 // of the block, advanced through an empty asm so that the compiler keeps one pointer live instead of
                 // hoisting (and spilling) one per block
+                if constexpr (kBoot) {
+                    boot_label_product(acc, p, kbase, lr0, q, c, r, ct);
+                    named_bar_sync(2 + c, 128);
+                    continue;
+                }
                 const uint32_t* bl = p.bits + (size_t)lr0 * p.words;
                 const size_t row8 = 8 * (size_t)p.words, block = (size_t)kPermBlock * p.words;
 #pragma unroll
@@ -544,10 +627,12 @@ kad_perm_tile_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_co
                 named_bar_sync(2 + c, 128);
             }
             // R of rows row0, row0 + 8: the quad's 4 lanes by a fixed xor tree
+            if constexpr (!kBoot) {
 #pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                for (int o = 1; o < 4; o <<= 1) rs[i] += __shfl_xor_sync(0xffffffffu, rs[i], o);
-                if (q == 0) p.rowsum[row0 + 8 * i] = rs[i];
+                for (int i = 0; i < 2; ++i) {
+                    for (int o = 1; o < 4; o <<= 1) rs[i] += __shfl_xor_sync(0xffffffffu, rs[i], o);
+                    if (q == 0) p.rowsum[row0 + 8 * i] = rs[i];
+                }
             }
         }
         double* part = p.partial + ((size_t)u * 2 + c) * p.blocks * kPermBlock * 2;
@@ -669,6 +754,75 @@ __global__ void kad_perm_reduce_kernel(const double* __restrict__ partial, int u
     double s = 0.0;
     for (int u = 0; u < 2 * units; ++u) s += partial[(size_t)u * 2 * n + t];
     pc[t] = s;
+}
+
+// ------------------------------------------------------------------------ bootstrap (DESIGN.md 5.18)
+// Resample b of F units: draw t = 0 .. F - 1 picks unit floor(key_b(t) F / 2^64) (the high word of the 128-bit
+// product: no modulo bias), key_b(t) = pair_mix64(pair_mix64(seed + b) ^ t); w_b(u) = #{t : the draw picks u}.
+// Resample 0 is the observed set, every multiplicity 1.
+constexpr int kBootThreads = 256;
+
+// one block per resample b = b0 + blockIdx.x: counts[blockIdx.x][u - u0] = w_b(u) for u in [u0, u0 + width); rows
+// b >= resamples (the call's B + 1) are zero.  Integer atomics, so the counts do not depend on the order.  limit > 0:
+// *over = 1 when a count exceeds it
+__global__ void __launch_bounds__(kBootThreads)
+boot_counts_kernel(long long F, long long u0, int width, int b0, int resamples, unsigned long long seed,
+                   uint32_t* __restrict__ counts, uint32_t limit, int* __restrict__ over) {
+    const int b = b0 + blockIdx.x;
+    uint32_t* row = counts + (size_t)blockIdx.x * width;
+    for (int k = threadIdx.x; k < width; k += kBootThreads) row[k] = b == 0 ? 1u : 0u;
+    if (b == 0 || b >= resamples) return;
+    __syncthreads();
+    const unsigned long long base = pair_mix64(seed + (unsigned long long)b);
+    for (long long t = threadIdx.x; t < F; t += kBootThreads) {
+        const long long u = (long long)__umul64hi(pair_mix64(base ^ (unsigned long long)t), (unsigned long long)F) - u0;
+        if (u >= 0 && u < width) atomicAdd(row + u, 1u);
+    }
+    if (limit == 0) return;
+    __syncthreads();
+    for (int k = threadIdx.x; k < width; k += kBootThreads)
+        if (__ldcg(row + k) > limit) *over = 1;
+}
+
+// unit_of[i] = the unit of row i (offsets [units + 1]); one thread per unit
+__global__ void boot_unit_index_kernel(const long long* __restrict__ offsets, int units, int* __restrict__ unit_of) {
+    for (int u = blockIdx.x * blockDim.x + threadIdx.x; u < units; u += gridDim.x * blockDim.x)
+        for (long long i = offsets[u]; i < offsets[u + 1]; ++i) unit_of[i] = u;
+}
+
+// weights[r][i] = counts[r][unit_of[i]] as fp16 (exact up to 2048), 0 for N <= i < Npad; grid (blocks, rows)
+__global__ void boot_weights_kernel(const uint32_t* __restrict__ counts, long long F, const int* __restrict__ unit_of,
+                                    int N, int Npad, __half* __restrict__ weights) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= Npad) return;
+    const size_t r = blockIdx.y;
+    weights[r * Npad + i] = __uint2half_rn(i < N ? counts[r * F + unit_of[i]] : 0u);
+}
+
+// one block per resample row of a pass: out[b] = (n_b, Q_b + sum_u n_u w_u (w_u - 1) / 2, sum_u w_u g_u) with
+// Q_b = pc[2 b] (the pass's label product), each sum over the units in a fixed order (perm_block_sum)
+__global__ void __launch_bounds__(kPermSumThreads)
+boot_unit_terms_kernel(const uint32_t* __restrict__ counts, long long F, const long long* __restrict__ offsets,
+                       const double* __restrict__ g, const double* __restrict__ pc, double* __restrict__ out) {
+    const uint32_t* w = counts + (size_t)blockIdx.x * F;
+    double n = 0.0, sxy = 0.0, self = 0.0;
+    for (long long u = threadIdx.x; u < F; u += kPermSumThreads) {
+        const double wu = (double)w[u], nu = (double)(offsets[u + 1] - offsets[u]);
+        n += wu * nu;
+        sxy += wu * g[u];
+        self += nu * (wu * (wu - 1.0) * 0.5);
+    }
+    n = perm_block_sum(n);
+    __syncthreads();
+    sxy = perm_block_sum(sxy);
+    __syncthreads();
+    self = perm_block_sum(self);
+    if (threadIdx.x == 0) {
+        double* o = out + 3 * (size_t)blockIdx.x;
+        o[0] = n;
+        o[1] = pc[2 * (size_t)blockIdx.x] + self;
+        o[2] = sxy;
+    }
 }
 
 // out[b] = (S_aa, S_bb, S_ab) = (P, ((T - L) - C) + P, (L + C) - 2 P) for the first `labellings` labellings

@@ -580,6 +580,10 @@ unit_records_kernel(const __half* __restrict__ emb, const long long* __restrict_
 // accumulator element runs the units in order, four per DMMA, from zero or from the value a previous launch stored:
 // when every launch but the last covers a multiple of 4 units (the host uses multiples of 64), the result is bitwise
 // the same however the units are cut into launches and the labellings into passes.  No atomics.
+//
+// kWeighted (the bootstrap, DESIGN.md 5.18): sums[b] += sum_u w_b(u) R_u, one accumulator, the A operand the integer
+// multiplicities w_b(u) of the launch's units (counts: [rows][count_stride], column 0 = the launch's first unit)
+// converted to fp64 in registers, exactly.  Same staging, order and invariance; bits and words are not read.
 constexpr int kRsTile = 64, kRsUnits = 16, kRsPitch = kRsTile + 4;
 constexpr int kRsUnitAlign = 64;                  // unit0 of every launch is a multiple of this
 
@@ -591,9 +595,12 @@ struct RecordSumsParams {
     int words;                   // words per labelling
     int rows;                    // labellings of this launch: rows past it are not read nor written
     int accumulate;              // 0: start from zero, 1: add to sums
-    double* sums;                // [rows][2][R]
+    double* sums;                // [rows][2][R]; kWeighted: [rows][R]
+    const uint32_t* counts;      // kWeighted: multiplicities [rows][count_stride] of the launch's units
+    long long count_stride;
 };
 
+template <bool kWeighted>
 __global__ void __launch_bounds__(256, 1)
 record_sums_kernel(const RecordSumsParams p)
 {
@@ -616,8 +623,12 @@ record_sums_kernel(const RecordSumsParams p)
                 const int m = m0 + wm + i * 8 + fr;
                 const long long n = n0 + wn + j * 8 + 2 * fk + e;
                 const bool in = p.accumulate && m < p.rows && n < R;
-                ca[i][j][e] = in ? p.sums[((size_t)m * 2) * R + n] : 0.0;
-                cb[i][j][e] = in ? p.sums[((size_t)m * 2 + 1) * R + n] : 0.0;
+                if constexpr (kWeighted) {
+                    ca[i][j][e] = in ? p.sums[(size_t)m * R + n] : 0.0;
+                } else {
+                    ca[i][j][e] = in ? p.sums[((size_t)m * 2) * R + n] : 0.0;
+                    cb[i][j][e] = in ? p.sums[((size_t)m * 2 + 1) * R + n] : 0.0;
+                }
             }
     const int mrow = m0 + wm + fr;                               // this thread's labelling rows: mrow + 8 i
     const uint32_t* lb = p.bits + (size_t)mrow * p.words;
@@ -640,6 +651,26 @@ record_sums_kernel(const RecordSumsParams p)
     for (int st = 0; st < stages; ++st) {
         const int buf = st & 1;
         if (st + 1 < stages) fetch(st + 1);
+        if constexpr (kWeighted) {
+            const uint32_t* cnt = p.counts + (size_t)mrow * p.count_stride + st * kRsUnits + fk;
+#pragma unroll
+            for (int kk = 0; kk < kRsUnits; kk += 4) {
+                const bool valid = st * kRsUnits + kk + fk < p.units;
+                double b[2];
+#pragma unroll
+                for (int j = 0; j < 2; ++j) b[j] = Rs[buf][kk + fk][wn + j * 8 + fr];
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const double a = valid && mrow + 8 * i < p.rows
+                        ? (double)__ldg(cnt + (size_t)8 * i * p.count_stride + kk) : 0.0;
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) sm90::dmma_884(ca[i][j][0], ca[i][j][1], a, b[j]);
+                }
+            }
+            if (st + 1 < stages) stage(buf ^ 1);
+            __syncthreads();
+            continue;
+        }
         const int ug = p.unit0 + st * kRsUnits;                  // a multiple of 16: the stage sits in one word
         uint32_t w[4];
 #pragma unroll
@@ -673,7 +704,9 @@ record_sums_kernel(const RecordSumsParams p)
             for (int e = 0; e < 2; ++e) {
                 const int m = m0 + wm + i * 8 + fr;
                 const long long n = n0 + wn + j * 8 + 2 * fk + e;
-                if (m < p.rows && n < R) {
+                if constexpr (kWeighted) {
+                    if (m < p.rows && n < R) p.sums[(size_t)m * R + n] = ca[i][j][e];
+                } else if (m < p.rows && n < R) {
                     p.sums[((size_t)m * 2) * R + n] = ca[i][j][e];
                     p.sums[((size_t)m * 2 + 1) * R + n] = cb[i][j][e];
                 }

@@ -14,6 +14,9 @@ error behaviour; the arithmetic runs on the H100 through the C ABI.
                                                               label-product tile pass (csrc/kad.cuh)
     calc_fad_comparison                                    -> permutation p-value of a FAD difference: file records,
                                                               labelled fp64 sums and batched Frechet chains (stats.cuh)
+    calc_fad_bootstrap, calc_kad_bootstrap                 -> bootstrap confidence intervals over the eval files:
+                                                              seeded multiplicities, weighted record sums (FAD) and a
+                                                              weighted label product (KAD)
     FrechetAudioDistance      fad.py:123-395 -> same methods; file <-> GPU staging is batched
 """
 from __future__ import annotations
@@ -131,6 +134,40 @@ class FADComparisonResults(NamedTuple):
     n_units_b: int
     n_rows_a: int
     n_rows_b: int
+
+
+class FADBootstrapResults(NamedTuple):
+    score: float                    # calc_frechet_distance(mu, cov, *calc_embd_statistics(all eval rows)), bitwise
+    observed: float                 # resample 0 (the observed set) on the weighted path
+    ci_low: float
+    ci_high: float
+    standard_error: float           # std(replicates, ddof=1)
+    bias: float                     # mean(replicates) - observed
+    replicates: np.ndarray          # float64 [resamples]
+    level: float
+    method: str                     # "percentile" or "basic"
+    resamples: int
+    seed: int
+    n_units: int
+    n_rows: int
+
+
+class KADBootstrapResults(NamedTuple):
+    score: float                    # calc_kernel_audio_distance_songs(emb_baseline, [all eval rows])[0].score, bitwise
+    observed: float
+    ci_low: float
+    ci_high: float
+    standard_error: float
+    bias: float
+    replicates: np.ndarray
+    level: float
+    method: str
+    resamples: int
+    seed: int
+    n_units: int
+    n_rows: int
+    bandwidth: float
+    n_baseline: int
 
 
 class PRDCResults(NamedTuple):
@@ -444,7 +481,7 @@ def calc_kad_comparison(emb_baseline, emb_a, emb_b, permutations: int = 999, see
                                 seed=seed, n_baseline=m, n_a=na, n_b=nb)
 
 
-def _fad_units(emb, what: str, d: int) -> list:
+def _fad_units(emb, what: str, d: int, metric: str = "the FAD comparison") -> list:
     """a list of fp16 [rows, d] arrays (files) or one 2-D fp16 array (one unit per row) -> the list of units"""
     if isinstance(emb, (list, tuple)):
         units = [np.asarray(u) for u in emb]
@@ -457,11 +494,11 @@ def _fad_units(emb, what: str, d: int) -> list:
         if u.ndim != 2 or u.shape[1] != d:
             raise ValueError(f"every {what} array must be [rows, {d}] (the baseline's width); got shape {u.shape}")
         if u.dtype != np.float16:
-            raise ValueError(f"the FAD comparison needs fp16 embeddings; {what} holds {u.dtype}")
+            raise ValueError(f"{metric} needs fp16 embeddings; {what} holds {u.dtype}")
         if u.shape[0] == 0:
             raise ValueError(f"every {what} file needs at least one row")
     if len(units) < 2:
-        raise ValueError(f"the FAD comparison needs at least two units (files) in {what}; got {len(units)}")
+        raise ValueError(f"{metric} needs at least two units (files) in {what}; got {len(units)}")
     return units
 
 
@@ -487,18 +524,24 @@ def calc_fad_comparison(baseline, eval_a, eval_b, permutations: int = 999, seed:
     [rows, d], an empty file, fewer than two units on a side, permutations outside [1, 9999] or a seed outside
     [0, 2**64), before any GPU work."""
     permutations, seed = _perm_args(permutations, seed, "a FAD comparison")
+    mu, cov, d = _fad_baseline(baseline, "the FAD comparison")
+    units_a, units_b = _fad_units(eval_a, "eval A", d), _fad_units(eval_b, "eval B", d)
+    return _fad_comparison(mu, cov, units_a, units_b, None, None, permutations, seed)
+
+
+def _fad_baseline(baseline, metric: str):
+    """(mu, cov) -> (mu, cov, d) as arrays, d a multiple of 64 up to 2048"""
     try:
         mu, cov = baseline
     except (TypeError, ValueError):
-        raise ValueError("the FAD comparison needs the baseline as (mu, cov)") from None
+        raise ValueError(f"{metric} needs the baseline as (mu, cov)") from None
     mu, cov = np.asarray(mu), np.asarray(cov)
     d = int(mu.shape[0]) if mu.ndim == 1 else -1
     if d <= 0 or cov.shape != (d, d):
         raise ValueError(f"the baseline must be (mu [d], cov [d, d]); got shapes {mu.shape} and {cov.shape}")
     if d % 64 != 0 or d > 2048:
-        raise ValueError(f"the FAD comparison needs an embedding width that is a multiple of 64 up to 2048; got {d}")
-    units_a, units_b = _fad_units(eval_a, "eval A", d), _fad_units(eval_b, "eval B", d)
-    return _fad_comparison(mu, cov, units_a, units_b, None, None, permutations, seed)
+        raise ValueError(f"{metric} needs an embedding width that is a multiple of 64 up to 2048; got {d}")
+    return mu, cov, d
 
 
 def _fad_comparison(mu, cov, units_a: list, units_b: list, score_a, score_b, permutations: int,
@@ -525,6 +568,142 @@ def _fad_comparison(mu, cov, units_a: list, units_b: list, score_a, score_b, per
                                 null_differences=diff[1:].copy(), permutations=permutations, seed=seed,
                                 n_units_a=len(units_a), n_units_b=len(units_b), n_rows_a=int(rows_a.shape[0]),
                                 n_rows_b=int(rows_b.shape[0]))
+
+
+def _boot_args(resamples, seed, level, method, metric: str):
+    if isinstance(resamples, bool) or not isinstance(resamples, (int, np.integer)) or not 2 <= resamples <= 9999:
+        raise ValueError(f"{metric} needs resamples in [2, 9999] (got {resamples!r})")
+    if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= seed < 2 ** 64:
+        raise ValueError(f"{metric} needs an integer seed in [0, 2**64) (got {seed!r})")
+    if isinstance(level, bool) or not isinstance(level, (int, float, np.floating)) or not 0.0 < level < 1.0:
+        raise ValueError(f"{metric} needs a level strictly between 0 and 1 (got {level!r})")
+    if method not in ("percentile", "basic"):
+        raise ValueError(f"{metric} needs method 'percentile' or 'basic' (got {method!r})")
+    return int(resamples), int(seed), float(level), method
+
+
+def _boot_interval(theta: np.ndarray, level: float, method: str):
+    """theta fp64 [B + 1] (theta[0] the observed set on the same path) -> (ci_low, ci_high, standard_error, bias)"""
+    rep, obs = theta[1:], float(theta[0])
+    q_lo, q_hi = (float(v) for v in np.quantile(rep, [(1.0 - level) / 2.0, (1.0 + level) / 2.0]))
+    lo, hi = (q_lo, q_hi) if method == "percentile" else (2.0 * obs - q_hi, 2.0 * obs - q_lo)
+    return lo, hi, float(np.std(rep, ddof=1)), float(np.mean(rep)) - obs
+
+
+def calc_fad_bootstrap(baseline, eval_units, resamples: int = 999, seed: int = 0, level: float = 0.95,
+                       method: str = "percentile") -> FADBootstrapResults:
+    """Bootstrap confidence interval of FAD: how precise is this score, given the eval files it was computed from?
+    baseline = (mu, cov) (as calc_fad_comparison takes it).  eval_units: a list of fp16 [rows, d] arrays, one per file,
+    or one 2-D fp16 array (one unit per row, which assumes independent rows).  Rows of one file are correlated, so whole
+    files are resampled: resample b >= 1 draws F files with replacement, draw t picking file
+    floor(pair_mix64(pair_mix64(seed + b) ^ t) F / 2^64) (DESIGN.md 5.18), and its replicate is the FAD of the multiset
+    of rows, each file's rows as often as the file was drawn, with its exact fp64 mean and ddof = 1 covariance.
+
+    The baseline is held fixed: the interval is the sampling spread of the eval set, conditional on the baseline (an
+    .npz baseline has no rows to resample).  With q_lo, q_hi the (1 -+ level) / 2 quantiles of the replicates (numpy's
+    default linear method), method "percentile" gives (q_lo, q_hi) and "basic" (2 observed - q_hi, 2 observed - q_lo);
+    standard_error = std(replicates, ddof=1), bias = mean(replicates) - observed.  FAD is biased upwards at small n,
+    and a resample's duplicate files add about the same bias again, so the percentile interval sits high; `bias` and
+    the basic interval are there for that reason.
+
+    score is calc_frechet_distance(mu, cov, *calc_embd_statistics(all rows)), the value FAD users see; `observed` is
+    resample 0 (the observed set) on the weighted path, which can differ from score by about 1e-4 relative because
+    calc_embd_statistics rounds the mean to fp16.  Raises ValueError for a baseline that is not (mu [d], cov [d, d])
+    with d a multiple of 64 up to 2048, arrays that are not fp16 [rows, d], an empty file, fewer than two units,
+    resamples outside [2, 9999], a seed outside [0, 2**64), a level outside (0, 1) or another method, before any GPU
+    work."""
+    resamples, seed, level, method = _boot_args(resamples, seed, level, method, "a FAD bootstrap")
+    mu, cov, d = _fad_baseline(baseline, "the FAD bootstrap")
+    units = _fad_units(eval_units, "eval", d, "the FAD bootstrap")
+    return _fad_bootstrap(mu, cov, units, None, resamples, seed, level, method)
+
+
+def _fad_bootstrap(mu, cov, units: list, score, resamples: int, seed: int, level: float,
+                   method: str) -> FADBootstrapResults:
+    """calc_fad_bootstrap on checked units; score None: the array score"""
+    from . import _native
+    rows = np.concatenate(units)
+    if score is None:
+        score = float(calc_frechet_distance(mu, cov, *calc_embd_statistics(rows)))
+    eng = _native.engine()
+    dev = eng.torch_device
+    base = _native.Baseline(eng, mu, cov)
+    offsets = torch.from_numpy(np.concatenate([[0], np.cumsum([u.shape[0] for u in units])]).astype(np.int64)).to(dev)
+    out, _ = base.frechet_boot(torch.from_numpy(rows).to(dev), offsets, resamples, seed)
+    theta = out[:, 0].cpu().numpy()
+    if not np.isfinite(theta).all():
+        raise ValueError("non-finite covariance statistics (NaN/Inf input)")
+    lo, hi, se, bias = _boot_interval(theta, level, method)
+    return FADBootstrapResults(score=score, observed=float(theta[0]), ci_low=lo, ci_high=hi, standard_error=se,
+                               bias=bias, replicates=theta[1:].copy(), level=level, method=method, resamples=resamples,
+                               seed=seed, n_units=len(units), n_rows=int(rows.shape[0]))
+
+
+def _kad_units(eval_units) -> list:
+    """a list of fp16 [rows, d] arrays or tensors (files) or one 2-D fp16 array (one unit per row) -> fp16 tensors"""
+    if isinstance(eval_units, (list, tuple)):
+        units = [_kad_rows(u, f"eval file {k}") for k, u in enumerate(eval_units)]
+    else:
+        y = _kad_rows(eval_units, "eval")
+        units = [y[i:i + 1] for i in range(y.shape[0])]
+    for u in units:
+        if u.shape[0] == 0:
+            raise ValueError("every eval file needs at least one row")
+        if u.shape[1] != units[0].shape[1]:
+            raise ValueError(f"embedding widths differ across the eval files ({units[0].shape[1]}, {u.shape[1]})")
+    if len(units) < 2:
+        raise ValueError(f"the KAD bootstrap needs at least two units (files) in eval; got {len(units)}")
+    return units
+
+
+def calc_kad_bootstrap(emb_baseline, eval_units, resamples: int = 999, seed: int = 0, level: float = 0.95,
+                       method: str = "percentile") -> KADBootstrapResults:
+    """Bootstrap confidence interval of KAD over the eval files (units as calc_fad_bootstrap takes them, resampled by
+    the same seeded rule).  Row i of a resample carries the multiplicity v_i of its file, n_b = sum v_i, and
+
+        S_yy(b) = sum_{i<j} v_i v_j K_ij + sum_u n_u w_u (w_u - 1) / 2,     S_xy(b) = sum_u w_u G_u,
+        KAD_b   = 1000 * (2 S_xx / (m (m - 1)) + 2 S_yy(b) / (n_b (n_b - 1)) - 2 S_xy(b) / (m n_b)),
+
+    the second term of S_yy counting the pairs of two copies of one row (K(y, y) = 1), G_u = sum_{x, i in u} k(x, y_i).
+    The baseline X [m, d] (fp16 rows, or a PairwiseBaseline) is held fixed, and so are sigma (X's bandwidth, as
+    calc_kernel_audio_distance uses it) and S_xx: the interval is the sampling spread of the eval set, conditional on the
+    baseline.  The quadratic form runs on the pair tiles of the eval rows with each kernel value rounded to fp16 once
+    and the multiplicities as exact fp16 weights (fad_kad_boot_sums); every other term is an fp64 unit sum.
+
+    Intervals, standard_error and bias as calc_fad_bootstrap (KAD is unbiased, but duplicate rows within a resample
+    still shift it).  score is bitwise calc_kernel_audio_distance_songs(emb_baseline, [all eval rows]); `observed` is
+    resample 0 on the fp16 path.  A PairwiseBaseline gives replicates bitwise equal to the rows'.  Raises ValueError as
+    calc_kad_test does, for fewer than two units or an empty file, and for resamples, seed, level or method as
+    calc_fad_bootstrap does, before any GPU work."""
+    from . import _native
+    resamples, seed, level, method = _boot_args(resamples, seed, level, method, "a KAD bootstrap")
+    units = _kad_units(eval_units)
+    parts, x_rows, m, (n,), prepared = _perm_pool(emb_baseline, [torch.cat(units)], ["eval"], "KAD")
+    sizes = np.array([int(u.shape[0]) for u in units], dtype=np.int64)
+    offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    eng = _native.engine()
+    dev = eng.torch_device
+    if prepared is not None:
+        yd = _kad_device_rows(parts[0], eng)
+        r = _kad_prepared(prepared, yd, np.array([0, n], dtype=np.int64))[0]
+        score, sigma, s_xx = r.score, prepared.sigma, prepared.s_xx
+        z = torch.cat([prepared.x, yd])
+    else:
+        z = _kad_device_rows(torch.cat([x_rows, parts[0]]), eng)
+        sigma = _kad_bandwidth(eng, z, m)
+        sig = torch.tensor([sigma], dtype=torch.float64, device=dev)
+        sums = eng.kad_song_sums(z, m, torch.tensor([0, n], dtype=torch.int64, device=dev), sig).cpu().numpy()
+        s_xx = float(sums[0])
+        score = _kad_score(s_xx, float(sums[1]), float(sums[2]), m, n)
+    sig = torch.tensor([sigma], dtype=torch.float64, device=dev)
+    offs = torch.from_numpy(offsets).to(dev)
+    g = eng.kad_eval_sums(z, m, offs, sig)[:, 1].contiguous()
+    s = eng.kad_boot_sums(z[m:], offs, sig, g, resamples, seed).cpu().numpy()
+    theta = _kad_score(s_xx, s[:, 1], s[:, 2], m, s[:, 0])
+    lo, hi, se, bias = _boot_interval(theta, level, method)
+    return KADBootstrapResults(score=score, observed=float(theta[0]), ci_low=lo, ci_high=hi, standard_error=se,
+                               bias=bias, replicates=theta[1:].copy(), level=level, method=method, resamples=resamples,
+                               seed=seed, n_units=len(units), n_rows=n, bandwidth=sigma, n_baseline=m)
 
 
 def calc_prdc(emb_baseline, emb_eval, k: int = 5, distributed: bool = False) -> PRDCResults:
@@ -1274,6 +1453,31 @@ class FrechetAudioDistance:
             arrs = [np.load(f) for f in _sorted_npy_files(Path(p) / "embeddings" / self.ml.name)]
             units.append(_fad_units([a for a in arrs if a.shape[0] > 0], what, d))
         return _fad_comparison(mu, cov, units[0], units[1], score_a, score_b, permutations, seed)
+
+    def score_fad_bootstrap(self, baseline: PathLike, eval_dir: PathLike, resamples: int = 999, seed: int = 0,
+                            level: float = 0.95, method: str = "percentile") -> FADBootstrapResults:
+        """Bootstrap confidence interval of score(baseline, eval_dir) (calc_fad_bootstrap), conditional on the baseline.
+        baseline is anything load_stats takes (a directory, an .npz file or a named set); the units are the sorted
+        cache files <eval_dir>/embeddings/<model>/*.npy, empty files dropped.  score is self.score's value."""
+        resamples, seed, level, method = _boot_args(resamples, seed, level, method, "a FAD bootstrap")
+        score = float(self.score(baseline, eval_dir))
+        mu, cov = self.load_stats(baseline)
+        d = int(np.asarray(mu).shape[0])
+        arrs = [np.load(f) for f in _sorted_npy_files(Path(eval_dir) / "embeddings" / self.ml.name)]
+        units = _fad_units([a for a in arrs if a.shape[0] > 0], "eval", d, "the FAD bootstrap")
+        return _fad_bootstrap(mu, cov, units, score, resamples, seed, level, method)
+
+    def score_kad_bootstrap(self, baseline_dir: PathLike, eval_dir: PathLike, resamples: int = 999, seed: int = 0,
+                            level: float = 0.95, method: str = "percentile", prepared: bool = False) -> KADBootstrapResults:
+        """Bootstrap confidence interval of KAD (calc_kad_bootstrap) between the cached embeddings of two directories,
+        read as score_kad reads them; the units are the eval directory's sorted cache files, empty files dropped.
+        prepared: against the baseline's saved pairwise preparation, with replicates bitwise the unprepared ones."""
+        resamples, seed, level, method = _boot_args(resamples, seed, level, method, "a KAD bootstrap")
+        x, _ = self._cached_sets(baseline_dir, eval_dir, "KAD", False)
+        if prepared:
+            x = self._prepared(baseline_dir, x, self._cached_offsets(baseline_dir, "KAD", False), 1, False)
+        arrs = [np.load(f) for f in _sorted_npy_files(kad_embedding_dir(eval_dir, self.ml.name))]
+        return calc_kad_bootstrap(x, [a for a in arrs if a.shape[0] > 0], resamples, seed, level, method)
 
     def _cached_offsets(self, baseline_dir: PathLike, metric: str, distributed: bool) -> np.ndarray:
         """the int64 row offsets of the baseline's cache files, from their headers"""

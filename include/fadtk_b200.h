@@ -543,6 +543,39 @@ int fad_frechet_perm(fad_handle* h, const double* mu1, const double* sqrt1, cons
                      const long long* offsets, long long n_units, long long a, int d, int labellings,
                      unsigned long long seed, int iters, void* shift_out, double* out, void* stream);
 
+/* ---- Bootstrap confidence intervals of FAD and KAD (DESIGN.md section 5.18).  An eval set of n_units >= 2 units
+ * (files: rows [offsets[u], offsets[u + 1]) of a fp16 [N, d] array, no empty unit) is resampled B = resamples times
+ * (2 <= B <= 9999) with replacement, whole units at a time; the baseline is held fixed.  Resample 0 is the observed
+ * set (every multiplicity 1); resample b >= 1 makes F = n_units draws t = 0 .. F - 1, draw t picking unit
+ * floor(pair_mix64(pair_mix64(seed + b) ^ t) * F / 2^64) (the high word of the 128-bit product), and w_b(u) counts
+ * the draws of u.  16-byte-aligned device pointers; every argument is checked first (offsets are read back, one
+ * stream synchronisation); a rejected call launches nothing and writes nothing.
+ *   fad_boot_counts      counts (device uint32 [B + 1][n_units]) = w_b(u); integer counts, bitwise reproducible
+ *   fad_boot_record_sums sums (device fp64 [B + 1][R(d)]) = sum_u counts[b][u] records[u] (records as
+ *                        fad_unit_records writes them, counts as fad_boot_counts does); fixed order, bitwise the same
+ *                        however the units are cut into chunks and the resamples into passes
+ *   fad_frechet_boot     out (device fp64 [B + 1][8], fad_frechet's layout, [7] = n_b) = the FAD of every resample
+ *                        against the baseline (mu1, sqrt1, scal1 as fad_frechet_records takes them): the weighted
+ *                        record sums of the units about the fp16 mean of all rows (written to shift_out, device fp16
+ *                        [d]), then fad_frechet_records' statistics and chain.  d a multiple of 64, at most 2048
+ *   fad_kad_boot_sums    out (device fp64 [B + 1][3]) = (n_b, S_yy(b), S_xy(b)) of every resample of the rows y_f16
+ *                        (d a multiple of 8): n_b = sum_u w_u n_u, S_yy(b) = sum_{i<j} v_i v_j K_ij + sum_u n_u w_u
+ *                        (w_u - 1) / 2 (v_i the multiplicity of row i's unit, K_ij = exp(-|y_i - y_j|^2 /
+ *                        (2 sigma^2)) rounded to fp16 once, weights fed to the tensor cores as fp16), S_xy(b) =
+ *                        sum_u w_u g_units[u] (g_units: device fp64 [n_units], per unit the sum of k(x, y) over the
+ *                        baseline rows and the unit's rows, e.g. column 1 of fad_kad_eval_sums).  sigma: device fp64
+ *                        scalar.  Fails (out not valid) if a multiplicity exceeds 2048, which n_units <= 2048 rules out */
+int fad_boot_counts(fad_handle* h, long long n_units, int resamples, unsigned long long seed, uint32_t* counts,
+                    void* stream);
+int fad_boot_record_sums(fad_handle* h, const double* records, long long n_units, int d, const uint32_t* counts,
+                         int resamples, double* sums, void* stream);
+int fad_frechet_boot(fad_handle* h, const double* mu1, const double* sqrt1, const double* scal1, const void* emb_f16,
+                     const long long* offsets, long long n_units, int d, int resamples, unsigned long long seed,
+                     int iters, void* shift_out, double* out, void* stream);
+int fad_kad_boot_sums(fad_handle* h, const void* y_f16, const long long* offsets, long long n_units, int d,
+                      const double* sigma, const double* g_units, int resamples, unsigned long long seed, double* out,
+                      void* stream);
+
 /* ---- audio conversion: replaces the torchaudio branch of FrechetAudioDistance.load_audio
  * (fadtk/fad.py:147-160): mono mix (:150), Resample(lowpass_filter_width=64, rolloff=0.9475937167399596,
  * sinc_interp_kaiser, beta=14.769656459379492) (:151-158), PCM16 quantisation (:160).
