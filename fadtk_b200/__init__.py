@@ -15,6 +15,7 @@ from .fad import RealismResults, calc_realism  # noqa: F401
 from .fad import NearestResults, calc_nearest  # noqa: F401
 from .fad import prepare_pairwise_baseline  # noqa: F401
 from .fad_batch import cache_embedding_files  # noqa: F401
+from .layers import cache_layer_embeddings, score_layers  # noqa: F401
 from .model_loader import ModelLoader, VGGishModel, CLAPLaionModel, WhisperModel, EncodecEmbModel, Wav2VecFamilyModel, W2V2Model, HuBERTModel, MERTModel, WavLMModel, UnbuiltModel, get_all_models  # noqa: F401
 from .utils import (PathLike, DeviceStatistics, calculate_embd_statistics_online,  # noqa: F401
                     find_sox_formats, get_cache_embedding_path, statistics_of_arrays)

@@ -76,6 +76,7 @@ SIGNATURES = {
     "fad_whisper_dec_layer": (C.c_int, [c_vp, C.c_int, c_vp, c_vp, c_ll, c_vp, c_vp]),
     "fad_w2v_load": (C.c_int, [c_vp, c_vp, c_vp, C.c_int, C.c_int, C.c_int]),
     "fad_w2v_forward": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, C.c_int, c_vp, c_vp]),
+    "fad_w2v_forward_taps": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, C.c_int, c_vp, c_vp]),
     "fad_w2v_normalize": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_w2v_conv": (C.c_int, [c_vp, C.c_int, c_vp, c_ll, C.c_int, c_vp, c_vp]),
     "fad_w2v_posconv": (C.c_int, [c_vp, c_vp, c_ll, C.c_int, c_vp, c_vp]),
@@ -578,6 +579,19 @@ class Engine:
         n, L = pcm.shape
         out = torch.empty((n, self.w2v_frames(L), self._w2v_d), dtype=torch.float16, device=pcm.device)
         _check(lib().fad_w2v_forward(self._h, pcm.data_ptr(), n, L, int(layer), out.data_ptr(), _stream()))
+        return out
+
+    def w2v_forward_taps(self, pcm: torch.Tensor, taps, out=None) -> torch.Tensor:
+        """pcm int16 [n_clips, L] (cuda, equal lengths), taps strictly increasing layers -> fp16
+        [n_taps, n_clips, frames, d_model], slice t = hidden_states[taps[t]] from ONE forward (written into `out` when
+        given)."""
+        assert pcm.dtype == torch.int16 and pcm.is_cuda and pcm.ndim == 2 and pcm.is_contiguous()
+        n, L = pcm.shape
+        taps = [int(t) for t in taps]
+        if out is None:
+            out = torch.empty((len(taps), n, self.w2v_frames(L), self._w2v_d), dtype=torch.float16, device=pcm.device)
+        arr = (C.c_int * max(1, len(taps)))(*taps)
+        _check(lib().fad_w2v_forward_taps(self._h, pcm.data_ptr(), n, L, arr, len(taps), _ptr(out), _stream()))
         return out
 
     # Stage entries of the loaded encoder: they write into the caller's cuda tensors (shapes in include/fadtk_b200.h)

@@ -150,25 +150,33 @@ def _convert_rest(part, clips, fad: FrechetAudioDistance, pool: ThreadPoolExecut
     return clips
 
 
-def _save_embeddings(ml: ModelLoader, group, flat: np.ndarray, rows, workers: int):
-    """``<dir>/embeddings/<model>/<stem>.npy`` for every file of ``group`` (fp16 [n_frames, d], as np.save writes it):
-    file i = the next rows[i] rows of ``flat``."""
-    paths, _ = _derived_paths(group, ml.name, ml.sr)
-    for d in {os.path.dirname(p) for p in paths}:
+def _save_embeddings(ml: ModelLoader, group, flat: np.ndarray, rows, workers: int, name: str = None, keep=None):
+    """``<dir>/embeddings/<name>/<stem>.npy`` (default name: the model's) for every file of ``group`` (fp16
+    [n_frames, d], as np.save writes it): file i = the next rows[i] rows of ``flat``.  ``keep`` (bool per file):
+    only those files are written."""
+    paths, _ = _derived_paths(group, ml.name if name is None else name, ml.sr)
+    sel = np.arange(len(group)) if keep is None else np.nonzero(np.asarray(keep, dtype=bool))[0]
+    for d in {os.path.dirname(paths[i]) for i in sel}:
         os.makedirs(d, exist_ok=True)
     rows = np.asarray(rows, dtype=np.int64)
     off = np.zeros(len(rows) + 1, dtype=np.int64)
     off[1:] = np.cumsum(rows)
     if flat.dtype == np.float16 and flat.ndim == 2:
-        st = _io_native.npy_write_f16(paths, np.ascontiguousarray(flat), off[:-1], rows, workers)
-        for i in np.nonzero(st != _io_native.OK)[0]:
+        st = _io_native.npy_write_f16([paths[i] for i in sel], np.ascontiguousarray(flat), off[sel], rows[sel], workers)
+        for k in np.nonzero(st != _io_native.OK)[0]:
             # the reference writes file by file and a failing np.save stops only that worker's loop (fad_batch.py:20-22);
             # here one bad path must not lose the embeddings of the other files of the batch: report it and go on - the
             # file stays without a cache entry and is picked up again by the next run
-            log.error(f"cannot write {paths[i]} (status {int(st[i])}); the other files of the batch were written")
+            log.error(f"cannot write {paths[sel[k]]} (status {int(st[k])}); the other files of the batch were written")
     else:                                                      # a plugin returning another dtype / rank: numpy decides the format
-        for i, p in enumerate(paths):
-            np.save(p, flat[off[i]:off[i + 1]])
+        for i in sel:
+            np.save(paths[i], flat[off[i]:off[i + 1]])
+
+
+def _save_outputs(ml: ModelLoader, names, group, flats, rows, missing, workers: int):
+    """every output j of a batch to the caches of names[j], only where that cache is missing (missing[file][j])"""
+    for j, (name, flat) in enumerate(zip(names, flats)):
+        _save_embeddings(ml, group, flat, rows, workers, name=name, keep=[missing[f][j] for f in group])
 
 
 def cache_embedding_files(files: Union[list[Path], str, Path], ml: ModelLoader, workers: int = 8, **kwargs):
@@ -177,17 +185,49 @@ def cache_embedding_files(files: Union[list[Path], str, Path], ml: ModelLoader, 
 
     Same signature as the reference; ``kwargs`` are forwarded to FrechetAudioDistance.
     """
+    def embed(clips):
+        flat, rows = ml.embed_pcm_batch_flat(clips)
+        return [flat], rows
+    _cache_outputs(files, ml, [ml.name], embed, workers, **kwargs)
+
+
+def cache_tapped_embedding_files(files: Union[list[Path], str, Path], ml: ModelLoader, taps, names, workers: int = 8,
+                                 **kwargs):
+    """Several layers of one forward per file: hidden_states[taps[t]] cached as ``<dir>/embeddings/<names[t]>/<stem>.npy``,
+    byte-identical to what cache_embedding_files writes with the loader of names[t].  ``ml`` is a loader with a tapped
+    path (model_loader.Wav2VecFamilyModel.embed_pcm_batch_flat_taps).  A file is embedded when any of its caches is
+    missing, and only the missing ones are written: an existing cache keeps its bytes and its mtime, which the
+    statistics caches' fingerprints depend on."""
+    taps = [int(t) for t in taps]
+    names = list(names)
+    if len(taps) != len(names) or not taps:
+        raise ValueError("one registry name per tap")
+
+    def embed(clips):
+        flat, rows = ml.embed_pcm_batch_flat_taps(clips, taps)
+        return list(flat), rows
+    _cache_outputs(files, ml, names, embed, workers, **kwargs)
+
+
+def _cache_outputs(files, ml: ModelLoader, names, embed, workers: int, **kwargs):
+    """The directory flow: embed(clips) -> (one flat array per output, rows per clip) for every file that lacks the
+    cache of any of ``names``; output j goes to the caches of names[j] that are missing."""
     if isinstance(files, (str, Path)):
         files = list(Path(files).glob('*.*'))
 
     files = [Path(f) for f in files]
+    missing = None
     if dist.rank() == 0:
-        emb_paths, _ = _derived_paths(files, ml.name, ml.sr)
-        done = {d: _names_in(d) for d in {os.path.dirname(p) for p in emb_paths}}
-        files = sorted(f for f, p in zip(files, emb_paths) if os.path.basename(p) not in done[os.path.dirname(p)])
+        miss = np.zeros((len(files), len(names)), dtype=bool)
+        for j, name in enumerate(names):
+            emb_paths, _ = _derived_paths(files, name, ml.sr)
+            done = {d: _names_in(d) for d in {os.path.dirname(p) for p in emb_paths}}
+            miss[:, j] = [os.path.basename(p) not in done[os.path.dirname(p)] for p in emb_paths]
+        missing = {f: tuple(bool(v) for v in m) for f, m in zip(files, miss) if m.any()}
+        files = sorted(f for f, m in zip(files, miss) if m.any())
     # ONE listing decides what is left to do: rank 0 filters the already-embedded files and every rank shards that
     # same list (a rank that lists the directory after another has started writing would see a different set)
-    files = dist.broadcast_object(files)
+    files, missing = dist.broadcast_object((files, missing))
     if len(files) == 0:
         log.info("All files already have embeddings, skipping.")
         return
@@ -216,11 +256,12 @@ def cache_embedding_files(files: Union[list[Path], str, Path], ml: ModelLoader, 
             clips = _convert_rest(part, clips, fad, pool)
             secs = [len(c) / ml.sr for c in clips]
             by_file = dict(zip(part, clips))
-            for group in _batches(part, secs, _BATCH_AUDIO_SECONDS):
-                flat, rows = ml.embed_pcm_batch_flat([by_file[f] for f in group])
+            # n outputs per file: the batch is cut n times shorter, so that the host copy of its outputs stays bounded
+            for group in _batches(part, secs, _BATCH_AUDIO_SECONDS / len(names)):
+                flats, rows = embed([by_file[f] for f in group])
                 if writer is not None:
                     writer.result()
-                writer = pool.submit(_save_embeddings, ml, group, flat, rows, workers)
+                writer = pool.submit(_save_outputs, ml, names, group, flats, rows, missing, workers)
         if writer is not None:
             writer.result()
     dist.barrier()

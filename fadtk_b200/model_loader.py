@@ -550,17 +550,32 @@ class Wav2VecFamilyModel(_DeviceBatch, ModelLoader):
         return self.embed_equal_length([pcm])[0]
 
     def _embed_device(self, clips):
+        return [e[0] for e in self._embed_device_taps(clips, [self.layer])]
+
+    def embed_equal_length(self, clips):
+        return list(self.embed_equal_length_taps(clips, [self.layer])[0])
+
+    def embed_pcm_batch_flat(self, clips):
+        flat, rows = self.embed_pcm_batch_flat_taps(clips, [self.layer])
+        return flat[0], rows
+
+    # ---- several layers of one forward (fad_w2v_forward_taps): the per-layer sweep of fadtk_b200.layers
+    def _embed_device_taps(self, clips, taps):
+        """list of int16 arrays -> one cuda fp16 tensor [n_taps, n_i, d] per clip (hidden_states[taps[t]]).  Clips of
+        equal length share one launch sequence; files over limit_minutes are truncated like the reference does."""
         clips = [np.asarray(c, dtype=np.int16)[:self.limit] for c in clips]
         out = [None] * len(clips)
         groups = {}
         for i, c in enumerate(clips):
             groups.setdefault(len(c), []).append(i)
         for _, idx in groups.items():
-            for i, e in zip(idx, self.embed_equal_length([clips[i] for i in idx])):
-                out[i] = e
+            emb = self.embed_equal_length_taps([clips[i] for i in idx], taps)
+            for j, i in enumerate(idx):
+                out[i] = emb[:, j]
         return out
 
-    def embed_equal_length(self, clips):
+    def embed_equal_length_taps(self, clips, taps):
+        """equal-length int16 clips -> cuda fp16 [n_taps, n_clips, frames, d]"""
         self._ensure_loaded()
         eng = self._engine
         L = len(clips[0])
@@ -569,7 +584,17 @@ class Wav2VecFamilyModel(_DeviceBatch, ModelLoader):
             eng.w2v_load(*self._packed, 1, max_len=L)
             self.max_clips = 1
         pcm = torch.from_numpy(flat_pcm(clips).reshape(len(clips), -1)).pin_memory().to(eng.torch_device, non_blocking=True)
-        return list(eng.w2v_forward(pcm, self.layer))
+        return eng.w2v_forward_taps(pcm, taps)
+
+    def embed_pcm_batch_flat_taps(self, clips, taps):
+        """list of int16 arrays -> (fp16 host array [n_taps, sum n_i, d], rows per clip) with ONE device -> host copy:
+        what the batch driver writes to the ``.npy`` caches of every tapped layer."""
+        parts = self._embed_device_taps(clips, taps)
+        rows = [int(p.shape[1]) for p in parts]
+        flat = torch.cat(parts, dim=1) if len(parts) > 1 else parts[0].contiguous()
+        host = torch.empty(flat.shape, dtype=flat.dtype, pin_memory=True)
+        host.copy_(flat)                                     # synchronous: pinned destination
+        return host.numpy(), rows
 
 
 def _layer_name(prefix: str, size: str, layer: int) -> str:

@@ -219,6 +219,13 @@ int fad_encodec_lstm(fad_handle* h, const float* z_f32, long long n_clips, int T
 int fad_w2v_load(fad_handle* h, const int* cfg, const void* const* tensors_host, int n_tensors, int max_clips, int max_len);
 /* pcm: int16 mono [n_clips][L] (device), equal lengths; emb_out: fp16 [n_clips][frames(L)][d_model]. */
 int fad_w2v_forward(fad_handle* h, const int16_t* pcm, long long n_clips, int L, int layer, void* emb_out_f16, void* stream);
+/* Several layers of one forward.  taps: host int[n_taps], strictly increasing, each in [0, layers]; out: fp16
+ * [n_taps][n_clips][frames(L)][d_model], 16-byte aligned, slice t = hidden_states[taps[t]], bitwise what
+ * fad_w2v_forward(..., taps[t], ...) writes.  The encoder runs once per max_clips chunk, up to the deepest tap.
+ * Fails, launching nothing and writing nothing, on a missing load, null pcm / taps / out, n_clips < 1,
+ * n_taps outside [1, layers + 1], taps out of order or range, a misaligned out, or L outside [400, max_len]. */
+int fad_w2v_forward_taps(fad_handle* h, const int16_t* pcm, long long n_clips, int L, const int* taps, int n_taps,
+                         void* out_f16, void* stream);
 /* Stage entries (parity tests); each calls the launch code fad_w2v_forward calls and fails, launching nothing and
  * writing nothing, on arguments it could not honour.  B in [1, max_clips]; 16-byte aligned device pointers.
  * fad_w2v_normalize (no load needed): pcm int16 [n_clips][L] -> out fp32 [n_clips][L], (x - mean) / sqrt(var + 1e-7).
